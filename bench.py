@@ -6,7 +6,7 @@
     python bench.py --impl reference ...      # the reference algorithm's CPU implementation (oracle port) on the host cores
 
 Workload (config.workload = "cfg2"): BASELINE.json configs[1], "neus_in_10_minutes BMVS-style object (LoTD + fused MLP),
-800x600, 1 B200": a CFG-sized LoTDNeuS (16-level LoTD, 12.13 M params, 32->64->1 SDF decoder, 58->64->64->3 radiance net,
+800x600, 1 GPU": a CFG-sized LoTDNeuS (16-level LoTD, 12.13 M params, 32->64->1 SDF decoder, 58->64->64->3 radiance net,
 64^3 occupancy grid), synthetic sphere-like SDF, one full 800x600 frame (480 000 rays) per step, rendered in ray chunks.
 A step = ray_test -> march -> 3-stage up-sampling -> boundary SDF (grad) -> alpha -> compression -> colour/normal query
 -> compositing -> scalar loss over rgb/depth/normals/mask -> backward to every parameter (-> one NCCL all-reduce of the
@@ -132,10 +132,9 @@ def loss_of(rendered):
 class ClockSampler:
     """SM clock + throttle reasons during the timed region.
 
-    Measured on this pool (profiles/diag_clock_sampler.sh, /tmp logs of round 1): ANY concurrent poller -- a looping `nvidia-smi -lms 100..1000`,
-    a thread forking nvidia-smi, an NVML thread -- makes 7 of 8 runs of this launch- and sync-heavy step show 80-230 ms stalls inside 15 ms steps
-    (NVML queries disturb CUDA submission for ~100 ms; even a query made between two steps shows up in the next ones, profiles/diag_*.sh); with no
-    poller -- and no NVML session inside this process -- steps are 14.2-15.8 ms.  So ONE sample is taken, by a separate one-shot `nvidia-smi`
+    Any concurrent poller -- a looping `nvidia-smi -lms 100..1000`, a thread forking nvidia-smi, an NVML thread -- was seen to stall a launch- and
+    sync-heavy step several-fold (NVML queries disturb CUDA submission; even a query made between two steps shows up in the next ones,
+    profiles/diag_*.sh).  So ONE sample is taken, by a separate one-shot `nvidia-smi`
     process, at the one moment it cannot perturb the measurement and is still "during" it: right after the LAST step of the resident loop has been
     enqueued -- the GPU is then executing the timed steps and nothing of ours is left to launch."""
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -236,7 +235,7 @@ def run_reference(args, rank):
 
 def use_reference_cuda_kernels():
     """BASELINE.md B1: route the SAME host orchestration through the REFERENCE'S OWN CUDA kernels (oracle/_ref: `_lotd`,
-    `_pack_ops`, `_occ_grid`, `_shencoder` compiled from /root/reference) and switch every fused path off, i.e. the op
+    `_pack_ops`, `_occ_grid`, `_shencoder` compiled from the reference project) and switch every fused path off, i.e. the op
     sequence nr3d_lib executes (16-level gather kernels, autocast cuBLAS MLPs, one-thread-per-pack pack_ops, fp16 atomics).
     Only used by `--impl reference-cuda` and the `reference_cuda` field; never by the product path."""
     sys.path.insert(0, os.path.join(ROOT, "oracle"))
@@ -504,6 +503,20 @@ def stats_of(ts):
     return dict(mean=float(a.mean()), median=float(np.median(a)), min=float(a.min()), max=float(a.max()))
 
 
+def dump_outputs(out_dir, rendered, loss, flat, n_grad=2 * 1024 * 1024):
+    """What one fwd+bwd step hands its caller: the rendered buffers, the loss and the parameter gradient (flat fp32 buffer) -- the
+    gradient as a fixed seeded sample of n_grad entries and their indices (24 MB), so that the files stay under 64 MB for a full
+    800x600 frame."""
+    os.makedirs(out_dir, exist_ok=True)
+    outs = {k: v.detach().float().cpu().numpy() for k, v in rendered.items()}
+    outs["loss"] = loss.detach().float().reshape(1).cpu().numpy()
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:n_grad].sort().values
+    outs["grad_sample"] = flat.detach()[idx.to(flat.device)].float().cpu().numpy()
+    outs["grad_sample_index"] = idx.double().numpy()
+    for k, v in outs.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), v)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -525,7 +538,14 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-ref-cuda", action="store_true")
     ap.add_argument("--dump-render", default=None, help="(internal) save the rendered buffers of view 0 to this file")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (rendered buffers, loss, a fixed sample of the "
+                         "parameter gradient) to DIR/<name>.npy, float32, < 64 MB in all")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "cfg2" or args.impl != "ours"):
+        raise SystemExit("bench.py: --dump-outputs is supported for --workload cfg2 --impl ours")
+    if args.dump_outputs and args.mode == "host" and 0 < args.rayschunk < args.rays:
+        raise SystemExit("bench.py: --dump-outputs needs the whole batch in one render call (--rayschunk 0 or >= --rays)")
 
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
@@ -566,7 +586,7 @@ def main():
     views_host, views_dev = [], []
     for k in range(N_VIEWS):
         if args.scaling == "strong":           # ONE frame per step, its rows dealt to the ranks round-robin (row r -> rank r mod N): contiguous
-            # blocks would give the ranks that own the object's rows most of the work (measured: 38 % efficiency at N = 8, profiles/r02s_*)
+            # blocks would give the ranks that own the object's rows most of the work
             o, d = pinhole_rays(H, W, orbit(k, N_VIEWS))
             o, d = strong_shard(o, d, rank, world, args.rays, n_rays, seed=(1000 + k) if args.random_rays else None)
             if o.shape[0] < n_rays:                # the last rank's block is padded with its own last ray
@@ -624,7 +644,7 @@ def main():
             loss = total
         if world > 1:
             dist.all_reduce(flat)                # the one collective of a step: sum of the flat gradient
-        last["rendered"] = rendered
+        last["rendered"], last["loss"] = rendered, loss
         return loss
 
     def timed(fn, k, sampler=None):
@@ -673,6 +693,8 @@ def main():
         torch.cuda.synchronize()
         t_res = timed(resident, args.steps, clocks)      # ... and the one clock query comes after its last launch (see ClockSampler)
         gc.enable()
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last["rendered"], last["loss"], flat)
         overflow = int(frame.counts()["overflow"]) if frame is not None else 0
         # a separate, instrumented pass for the roofline: the same step launched kernel by kernel with CUDA events around every launch of
         # the hash-gather kernels (not part of `value`); sizes are read back after every step to count the points that were processed
@@ -729,27 +751,19 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (6650.0, "fallback")
+    peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (3350.0, "H100 SXM data sheet")
     kt = _lib.KERNEL_TIMER.summary()
-    # the dominant kernel: the boundary SDF query (k_fused_sdf_tc, "fused_sdf_fwd": hash gather + tcgen05 decoder over the 65 coarse + 51 fine
-    # samples of every ray) -- 35-40 % of the step.  (The no-grad queries of the up-sampling half run inside the persistent per-ray kernel.)
+    # the dominant kernel: the boundary SDF query (k_fused_sdf_tc, "fused_sdf_fwd": hash gather + wgmma decoder over the 65 coarse + 51 fine
+    # samples of every ray).  (The no-grad queries of the up-sampling half run inside the persistent per-ray kernel.)
     gather = dict(kt["fused_sdf_fwd"]) if "fused_sdf_fwd" in kt else None
     if gather and frame is not None:
         gather["units"] = points["boundary"]          # points actually processed (the launch is sized by capacity)
-    traffic, traffic_note = None, None
-    try:       # dram bytes of the dominant gather launch, from the committed ncu --set full capture (per launch, like `achieved`)
-        tj = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))
-        traffic = tj["traffic_bytes_per_launch"]
-        traffic_note = {"unit": "bytes per launch (dram read + write)", "algorithmic_bytes_of_that_launch": tj["algorithmic_bytes_per_launch"], "source": tj["source"]}
-    except Exception:
-        pass
     roof = None
     if gather and gather["ms"] > 0:
         achieved = gather["units"] * 512.0 / (gather["ms"] * 1e-3) / 1e9     # 512 B of table per encoded point (SURVEY §8d)
         per_ms = {k: v["ms"] / inst_steps for k, v in kt.items()}
-        roof = {"kernel": "LoTD hash gather: k_fused_sdf_tc (gather + tcgen05 decoder), the boundary SDF query of the step (one launch per step)", "bound": "hbm",
-                "achieved": achieved, "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                "traffic_note": traffic_note, "points_per_launch": gather["units"] / max(gather["launches"], 1), "launches": gather["launches"],
+        roof = {"kernel": "LoTD hash gather: k_fused_sdf_tc (gather + wgmma decoder), the boundary SDF query of the step (one launch per step)", "bound": "hbm",
+                "achieved": achieved, "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": achieved / peak, "points_per_launch": gather["units"] / max(gather["launches"], 1), "launches": gather["launches"],
                 "avg_launch_ms": gather["ms"] / max(gather["launches"], 1), "share_of_step": gather["ms"] / max(sum(t_inst), 1e-9),
                 "per_kernel_ms_per_step": per_ms, "points_per_step": {k: v / inst_steps for k, v in points.items()} if frame is not None else None,
                 "how": "CUDA events around every launch of these kernels in a separate kernel-by-kernel pass of the same step (events cannot sit inside the graph)"}
@@ -765,7 +779,7 @@ def main():
                    "step": {"graph": "one CUDA-graph launch per step, no host read (sizes stay on the device)", "static": "kernel-by-kernel, no host read",
                             "host": "kernel-by-kernel, three host reads per step"}[mode],
                    "samples_per_ray": "<=116 boundary, <=1024 marched",
-                   "parallelism": f"dp{world} ray-shard ({args.scaling}), 1 all-reduce/step", "l2": "256 MiB L2 flush between steps; per-step working set >> 126 MB",
+                   "parallelism": f"dp{world} ray-shard ({args.scaling}), 1 all-reduce/step", "l2": "256 MiB L2 flush between steps; per-step working set >> 50 MB",
                    "camera_poses": n_views, "arena_overflow": overflow,
                    "arenas": {"march_cap": frame.march_cap, "kept_cap": frame.kept_cap} if frame is not None else None},
         "e2e": {"value": tot_rays / (ms_e2e * 1e-3) / 1e6, "unit": "Mrays/s", "ms_per_step": ms_e2e,
@@ -793,7 +807,7 @@ def main():
             rl = json.loads(r.stdout.strip().splitlines()[-1])
             line["reference_cuda"] = {"value": rl["value"], "unit": "Mrays/s", "ms_per_step": rl["ms_per_step"], "median_ms_per_step": rl["median"]["ms_per_step"],
                                       "e2e": rl["e2e"]["value"], "steps": rl["steps"], "warmup": rl["warmup"],
-                                      "what": "reference nr3d_lib CUDA kernels compiled from /root/reference (oracle/_ref), same B200, same workload"}
+                                      "what": "reference nr3d_lib CUDA kernels compiled by oracle/build_ref.py (oracle/_ref), same GPU, same workload"}
             line["vs_reference_cuda"] = {"value_ratio": line["value"] / rl["value"], "e2e_ratio": line["e2e"]["value"] / rl["e2e"]["value"],
                                          "median_ratio": line["median"]["value"] / rl["median"]["value"]}
             if os.path.exists(dump):

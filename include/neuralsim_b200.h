@@ -1,8 +1,8 @@
-/* neuralsim_b200 -- C ABI of the B200-native NeuS volume-rendering hot path.
+/* neuralsim_b200 -- C ABI of the H100-native (sm_90a) NeuS volume-rendering hot path.
  *
  * This header is the drop-in boundary (SURVEY.md §8b): every entry point is what the reference's own
  * native extensions (`nr3d_lib.bindings._lotd / _pack_ops / _occ_grid / _shencoder`, built by
- * /root/reference/nr3d_lib/setup.py:134,184,239,516) expose to Python, restated as plain C: raw *device*
+ * nr3d_lib/setup.py:134,184,239,516) expose to Python, restated as plain C: raw *device*
  * pointers + sizes + a stream, no torch / ATen types.  The pybind11 / ctypes shim a maintainer would put on
  * top is shown in INTEGRATION.md; `neuralsim_b200/bindings/*.py` is that shim over ctypes.
  *
@@ -350,7 +350,7 @@ int nsb_occ_ema_update(const float *pts, const float *val, int64_t n, int32_t va
 
 /* ---------------------------------------------------------------- fused colour / normal query (csrc/color_tc.cu)
  * The whole LoTDNeuS.forward of the reference for packed samples (nr3d_lib/models/fields/neus/lotd_neus.py:141-167 =
- * LoTDSDF.forward_sdf_nablas, lotd_sdf.py:201-257, + RadianceNet.forward, mlp_nerf.py:267-289) as one tcgen05 kernel, and
+ * LoTDSDF.forward_sdf_nablas, lotd_sdf.py:201-257, + RadianceNet.forward, mlp_nerf.py:267-289) as one wgmma kernel, and
  * its backward including the second-order pass through nablas (LoTDFunctionBwdDydx.backward, lotd.py:193-268) as two.
  * All weight pointers are fp16 device images of the fp32 masters (what autocast feeds the GEMMs). */
 typedef struct nsb_color_net {

@@ -1,4 +1,4 @@
-"""neuralsim_b200 -- B200-native (sm_100a) NeuS volume-rendering hot path behind the nr3d_lib operator boundary.
+"""neuralsim_b200 -- H100-native (sm_90a) NeuS volume-rendering hot path behind the nr3d_lib operator boundary.
 
 Layout
   csrc/        hand-written CUDA kernels + the C ABI (include/neuralsim_b200.h) -> libneuralsim_b200.so

@@ -52,7 +52,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"neuralsim_b200: {LIB_PATH} is missing. Build it with `python -m neuralsim_b200.build` "
-                "(nvcc, sm_100a). There is no CPU fallback for this package.")
+                "(nvcc, sm_90a). There is no CPU fallback for this package.")
         _lib = ctypes.CDLL(LIB_PATH)
         _lib.nsb_last_error.restype = ctypes.c_char_p
         _lib.nsb_launch_count.restype = ctypes.c_uint64

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's native-extension modules (`nr3d_lib.bindings._*`).
 
 `neuralsim_b200.bindings._lotd / _pack_ops / _occ_grid / _shencoder` export the functions, argument orders and
-error behaviour of the pybind11 modules built by /root/reference/nr3d_lib/setup.py, implemented by ctypes calls
+error behaviour of the pybind11 modules built by nr3d_lib/setup.py, implemented by ctypes calls
 into libneuralsim_b200.so.  `install_as_nr3d_lib_bindings()` registers them under the reference's module names so
 that an unmodified `nr3d_lib` Python tree imports them (INTEGRATION.md).
 

@@ -1,7 +1,7 @@
 """Drop-in for `nr3d_lib.bindings._lotd` (reference: nr3d_lib/csrc/lotd/src/lotd.cpp:22-107) over the C ABI.
 
 Same names, argument order and error behaviour (RuntimeError) as the pybind11 module; the encoding kernels
-are the sm_100a ones of neuralsim_b200/csrc/lotd.cu.  Supported: Dense / Hash levels, linear interpolation,
+are the sm_90a ones of neuralsim_b200/csrc/lotd.cu.  Supported: Dense / Hash levels, linear interpolation,
 single (non-batched, non-forest) tables -- the `c_hash_only` configuration every NeuS config of the reference
 uses.  Unsupported arguments raise instead of silently taking another path.
 """

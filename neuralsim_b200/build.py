@@ -1,4 +1,4 @@
-"""Builds libneuralsim_b200.so (C ABI, sm_100a only) in-tree with nvcc.
+"""Builds libneuralsim_b200.so (C ABI, sm_90a only: H100) in-tree with nvcc.
 
     python -m neuralsim_b200.build            # incremental
     python -m neuralsim_b200.build --force
@@ -19,7 +19,8 @@ OBJ = os.path.join(CSRC, "_build")
 LIB = os.path.join(HERE, "libneuralsim_b200.so")
 SOURCES = ["common.cu", "lotd.cu", "march.cu", "pack_ops.cu", "sh.cu", "fused.cu", "fused_tc.cu", "neus_fused.cu", "neus_glue.cu", "color_tc.cu", "ray_upsample.cu", "occ_ema.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v", "-I", os.path.join(os.path.dirname(HERE), "include")]
 
 
@@ -53,8 +54,7 @@ def build_library(force=False, verbose=False):
         res = list(ex.map(lambda s: _compile(s, force, hdr, verbose), SOURCES))
     objs = [o for o, _ in res]
     if force or not os.path.exists(LIB) or any(os.path.getmtime(o) > os.path.getmtime(LIB) for o in objs):
-        r = subprocess.run([NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a",
-                            "-cudart", "static"], capture_output=True, text=True)
+        r = subprocess.run([NVCC, "-shared", "-o", LIB, *objs, *ARCH, "-cudart", "static"], capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
     if verbose:

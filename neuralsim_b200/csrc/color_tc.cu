@@ -1,6 +1,6 @@
 // Fused colour / normal query of the NeuS field and its backward (incl. the second-order path through nablas) on the
-// 5th-generation tensor cores (tcgen05 + TMEM), sm_100a.  One CTA = 128 threads = one tile of 128 points, thread r owns
-// point r (TMEM lane r).  Replaces, for the packed samples that survive compression, the reference's chain
+// Hopper tensor cores (wgmma), sm_90a.  One CTA = 128 threads = one warpgroup = one tile of 128 points, thread r owns
+// point r (row r of the accumulators staged in shared memory, tc_util.cuh).  Replaces, for the packed samples that survive compression, the reference's chain
 //   LoTDNeuS.forward (lotd_neus.py:141-167) = LoTDSDF.forward_sdf_nablas (lotd_sdf.py:201-257: LoTDFunctionFwdDydx ->
 //   decoder -> autograd.grad -> LoTDFunctionBwdDydx) + RadianceNet.forward (mlp_nerf.py:267-289)
 // and its autograd backward (LoTDFunctionBwdDydx.backward = lod_bwd_bwd_input, lotd.py:193-268; the autocast MLP
@@ -10,7 +10,7 @@
 //                    nablas = J^T g (J recomputed per level, never stored) -> radiance input row -> MMA -> relu -> MMA ->
 //                    relu -> 64->3 -> sigmoid.   Saves the fp16 activation tiles Z, X, Y1, Y2 in core-matrix layout.
 //   k_color_rad_bwd  radiance backward from the saved tiles: dZ2, dZ1 (MMA), dh (MMA), weight gradients accumulated in
-//                    TMEM over all tiles of the persistent CTA (MN-major MMAs contracting over the 128 points).
+//                    shared memory over all tiles of the persistent CTA (MN-major MMAs contracting over the 128 points).
 //   k_color_sdf_bwd  gather pass for dg = J.dn, MMA du = dG.W1^T, MMA g = U.W1, dz (softplus'' term + sdf term),
 //                    MMA dh = dZ.W1, weight-gradient MMAs, one merged scatter (g (x) second-order weights + dh (x) trilinear
 //                    weights) into the fp32 table gradient.
@@ -122,7 +122,7 @@ __device__ __forceinline__ void load_point_net(const PointSrc &ps, int64_t i, bo
     for (int d = 0; d < 3; ++d) xs[d] = fminf(fmaxf(__fmaf_rn(xn[d], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
 }
 
-// The colour kernels run at 2-3 CTAs per SM (TMEM / shared-memory bound), i.e. 8-12 warps: their gathers live on loads in flight PER THREAD, and
+// The colour kernels run at 1-2 CTAs per SM (shared-memory bound), i.e. 4-8 warps: their gathers live on loads in flight PER THREAD, and
 // registers are plentiful -> four levels (32 corner loads) per gather trip instead of the two of k_fused_sdf_tc (which runs 24 warps per SM).
 constexpr int kColorGatherU = 4;
 
@@ -141,12 +141,12 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
     uint8_t *sW1T = sW1 + HW * NF * 2;                         //  4 KB W1^T [32 x 64]
     uint8_t *sR1 = sW1T + HW * NF * 2;                         //  8 KB R1 [64 x 64] (internal column order)
     uint8_t *sR2 = sR1 + XW * XW * 2;                          //  8 KB R2 [64 x 64]
+    constexpr int kS = tc::acc_stride(64);
+    float *acc = reinterpret_cast<float *>(sR2 + XW * XW * 2); // 34 KB staged accumulator rows (Z, g, Y1, Y2 in turn)
     __shared__ float sb1[HW], sW2[HW], srb1[XW], srb2[XW], sR3[3][XW];
     __shared__ float sb2, srb3[3];
-    __shared__ __align__(8) uint64_t mbar;
-    __shared__ uint32_t tmem_slot;
 
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     {
         DecoderDevTC dec{net.W1, net.b1, net.W2, net.b2, net.width, net.beta};
         stage_W1(dec, sW1, tid);
@@ -171,21 +171,12 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
     if (tid == 0) {
         sb2 = __half2float(net.b2[0]);
         for (int k = 0; k < 3; ++k) srb3[k] = __half2float(net.rb3[k]);
-        tc::mbar_init(&mbar, 1);
-        tc::fence_mbar_init();
     }
-    if (warp == 0) tc::tmem_alloc<128>(&tmem_slot);
     tc::fence_async_smem();
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = tmem_slot;
-    const uint32_t id64 = tc::make_idesc(kTile, 64, 0, 0), id32 = tc::make_idesc(kTile, 32, 0, 0);
     const uint32_t x_addr = tc::smem_u32(sX), u_addr = tc::smem_u32(sU), w1_addr = tc::smem_u32(sW1), w1t_addr = tc::smem_u32(sW1T);
     const uint32_t r1_addr = tc::smem_u32(sR1), r2_addr = tc::smem_u32(sR2);
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
     const SoftplusK spk(net.beta);
-    uint32_t phase = 0;
 
     const int64_t n_tiles = (n + kTile - 1) / kTile;
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -197,24 +188,15 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         gather_row_to_tile<kTile, kColorGatherU>(m, grid, xs, max_level, sX, tid);          // h -> chunks 0..3 of X
         tc::fence_async_smem();
         __syncthreads();
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < NF / 16; ++ks)
-                tc::mma_f16_ss(tmem, tc::make_desc(x_addr + ks * 2 * kChunk, kChunk, 128), tc::make_desc(w1_addr + ks * 2 * (HW * 16), HW * 16, 128),
-                               id64, ks > 0);
-            tc::commit(&mbar);
-        }
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
+        tc::mma_to_rows<64, 0, 0, NF / 16>(acc, kS, 0, tc::kmajor(x_addr, kTile), tc::kmajor(w1_addr, HW), false);   // Z = H . W1^T
+        __syncthreads();
         // ---- decoder epilogue: z, a -> sdf ; u = fp16(w2 * s) (first-order cotangent at z)
         float out = 0.f;
         uint8_t *zt = Zt ? Zt + tile * kTileBytes : nullptr;
 #pragma unroll 1
         for (int c = 0; c < HW / 8; ++c) {
             float z[8], uu[8];
-            tc::tmem_ld8(tmem + lane_base + c * 8, z);
+            tc::acc_ld8(acc, kS, tid, c * 8, z);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 z[j] = r16f(z[j] + sb1[c * 8 + j]);
@@ -228,25 +210,15 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         }
         const float sdf = r16f(out + sb2);
         tc::fence_async_smem();
-        tc::fence_before_sync();
         __syncthreads();
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < HW / 16; ++ks)                             // g = U . W1
-                tc::mma_f16_ss(tmem + 64, tc::make_desc(u_addr + ks * 2 * kChunk, kChunk, 128),
-                               tc::make_desc(w1t_addr + ks * 2 * (NF * 16), NF * 16, 128), id32, ks > 0);
-            tc::commit(&mbar);
-        }
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
+        tc::mma_to_rows<32, 0, 0, HW / 16>(acc, kS, 0, tc::kmajor(u_addr, kTile), tc::kmajor(w1t_addr, NF), false);   // g = U . W1
+        __syncthreads();
         // ---- second gather pass: nablas01 = J^T g, f ascending (k_lotd_bwd_input order)
-        float acc[3] = {0.f, 0.f, 0.f};
+        float nacc[3] = {0.f, 0.f, 0.f};
 #pragma unroll 1
         for (uint32_t g4 = 0; g4 < 4; ++g4) {
             float gg[8];
-            tc::tmem_ld8(tmem + 64 + lane_base + g4 * 8, gg);
+            tc::acc_ld8(acc, kS, tid, g4 * 8, gg);
 #pragma unroll
             for (uint32_t q = 0; q < 4; ++q) {
                 const uint32_t p = g4 * 4 + q;
@@ -255,15 +227,15 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
                     level_jacobian(m, p, xs, grid, J0, J1);
                     const float g0 = r16f(gg[2 * q]), g1 = r16f(gg[2 * q + 1]);
 #pragma unroll
-                    for (int d = 0; d < 3; ++d) acc[d] = __fmaf_rn(g0, J0[d], acc[d]);
+                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g0, J0[d], nacc[d]);
 #pragma unroll
-                    for (int d = 0; d < 3; ++d) acc[d] = __fmaf_rn(g1, J1[d], acc[d]);
+                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g1, J1[d], nacc[d]);
                 }
             }
         }
         float nab[3];
 #pragma unroll
-        for (int d = 0; d < 3; ++d) nab[d] = __fmul_rn(__fmul_rn(acc[d], 0.5f), net.fac[d]);
+        for (int d = 0; d < 3; ++d) nab[d] = __fmul_rn(__fmul_rn(nacc[d], 0.5f), net.fac[d]);
         // ---- radiance input, columns 32..63: [x | SH(v) | clamp(n) | h_appear | 0]
         {
             float xr[32];
@@ -295,24 +267,14 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
             }
         }
         tc::fence_async_smem();
-        tc::fence_before_sync();
         __syncthreads();
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < XW / 16; ++ks)                             // Y1 = X . R1^T
-                tc::mma_f16_ss(tmem, tc::make_desc(x_addr + ks * 2 * kChunk, kChunk, 128), tc::make_desc(r1_addr + ks * 2 * (XW * 16), XW * 16, 128),
-                               id64, ks > 0);
-            tc::commit(&mbar);
-        }
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
+        tc::mma_to_rows<64, 0, 0, XW / 16>(acc, kS, 0, tc::kmajor(x_addr, kTile), tc::kmajor(r1_addr, XW), false);   // Y1 = X . R1^T
+        __syncthreads();
         uint8_t *y1t = Y1t ? Y1t + tile * kTileBytes : nullptr;
 #pragma unroll 1
         for (int c = 0; c < XW / 8; ++c) {
             float y[8];
-            tc::tmem_ld8(tmem + lane_base + c * 8, y);
+            tc::acc_ld8(acc, kS, tid, c * 8, y);
 #pragma unroll
             for (int j = 0; j < 8; ++j) y[j] = fmaxf(r16f(y[j] + srb1[c * 8 + j]), 0.f);
             const uint4 q = tc::pack8_f16(y);
@@ -320,25 +282,15 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
             if (y1t) *reinterpret_cast<uint4 *>(y1t + c * kChunk + tid * 16) = q;
         }
         tc::fence_async_smem();
-        tc::fence_before_sync();
         __syncthreads();
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < XW / 16; ++ks)                             // Y2 = relu(Y1) . R2^T
-                tc::mma_f16_ss(tmem + 64, tc::make_desc(u_addr + ks * 2 * kChunk, kChunk, 128),
-                               tc::make_desc(r2_addr + ks * 2 * (XW * 16), XW * 16, 128), id64, ks > 0);
-            tc::commit(&mbar);
-        }
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
+        tc::mma_to_rows<64, 0, 0, XW / 16>(acc, kS, 0, tc::kmajor(u_addr, kTile), tc::kmajor(r2_addr, XW), false);   // Y2 = relu(Y1) . R2^T
+        __syncthreads();
         float o3[3] = {0.f, 0.f, 0.f};
         uint8_t *y2t = Y2t ? Y2t + tile * kTileBytes : nullptr;
 #pragma unroll 1
         for (int c = 0; c < XW / 8; ++c) {
             float y[8];
-            tc::tmem_ld8(tmem + 64 + lane_base + c * 8, y);
+            tc::acc_ld8(acc, kS, tid, c * 8, y);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 y[j] = fmaxf(r16f(y[j] + srb2[c * 8 + j]), 0.f);
@@ -358,10 +310,8 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
                 if (x_out) x_out[i * 3 + d] = xn[d];
             }
         }
-        tc::fence_before_sync();
         __syncthreads();
     }
-    if (warp == 0) tc::tmem_free<128>(tmem);
 }
 
 // ===================================================================================================================== radiance backward
@@ -388,13 +338,14 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     uint8_t *sXe = sY1 + kTile * NE * 2;                       // 20 KB [X | 1 gy3 | 0]
     uint8_t *sR2T = sXe + kTile * NE * 2;                      //  8 KB (N = in i, K = out j) = R2[j][i]
     uint8_t *sR1h = sR2T + XW * XW * 2;                        //  4 KB (N = h column k, K = out j) = R1[j][22 + k]
+    constexpr uint32_t cDY1 = 0, cDH = 0, cXA = 64, cXB = 64 + NE;   // staged accumulator columns (dY1, then dh; XA, XB persist)
+    constexpr int kS = tc::acc_stride(64 + 2 * NE);
+    float *acc = reinterpret_cast<float *>(sR1h + NF * XW * 2); // 114 KB
     __shared__ float sR3[3][XW];
     __shared__ float sdb3[3];
-    __shared__ __align__(8) uint64_t mbar;
     __shared__ __align__(8) uint64_t mbar_ld;
-    __shared__ uint32_t tmem_slot;
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, lane = tid & 31;
     for (int e = tid; e < XW * XW; e += kTile) {
         const int i = e % XW, j = e / XW;
         const __half v = (j < net.rw && i < net.rw) ? net.R2[j * net.rw + i] : __float2half_rn(0.f);
@@ -412,24 +363,17 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     *reinterpret_cast<uint4 *>(sY1 + 8 * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);       // [1, 0, ...]
     *reinterpret_cast<uint4 *>(sY1 + 9 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
     *reinterpret_cast<uint4 *>(sXe + 9 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
+    for (int c = cXA; c < cXB + NE; ++c) acc[tid * kS + c] = 0.f;
     if (tid == 0) {
         sdb3[0] = sdb3[1] = sdb3[2] = 0.f;
-        tc::mbar_init(&mbar, 1);
         tc::mbar_init(&mbar_ld, 1);
         tc::fence_mbar_init();
     }
-    if (warp == 0) tc::tmem_alloc<256>(&tmem_slot);
     tc::fence_async_smem();
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = tmem_slot;
-    const uint32_t id64 = tc::make_idesc(kTile, 64, 0, 0), id32 = tc::make_idesc(kTile, 32, 0, 0), idw = tc::make_idesc(kTile, NE, 1, 1);
     const uint32_t t_addr = tc::smem_u32(sT), y1_addr = tc::smem_u32(sY1), xe_addr = tc::smem_u32(sXe);
     const uint32_t r2t_addr = tc::smem_u32(sR2T), r1h_addr = tc::smem_u32(sR1h);
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    constexpr uint32_t cDY1 = 0, cDH = 64, cXA = 96, cXB = 176;
-    uint32_t phase = 0, ld_phase = 0;
+    uint32_t ld_phase = 0;
     bool first_tile = true;
 
     const int64_t n_tiles = (n + kTile - 1) / kTile;
@@ -484,75 +428,49 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
             *reinterpret_cast<uint4 *>(sT + c * kChunk + tid * 16) = tc::pack8_f16(d);
         }
         tc::fence_async_smem();
-        tc::fence_before_sync();
         __syncthreads();
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < XW / 16; ++ks)
-                tc::mma_f16_ss(tmem + cDY1, tc::make_desc(t_addr + ks * 2 * kChunk, kChunk, 128),
-                               tc::make_desc(r2t_addr + ks * 2 * (XW * 16), XW * 16, 128), id64, ks > 0);
-            tc::commit(&mbar);
-        }
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
+        tc::mma_to_rows<64, 0, 0, XW / 16>(acc, kS, cDY1, tc::kmajor(t_addr, kTile), tc::kmajor(r2t_addr, XW), false);   // dY1 = dZ2 . R2
+        __syncthreads();
 #pragma unroll 1
         for (int c = 0; c < 8; ++c) {
             float dy[8], y1[8];
-            tc::tmem_ld8(tmem + cDY1 + lane_base + c * 8, dy);
+            tc::acc_ld8(acc, kS, tid, cDY1 + c * 8, dy);
             unpack8(*reinterpret_cast<const uint4 *>(sY1 + c * kChunk + tid * 16), y1);
 #pragma unroll
             for (int j = 0; j < 8; ++j) dy[j] = y1[j] > 0.f ? dy[j] : 0.f;
             *reinterpret_cast<uint4 *>(sT + kTileBytes + c * kChunk + tid * 16) = tc::pack8_f16(dy);
         }
         tc::fence_async_smem();
-        tc::fence_before_sync();
         __syncthreads();
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < XW / 16; ++ks)                              // dh = dZ1 . R1[:, h]
-                tc::mma_f16_ss(tmem + cDH, tc::make_desc(t_addr + kTileBytes + ks * 2 * kChunk, kChunk, 128),
-                               tc::make_desc(r1h_addr + ks * 2 * (NF * 16), NF * 16, 128), id32, ks > 0);
-#pragma unroll
-            for (int ks = 0; ks < kTile / 16; ++ks) {                         // weight gradients: contract over the 128 points
-                tc::mma_f16_ss(tmem + cXA, tc::make_desc(t_addr + ks * 256, 128, kChunk), tc::make_desc(y1_addr + ks * 256, 128, kChunk), idw,
-                               (ks > 0) || !first_tile);
-                tc::mma_f16_ss(tmem + cXB, tc::make_desc(t_addr + kTileBytes + ks * 256, 128, kChunk), tc::make_desc(xe_addr + ks * 256, 128, kChunk),
-                               idw, (ks > 0) || !first_tile);
-            }
-            tc::commit(&mbar);
-        }
+        tc::mma_to_rows<32, 0, 0, XW / 16>(acc, kS, cDH, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(r1h_addr, NF), false);   // dh = dZ1 . R1[:, h]
+        // weight gradients: contract over the 128 points
+        tc::mma_to_rows<NE, 1, 1, kTile / 16>(acc, kS, cXA, tc::mnmajor(t_addr, kTile), tc::mnmajor(y1_addr, kTile), true);
+        tc::mma_to_rows<NE, 1, 1, kTile / 16>(acc, kS, cXB, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(xe_addr, kTile), true);
         first_tile = false;
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
+        __syncthreads();
         if (TMA && tid == 0 && tile + gridDim.x < n_tiles) {
             // every reader of the three tiles is done: the threads' own reads precede the __syncthreads before the MMAs above, and those MMAs
-            // (the last readers) have completed -> the next tile's activations may overwrite them while this tile is finished
+            // (the last readers) have completed before the barrier above -> the next tile's activations may overwrite them while this tile is finished
             tc::fence_async_smem();
             fetch(tile + gridDim.x);
         }
 #pragma unroll 1
         for (int c = 0; c < 4; ++c) {
             float dh[8];
-            tc::tmem_ld8(tmem + cDH + lane_base + c * 8, dh);
+            tc::acc_ld8(acc, kS, tid, cDH + c * 8, dh);
             if (valid) {
                 *reinterpret_cast<float4 *>(dh_out + i * NF + c * 8) = make_float4(dh[0], dh[1], dh[2], dh[3]);
                 *reinterpret_cast<float4 *>(dh_out + i * NF + c * 8 + 4) = make_float4(dh[4], dh[5], dh[6], dh[7]);
             }
         }
-        tc::fence_before_sync();
         __syncthreads();
     }
     if (!first_tile) {
-        tc::fence_after_sync();
 #pragma unroll 1
         for (int c = 0; c < 9; ++c) {
             float a[8], b[8];
-            tc::tmem_ld8(tmem + cXA + lane_base + c * 8, a);
-            tc::tmem_ld8(tmem + cXB + lane_base + c * 8, b);
+            tc::acc_ld8(acc, kS, tid, cXA + c * 8, a);
+            tc::acc_ld8(acc, kS, tid, cXB + c * 8, b);
             if (tid < net.rw) {
                 if (c < 8) {
 #pragma unroll
@@ -573,9 +491,6 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         }
         if (tid < 3) atomicAdd(drb3 + tid, sdb3[tid]);
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_free<256>(tmem);
 }
 
 // ===================================================================================================================== sdf / nablas backward
@@ -606,13 +521,14 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
     uint8_t *sW1 = sGe + kTile * NX * 2;                       //  4 KB
     uint8_t *sW1T = sW1 + HW * NF * 2;                         //  4 KB
     uint8_t *sZ = sW1T + NF * HW * 2;                          // 16 KB saved pre-activations (TMA only)
+    constexpr uint32_t cDU = 0, cDHZ = 0, cG = 64, cX1 = 96, cX2 = 96 + NX;   // staged accumulator columns (du, then dhz; X1, X2 persist)
+    constexpr int kS = tc::acc_stride(96 + 2 * NX);
+    float *acc = reinterpret_cast<float *>(sZ + kTileBytes);   // 98 KB
     __shared__ float sW2[HW];
     __shared__ float sdb2;
-    __shared__ __align__(8) uint64_t mbar;
     __shared__ __align__(8) uint64_t mbar_ld;
-    __shared__ uint32_t tmem_slot;
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, lane = tid & 31;
     {
         DecoderDevTC dec{net.W1, net.b1, net.W2, net.b2, net.width, net.beta};
         stage_W1(dec, sW1, tid);
@@ -623,25 +539,18 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
     *reinterpret_cast<uint4 *>(sGe + 4 * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);
     *reinterpret_cast<uint4 *>(sHe + 5 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
     *reinterpret_cast<uint4 *>(sGe + 5 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
+    for (int c = cX1; c < cX2 + NX; ++c) acc[tid * kS + c] = 0.f;
     if (tid == 0) {
         sdb2 = 0.f;
-        tc::mbar_init(&mbar, 1);
         tc::mbar_init(&mbar_ld, 1);
         tc::fence_mbar_init();
     }
-    if (warp == 0) tc::tmem_alloc<256>(&tmem_slot);
     tc::fence_async_smem();
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = tmem_slot;
-    const uint32_t id64 = tc::make_idesc(kTile, 64, 0, 0), id32 = tc::make_idesc(kTile, 32, 0, 0), idw = tc::make_idesc(kTile, NX, 1, 1);
     const uint32_t t_addr = tc::smem_u32(sT), he_addr = tc::smem_u32(sHe), ge_addr = tc::smem_u32(sGe), w1_addr = tc::smem_u32(sW1),
                    w1t_addr = tc::smem_u32(sW1T);
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    constexpr uint32_t cDU = 0, cG = 64, cDHZ = 96, cX1 = 128, cX2 = 176;
     const SoftplusK spk(net.beta);
-    uint32_t phase = 0, ld_phase = 0;
+    uint32_t ld_phase = 0;
     bool first_tile = true;
 
     const int64_t n_tiles = (n + kTile - 1) / kTile;
@@ -702,27 +611,14 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
             *reinterpret_cast<uint32_t *>(sGe + (p >> 2) * kChunk + tid * 16 + (p & 3) * 4) = packed;
         }
         tc::fence_async_smem();
-        tc::fence_before_sync();
         __syncthreads();
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < NF / 16; ++ks)                              // du = dG . W1^T
-                tc::mma_f16_ss(tmem + cDU, tc::make_desc(ge_addr + ks * 2 * kChunk, kChunk, 128),
-                               tc::make_desc(w1_addr + ks * 2 * (HW * 16), HW * 16, 128), id64, ks > 0);
-#pragma unroll
-            for (int ks = 0; ks < HW / 16; ++ks)                              // g = U . W1
-                tc::mma_f16_ss(tmem + cG, tc::make_desc(t_addr + kTileBytes + ks * 2 * kChunk, kChunk, 128),
-                               tc::make_desc(w1t_addr + ks * 2 * (NF * 16), NF * 16, 128), id32, ks > 0);
-            tc::commit(&mbar);
-        }
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
+        tc::mma_to_rows<64, 0, 0, NF / 16>(acc, kS, cDU, tc::kmajor(ge_addr, kTile), tc::kmajor(w1_addr, HW), false);                // du = dG . W1^T
+        tc::mma_to_rows<32, 0, 0, HW / 16>(acc, kS, cG, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(w1t_addr, NF), false);    // g = U . W1
+        __syncthreads();
 #pragma unroll 1
         for (int c = 0; c < 8; ++c) {
             float du[8], z[8], dz[8], vv[8];
-            tc::tmem_ld8(tmem + cDU + lane_base + c * 8, du);
+            tc::acc_ld8(acc, kS, tid, cDU + c * 8, du);
             unpack8(*reinterpret_cast<const uint4 *>(zt + c * kChunk + tid * 16), z);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
@@ -737,29 +633,14 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
             *reinterpret_cast<uint4 *>(sT + 2 * kTileBytes + c * kChunk + tid * 16) = tc::pack8_f16(vv);
         }
         tc::fence_async_smem();
-        tc::fence_before_sync();
         __syncthreads();
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < HW / 16; ++ks)                              // dhz = dZ . W1
-                tc::mma_f16_ss(tmem + cDHZ, tc::make_desc(t_addr + ks * 2 * kChunk, kChunk, 128),
-                               tc::make_desc(w1t_addr + ks * 2 * (NF * 16), NF * 16, 128), id32, ks > 0);
-#pragma unroll
-            for (int ks = 0; ks < kTile / 16; ++ks) {
-                tc::mma_f16_ss(tmem + cX1, tc::make_desc(t_addr + ks * 256, 128, kChunk), tc::make_desc(he_addr + ks * 256, 128, kChunk), idw,
-                               (ks > 0) || !first_tile);
-                tc::mma_f16_ss(tmem + cX2, tc::make_desc(t_addr + kTileBytes + ks * 256, 128, kChunk), tc::make_desc(ge_addr + ks * 256, 128, kChunk),
-                               idw, (ks > 0) || !first_tile);
-            }
-            tc::commit(&mbar);
-        }
+        tc::mma_to_rows<32, 0, 0, HW / 16>(acc, kS, cDHZ, tc::kmajor(t_addr, kTile), tc::kmajor(w1t_addr, NF), false);               // dhz = dZ . W1
+        tc::mma_to_rows<NX, 1, 1, kTile / 16>(acc, kS, cX1, tc::mnmajor(t_addr, kTile), tc::mnmajor(he_addr, kTile), true);
+        tc::mma_to_rows<NX, 1, 1, kTile / 16>(acc, kS, cX2, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(ge_addr, kTile), true);
         first_tile = false;
         const float dsum = warp_sum(dsdf);
         if (lane == 0 && dsum != 0.f) atomicAdd(&sdb2, dsum);
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
+        __syncthreads();
         if (TMA && tid == 0 && tile + gridDim.x < n_tiles) {
             // sZ was last read by the threads before the __syncthreads that precedes the MMAs above, sHe by those MMAs, which have completed
             tc::fence_async_smem();
@@ -769,8 +650,8 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
 #pragma unroll 1
         for (uint32_t g4 = 0; g4 < 4; ++g4) {
             float gg[8], hz[8];
-            tc::tmem_ld8(tmem + cG + lane_base + g4 * 8, gg);
-            tc::tmem_ld8(tmem + cDHZ + lane_base + g4 * 8, hz);
+            tc::acc_ld8(acc, kS, tid, cG + g4 * 8, gg);
+            tc::acc_ld8(acc, kS, tid, cDHZ + g4 * 8, hz);
             if (valid && dh_r) {
                 const float4 r0 = *reinterpret_cast<const float4 *>(dh_r + i * NF + g4 * 8), r1 = *reinterpret_cast<const float4 *>(dh_r + i * NF + g4 * 8 + 4);
                 hz[0] += r0.x; hz[1] += r0.y; hz[2] += r0.z; hz[3] += r0.w; hz[4] += r1.x; hz[5] += r1.y; hz[6] += r1.z; hz[7] += r1.w;
@@ -809,31 +690,26 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
                 }
             }
         }
-        tc::fence_before_sync();
         __syncthreads();
     }
     if (!first_tile) {
-        tc::fence_after_sync();
 #pragma unroll 1
         for (int c = 0; c < NF / 8; ++c) {
             float a[8], b[8];
-            tc::tmem_ld8(tmem + cX1 + lane_base + c * 8, a);
-            tc::tmem_ld8(tmem + cX2 + lane_base + c * 8, b);
+            tc::acc_ld8(acc, kS, tid, cX1 + c * 8, a);
+            tc::acc_ld8(acc, kS, tid, cX2 + c * 8, b);
             if (tid < net.width) {
 #pragma unroll
                 for (int k = 0; k < 8; ++k) atomicAdd(d_W1 + tid * NF + c * 8 + k, a[k] + b[k]);
             }
         }
         float a1[8], b1[8];
-        tc::tmem_ld8(tmem + cX1 + 32 + lane_base, a1);
-        tc::tmem_ld8(tmem + cX2 + 32 + lane_base, b1);
+        tc::acc_ld8(acc, kS, tid, cX1 + 32, a1);
+        tc::acc_ld8(acc, kS, tid, cX2 + 32, b1);
         if (tid < HW) { if (tid < net.width) atomicAdd(d_b1 + tid, a1[0]); }
         else if (tid - HW < net.width) atomicAdd(d_W2 + (tid - HW), b1[0]);
         if (tid == 0) atomicAdd(d_b2, sdb2);
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_free<256>(tmem);
 }
 
 }  // namespace nsb
@@ -875,12 +751,12 @@ extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params
     ColorNetDev d;
     if (int rc = make_net(net, meta, &m, &d, "nsb_fused_color_fwd")) return rc;
     NSB_REQUIRE(d.n_appear == 0 || h_appear, "nsb_fused_color_fwd: h_appear is NULL but the net has %d appearance channels", d.n_appear);
-    constexpr int kSmem = 2 * kTileBytes + 2 * HW * NF * 2 + 2 * XW * XW * 2 + 1024;
+    constexpr int kSmem = 2 * kTileBytes + 2 * HW * NF * 2 + 2 * XW * XW * 2 + kTile * tc::acc_stride(64) * 4 + 1024;
     opt_in_smem(k_color_fwd, kSmem);
     PointSrc ps{x, rays_o, rays_d, t, ridx};
     OccCollect oc{nullptr, 1, 1, 1, 0.f};
     if (collect && collect->grid_pcl) oc = OccCollect{collect->grid_pcl, collect->res[0], collect->res[1], collect->res[2], collect->inv_s};
-    k_color_fwd<<<tiles_grid(n, 3), kTile, kSmem, (cudaStream_t)stream>>>(m, (const __half *)params_half, d, ps, view_dirs, h_appear, n,
+    k_color_fwd<<<tiles_grid(n, 2), kTile, kSmem, (cudaStream_t)stream>>>(m, (const __half *)params_half, d, ps, view_dirs, h_appear, n,
                                                                           max_level < 0 ? -1 : max_level, sdf, nablas, rgb, x_out, (uint8_t *)act_z,
                                                                           (uint8_t *)act_x, (uint8_t *)act_y1, (uint8_t *)act_y2, oc, dn.a);
     return check_launch("nsb_fused_color_fwd");
@@ -903,27 +779,27 @@ extern "C" int nsb_fused_color_bwd(const nsb_lotd_meta *meta, const void *params
     cudaStream_t s = (cudaStream_t)stream;
     const float *dh = nullptr;
     if (g_rgb) {
-        constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + 1024;
+        constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + kTile * tc::acc_stride(64 + 2 * 80) * 4 + 1024;   // 1 CTA / SM
         opt_in_smem(k_color_rad_bwd<true>, kSmemR);
         opt_in_smem(k_color_rad_bwd<false>, kSmemR);
         if (g_opt_color_tma.load())
-            k_color_rad_bwd<true><<<tiles_grid(n, 2), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n,
+            k_color_rad_bwd<true><<<tiles_grid(n, 1), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n,
                                                                           dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, dn.a);
         else
-            k_color_rad_bwd<false><<<tiles_grid(n, 2), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n,
+            k_color_rad_bwd<false><<<tiles_grid(n, 1), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n,
                                                                            dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, dn.a);
         if (int rc = check_launch("nsb_fused_color_bwd(radiance)")) return rc;
         dh = dh_scratch;
     }
-    constexpr int kSmemS = 3 * kTileBytes + 2 * kTile * 48 * 2 + 2 * HW * NF * 2 + kTileBytes + 1024;      // 97 KB: still 2 CTAs / SM (TMEM-bound anyway)
+    constexpr int kSmemS = 3 * kTileBytes + 2 * kTile * 48 * 2 + 2 * HW * NF * 2 + kTileBytes + kTile * tc::acc_stride(96 + 2 * 48) * 4 + 1024;   // 1 CTA / SM
     opt_in_smem(k_color_sdf_bwd<true>, kSmemS);
     opt_in_smem(k_color_sdf_bwd<false>, kSmemS);
     PointSrc ps{x, rays_o, rays_d, t, ridx};
     if (g_opt_color_tma.load() >= 2)
-        k_color_sdf_bwd<true><<<tiles_grid(n, 2), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
+        k_color_sdf_bwd<true><<<tiles_grid(n, 1), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
                                                                       g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level, d_grid, d_W1, d_b1, d_W2, d_b2, dn.a);
     else
-        k_color_sdf_bwd<false><<<tiles_grid(n, 2), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
+        k_color_sdf_bwd<false><<<tiles_grid(n, 1), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
                                                                        g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level, d_grid, d_W1, d_b1, d_W2, d_b2, dn.a);
     return check_launch("nsb_fused_color_bwd(sdf)");
 }

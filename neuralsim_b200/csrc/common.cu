@@ -49,7 +49,7 @@ extern "C" int nsb_bind_device_counts(const int64_t *count0, const int64_t *coun
 }
 
 // Tunables / self-check switches.  "sdf_simt" = 1 routes nsb_fused_sdf* through the CUDA-core reference kernel of
-// csrc/fused.cu instead of the tcgen05 kernel (used by the tests to cross-check the two).
+// csrc/fused.cu instead of the wgmma kernel (used by the tests to cross-check the two).
 extern "C" int nsb_set_option(const char *key, int value) {
     if (key && !strcmp(key, "sdf_simt")) { nsb::g_opt_sdf_simt.store(value); return 0; }
     if (key && !strcmp(key, "color_tma")) { nsb::g_opt_color_tma.store(value); return 0; }       // 0: plain 16-byte loads of the saved activation tiles (A/B)

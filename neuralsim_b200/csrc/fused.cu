@@ -1,4 +1,4 @@
-// Fused "forward_sdf" for sm_100a: LoTD gather -> SDF decoder MLP (F -> W -> 1, Softplus(beta)) in one kernel.
+// Fused "forward_sdf" for sm_90a: LoTD gather -> SDF decoder MLP (F -> W -> 1, Softplus(beta)) in one kernel.
 //
 // Replaces, for no-grad SDF queries, the chain
 //   LoTDEncoding.forward (lotd_encoding.py:150-166)  -> 16 gather kernels + transpose
@@ -10,7 +10,7 @@
 //   a   : fp16( softplus_beta(float(z)) )                   softplus evaluated in fp32 (autocast fp32 list)
 //   sdf : fp16( sum_j a_j*W2_j [fp32] + b2 )
 // The 32x64 layer is evaluated here on CUDA cores with weights staged once per CTA in shared memory
-// (fp32, float4 broadcast loads); the tcgen05 variant of the same contract lives in mlp_tc.cu.
+// (fp32, float4 broadcast loads); the tensor-core variant of the same contract lives in fused_tc.cu.
 #include "lotd_device.cuh"
 
 namespace nsb {

@@ -1,13 +1,12 @@
-// Fused forward_sdf and its backward with the decoder GEMMs on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a.
+// Fused forward_sdf and its backward with the decoder GEMMs on the Hopper tensor cores (wgmma), sm_90a.
 //
-// One CTA = 128 threads = one tile of 128 points; thread r owns point r for the whole pipeline (TMEM lane r == point r):
+// One CTA = 128 threads = one warpgroup = one tile of 128 points; thread r owns point r for the gather and the scatter:
 //   gather   thread r walks the 16 LoTD levels of its point (8 corner loads each); every level's two fp16 features go
 //            straight into its row of the A tile in shared memory (core-matrix layout of tc_util.cuh)
-//   MMA      one elected thread issues tcgen05.mma (M=128, N=64, K=16) x2: Z[128 x 64] (fp32, TMEM) = H[128 x 32] . W1^T
-//   epilogue thread r reads its own TMEM lane 8 columns at a time (tcgen05.ld), applies bias + Softplus(beta) with the
-//            autocast rounding points, and folds the 64 -> 1 layer into a running dot product -> sdf[r]
-// All loops over levels / hidden units are rolled on purpose: the first, fully unrolled version was 10k SASS instructions
-// (168 KB) and spent most issue slots in instruction-cache misses (ncu: stall_no_instruction 5.9/issue; profiles/r01_*).
+//   MMA      the warpgroup issues wgmma (M=64, N=64, K=16) x2 per 64-row half: Z[128 x 64] (fp32, registers) = H[128 x 32] . W1^T
+//   epilogue bias + Softplus(beta) with the autocast rounding points on the accumulator fragments, the 64 -> 1 layer as a
+//            dot product per row (16 hidden units per lane, summed over the lane quad) -> sdf[r]
+// The loop over levels is rolled on purpose (instruction cache: a fully unrolled gather is several thousand instructions).
 // W1 is staged once per persistent CTA.  Numerics: the fp16 rounding points of the reference's autocast graph (DESIGN.md).
 #include <stdlib.h>
 
@@ -18,8 +17,7 @@ namespace nsb {
 // MODE 0: points x[n,3];  MODE 1: x = o[ridx[i]] + d[ridx[i]] t[i] in the given (ray-major) order;
 // MODE 2: the same packed samples traversed RAY-TILED: a tile = 32 consecutive packs (rays) x 4 consecutive samples, lane = ray,
 //         warp = sample ordinal.  For coherent rays (an image) the 32 lanes of a gather instruction then sit in neighbouring
-//         cells -> few 128 B lines per request; the L1 tag stage (one line per ~2 cycles) is what bounds this kernel
-//         (profiles/r01d_ab.txt: 12.6 -> 7.4 ms on the boundary points of a frame).  sdf is written to the packed slot, so
+//         cells -> few 128 B lines per request; the L1 tag stage is what bounds this kernel.  sdf is written to the packed slot, so
 //         nothing downstream changes.  Incoherent rays (random training pixels) keep MODE 1: locality along the ray.
 template <int MODE, bool FAST_SP = false, int UNROLL = 2, bool PAIRED = false>
 __global__ void __launch_bounds__(kTile)
@@ -28,12 +26,10 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
                const float *__restrict__ t, int64_t n, int max_level, float *__restrict__ sdf, const int64_t *__restrict__ pack_infos,
                const int64_t *__restrict__ pack_ray, int64_t n_packs, const OccCollect oc, const int64_t *__restrict__ n_dev) {
     if (MODE == 2) n_packs = eff_n(n_packs, n_dev); else n = eff_n(n, n_dev);       // device-resident count (nsb_bind_device_counts)
-    __shared__ __align__(1024) uint8_t sA[kTile * NF * 2];   // 8 KB : features, chunk-major core-matrix layout
-    __shared__ __align__(1024) uint8_t sB[HW * NF * 2];      // 4 KB : W1 [64 x 32], same layout
-    __shared__ float sb1[HW], sW2[HW];
+    __shared__ __align__(128) uint8_t sA[kTile * NF * 2];    // 8 KB : features, chunk-major core-matrix layout
+    __shared__ __align__(128) uint8_t sB[HW * NF * 2];       // 4 KB : W1 [64 x 32], same layout
+    __shared__ float sb1[HW], sW2[HW], srow[kTile];
     __shared__ float sb2;
-    __shared__ __align__(8) uint64_t mbar;
-    __shared__ uint32_t tmem_slot;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     stage_W1(dec, sB, tid);
@@ -41,19 +37,10 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
         sb1[tid] = tid < dec.width ? __half2float(dec.b1[tid]) : 0.f;
         sW2[tid] = tid < dec.width ? __half2float(dec.W2[tid]) : 0.f;
     }
-    if (tid == 0) {
-        sb2 = __half2float(dec.b2[0]);
-        tc::mbar_init(&mbar, 1);
-        tc::fence_mbar_init();
-    }
-    if (warp == 0) tc::tmem_alloc<64>(&tmem_slot);
+    if (tid == 0) sb2 = __half2float(dec.b2[0]);
     tc::fence_async_smem();
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), tc::make_idesc(kTile, HW, 0, 0), tmem_slot,
-                      (uint32_t)(warp * 32) << 16, &mbar, sb1, sW2, sb2, SoftplusK(dec.beta)};
-    uint32_t phase = 0;
+    const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
 
     if (MODE == 2) {
         const int64_t n_groups = (n_packs + 31) / 32;
@@ -80,7 +67,7 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
                 }
 #pragma unroll
                 for (int q = 0; q < 3; ++q) xs[q] = fminf(fmaxf(__fmaf_rn(xs[q], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
-                const float v = sdf_of_tile<FAST_SP, UNROLL, PAIRED>(ctx, xs, tid, phase);
+                const float v = sdf_of_tile<FAST_SP, UNROLL, PAIRED>(ctx, xs, tid);
                 if (valid) {
                     sdf[first + k] = v;
                     if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -94,26 +81,25 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
             const bool valid = i < n;
             float xs[3];
             load_point(MODE == 1, x, rays_o, rays_d, ridx, t, i, valid, xs);
-            const float v = sdf_of_tile<FAST_SP, UNROLL, PAIRED>(ctx, xs, tid, phase);
+            const float v = sdf_of_tile<FAST_SP, UNROLL, PAIRED>(ctx, xs, tid);
             if (valid) {
                 sdf[i] = v;
                 if (oc.pcl) occ_collect_point(oc, xs, v);
             }
         }
     }
-    if (warp == 0) tc::tmem_free<64>(ctx.tmem);
 }
 
 // =====================================================================================================================
 // Backward of forward_sdf wrt. the LoTD table and the decoder weights, one kernel, nothing saved by the forward.
-// Per tile of 128 points (thread r = point r = TMEM lane r), d = dL/dsdf[r]:
-//   recompute  gather -> A tile [H | 1 | 0..];  MMA1: Z = H.W1^T (TMEM cols 0..63);  z = fp16(Z + b1); s = sigmoid(beta z), a = fp16(softplus)
+// Per tile of 128 points (thread r = point r = staged accumulator row r), d = dL/dsdf[r]:
+//   recompute  gather -> A tile [H | 1 | 0..];  MMA1: Z = H.W1^T (staged cols 0..63);  z = fp16(Z + b1); s = sigmoid(beta z), a = fp16(softplus)
 //   row r of the G tile [128 x 128] fp16 :=  [ dz_0..dz_63 | d*a_0..d*a_63 ],  dz_j = d * w2_j * s_j
 //              (the reference rounds grad_z to fp16 at the same place, layers.py autocast backward)
-//   MMA2: dH[128 x 32]  = dZ . W1                 A = G cols 0..63 (K-major), B = W1^T tile          -> TMEM cols 0..31
+//   MMA2: dH[128 x 32]  = dZ . W1                 A = G cols 0..63 (K-major), B = W1^T tile          -> staged cols 0..31
 //   MMA3: X[128 x 40]  += G^T . [H | 1 | 0..]     both operands are the tiles above read MN-major, K = the 128 points;
 //              rows 0..63 of X = [ dW1 | db1 ], rows 64..127, column 32 = dW2; accumulated over all tiles of the
-//              persistent CTA in TMEM cols 64..103
+//              persistent CTA in staged cols 64..103
 //   scatter dH into the fp32 table gradient (8 corners x 16 levels, red.global.add.v2.f32);  db2 via a warp sum.
 // =====================================================================================================================
 template <bool FROM_RAYS>
@@ -125,18 +111,18 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
              const int64_t *__restrict__ keep, const int64_t *__restrict__ n_dev) {
     n = eff_n(n, n_dev);
     constexpr int NX = 40, GW = 128;                          // NX: features + [1,0,..] chunk; GW: dz | d*a
-    extern __shared__ uint8_t dyn_smem[];                     // 50 KB of tiles (> the 48 KB static limit), 1 KB aligned by hand
-    uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
+    constexpr int kCols = HW + NX, kS = tc::acc_stride(kCols);  // staged accumulators: Z / dH in cols 0..63, X in cols 64..103
+    extern __shared__ uint8_t dyn_smem[];                     // 104 KB of tiles and staged accumulators (> the 48 KB static limit)
+    uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 127) & ~uintptr_t(127));
     uint8_t *sA = tiles;                                      // 10 KB : [H | 1 | 0..]
     uint8_t *sG = sA + kTile * NX * 2;                        // 32 KB : [dz | d*a]
     uint8_t *sB = sG + kTile * GW * 2;                        //  4 KB : W1   [64 x 32]  (B of MMA1)
     uint8_t *sBT = sB + HW * NF * 2;                          //  4 KB : W1^T [32 x 64]  (B of MMA2)
+    float *acc = reinterpret_cast<float *>(sBT + NF * HW * 2);   // 54 KB : [128 x kS] fp32
     __shared__ float sb1[HW], sW2[HW];
     __shared__ float sdb2;
-    __shared__ __align__(8) uint64_t mbar;
-    __shared__ uint32_t tmem_slot;
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, lane = tid & 31;
     stage_W1(dec, sB, tid);
     for (int e = tid; e < NF * HW; e += kTile) {              // W1^T: row = feature k, col = hidden j
         const int k = e % NF, j = e / NF;
@@ -148,24 +134,12 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         sW2[tid] = tid < dec.width ? __half2float(dec.W2[tid]) : 0.f;
     }
     *reinterpret_cast<uint4 *>(sA + 4 * (kTile * 16) + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);   // constant chunk: [1,0,..]
-    if (tid == 0) {
-        sdb2 = 0.f;
-        tc::mbar_init(&mbar, 1);
-        tc::fence_mbar_init();
-    }
-    if (warp == 0) tc::tmem_alloc<128>(&tmem_slot);
+    for (int c = HW; c < kCols; ++c) acc[tid * kS + c] = 0.f;
+    if (tid == 0) sdb2 = 0.f;
     tc::fence_async_smem();
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = tmem_slot;
-    const uint32_t idesc1 = tc::make_idesc(kTile, HW, 0, 0);   // Z  = H  . W1^T
-    const uint32_t idesc2 = tc::make_idesc(kTile, NF, 0, 0);   // dH = dZ . W1
-    const uint32_t idesc3 = tc::make_idesc(GW, NX, 1, 1);      // X  = G^T . [H|1]   (MN-major operands)
     const uint32_t a_addr = tc::smem_u32(sA), g_addr = tc::smem_u32(sG), b_addr = tc::smem_u32(sB), bt_addr = tc::smem_u32(sBT);
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
     const SoftplusK spk(dec.beta);
-    uint32_t phase = 0;
     bool first_tile = true;
 
     const int64_t n_tiles = (n + kTile - 1) / kTile;
@@ -179,22 +153,13 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         gather_row_to_tile<kTile>(m, grid, xs, max_level, sA, tid);
         tc::fence_async_smem();
         __syncthreads();
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < NF / 16; ++ks)
-                tc::mma_f16_ss(tmem, tc::make_desc(a_addr + ks * 2 * (kTile * 16), kTile * 16, 128),
-                               tc::make_desc(b_addr + ks * 2 * (HW * 16), HW * 16, 128), idesc1, ks > 0);
-            tc::commit(&mbar);
-        }
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
+        tc::mma_to_rows<HW, 0, 0, NF / 16>(acc, kS, 0, tc::kmajor(a_addr, kTile), tc::kmajor(b_addr, HW), false);   // Z = H . W1^T
+        __syncthreads();
         // ---- my G row: dz (chunks 0..7) and d*a (chunks 8..15)
 #pragma unroll 1
         for (int c = 0; c < HW / 8; ++c) {
             float z[8], dz[8], da[8];
-            tc::tmem_ld8(tmem + lane_base + c * 8, z);
+            tc::acc_ld8(acc, kS, tid, c * 8, z);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const float zz = __half2float(__float2half_rn(z[j] + sb1[c * 8 + j]));
@@ -207,34 +172,20 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
             *reinterpret_cast<uint4 *>(sG + (8 + c) * (kTile * 16) + tid * 16) = tc::pack8_f16(da);
         }
         tc::fence_async_smem();
-        tc::fence_before_sync();
         __syncthreads();                                         // every thread has read Z and written its G row
-        if (tid == 0) {
-            tc::fence_after_sync();
-#pragma unroll
-            for (int ks = 0; ks < HW / 16; ++ks)                 // dH = dZ . W1 : K = 64 hidden
-                tc::mma_f16_ss(tmem, tc::make_desc(g_addr + ks * 2 * (kTile * 16), kTile * 16, 128),
-                               tc::make_desc(bt_addr + ks * 2 * (NF * 16), NF * 16, 128), idesc2, ks > 0);
-#pragma unroll
-            for (int ks = 0; ks < kTile / 16; ++ks)              // X += G^T . [H|1] : K = 128 points
-                tc::mma_f16_ss(tmem + 64, tc::make_desc(g_addr + ks * 256, 128, kTile * 16),
-                               tc::make_desc(a_addr + ks * 256, 128, kTile * 16), idesc3, (ks > 0) || !first_tile);
-            tc::commit(&mbar);
-        }
+        tc::mma_to_rows<NF, 0, 0, HW / 16>(acc, kS, 0, tc::kmajor(g_addr, kTile), tc::kmajor(bt_addr, NF), false);          // dH = dZ . W1 : K = 64 hidden
+        tc::mma_to_rows<NX, 1, 1, kTile / 16>(acc, kS, HW, tc::mnmajor(g_addr, kTile), tc::mnmajor(a_addr, kTile), true);   // X += G^T . [H|1] : K = 128 points
         first_tile = false;
         const float dsum = warp_sum(dd);
         if (lane == 0 && dsum != 0.f) atomicAdd(&sdb2, dsum);
-        tc::mbar_wait(&mbar, phase);
-        phase ^= 1;
-        tc::fence_after_sync();
-        // ---- my dH row -> scatter into the table gradient.  The TMEM loads are warp-collective (.sync.aligned), so every
-        //      thread runs them; only the reductions are predicated on "this point carries gradient".
+        __syncthreads();
+        // ---- my dH row -> scatter into the table gradient; only the reductions are predicated on "this point carries gradient".
         const bool active = valid && dd != 0.f;
         const bool warp_active = __any_sync(0xffffffffu, active);
 #pragma unroll 1
         for (uint32_t g4 = 0; g4 < 4; ++g4) {
             float dh[8];
-            tc::tmem_ld8(tmem + lane_base + g4 * 8, dh);            // 4 levels x 2 features
+            tc::acc_ld8(acc, kS, tid, g4 * 8, dh);                  // 4 levels x 2 features
             if (!warp_active) continue;
 #pragma unroll
             for (uint32_t q = 0; q < 4; ++q) {
@@ -255,35 +206,35 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
                 }
             }
         }
-        tc::fence_before_sync();
-        __syncthreads();                                         // tiles + TMEM free for the next iteration
+        __syncthreads();                                         // tiles + staged rows free for the next iteration
     }
     // ---- flush the CTA's weight-gradient accumulators: X rows 0..63 = [dW1 | db1], rows 64..127 col 32 = dW2
     if (!first_tile) {                                           // uniform per CTA
-        tc::fence_after_sync();
 #pragma unroll 1
         for (int c = 0; c < NF / 8; ++c) {
             float r[8];
-            tc::tmem_ld8(tmem + 64 + lane_base + c * 8, r);
+            tc::acc_ld8(acc, kS, tid, HW + c * 8, r);
             if (tid < dec.width) {
 #pragma unroll
                 for (int k = 0; k < 8; ++k) atomicAdd(d_W1 + tid * NF + c * 8 + k, r[k]);
             }
         }
         float r1[8];
-        tc::tmem_ld8(tmem + 64 + 32 + lane_base, r1);
+        tc::acc_ld8(acc, kS, tid, HW + 32, r1);
         if (tid < HW) { if (tid < dec.width) atomicAdd(d_b1 + tid, r1[0]); }
         else if (tid - HW < dec.width) atomicAdd(d_W2 + (tid - HW), r1[0]);
         if (tid == 0) atomicAdd(d_b2, sdb2);
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_free<128>(tmem);
 }
 
 }  // namespace nsb
 
 using namespace nsb;
+
+// CTAs of k_fused_sdf_tc per SM in the persistent grid.  5 would fit (90-101 registers, ~13 KB of shared memory), but the gather
+// is L1-bound and more warps gathering at once evict each other's lines: on an H100 (NVIDIA H100 80GB HBM3, 700 W) the boundary
+// query of an 800x600 frame took 5.8 ms per launch at 4 CTAs / SM, 7.3-7.4 ms at 5 and 6.5 ms at 6 (bench.py, NSB_SDF_CTAS, alternated).
+constexpr int kSdfCtasPerSM = 4;
 
 static inline unsigned persistent_grid(int64_t n, int ctas_per_sm) {
     const int64_t n_tiles = (n + kTile - 1) / kTile;
@@ -295,10 +246,9 @@ template <int MODE>
 static void launch_sdf(int variant, unsigned grid, cudaStream_t s, const PLMeta &m, const __half *g, const DecoderDevTC &d, const float *x, const float *ro,
                        const float *rd, const int64_t *ridx, const float *t, int64_t n, int ml, float *sdf, const int64_t *pi, const int64_t *pr, int64_t np,
                        const OccCollect &oc, const int64_t *nd) {
-    // default (variant 1): SFU softplus, two levels per gather trip -- fastest in both point orders (profiles/r01f_ab.txt: 4.3 ms ray-tiled,
-    // 5.0 ms ray-major on the 25.4 M boundary points of a frame; the SFU epilogue with ONE level per trip thrashes L1 in ray-major order: 13 ms).
+    // default (variant 1): SFU softplus, two levels per gather trip (one level per trip thrashes L1 in ray-major order).
     // variants: 0 libm / 2 levels per trip, 1 SFU / 2, 2 libm / 1, 3 SFU / 1, 4 SFU / 2 + paired corner loads (experiment, lotd_device.cuh)
-    if (variant < 0) variant = 1;                      // SFU softplus, two levels per trip: best in both orders (profiles/r01f_ab.txt)
+    if (variant < 0) variant = 1;                      // SFU softplus, two levels per trip
     if (variant == 1) k_fused_sdf_tc<MODE, true, 2><<<grid, kTile, 0, s>>>(m, g, d, x, ro, rd, ridx, t, n, ml, sdf, pi, pr, np, oc, nd);
     else if (variant == 2) k_fused_sdf_tc<MODE, false, 1><<<grid, kTile, 0, s>>>(m, g, d, x, ro, rd, ridx, t, n, ml, sdf, pi, pr, np, oc, nd);
     else if (variant == 3) k_fused_sdf_tc<MODE, true, 1><<<grid, kTile, 0, s>>>(m, g, d, x, ro, rd, ridx, t, n, ml, sdf, pi, pr, np, oc, nd);
@@ -323,7 +273,7 @@ extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *pa
     // read per call on purpose: profiles/ab_gather.py flips them between launches (two getenv of short names, ~50 ns)
     const char *ev = getenv("NSB_SDF_VARIANT"), *ec = getenv("NSB_SDF_CTAS");
     const int variant = ev ? atoi(ev) : -1;
-    const int ctas = ec ? atoi(ec) : 6;      // <= 8 (TMEM: 8 x 64 columns); 6 measured best
+    const int ctas = ec ? atoi(ec) : kSdfCtasPerSM;
     cudaStream_t s = (cudaStream_t)stream;
     const int ml = max_level < 0 ? -1 : max_level;
     const __half *g = (const __half *)params_half;
@@ -359,10 +309,10 @@ extern "C" int nsb_fused_sdf_bwd_indexed(const nsb_lotd_meta *meta, const void *
     NSB_REQUIRE(dec->width >= 1 && dec->width <= 64, "nsb_fused_sdf_bwd: decoder width must be <= 64");
     DecoderDevTC d{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2, dec->width,
                    dec->beta};
-    constexpr int kBwdSmem = (128 * 40 + 128 * 128 + 64 * 32 + 32 * 64) * 2 + 1024;
+    constexpr int kBwdSmem = (128 * 40 + 128 * 128 + 64 * 32 + 32 * 64) * 2 + 128 * tc::acc_stride(64 + 40) * 4 + 128;
     opt_in_smem(k_sdf_bwd_tc<true>, kBwdSmem);
     opt_in_smem(k_sdf_bwd_tc<false>, kBwdSmem);
-    const unsigned grid = persistent_grid(n, 4);           // TMEM: 4 x 128 columns per SM; smem 4 x 51 KB
+    const unsigned grid = persistent_grid(n, 2);           // shared memory: 2 x 104 KB per SM
     cudaStream_t s = (cudaStream_t)stream;
     const int ml = max_level < 0 ? -1 : max_level;
     if (x == nullptr) k_sdf_bwd_tc<true><<<grid, kTile, kBwdSmem, s>>>(m, (const __half *)params_half, d, nullptr, rays_o, rays_d, ridx, t, d_sdf, n, ml,

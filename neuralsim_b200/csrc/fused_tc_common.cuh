@@ -1,4 +1,4 @@
-// Building blocks shared by the tcgen05 fused kernels (fused_tc.cu, color_tc.cu): tile constants, the per-thread
+// Building blocks shared by the wgmma fused kernels (fused_tc.cu, color_tc.cu): tile constants, the per-thread
 // LoTD gather that writes straight into a core-matrix A tile, point loading and W1 staging.
 #pragma once
 #include "lotd_device.cuh"
@@ -118,53 +118,52 @@ __device__ __forceinline__ void stage_W1(const DecoderDevTC &dec, uint8_t *sB, i
     }
 }
 
-// ---- one 128-point tile of the fused SDF query: gather -> tcgen05 MMA -> SFU epilogue (used by k_fused_sdf_tc and by the per-ray kernels)
+// ---- one 128-point tile of the fused SDF query: gather -> wgmma -> SFU epilogue (used by k_fused_sdf_tc and by the per-ray kernels)
 struct SdfTile {
     const PLMeta &m;
     const __half *grid;
     int max_level;
     uint8_t *sA;
-    uint32_t a_addr, b_addr, idesc, tmem, lane_base;
-    uint64_t *mbar;
+    uint32_t a_addr, b_addr;
+    float *srow;                           // [kTile] shared: the sdf of each row, handed from the fragment owners to the row's thread
     const float *sb1, *sW2;
     float sb2;
     SoftplusK spk;
 };
 
-// all 128 threads: my point's table coordinates -> my sdf (fp16-rounded, as fp32).  Ends with the CTA barrier that frees tile + TMEM.
+// all 128 threads: my point's table coordinates -> my sdf (fp16-rounded, as fp32).  Ends with the CTA barrier that frees the tile.
+// The epilogue runs on the accumulator fragments: each lane folds its 16 of a row's 64 hidden units, the quad sums the four parts
+// in a fixed order (the same for every row, so a point's sdf does not depend on where it sits in the tile).
 template <bool FAST_SP, int UNROLL, bool PAIRED>
-__device__ __forceinline__ float sdf_of_tile(const SdfTile &c, const float (&xs)[3], int tid, uint32_t &phase) {
+__device__ __forceinline__ float sdf_of_tile(const SdfTile &c, const float (&xs)[3], int tid) {
     gather_row_to_tile<kTile, UNROLL, PAIRED>(c.m, c.grid, xs, c.max_level, c.sA, tid);
     tc::fence_async_smem();                // generic-proxy smem writes -> visible to the tensor core (async proxy)
     __syncthreads();
-    if (tid == 0) {
-        tc::fence_after_sync();
+    float z[2][HW / 2];
+    tc::mma_m128<HW, 0, 0, NF / 16>(z, tc::kmajor(c.a_addr, kTile), tc::kmajor(c.b_addr, HW), false);
+    const int lane = tid & 31, q = lane & 3;
 #pragma unroll
-        for (int ks = 0; ks < NF / 16; ++ks)
-            tc::mma_f16_ss(c.tmem, tc::make_desc(c.a_addr + ks * 2 * (kTile * 16), kTile * 16, 128),
-                           tc::make_desc(c.b_addr + ks * 2 * (HW * 16), HW * 16, 128), c.idesc, ks > 0);
-        tc::commit(c.mbar);
-    }
-    tc::mbar_wait(c.mbar, phase);
-    phase ^= 1;
-    tc::fence_after_sync();
-    float out = 0.f;
-#pragma unroll 1
-    for (int ch = 0; ch < HW / 8; ++ch) {
-        float z[8];
-        tc::tmem_ld8(c.tmem + c.lane_base + ch * 8, z);
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float zz = __half2float(__float2half_rn(z[j] + c.sb1[ch * 8 + j]));
-            float sp;
-            if (FAST_SP) sp = softplus_a(zz, c.spk);
-            else { const float zb = zz * c.spk.beta; sp = zb > 20.f ? zz : log1pf(expf(zb)) * (1.f / c.spk.beta); }
-            out = fmaf(__half2float(__float2half_rn(sp)), c.sW2[ch * 8 + j], out);
+        for (int i = 0; i < 2; ++i) {
+            float out = 0.f;
+#pragma unroll
+            for (int ch = 0; ch < HW / 8; ++ch)
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const int col = ch * 8 + 2 * q + j;
+                    const float zz = __half2float(__float2half_rn(z[h][4 * ch + 2 * i + j] + c.sb1[col]));
+                    float sp;
+                    if (FAST_SP) sp = softplus_a(zz, c.spk);
+                    else { const float zb = zz * c.spk.beta; sp = zb > 20.f ? zz : log1pf(expf(zb)) * (1.f / c.spk.beta); }
+                    out = fmaf(__half2float(__float2half_rn(sp)), c.sW2[col], out);
+                }
+            out += __shfl_xor_sync(0xffffffffu, out, 1);
+            out += __shfl_xor_sync(0xffffffffu, out, 2);
+            if (q == 0) c.srow[h * 64 + (tid >> 5) * 16 + (lane >> 2) + 8 * i] = out;
         }
-    }
-    tc::fence_before_sync();               // TMEM reads done before the next tile's MMA overwrites Z
     __syncthreads();
-    return __half2float(__float2half_rn(out + c.sb2));
+    return __half2float(__float2half_rn(c.srow[tid] + c.sb2));
 }
 
 }  // namespace nsb

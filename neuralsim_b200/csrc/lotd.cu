@@ -1,7 +1,7 @@
-// LoTD (Dense + Hash multi-resolution grid) encoding kernels for sm_100a and their C entry points.
+// LoTD (Dense + Hash multi-resolution grid) encoding kernels for sm_90a and their C entry points.
 //
 // Replaces the reference's `_lotd` extension for the c_hash_only path
-// (/root/reference/nr3d_lib/csrc/lotd/include/lotd/lotd_hash_only.h).  Different design:
+// (nr3d_lib/csrc/lotd/include/lotd/lotd_hash_only.h).  Different design:
 //   * point-major: one thread walks all pseudo-levels of its point, so the [N,F] feature row is produced
 //     contiguously (the reference runs a (points x levels) grid and writes a transposed [F,N] tensor);
 //   * fp32 gradient accumulation with vector reductions (red.global.add.v2.f32) instead of fp16 atomics;

@@ -1,5 +1,5 @@
 // Device-side building blocks of the LoTD encoding shared by lotd.cu and the fused kernels.
-// Index / hash arithmetic follows /root/reference/nr3d_lib/csrc/lotd/include/lotd/lotd_cuda.h:92-143,
+// Index / hash arithmetic follows nr3d_lib/csrc/lotd/include/lotd/lotd_cuda.h:92-143,
 // position arithmetic lotd_cuda.h:959-984 (InterpolationType::Linear).
 #pragma once
 #include <type_traits>
@@ -277,8 +277,8 @@ __device__ __forceinline__ void red_add2(float2 *dst, float a, float b) {
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(a), "f"(b) : "memory");
 }
 
-// ---- warp-merged table-gradient updates.  Measured (profiles/r01g_ab_scatter.txt): the fp32 atomics themselves bound the table
-// backward (80 G corner-updates/s whether the points are ordered or shuffled, at any occupancy), so the lever is FEWER atomics.
+// ---- warp-merged table-gradient updates.  The fp32 atomics themselves bound the table
+// backward (the same rate whether the points are ordered or shuffled, at any occupancy), so the lever is FEWER atomics.
 // The lanes of a warp are consecutive samples of a ray; on the coarse / middle levels neighbouring samples fall into the same cell
 // and update the same 8 corners.  Runs of lanes with equal integer cell coordinates are summed with shuffles (segmented reduction
 // over contiguous runs; the run structure is one ballot) and only the run's first lane issues the 8 reductions.

@@ -1,10 +1,11 @@
-// Occupancy-grid ray marching for sm_100a (single grid and batched grids, AABB contraction).
+// Occupancy-grid ray marching for sm_90a (single grid and batched grids, AABB contraction).
 //
 // Replaces `_occ_grid.ray_marching / batched_ray_marching`
-// (/root/reference/nr3d_lib/csrc/occ_grid/src/ray_marching.cu:17-244, batched_marching.cu:18-287).
+// (nr3d_lib/csrc/occ_grid/src/ray_marching.cu:17-244, batched_marching.cu:18-287).
 // The sample counts / voxel ids are integer results and are kept bit-exact with the reference by issuing the
-// same sequence of fp32 roundings (explicit _rn intrinsics; the sequence was read off the SASS nvcc 12.9
-// emits for the reference at -O3/sm_100a -- see oracle/march.c and DESIGN.md).
+// same sequence of fp32 roundings (explicit _rn intrinsics; the sequence was read off the SASS nvcc 12.9 emitted
+// for the reference at -O3 for sm_100a -- see oracle/march.c and DESIGN.md; that the reference's sm_90a build gives the same
+// counts, samples and voxel ids bit for bit is checked against its stored outputs, tests/test_ref_parity_gpu.py).
 // Differences in design: the bool grid is bit-packed into shared memory once per CTA when it fits
 // (64^3 -> 32 KB), so the inner loop never touches global memory; rays are processed grid-stride by
 // a wave-sized grid.

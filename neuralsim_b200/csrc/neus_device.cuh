@@ -1,5 +1,5 @@
 // Per-ray NeuS stage bodies shared by the stand-alone stage kernels (neus_fused.cu, neus_glue.cu) and -- round 2 -- the persistent per-ray
-// kernel (profiles/NEXT_persistent_ray_kernel.md): they take plain pointers, so they run on global packs and on a ray's samples in shared memory alike.
+// kernel (ray_upsample.cu): they take plain pointers, so they run on global packs and on a ray's samples in shared memory alike.
 #pragma once
 #include "nsb_common.cuh"
 

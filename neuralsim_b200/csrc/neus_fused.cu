@@ -1,4 +1,4 @@
-// Fused per-ray NeuS stages for sm_100a: one warp owns one ray (pack) and keeps the ray's state in registers / shuffles.
+// Fused per-ray NeuS stages for sm_90a: one warp owns one ray (pack) and keeps the ray's state in registers / shuffles.
 // Each kernel replaces a chain of ~10-40 ATen / pack_ops launches of the reference's Python layer:
 //   k_upsample_cdf      neus_packed_sdf_to_upsample_alpha | neus_packed_sdf_to_alpha -> packed_alpha_to_vw -> packed_cumsum(excl)
 //                       -> / clamp_min(last,1e-5)                     (graphics/neus/neus_ray_query.py:873-884, neus_utils.py:164-188)

@@ -1,4 +1,4 @@
-// Glue of the per-ray NeuS query for sm_100a: the index bookkeeping between the big kernels (march -> up-sample -> boundary
+// Glue of the per-ray NeuS query for sm_90a: the index bookkeeping between the big kernels (march -> up-sample -> boundary
 // SDF -> alpha -> colour -> composite) that the reference does with ~200 ATen launches and ~20 host syncs per call
 // (graphics/neus/neus_ray_query.py:732-1104, pack_ops.py, occgrid_raymarch.py:60-112) -- here one launch per step:
 //

@@ -1,4 +1,4 @@
-// Shared helpers of the neuralsim_b200 CUDA library (sm_100a only).
+// Shared helpers of the neuralsim_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -47,7 +47,7 @@ inline int sm_count() {
     int n = cache[dev].load(std::memory_order_relaxed);
     if (n == 0) {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
         cache[dev].store(n, std::memory_order_relaxed);
     }
     return n;

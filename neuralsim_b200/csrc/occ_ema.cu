@@ -1,4 +1,4 @@
-// Occupancy-grid EMA maintenance on the device (SURVEY.md §8 a11 / f3), sm_100a.
+// Occupancy-grid EMA maintenance on the device (SURVEY.md §8 a11 / f3), sm_90a.
 //
 // Reference: OccGridEma._step_update_occ (nr3d_lib/models/accelerations/occgrid/ema_single.py:176-190) ->
 //   occ_val = normalized_logistic_density(sdf_half, inv_s)            (occgrid/utils.py:63-68, maths/common.py:122-133)

@@ -1,6 +1,6 @@
-// Packed-tensor ("ragged per-ray arrays") operators for sm_100a.
+// Packed-tensor ("ragged per-ray arrays") operators for sm_90a.
 //
-// Replaces the reference's `_pack_ops` extension (/root/reference/nr3d_lib/csrc/pack_ops/pack_ops_cuda.cu).
+// Replaces the reference's `_pack_ops` extension (nr3d_lib/csrc/pack_ops/pack_ops_cuda.cu).
 // The reference runs ONE THREAD PER PACK with serial inner loops, so neighbouring threads stride by the pack
 // length (uncoalesced) and every wrapper syncs the host.  Here a WARP owns a pack: lanes sweep the pack in
 // 32-element, fully coalesced chunks; reductions / scans use shuffles with a running carry; nothing

@@ -4,7 +4,7 @@
 // (graphics/neus.py:_query_fused, reference neus_ray_query.py:861-905) and keeps the ray's samples in shared memory in between.
 // A CTA of 128 threads owns a group of 4 consecutive hit rays: warp w <-> ray w for the per-ray stages (the bodies are the stand-alone kernels'
 // own device functions, neus_device.cuh, so the results are bit-identical by construction); for the SDF evaluations the four rays' pending samples
-// are concatenated into 128-point tiles of the usual gather -> tcgen05 -> SFU pipeline (sdf_of_tile, fused_tc_common.cuh).
+// are concatenated into 128-point tiles of the usual gather -> wgmma -> SFU pipeline (sdf_of_tile, fused_tc_common.cuh).
 // Output: fine[n_hit, sum(n_fine)] -- what `torch.cat(fine_stages, -1)` is on the multi-kernel path.  A ray whose samples do not fit the
 // per-ray shared-memory capacity (kCap) works on a slice of a global scratch buffer instead (same code: the stage bodies take plain
 // pointers); `overflow` is only raised for a ray longer than that slice (`long_cap`, sized from max_steps by the caller: cannot happen then).
@@ -97,12 +97,10 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
                       int nf_total, int32_t *__restrict__ overflow, float *__restrict__ scratch, int long_cap, const OccCollect oc,
                       const int64_t *__restrict__ n_dev) {
     n_hit = eff_n(n_hit, n_dev);
-    __shared__ __align__(1024) uint8_t sA[kTile * NF * 2];
-    __shared__ __align__(1024) uint8_t sB[HW * NF * 2];
-    __shared__ float sb1[HW], sW2[HW];
+    __shared__ __align__(128) uint8_t sA[kTile * NF * 2];
+    __shared__ __align__(128) uint8_t sB[HW * NF * 2];
+    __shared__ float sb1[HW], sW2[HW], srow[kTile];
     __shared__ float sb2;
-    __shared__ __align__(8) uint64_t mbar;
-    __shared__ uint32_t tmem_slot;
     __shared__ float s_t[2][kG][kCap], s_sdf[2][kG][kCap], s_cdf[kG][kCap];
     __shared__ float s_fine[kG][kMaxFine], s_fsdf[kG][kMaxFine];
     __shared__ float s_o[kG][3], s_d[kG][3];
@@ -115,19 +113,10 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
         sb1[tid] = tid < dec.width ? __half2float(dec.b1[tid]) : 0.f;
         sW2[tid] = tid < dec.width ? __half2float(dec.W2[tid]) : 0.f;
     }
-    if (tid == 0) {
-        sb2 = __half2float(dec.b2[0]);
-        tc::mbar_init(&mbar, 1);
-        tc::fence_mbar_init();
-    }
-    if (warp == 0) tc::tmem_alloc<64>(&tmem_slot);
+    if (tid == 0) sb2 = __half2float(dec.b2[0]);
     tc::fence_async_smem();
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), tc::make_idesc(kTile, HW, 0, 0), tmem_slot,
-                      (uint32_t)(warp * 32) << 16, &mbar, sb1, sW2, sb2, SoftplusK(dec.beta)};
-    uint32_t phase = 0;
+    const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
     int room = kCap;                                     // a ray must hold its marched samples + every merged stage
     for (int i = 0; i + 1 < ua.n_stage; ++i) room -= ua.n_fine[i];
 
@@ -180,7 +169,7 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
                 }
 #pragma unroll
                 for (int c = 0; c < 3; ++c) xs[c] = fminf(fmaxf(__fmaf_rn(xs[c], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
-                const float v = sdf_of_tile<true, 2, false>(ctx, xs, tid, phase);
+                const float v = sdf_of_tile<true, 2, false>(ctx, xs, tid);
                 if (valid) {
                     p_sdf[0][q][r] = v;
                     if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -215,7 +204,7 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
                 }
 #pragma unroll
                 for (int c = 0; c < 3; ++c) xs[c] = fminf(fmaxf(__fmaf_rn(xs[c], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
-                const float v = sdf_of_tile<true, 2, false>(ctx, xs, tid, phase);
+                const float v = sdf_of_tile<true, 2, false>(ctx, xs, tid);
                 if (valid) {
                     s_fsdf[q][k] = v;
                     if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -232,7 +221,6 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
         }
         __syncthreads();                                 // the group's shared memory is free for the next one
     }
-    if (warp == 0) tc::tmem_free<64>(ctx.tmem);
 }
 
 }  // namespace nsb

@@ -1,5 +1,5 @@
-// Real spherical-harmonics embedding of view directions (degree <= 4 -> up to 16 channels) for sm_100a.
-// Replaces `_shencoder.sh_encode_forward/backward` (/root/reference/nr3d_lib/externals/shencoder/shencoder.cu:33-,
+// Real spherical-harmonics embedding of view directions (degree <= 4 -> up to 16 channels) for sm_90a.
+// Replaces `_shencoder.sh_encode_forward/backward` (nr3d_lib/externals/shencoder/shencoder.cu:33-,
 // 364-387) for the degrees the path uses (CFG `degree: 4`); launches on the caller's stream (the reference ignores
 // the current stream).  Outputs are [N, C^2] fp32, the optional Jacobian is [N, 3, C^2] as in the reference.
 #include "sh_device.cuh"

@@ -1,5 +1,5 @@
 // Real spherical-harmonics basis (degree <= 4), shared by sh.cu and the fused colour kernel.
-// Follows /root/reference/nr3d_lib/externals/shencoder/shencoder.cu:33-80.
+// Follows nr3d_lib/externals/shencoder/shencoder.cu:33-80.
 #pragma once
 #include "nsb_common.cuh"
 

@@ -1,5 +1,6 @@
-// Blackwell tensor-core plumbing used by the fused MLP kernels: tcgen05.mma with shared-memory operands,
-// accumulators in TMEM, completion through an mbarrier.  Inline PTX only (no CUTLASS dependency).
+// Hopper tensor-core plumbing used by the fused MLP kernels: warpgroup MMAs (wgmma) with both operands in shared memory
+// and fp32 accumulators in registers.  Inline PTX only (no CUTLASS dependency).  Every kernel that uses it runs one
+// warpgroup (128 threads) per CTA; the MMA helpers are collective over it and must be reached by all 128 threads.
 //
 // Shared-memory operand layout ("canonical K-major, no swizzle", what cute calls Layout_K_INTER_Atom):
 //   the tile is cut into core matrices of 8 rows x 16 bytes (8 fp16 along K); a core matrix is 128 contiguous
@@ -8,8 +9,13 @@
 //   We store a [R x K] fp16 tile chunk-major:   byte(r, k) = (k/8) * (R*16) + r*16 + (k%8)*2
 //   => SBO = 128, LBO = R*16.  Thread r owns row r and writes K/8 16-byte vectors with a stride of R*16 bytes:
 //   consecutive threads hit consecutive 16-byte slots, i.e. conflict-free st.shared.v4.
-//   The very same bytes read as an MN-major operand (rows <-> K) are described by swapping the two offsets
-//   (LBO = 128, SBO = R*16) -- used by the weight-gradient MMA that contracts over the points of a tile.
+//   The very same bytes read as an MN-major (transposed) operand (rows <-> K) are described by swapping the two
+//   offsets (LBO = 128, SBO = R*16) -- used by the weight-gradient MMAs that contract over the points of a tile.
+//
+// A 128-row tile is two m64 wgmma row blocks.  The accumulator of rows [64h, 64h + 64) lives in d[h][] in the wgmma
+// fragment layout: warp w, lane l holds rows 64h + 16w + l/4 (+8) and columns 8c + 2(l%4) (+1).  Kernels whose
+// epilogue wants "thread r owns row r" stage the fragments in a padded fp32 row buffer in shared memory (frag_store,
+// then a CTA barrier, then acc_ld8 of the own row).
 #pragma once
 #include "nsb_common.cuh"
 
@@ -18,35 +24,161 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// 64-bit shared-memory matrix descriptor (PTX "tcgen05 matrix descriptor"; fields as in cute::UMMA::SmemDescriptor):
-//   [0,14) start address >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [46,48) version = 1 | [61,64) swizzle = 0 (none)
+// 64-bit wgmma shared-memory matrix descriptor (cute::GMMA::GmmaDescriptor):
+//   [0,14) start address >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [49,52) base offset = 0 | [62,64) swizzle = 0 (none)
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
 
-// 32-bit instruction descriptor for kind::f16 (cute::UMMA::InstrDescriptor): fp16 x fp16 -> fp32.
-//   [4,6) D format 1 = F32 | [7,10) A format 0 = F16 | [10,13) B format 0 = F16 | [15] A major | [16] B major
-//   (0 = K-major, 1 = MN-major) | [17,23) N >> 3 | [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// One chunk-major fp16 tile in shared memory as an MMA operand; kstep = bytes between consecutive K = 16 slices.
+struct Operand {
+    uint32_t addr, lbo, sbo, kstep;
+};
+// a [rows x K] tile contracted over its columns (K-major)
+__device__ __forceinline__ Operand kmajor(uint32_t addr, int rows) { return Operand{addr, (uint32_t)rows * 16, 128, (uint32_t)rows * 32}; }
+// the same bytes contracted over its rows (MN-major: K = the rows, M or N = the columns)
+__device__ __forceinline__ Operand mnmajor(uint32_t addr, int rows) { return Operand{addr, 128, (uint32_t)rows * 16, 256}; }
+
+// wgmma.mma_async m64nNk16, fp16 x fp16 -> fp32, A and B from shared memory; TA / TB = 1: the operand is MN-major.
+template <int N, int TA, int TB>
+struct Wgmma;
+template <int TA, int TB>
+struct Wgmma<32, TA, TB> {
+    __device__ __forceinline__ static void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
+template <int TA, int TB>
+struct Wgmma<40, TA, TB> {
+    __device__ __forceinline__ static void mma(float (&d)[20], uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n40k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, %20, %21, p, 1, 1, %23, %24;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+            : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
+template <int TA, int TB>
+struct Wgmma<48, TA, TB> {
+    __device__ __forceinline__ static void mma(float (&d)[24], uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %27, %28;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
+template <int TA, int TB>
+struct Wgmma<64, TA, TB> {
+    __device__ __forceinline__ static void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
+template <int TA, int TB>
+struct Wgmma<80, TA, TB> {
+    __device__ __forceinline__ static void mma(float (&d)[40], uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, %43, %44;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+            : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of an accumulator register across the asynchronous MMA
+__device__ __forceinline__ void fence_operand(float &r) { asm volatile("" : "+f"(r)::"memory"); }
+
+// D[128 x N] (+)= A[128 x 16 KSTEPS] . B[16 KSTEPS x N] by the whole warpgroup; returns when the result is in d.
+// The shared-memory operands must have been made visible to the async proxy (fence_async_smem + barrier) before.
+template <int N, int TA, int TB, int KSTEPS>
+__device__ __forceinline__ void mma_m128(float (&d)[2][N / 2], const Operand &a, const Operand &b, bool accumulate) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) fence_operand(d[h][i]);
+    wgmma_fence();
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int ks = 0; ks < KSTEPS; ++ks)
+            Wgmma<N, TA, TB>::mma(d[h], make_desc(a.addr + h * 8 * a.sbo + ks * a.kstep, a.lbo, a.sbo), make_desc(b.addr + ks * b.kstep, b.lbo, b.sbo),
+                                  (ks > 0 || accumulate) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait_all();
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) fence_operand(d[h][i]);
 }
 
-__device__ __forceinline__ void mma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+// Row buffer of staged accumulators: row r at acc + r * stride (floats).  A stride = 4 (mod 8) keeps the row reads of
+// acc_ld8 free of bank conflicts.
+constexpr int acc_stride(int cols) { return cols + 4; }
+
+// this thread's fragments of D[128 x N] -> columns [col0, col0 + N) of the row buffer (fp32, exact)
+template <int N>
+__device__ __forceinline__ void frag_store(const float (&d)[2][N / 2], float *acc, int stride, int col0) {
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int c = 0; c < N / 8; ++c)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int row = h * 64 + w * 16 + (l >> 2) + 8 * i, col = col0 + c * 8 + 2 * (l & 3);
+                *reinterpret_cast<float2 *>(acc + row * stride + col) = make_float2(d[h][4 * c + 2 * i], d[h][4 * c + 2 * i + 1]);
+            }
+}
+template <int N>
+__device__ __forceinline__ void frag_load(float (&d)[2][N / 2], const float *acc, int stride, int col0) {
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int c = 0; c < N / 8; ++c)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int row = h * 64 + w * 16 + (l >> 2) + 8 * i, col = col0 + c * 8 + 2 * (l & 3);
+                const float2 v = *reinterpret_cast<const float2 *>(acc + row * stride + col);
+                d[h][4 * c + 2 * i] = v.x;
+                d[h][4 * c + 2 * i + 1] = v.y;
+            }
+}
+// D[128 x N] (+)= A . B with D kept in columns [col0, col0 + N) of the row buffer: load (if accumulating), MMA, store.
+// Only this thread's own fragment positions are read and written; the rows are readable by their owners after a barrier.
+template <int N, int TA, int TB, int KSTEPS>
+__device__ __forceinline__ void mma_to_rows(float *acc, int stride, int col0, const Operand &a, const Operand &b, bool accumulate) {
+    float d[2][N / 2];
+    if (accumulate) frag_load<N>(d, acc, stride, col0);
+    else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) d[h][i] = 0.f;
+    }
+    mma_m128<N, TA, TB, KSTEPS>(d, a, b, accumulate);
+    frag_store<N>(d, acc, stride, col0);
 }
 
-// all previously issued MMAs of this thread arrive on the mbarrier when they complete
-__device__ __forceinline__ void commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// 8 consecutive staged fp32 columns of one row
+__device__ __forceinline__ void acc_ld8(const float *acc, int stride, int row, int col, float (&v)[8]) {
+    const float4 a = *reinterpret_cast<const float4 *>(acc + row * stride + col), b = *reinterpret_cast<const float4 *>(acc + row * stride + col + 4);
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
@@ -74,49 +206,6 @@ __device__ __forceinline__ void tma_load_bulk(void *smem_dst, const void *gmem_s
 
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// one full warp allocates / frees `cols` TMEM columns (power of two >= 32); the base address lands in *slot (shared)
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t *slot) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "n"(COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_free(uint32_t base) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "n"(COLS) : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread i gets lane 32*(warp%4)+i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// TMEM -> registers, 8 consecutive fp32 columns (used inside rolled loops: small code, dynamic column address)
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
 
 __device__ __forceinline__ uint4 pack8_f16(const float (&v)[8]) {
     __half2 h0 = __floats2half2_rn(v[0], v[1]), h1 = __floats2half2_rn(v[2], v[3]);

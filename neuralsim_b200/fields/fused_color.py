@@ -1,4 +1,4 @@
-"""The colour / normal query of LoTDNeuS as ONE differentiable op over the tcgen05 kernels of csrc/color_tc.cu.
+"""The colour / normal query of LoTDNeuS as ONE differentiable op over the wgmma kernels of csrc/color_tc.cu.
 
 `fused_color(model, ridx, t, rays_o, rays_d, view_dirs, h_appear)` computes, for the packed samples x = o[ridx] + d[ridx] t,
 what `LoTDNeuS.forward(x, v=, h_appear=, nablas_has_grad=True)` computes in the reference

@@ -4,7 +4,7 @@
 fields/nerf/mlp_nerf.py:188-289, embedders/spherical_harmonics/sphere_harmonics.py:14-82, fields/neus/variance.py:122-142).
 
 fp32 master weights, fp16 autocast evaluation -- the numerics contract of the reference.  The modules below are the
-reference's layers (torch autocast, cuBLAS) and remain the specification; the hot path replaces them by fused tcgen05
+reference's layers (torch autocast, cuBLAS) and remain the specification; the hot path replaces them by fused wgmma
 kernels with the same rounding points: SDF queries (with or without grad) by `nsb_fused_sdf*` + `nsb_fused_sdf_bwd`
 (`_FusedSDF`, csrc/fused_tc.cu), the colour / normal query by `nsb_fused_color_*` (fields/fused_color.py, csrc/color_tc.cu).
 """

@@ -29,10 +29,9 @@ from . import neus_fused
 FUSED_STAGES = True
 import os as _os
 # The no-grad half of the fused query (sdf of the marched samples + the up-sampling stages) as ONE persistent per-ray kernel
-# (csrc/ray_upsample.cu) or as one launch per stage -- same values either way (tests/test_ray_upsample_gpu.py).  Measured on the B200
-# (profiles/r02d_*): the persistent kernel wins on small batches (4096 random rays: 0.819 vs 0.840 ms / step, 25 instead of 35 launches) and loses
-# on large ones (800x600 frame: 14.06 vs 13.30 ms; its 128-point tiles are filled by 4 rays' 9-sample stages to 28 %), so: True / False force it,
-# "auto" (default) takes it below PERSISTENT_MAX_RAYS tested rays.  perturb=True always runs the stage kernels.
+# (csrc/ray_upsample.cu) or as one launch per stage -- same values either way (tests/test_ray_upsample_gpu.py).  The persistent kernel saves
+# launches on small batches (25 instead of 35 for 4096 random rays) and loses on large ones (its 128-point tiles are filled by 4 rays' 9-sample
+# stages to 28 %), so: True / False force it, "auto" (default) takes it below PERSISTENT_MAX_RAYS tested rays.  perturb=True always runs the stage kernels.
 _pu = _os.environ.get("NSB_PERSISTENT_UPSAMPLE", "auto")
 PERSISTENT_UPSAMPLE = "auto" if _pu == "auto" else (_pu != "0")
 PERSISTENT_MAX_RAYS = 8192
@@ -40,7 +39,7 @@ PERSISTENT_MAX_RAYS = 8192
 
 def use_persistent_upsample(n_rays: int) -> bool:
     return (n_rays < PERSISTENT_MAX_RAYS) if PERSISTENT_UPSAMPLE == "auto" else bool(PERSISTENT_UPSAMPLE)
-MARCHED_TILED = _os.environ.get("NSB_MARCHED_TILED", "0") != "0"     # measured: 0.71 ms ray-major vs 0.99 ms ray-tiled per frame (profiles/README.md)
+MARCHED_TILED = _os.environ.get("NSB_MARCHED_TILED", "0") != "0"     # ray-tiled traversal of the marched samples (off: ray-major was the faster order)
 
 __all__ = ["neus_cdf", "neus_ray_cdf_to_alpha", "neus_ray_sdf_to_alpha", "neus_ray_sdf_to_vw", "neus_packed_cdf_to_alpha",
            "neus_packed_sdf_to_alpha", "neus_packed_sdf_to_upsample_alpha", "neus_ray_sdf_to_upsample_alpha",

@@ -1,22 +1,32 @@
-"""Compiles the REFERENCE's own CUDA extensions, from the sources where they lie under /root/reference, into
-oracle/_ref/*.so (git-ignored, shipped to the GPU box with the snapshot).  TEST INFRASTRUCTURE.
+"""Compiles the REFERENCE's own CUDA extensions, from the sources of a checkout of the reference project (neuralsim with its
+nr3d_lib submodule), into oracle/_ref/*.so (git-ignored).  TEST INFRASTRUCTURE.  The checkout is found by reference_root():
+the NR3D_REFERENCE environment variable if set, else a directory named `reference` next to this repository's checkout.
 
     python oracle/build_ref.py            # all four hot-path extensions, incremental
 
 This is not the reference's build system (nr3d_lib/setup.py refuses to run without a CUDA device, setup.py:81-83):
 the source lists, include directories and nvcc flags of setup.py:86-134 (_lotd), :140-184 (_pack_ops), :495-516
 (_occ_grid) and :523-554 (_shencoder) are restated here and handed to torch.utils.cpp_extension.load with
-TORCH_CUDA_ARCH_LIST=10.0 (what `compute_{cc}` resolves to on a B200).  No reference source is copied.
+TORCH_CUDA_ARCH_LIST=9.0a (what `compute_{cc}` resolves to on an H100).  No reference source is copied.
 
 Uses: (1) GPU parity tests of our kernels against the reference kernels on identical inputs
-(tests/test_ref_parity_gpu.py); (2) the "reference nr3d_lib CUDA path on the same B200" timing of BASELINE.md B1.
+(tests/golden/make_ref_golden.py records their outputs for tests/test_ref_parity_gpu.py); (2) the "reference nr3d_lib CUDA path on the
+same GPU" timing of BASELINE.md B1.
 """
 from __future__ import annotations
 
 import os
 import sys
 
-REF = "/root/reference/nr3d_lib"
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def reference_root():
+    """the reference checkout: $NR3D_REFERENCE, else <parent of this repository>/reference; None if neither is a directory"""
+    root = os.environ.get("NR3D_REFERENCE") or os.path.join(os.path.dirname(ROOT), "reference")
+    return root if os.path.isdir(os.path.join(root, "nr3d_lib")) else None
+
+
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")
 
 COMMON = ["-O3", "-DNDEBUG", "-std=c++17", "-Xcompiler=-mf16c", "-Xcompiler=-Wno-float-conversion", "-Xcompiler=-fno-strict-aliasing",
@@ -41,10 +51,12 @@ EXTS = {
 
 
 def build(names=None, verbose=False):
-    if not os.path.isdir(REF):
-        print("oracle/build_ref.py: /root/reference is absent (GPU box) -- using prebuilt oracle/_ref if any")
+    if reference_root() is None:
+        print("oracle/build_ref.py: no reference checkout (set NR3D_REFERENCE, or place it next to this repository as `reference`) "
+              "-- using prebuilt oracle/_ref if any")
         return []
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    REF = os.path.join(reference_root(), "nr3d_lib")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", str(os.cpu_count() or 8))
     from torch.utils import cpp_extension
     built = []

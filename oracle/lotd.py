@@ -1,6 +1,6 @@
 """CPU restatement of the LoTD Dense+Hash ("hash-only") grid encoding.  TEST INFRASTRUCTURE.
 
-Follows (paths relative to /root/reference/nr3d_lib):
+Follows (paths relative to nr3d_lib):
   meta            csrc/lotd/src/lotd_torch_api.cu:29-230   (LoDMeta::create_meta)
   config          nr3d_lib/models/grid_encodings/lotd/lotd_cfg.py:48-57 (gen_ngp_cfg)
   index / hash    csrc/lotd/include/lotd/lotd_cuda.h:92-143

@@ -1,6 +1,6 @@
 /* CPU restatement of the reference occupancy-grid ray marching kernels.  TEST INFRASTRUCTURE.
  *
- * Follows /root/reference/nr3d_lib/csrc/occ_grid:
+ * Follows nr3d_lib/csrc/occ_grid:
  *   src/ray_marching.cu:17-134        (ray_marching_kernel, AABB contraction only)
  *   src/batched_marching.cu:18-152    (batched_ray_marching_kernel)
  *   include/occ_grid/helpers_march.h:11-76, helpers_contraction.h:10-21
@@ -9,7 +9,8 @@
  * bit-exact, so the exact sequence of fp32 roundings matters.  The sequence below (which products are
  * fused into an FMA, which divisions are IEEE) was read off the SASS that nvcc 12.9 generates for the
  * reference source at -O3 for sm_100a (cuobjdump of ray_marching.cu, see DESIGN.md "March: rounding
- * sequence"):
+ * sequence"); the reference's sm_90a build produces the same outputs bit for bit (digests stored under tests/golden/,
+ * tests/test_ref_parity_gpu.py):
  *   xyz          = fma(t_mid, dir, origin)
  *   unit         = (xyz - roi_min) / (roi_max - roi_min)               IEEE division
  *   ixyz         = trunc(unit * float(res))                            one multiply

@@ -1,7 +1,7 @@
 """CPU restatement of the tiny networks on the path: SH view-direction embedding, the autocast(fp16)
 DenseLayer/MLP stack, the LoTD-SDF decoder with analytic nablas and the radiance net.  TEST INFRASTRUCTURE.
 
-Follows (paths relative to /root/reference/nr3d_lib):
+Follows (paths relative to nr3d_lib):
   SH basis        externals/shencoder/shencoder.cu:33-80 (real SH, degree<=4 as used by CFG `degree: 4`)
   DenseLayer/MLP  nr3d_lib/models/layers.py:228-312, nr3d_lib/models/blocks/mlp.py:26-125
   LoTDSDF         nr3d_lib/models/fields/sdf/lotd_sdf.py:176-257 (forward, forward_sdf_nablas)

@@ -1,7 +1,7 @@
 """CPU restatement of the reference `_pack_ops` native extension.  TEST INFRASTRUCTURE.
 
 "Packed" tensors are ragged per-ray arrays described by pack_infos[P,2] = (first index, length).
-Every function follows a kernel of /root/reference/nr3d_lib/csrc/pack_ops/pack_ops_cuda.cu (cited per
+Every function follows a kernel of nr3d_lib/csrc/pack_ops/pack_ops_cuda.cu (cited per
 function) and keeps its serial, one-thread-per-pack evaluation order so that fp32 results are the
 ones a sequential loop produces.  Call signatures are those exported by
 csrc/pack_ops/pack_ops.cpp:20-58, on CPU torch tensors.

@@ -1,7 +1,7 @@
 """CPU restatement of the per-ray NeuS rendering path (Python/PyTorch layer of the reference).
 TEST INFRASTRUCTURE.
 
-Follows (paths relative to /root/reference):
+Follows (paths relative to the reference project):
   ray test          nr3d_lib/nr3d_lib/models/spatial/aabb.py:85-99, graphics/raytest.py:162-167
   coarse sampling   nr3d_lib/nr3d_lib/graphics/raysample.py:285-310 (batch_sample_step_linear)
   fine sampling     nr3d_lib/nr3d_lib/graphics/raysample.py:38-61 (packed_sample_cdf)

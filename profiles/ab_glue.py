@@ -1,8 +1,8 @@
-"""A/B of the step's glue on one B200, one process, same model and poses (not a bench value; bench.py is):
+"""A/B of the step's glue on one GPU, one process, same model and poses (not a bench value; bench.py is):
    asm_chunk   1 = every ray of nsb_assemble_boundary searches the hit list, 8 = one search per 8 consecutive rays
    onepass     0 = two-round march, 1 = march once recording the samples per ray + copy (auto: only when the record fits 64 MB)
 (r02j: the first version of this script captured its second frame with all-zero input rays and hung in the march until its timeout; only the
-first configuration of each run was recorded, profiles/r02j_ab_old_config.jsonl.  Fixed below, not re-run: no GPU time was left.)
+first configuration of each run was recorded.  Fixed below.)
 Usage: python profiles/ab_glue.py [--rays 480000 | --rays 4096 --random-rays] [--steps 20] [--rounds 2]"""
 import argparse
 import ctypes

@@ -22,7 +22,7 @@ WANT = [
     ("l1tex__t_requests_pipe_lsu_mem_global_op_red.sum", "global red requests"),
     ("l1tex__t_sectors_pipe_lsu_mem_global_op_red.sum", "global red sectors"),
     ("lts__t_sectors_op_red.sum", "L2 red sectors"), ("lts__t_sectors_op_atom.sum", "L2 atom sectors"),
-    ("sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active", "tensor pipe % (tcgen05 MMAs; sm__pipe_tensor_cycles_active)"),
+    ("sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active", "tensor pipe % (MMAs; sm__pipe_tensor_cycles_active)"),
     ("sm__pipe_tensor_subpipe_hmma_cycles_active.avg.pct_of_peak_sustained_active", "tensor pipe % (hmma)"),
     ("smsp__average_warps_issue_stalled_long_scoreboard_per_issue_active.ratio", "stall long_scoreboard"),
     ("smsp__average_warps_issue_stalled_lg_throttle_per_issue_active.ratio", "stall lg_throttle"),

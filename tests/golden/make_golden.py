@@ -1,5 +1,5 @@
 """Generates tests/golden/ref_python.npz by IMPORTING THE REFERENCE'S OWN PYTHON (pure-PyTorch layer of nr3d_lib)
-in the build container.  /root/reference cannot travel to the GPU box, so the vectors are committed.
+where a checkout of the reference project is found (oracle/build_ref.py: reference_root).  The reference is not part of this repository, so the vectors are committed.
 
     python tests/golden/make_golden.py
 
@@ -24,7 +24,11 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = "/root/reference/nr3d_lib/nr3d_lib"
+from oracle.build_ref import reference_root  # noqa: E402
+
+if reference_root() is None:
+    raise SystemExit("make_golden.py: no reference checkout found (set NR3D_REFERENCE, or place it next to this repository as `reference`)")
+REF = os.path.join(reference_root(), "nr3d_lib", "nr3d_lib")
 
 
 def _pkg(name, path):

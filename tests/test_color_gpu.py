@@ -1,4 +1,4 @@
-"""Fused colour / normal query (csrc/color_tc.cu: three tcgen05 kernels) against the module path it replaces
+"""Fused colour / normal query (csrc/color_tc.cu: three wgmma kernels) against the module path it replaces
 (LoTDNeuS.forward = LoTDFunctionFwdDydx -> autocast decoder -> autograd.grad -> LoTDFunctionBwdDydx -> RadianceNet, which the
 render tests pin against the CPU oracle) and against the CPU oracle directly."""
 import numpy as np

@@ -1,18 +1,24 @@
 """Parity AT THE BENCHMARK'S OWN SIZE (BASELINE.json: "PSNR vs ref"; north_star: rgb / depth / normals within 1e-4 relative L2 on identical rays
 and weights): the 800x600 frame of bench.py rendered by our kernels (host-sized fused path AND the static / graph path) against the render of the
-REFERENCE'S OWN KERNELS (oracle/_ref: `_lotd`, `_pack_ops`, `_occ_grid`, `_shencoder` compiled from /root/reference, driven op by op).  The
-reference arm runs in a child process (it patches module-level back ends).  Also: 4096 random rays (MODE-1 traversal, the training batch)."""
+REFERENCE'S OWN KERNELS (oracle/_ref: `_lotd`, `_pack_ops`, `_occ_grid`, `_shencoder` compiled by oracle/build_ref.py, driven op by op).  The
+reference renders are stored for a fixed sample of pixels in tests/golden/ref_frames.npz; NSB_RECORD_REF=<dir> re-records them where oracle/_ref
+is built (the reference arm runs in a child process: it patches module-level back ends).  Also: 4096 random rays (MODE-1 traversal, the
+training batch)."""
 import json
 import os
 import subprocess
 import sys
 
+import numpy as np
 import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = pytest.mark.gpu
 KEYS = ("rgb_volume", "depth_volume", "normals_volume", "mask_volume")
+RECORD = os.environ.get("NSB_RECORD_REF")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "ref_frames.npz")
+N_PIX = 8192                                  # pixels of a frame kept: a fixed seeded sample
 
 CHILD = r'''
 import sys, torch
@@ -34,13 +40,25 @@ torch.save({k: v.cpu() for k, v in out.items()}, %(path)r)
 '''
 
 
+def _pixels(n):
+    return torch.randperm(n, generator=torch.Generator().manual_seed(3))[:N_PIX].sort().values if n > N_PIX else torch.arange(n)
+
+
 def _reference_render(tmp_path, view, train, random, collect=False):
-    if not os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "_lotd")):
-        pytest.skip("oracle/_ref is not built")
-    path = str(tmp_path / f"ref_{view}_{int(train)}_{int(random)}.pt")
-    code = CHILD % dict(root=ROOT, view=view, train=train, random=random, collect=collect, path=path)
-    subprocess.run([sys.executable, "-c", code], check=True, timeout=600)
-    return torch.load(path)
+    """the reference kernels' render at the pixels _pixels(number of rays)"""
+    tag = f"view{view}_{int(train)}_{int(random)}"
+    if RECORD:
+        path = str(tmp_path / f"ref_{tag}.pt")
+        code = CHILD % dict(root=ROOT, view=view, train=train, random=random, collect=collect, path=path)
+        subprocess.run([sys.executable, "-c", code], check=True, timeout=600)
+        full = torch.load(path)
+        sel = _pixels(full[KEYS[0]].shape[0])
+        rec = dict(np.load(os.path.join(RECORD, "ref_frames.npz"))) if os.path.exists(os.path.join(RECORD, "ref_frames.npz")) else {}
+        rec.update({f"{tag}.{k}": full[k][sel].numpy() for k in KEYS})
+        os.makedirs(RECORD, exist_ok=True)
+        np.savez_compressed(os.path.join(RECORD, "ref_frames.npz"), **rec)
+    gold = np.load(GOLDEN) if not RECORD else np.load(os.path.join(RECORD, "ref_frames.npz"))
+    return {k: torch.from_numpy(gold[f"{tag}.{k}"]) for k in KEYS}
 
 
 def _report(tag, got, ref):
@@ -50,9 +68,6 @@ def _report(tag, got, ref):
         mse = float((x - y).square().mean())
         res[k] = dict(rel_l2=float((x - y).norm() / y.norm().clamp_min(1e-30)), psnr_db=(None if mse == 0 else -10.0 * float(torch.log10(torch.tensor(mse)))))
     print(tag, json.dumps(res))
-    if os.path.isdir(os.path.join(ROOT, "gpurun_out")):
-        with open(os.path.join(ROOT, "gpurun_out", "frame_parity.jsonl"), "a") as f:
-            f.write(json.dumps({"case": tag, **res}) + "\n")
     return res
 
 
@@ -62,12 +77,13 @@ def test_800x600_frame_vs_the_reference_kernels(cuda, tmp_path, view, train):
     from neuralsim_b200.renderer import SingleVolumeRenderer
     from neuralsim_b200.graphics.neus_static import StaticFrame
     ref = _reference_render(tmp_path, view, train, False)
+    sel = _pixels(bench.H * bench.W)
     model = bench.build_model(cuda).train(train)
     o, d = bench.pinhole_rays(bench.H, bench.W, bench.orbit(view, 8))
     o, d, ha = o.to(cuda), d.to(cuda), torch.zeros(bench.H * bench.W, 4, device=cuda)
     with torch.no_grad():
         got = SingleVolumeRenderer(dict(near=0.01)).train(train).render(model, o, d, rays_h_appear=ha)["rendered"]
-        res = _report(f"frame view {view} {'train' if train else 'eval'} (host-sized fused path)", got, ref)
+        res = _report(f"frame view {view} {'train' if train else 'eval'} (host-sized fused path, {N_PIX} pixels)", {k: got[k][sel.to(cuda)] for k in KEYS}, ref)
         for k in ("rgb_volume", "depth_volume", "normals_volume"):
             assert res[k]["rel_l2"] <= 1e-4, (k, res[k])
         assert res["rgb_volume"]["psnr_db"] is None or res["rgb_volume"]["psnr_db"] >= 80.0

@@ -52,7 +52,7 @@ def test_fused_sdf_rays_matches_points(cuda):
 
 
 def test_tensor_core_kernel_matches_cuda_core_kernel(cuda):
-    """csrc/fused_tc.cu (tcgen05 + TMEM) against csrc/fused.cu (CUDA cores): same rounding points, fp32 accumulation order differs."""
+    """csrc/fused_tc.cu (wgmma) against csrc/fused.cu (CUDA cores): same rounding points, fp32 accumulation order differs."""
     from neuralsim_b200 import _lib
     P, model = make_pair(cuda)
     g = torch.Generator().manual_seed(11)
@@ -68,7 +68,7 @@ def test_tensor_core_kernel_matches_cuda_core_kernel(cuda):
 
 
 def test_fused_backward_matches_autograd_chain(cuda):
-    """nsb_fused_sdf_bwd (one tcgen05 kernel) against the unfused chain LoTDFunction + autocast MLP differentiated by torch."""
+    """nsb_fused_sdf_bwd (one wgmma kernel) against the unfused chain LoTDFunction + autocast MLP differentiated by torch."""
     P, model = make_pair(cuda)
     surf = model.implicit_surface
     g = torch.Generator().manual_seed(12)
