@@ -53,8 +53,7 @@ const char *nsb_last_error(void);
 int nsb_version(void);
 /* Number of kernels this library has launched in the calling process (bench.py's `gpu_launches`). */
 uint64_t nsb_launch_count(void);
-/* Self-check / A-B switches: key "sdf_simt" (0|1) routes nsb_fused_sdf* through the CUDA-core cross-check kernel; "color_tma" (0|1|2) the
- * TMA fetch of the saved activation tiles in the colour backward; "asm_chunk" (1|8) rays per search of the hit list in nsb_assemble_boundary. */
+/* Self-check switch: key "sdf_simt" (0|1) routes nsb_fused_sdf* through the CUDA-core cross-check kernel.  Any other key is an error. */
 int nsb_set_option(const char *key, int value);
 
 /* ------------------------------------------------------------------------------------------------

@@ -57,10 +57,6 @@ def lib():
         _lib.nsb_last_error.restype = ctypes.c_char_p
         _lib.nsb_launch_count.restype = ctypes.c_uint64
         _lib.nsb_color_tile_bytes.restype = ctypes.c_int64
-        if os.environ.get("NSB_COLOR_TMA") is not None:       # A/B switch: 0 = plain loads of the saved activation tiles in the radiance backward
-            _lib.nsb_set_option(b"color_tma", ctypes.c_int(int(os.environ["NSB_COLOR_TMA"])))
-        if os.environ.get("NSB_ASM_CHUNK") is not None:       # A/B switch: 1 = every ray of nsb_assemble_boundary searches the hit list
-            _lib.nsb_set_option(b"asm_chunk", ctypes.c_int(int(os.environ["NSB_ASM_CHUNK"])))
     return _lib
 
 

@@ -25,10 +25,9 @@
 namespace nsb {
 
 struct ColorNetDev {
-    const __half *W1, *b1, *W2, *b2;                    // sdf decoder: [width x 32], [width], [width], [1]
+    DecoderDevTC dec;                                   // sdf decoder: [width x 32], [width], [width], [1]
     const __half *R1, *rb1, *R2, *rb2, *R3, *rb3;       // radiance net: [rw x rin], [rw], [rw x rw], [rw], [3 x rw], [3]
-    int width, rw, rin, n_appear;
-    float beta;
+    int rw, rin, n_appear;
     float fac[3];                                       // sdf_scale / radius3d_original per axis
 };
 
@@ -82,44 +81,10 @@ __device__ __forceinline__ void level_jacobian(const PLMeta &m, uint32_t p, cons
     }
 }
 
-__device__ __forceinline__ float r16f(float v) { return __half2float(__float2half_rn(v)); }
-
 __device__ __forceinline__ void unpack8(const uint4 &q, float (&v)[8]) {
     const __half2 *h = reinterpret_cast<const __half2 *>(&q);
 #pragma unroll
     for (int i = 0; i < 4; ++i) { const float2 f = __half22float2(h[i]); v[2 * i] = f.x; v[2 * i + 1] = f.y; }
-}
-
-__device__ __forceinline__ void stage_W1T(const __half *W1, int width, uint8_t *sBT, int tid) {
-    for (int e = tid; e < NF * HW; e += kTile) {              // W1^T: row = feature k, col = hidden j
-        const int k = e % NF, j = e / NF;
-        const __half v = j < width ? W1[j * NF + k] : __float2half_rn(0.f);
-        *reinterpret_cast<__half *>(sBT + (j / 8) * (NF * 16) + k * 16 + (j % 8) * 2) = v;
-    }
-}
-
-struct PointSrc {
-    const float *x, *rays_o, *rays_d, *t;
-    const int64_t *ridx;
-};
-
-__device__ __forceinline__ void load_point_net(const PointSrc &ps, int64_t i, bool valid, float (&xn)[3], float (&xs)[3], int64_t &ray) {
-    xn[0] = xn[1] = xn[2] = 0.f;
-    ray = 0;
-    if (valid) {
-        if (ps.x) {
-#pragma unroll
-            for (int d = 0; d < 3; ++d) xn[d] = ps.x[i * 3 + d];
-            ray = ps.ridx ? ps.ridx[i] : i;
-        } else {
-            ray = ps.ridx ? ps.ridx[i] : i;
-            const float tt = ps.t[i];
-#pragma unroll
-            for (int d = 0; d < 3; ++d) xn[d] = __fmaf_rn(ps.rays_d[ray * 3 + d], tt, ps.rays_o[ray * 3 + d]);
-        }
-    }
-#pragma unroll
-    for (int d = 0; d < 3; ++d) xs[d] = fminf(fmaxf(__fmaf_rn(xn[d], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
 }
 
 // The colour kernels run at 1-2 CTAs per SM (shared-memory bound), i.e. 4-8 warps: their gathers live on loads in flight PER THREAD, and
@@ -147,11 +112,8 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
     __shared__ float sb2, srb3[3];
 
     const int tid = threadIdx.x;
-    {
-        DecoderDevTC dec{net.W1, net.b1, net.W2, net.b2, net.width, net.beta};
-        stage_W1(dec, sW1, tid);
-        stage_W1T(net.W1, net.width, sW1T, tid);
-    }
+    stage_W1(net.dec, sW1, tid);
+    stage_W1T(net.dec, sW1T, tid);
     for (int e = tid; e < XW * XW; e += kTile) {
         const int j = e % XW, k = e / XW;                      // (out j, in k)
         const int rc = ref_col(k, net.n_appear);
@@ -160,23 +122,21 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         *reinterpret_cast<__half *>(sR1 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v1;
         *reinterpret_cast<__half *>(sR2 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v2;
     }
-    if (tid < HW) {
-        sb1[tid] = tid < net.width ? __half2float(net.b1[tid]) : 0.f;
-        sW2[tid] = tid < net.width ? __half2float(net.W2[tid]) : 0.f;
+    stage_decoder_vectors(net.dec, sb1, sW2, &sb2, tid);
+    if (tid < XW) {
         srb1[tid] = tid < net.rw ? __half2float(net.rb1[tid]) : 0.f;
         srb2[tid] = tid < net.rw ? __half2float(net.rb2[tid]) : 0.f;
 #pragma unroll
         for (int k = 0; k < 3; ++k) sR3[k][tid] = tid < net.rw ? __half2float(net.R3[k * net.rw + tid]) : 0.f;
     }
     if (tid == 0) {
-        sb2 = __half2float(net.b2[0]);
         for (int k = 0; k < 3; ++k) srb3[k] = __half2float(net.rb3[k]);
     }
     tc::fence_async_smem();
     __syncthreads();
     const uint32_t x_addr = tc::smem_u32(sX), u_addr = tc::smem_u32(sU), w1_addr = tc::smem_u32(sW1), w1t_addr = tc::smem_u32(sW1T);
     const uint32_t r1_addr = tc::smem_u32(sR1), r2_addr = tc::smem_u32(sR2);
-    const SoftplusK spk(net.beta);
+    const SoftplusK spk(net.dec.beta);
 
     const int64_t n_tiles = (n + kTile - 1) / kTile;
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -184,7 +144,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         const bool valid = i < n;
         float xn[3], xs[3];
         int64_t ray;
-        load_point_net(ps, i, valid, xn, xs, ray);
+        load_point(ps, ps.x == nullptr, i, valid, xn, xs, ray);
         gather_row_to_tile<kTile, kColorGatherU>(m, grid, xs, max_level, sX, tid);          // h -> chunks 0..3 of X
         tc::fence_async_smem();
         __syncthreads();
@@ -199,16 +159,16 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
             tc::acc_ld8(acc, kS, tid, c * 8, z);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                z[j] = r16f(z[j] + sb1[c * 8 + j]);
+                z[j] = r16(z[j] + sb1[c * 8 + j]);
                 float a, s;
                 softplus_as(z[j], spk, a, s);
-                out = fmaf(r16f(a), sW2[c * 8 + j], out);
+                out = fmaf(r16(a), sW2[c * 8 + j], out);
                 uu[j] = sW2[c * 8 + j] * s;
             }
             *reinterpret_cast<uint4 *>(sU + c * kChunk + tid * 16) = tc::pack8_f16(uu);
             if (zt) *reinterpret_cast<uint4 *>(zt + c * kChunk + tid * 16) = tc::pack8_f16(z);
         }
-        const float sdf = r16f(out + sb2);
+        const float sdf = r16(out + sb2);
         tc::fence_async_smem();
         __syncthreads();
         tc::mma_to_rows<32, 0, 0, HW / 16>(acc, kS, 0, tc::kmajor(u_addr, kTile), tc::kmajor(w1t_addr, NF), false);   // g = U . W1
@@ -225,7 +185,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
                 if ((int)m.level[p] <= max_level) {
                     float J0[3], J1[3];
                     level_jacobian(m, p, xs, grid, J0, J1);
-                    const float g0 = r16f(gg[2 * q]), g1 = r16f(gg[2 * q + 1]);
+                    const float g0 = r16(gg[2 * q]), g1 = r16(gg[2 * q + 1]);
 #pragma unroll
                     for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g0, J0[d], nacc[d]);
 #pragma unroll
@@ -276,7 +236,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
             float y[8];
             tc::acc_ld8(acc, kS, tid, c * 8, y);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) y[j] = fmaxf(r16f(y[j] + srb1[c * 8 + j]), 0.f);
+            for (int j = 0; j < 8; ++j) y[j] = fmaxf(r16(y[j] + srb1[c * 8 + j]), 0.f);
             const uint4 q = tc::pack8_f16(y);
             *reinterpret_cast<uint4 *>(sU + c * kChunk + tid * 16) = q;
             if (y1t) *reinterpret_cast<uint4 *>(y1t + c * kChunk + tid * 16) = q;
@@ -293,7 +253,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
             tc::acc_ld8(acc, kS, tid, c * 8, y);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                y[j] = fmaxf(r16f(y[j] + srb2[c * 8 + j]), 0.f);
+                y[j] = fmaxf(r16(y[j] + srb2[c * 8 + j]), 0.f);
 #pragma unroll
                 for (int k = 0; k < 3; ++k) o3[k] = fmaf(y[j], sR3[k][c * 8 + j], o3[k]);
             }
@@ -305,8 +265,8 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 #pragma unroll
             for (int d = 0; d < 3; ++d) {
                 nab_out[i * 3 + d] = nab[d];
-                const float y3 = r16f(o3[d] + srb3[d]);
-                rgb_out[i * 3 + d] = r16f(1.f / (1.f + expf(-y3)));
+                const float y3 = r16(o3[d] + srb3[d]);
+                rgb_out[i * 3 + d] = r16(1.f / (1.f + expf(-y3)));
                 if (x_out) x_out[i * 3 + d] = xn[d];
             }
         }
@@ -320,10 +280,9 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 //   dh  = dZ1 . R1[:, h columns]   (M128 N32 K64)    A = T block 1,                     B = R1h^T tile
 //   XA += [dZ2 | dZ1]^T . [Y1 | 1]           (M128 N72 K128, MN-major): rows 0..63  = [dR2 | drb2]
 //   XB += [dZ1 | y2 ]^T . [X | 1 gy3 0..]    (M128 N72 K128, MN-major): rows 0..63  = [dR1 | drb1], rows 64..127, cols 65..67 = dR3^T
-// TMA = true: the three saved activation tiles of a point tile (X, Y1, Y2: 3 x 16 KB, each contiguous in global memory and in shared
-// memory) are fetched by the bulk async copy engine (cp.async.bulk -> mbarrier), issued by one thread; the fetch of the NEXT tile starts as soon
+// The three saved activation tiles of a point tile (X, Y1, Y2: 3 x 16 KB, each contiguous in global memory and in shared memory) are
+// fetched by the bulk async copy engine (cp.async.bulk -> mbarrier), issued by one thread; the fetch of the NEXT tile starts as soon
 // as the last MMA that reads the current tiles has completed, so it overlaps the epilogue, the dh store and the next prologue.
-template <bool TMA>
 __global__ void __launch_bounds__(kTile)
 k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uint8_t *__restrict__ Y1t, const uint8_t *__restrict__ Y2t,
                 const float *__restrict__ rgb, const float *__restrict__ g_rgb, int64_t n, float *__restrict__ dh_out,
@@ -383,28 +342,18 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         tc::tma_load_bulk(sY1, Y1t + tile * kTileBytes, kTileBytes, &mbar_ld);
         tc::tma_load_bulk(sXe, Xt + tile * kTileBytes, kTileBytes, &mbar_ld);
     };
-    if (TMA && tid == 0 && (int64_t)blockIdx.x < n_tiles) fetch(blockIdx.x);
+    if (tid == 0 && (int64_t)blockIdx.x < n_tiles) fetch(blockIdx.x);
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int64_t i = tile * kTile + tid;
         const bool valid = i < n;
-        if (TMA) {
-            tc::mbar_wait(&mbar_ld, ld_phase);                // the tiles of this iteration have landed
-            ld_phase ^= 1;
-        } else {
-            const uint8_t *xt = Xt + tile * kTileBytes, *y1t = Y1t + tile * kTileBytes, *y2t = Y2t + tile * kTileBytes;
-#pragma unroll 1
-            for (int c = 0; c < 8; ++c) {
-                *reinterpret_cast<uint4 *>(sT + 2 * kTileBytes + c * kChunk + tid * 16) = *reinterpret_cast<const uint4 *>(y2t + c * kChunk + tid * 16);
-                *reinterpret_cast<uint4 *>(sY1 + c * kChunk + tid * 16) = *reinterpret_cast<const uint4 *>(y1t + c * kChunk + tid * 16);
-                *reinterpret_cast<uint4 *>(sXe + c * kChunk + tid * 16) = *reinterpret_cast<const uint4 *>(xt + c * kChunk + tid * 16);
-            }
-        }
+        tc::mbar_wait(&mbar_ld, ld_phase);                    // the tiles of this iteration have landed
+        ld_phase ^= 1;
         float gy[3] = {0.f, 0.f, 0.f};
         if (valid && g_rgb) {
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
                 const float y = rgb[i * 3 + k];
-                gy[k] = r16f(r16f(g_rgb[i * 3 + k]) * ((1.f - y) * y));          // sigmoid backward on the fp16 output
+                gy[k] = r16(r16(g_rgb[i * 3 + k]) * ((1.f - y) * y));          // sigmoid backward on the fp16 output
             }
         }
         {
@@ -448,7 +397,7 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         tc::mma_to_rows<NE, 1, 1, kTile / 16>(acc, kS, cXB, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(xe_addr, kTile), true);
         first_tile = false;
         __syncthreads();
-        if (TMA && tid == 0 && tile + gridDim.x < n_tiles) {
+        if (tid == 0 && tile + gridDim.x < n_tiles) {
             // every reader of the three tiles is done: the threads' own reads precede the __syncthreads before the MMAs above, and those MMAs
             // (the last readers) have completed before the barrier above -> the next tile's activations may overwrite them while this tile is finished
             tc::fence_async_smem();
@@ -502,10 +451,9 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
 //   X1 += [dz | u]^T . [H | 1]   rows 0..63 = [dW1 (z part) | db1]
 //   X2 += [u | v]^T . [dG | 1]   rows 0..63, cols 0..31 = dW1 (second-order part);  rows 64..127, col 32 = dW2
 //   scatter per level / corner:  g_f * wsum_c(gin) + (dhz_f + dh_r_f) * w_c
-// TMA = true: the saved Z tile (16 KB) and the H half of the saved X tile (8 KB) are fetched by the bulk async copy engine into shared memory, and
-// the NEXT tile's fetch is issued right after the last MMA of the current tile -- it runs behind the whole scatter phase.  (Without it the two
-// epilogue loops read Z straight from global memory, 16 dependent round trips per tile at 8 warps per SM.)
-template <bool TMA>
+// The saved Z tile (16 KB) and the H half of the saved X tile (8 KB) are fetched by the bulk async copy engine into shared memory, and
+// the NEXT tile's fetch is issued right after the last MMA of the current tile -- it runs behind the whole scatter phase.  (Reading Z
+// straight from global memory in the two epilogue loops costs 16 dependent round trips per tile at 8 warps per SM.)
 __global__ void __launch_bounds__(kTile)
 k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev net, const PointSrc ps, const uint8_t *__restrict__ Zt,
                 const uint8_t *__restrict__ Xt, const float *__restrict__ g_nab, const float *__restrict__ g_sdf, const float *__restrict__ dh_r,
@@ -520,7 +468,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
     uint8_t *sGe = sHe + kTile * NX * 2;                       // 12 KB [dG | 1 | 0]
     uint8_t *sW1 = sGe + kTile * NX * 2;                       //  4 KB
     uint8_t *sW1T = sW1 + HW * NF * 2;                         //  4 KB
-    uint8_t *sZ = sW1T + NF * HW * 2;                          // 16 KB saved pre-activations (TMA only)
+    uint8_t *sZ = sW1T + NF * HW * 2;                          // 16 KB saved pre-activations
     constexpr uint32_t cDU = 0, cDHZ = 0, cG = 64, cX1 = 96, cX2 = 96 + NX;   // staged accumulator columns (du, then dhz; X1, X2 persist)
     constexpr int kS = tc::acc_stride(96 + 2 * NX);
     float *acc = reinterpret_cast<float *>(sZ + kTileBytes);   // 98 KB
@@ -529,12 +477,9 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
     __shared__ __align__(8) uint64_t mbar_ld;
 
     const int tid = threadIdx.x, lane = tid & 31;
-    {
-        DecoderDevTC dec{net.W1, net.b1, net.W2, net.b2, net.width, net.beta};
-        stage_W1(dec, sW1, tid);
-        stage_W1T(net.W1, net.width, sW1T, tid);
-    }
-    if (tid < HW) sW2[tid] = tid < net.width ? __half2float(net.W2[tid]) : 0.f;
+    stage_W1(net.dec, sW1, tid);
+    stage_W1T(net.dec, sW1T, tid);
+    stage_decoder_vectors(net.dec, nullptr, sW2, nullptr, tid);
     *reinterpret_cast<uint4 *>(sHe + 4 * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);
     *reinterpret_cast<uint4 *>(sGe + 4 * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);
     *reinterpret_cast<uint4 *>(sHe + 5 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
@@ -549,7 +494,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
     __syncthreads();
     const uint32_t t_addr = tc::smem_u32(sT), he_addr = tc::smem_u32(sHe), ge_addr = tc::smem_u32(sGe), w1_addr = tc::smem_u32(sW1),
                    w1t_addr = tc::smem_u32(sW1T);
-    const SoftplusK spk(net.beta);
+    const SoftplusK spk(net.dec.beta);
     uint32_t ld_phase = 0;
     bool first_tile = true;
 
@@ -559,34 +504,26 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         tc::tma_load_bulk(sZ, Zt + tile * kTileBytes, kTileBytes, &mbar_ld);
         tc::tma_load_bulk(sHe, Xt + tile * kTileBytes, 4 * kChunk, &mbar_ld);
     };
-    if (TMA && tid == 0 && (int64_t)blockIdx.x < n_tiles) fetch(blockIdx.x);
+    if (tid == 0 && (int64_t)blockIdx.x < n_tiles) fetch(blockIdx.x);
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int64_t i = tile * kTile + tid;
         const bool valid = i < n;
         float xn[3], xs[3];
         int64_t ray;
-        load_point_net(ps, i, valid, xn, xs, ray);
+        load_point(ps, ps.x == nullptr, i, valid, xn, xs, ray);
         float gin[3] = {0.f, 0.f, 0.f};
         if (valid && g_nab) {
 #pragma unroll
             for (int d = 0; d < 3; ++d) gin[d] = g_nab[i * 3 + d] * net.fac[d] * 0.5f;
         }
         const float dsdf = (valid && g_sdf) ? g_sdf[i] : 0.f;
-        const uint8_t *zt = TMA ? sZ : Zt + tile * kTileBytes;
-        if (TMA) {
-            tc::mbar_wait(&mbar_ld, ld_phase);                // this tile's Z and H have landed
-            ld_phase ^= 1;
-        } else {
-            const uint8_t *xt = Xt + tile * kTileBytes;
-#pragma unroll
-            for (int c = 0; c < 4; ++c)
-                *reinterpret_cast<uint4 *>(sHe + c * kChunk + tid * 16) = *reinterpret_cast<const uint4 *>(xt + c * kChunk + tid * 16);
-        }
+        tc::mbar_wait(&mbar_ld, ld_phase);                    // this tile's Z and H have landed
+        ld_phase ^= 1;
         // u = fp16(w2 s)
 #pragma unroll 1
         for (int c = 0; c < 8; ++c) {
             float z[8], uu[8];
-            unpack8(*reinterpret_cast<const uint4 *>(zt + c * kChunk + tid * 16), z);
+            unpack8(*reinterpret_cast<const uint4 *>(sZ + c * kChunk + tid * 16), z);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 float a, s;
@@ -619,15 +556,15 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         for (int c = 0; c < 8; ++c) {
             float du[8], z[8], dz[8], vv[8];
             tc::acc_ld8(acc, kS, tid, cDU + c * 8, du);
-            unpack8(*reinterpret_cast<const uint4 *>(zt + c * kChunk + tid * 16), z);
+            unpack8(*reinterpret_cast<const uint4 *>(sZ + c * kChunk + tid * 16), z);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 float a, s;
                 softplus_as(z[j], spk, a, s);
-                const float w2 = sW2[c * 8 + j], d = r16f(du[j]);
+                const float w2 = sW2[c * 8 + j], d = r16(du[j]);
                 const float curv = (z[j] * spk.k > spk.thr) ? 0.f : spk.beta * s * (1.f - s);
                 dz[j] = d * w2 * curv + dsdf * w2 * s;
-                vv[j] = d * s + dsdf * r16f(a);
+                vv[j] = d * s + dsdf * r16(a);
             }
             *reinterpret_cast<uint4 *>(sT + c * kChunk + tid * 16) = tc::pack8_f16(dz);
             *reinterpret_cast<uint4 *>(sT + 2 * kTileBytes + c * kChunk + tid * 16) = tc::pack8_f16(vv);
@@ -641,7 +578,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         const float dsum = warp_sum(dsdf);
         if (lane == 0 && dsum != 0.f) atomicAdd(&sdb2, dsum);
         __syncthreads();
-        if (TMA && tid == 0 && tile + gridDim.x < n_tiles) {
+        if (tid == 0 && tile + gridDim.x < n_tiles) {
             // sZ was last read by the threads before the __syncthreads that precedes the MMAs above, sHe by those MMAs, which have completed
             tc::fence_async_smem();
             fetch(tile + gridDim.x);
@@ -663,7 +600,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
                 uint32_t cell[8];
                 float w[8], fr[3], sc[3], ua[8], ub[8];
                 level_cells3(m, p, xs, cell, w, fr, sc);
-                const float g0 = valid ? r16f(gg[2 * q]) : 0.f, g1 = valid ? r16f(gg[2 * q + 1]) : 0.f;
+                const float g0 = valid ? r16(gg[2 * q]) : 0.f, g1 = valid ? r16(gg[2 * q + 1]) : 0.f;
                 const float h0 = valid ? hz[2 * q] : 0.f, h1 = valid ? hz[2 * q + 1] : 0.f;
 #pragma unroll
                 for (int c = 0; c < 8; ++c) {
@@ -698,7 +635,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
             float a[8], b[8];
             tc::acc_ld8(acc, kS, tid, cX1 + c * 8, a);
             tc::acc_ld8(acc, kS, tid, cX2 + c * 8, b);
-            if (tid < net.width) {
+            if (tid < net.dec.width) {
 #pragma unroll
                 for (int k = 0; k < 8; ++k) atomicAdd(d_W1 + tid * NF + c * 8 + k, a[k] + b[k]);
             }
@@ -706,8 +643,8 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         float a1[8], b1[8];
         tc::acc_ld8(acc, kS, tid, cX1 + 32, a1);
         tc::acc_ld8(acc, kS, tid, cX2 + 32, b1);
-        if (tid < HW) { if (tid < net.width) atomicAdd(d_b1 + tid, a1[0]); }
-        else if (tid - HW < net.width) atomicAdd(d_W2 + (tid - HW), b1[0]);
+        if (tid < HW) { if (tid < net.dec.width) atomicAdd(d_b1 + tid, a1[0]); }
+        else if (tid - HW < net.dec.width) atomicAdd(d_W2 + (tid - HW), b1[0]);
         if (tid == 0) atomicAdd(d_b2, sdb2);
     }
 }
@@ -718,25 +655,22 @@ using namespace nsb;
 
 namespace {
 int make_net(const nsb_color_net *c, const nsb_lotd_meta *meta, PLMeta *m, ColorNetDev *d, const char *who) {
-    if (make_plmeta(meta, m)) return 2;
-    NSB_REQUIRE(m->n_pseudo == 16 && m->F == 2 && m->D == 3 && plmeta_two_feature_cells(*m), "%s: built for 16 x 2 LoTD features in 3-D", who);
-    NSB_REQUIRE(c->width >= 1 && c->width <= 64 && c->rad_width >= 1 && c->rad_width <= 64, "%s: hidden widths must be <= 64", who);
+    const nsb_sdf_decoder dec{c->W1, c->b1, c->W2, c->b2, c->width, c->beta};
+    if (int rc = make_decoder(meta, &dec, m, &d->dec, who)) return rc;
+    NSB_REQUIRE(c->rad_width >= 1 && c->rad_width <= 64, "%s: radiance width must be <= 64", who);
     NSB_REQUIRE(c->n_appear >= 0 && c->n_appear <= 8 && c->rad_in == 54 + c->n_appear,
                 "%s: radiance input must be [x(3), SH deg 4 (16), n(3), h(32), h_appear(<=8)]", who);
-    *d = ColorNetDev{(const __half *)c->W1, (const __half *)c->b1, (const __half *)c->W2, (const __half *)c->b2, (const __half *)c->R1,
-                     (const __half *)c->rb1, (const __half *)c->R2, (const __half *)c->rb2, (const __half *)c->R3, (const __half *)c->rb3,
-                     c->width, c->rad_width, c->rad_in, c->n_appear, c->beta, {c->nablas_scale[0], c->nablas_scale[1], c->nablas_scale[2]}};
+    d->R1 = (const __half *)c->R1; d->rb1 = (const __half *)c->rb1; d->R2 = (const __half *)c->R2; d->rb2 = (const __half *)c->rb2;
+    d->R3 = (const __half *)c->R3; d->rb3 = (const __half *)c->rb3;
+    d->rw = c->rad_width; d->rin = c->rad_in; d->n_appear = c->n_appear;
+    for (int k = 0; k < 3; ++k) d->fac[k] = c->nablas_scale[k];
     return 0;
-}
-inline unsigned tiles_grid(int64_t n, int ctas_per_sm) {
-    const int64_t n_tiles = (n + kTile - 1) / kTile, wave = (int64_t)sm_count() * ctas_per_sm;
-    return (unsigned)(n_tiles < wave ? n_tiles : wave);
 }
 }  // namespace
 
-namespace nsb { extern std::atomic<int> g_opt_color_tma; }
+static int64_t n_tiles(int64_t n) { return (n + kTile - 1) / kTile; }
 
-extern "C" int64_t nsb_color_tile_bytes(int64_t n) { return ((n + kTile - 1) / kTile) * (int64_t)kTileBytes; }
+extern "C" int64_t nsb_color_tile_bytes(int64_t n) { return n_tiles(n) * (int64_t)kTileBytes; }
 
 extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x, const float *rays_o,
                                    const float *rays_d, const int64_t *ridx, const float *t, const float *view_dirs, const float *h_appear,
@@ -753,12 +687,11 @@ extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params
     NSB_REQUIRE(d.n_appear == 0 || h_appear, "nsb_fused_color_fwd: h_appear is NULL but the net has %d appearance channels", d.n_appear);
     constexpr int kSmem = 2 * kTileBytes + 2 * HW * NF * 2 + 2 * XW * XW * 2 + kTile * tc::acc_stride(64) * 4 + 1024;
     opt_in_smem(k_color_fwd, kSmem);
-    PointSrc ps{x, rays_o, rays_d, t, ridx};
-    OccCollect oc{nullptr, 1, 1, 1, 0.f};
-    if (collect && collect->grid_pcl) oc = OccCollect{collect->grid_pcl, collect->res[0], collect->res[1], collect->res[2], collect->inv_s};
-    k_color_fwd<<<tiles_grid(n, 2), kTile, kSmem, (cudaStream_t)stream>>>(m, (const __half *)params_half, d, ps, view_dirs, h_appear, n,
-                                                                          max_level < 0 ? -1 : max_level, sdf, nablas, rgb, x_out, (uint8_t *)act_z,
-                                                                          (uint8_t *)act_x, (uint8_t *)act_y1, (uint8_t *)act_y2, oc, dn.a);
+    const PointSrc ps{x, rays_o, rays_d, t, ridx};
+    k_color_fwd<<<persistent_grid(n_tiles(n), 2), kTile, kSmem, (cudaStream_t)stream>>>(m, (const __half *)params_half, d, ps, view_dirs, h_appear, n,
+                                                                                        max_level < 0 ? -1 : max_level, sdf, nablas, rgb, x_out, (uint8_t *)act_z,
+                                                                                        (uint8_t *)act_x, (uint8_t *)act_y1, (uint8_t *)act_y2,
+                                                                                        occ_collect_of(collect), dn.a);
     return check_launch("nsb_fused_color_fwd");
 }
 
@@ -780,26 +713,16 @@ extern "C" int nsb_fused_color_bwd(const nsb_lotd_meta *meta, const void *params
     const float *dh = nullptr;
     if (g_rgb) {
         constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + kTile * tc::acc_stride(64 + 2 * 80) * 4 + 1024;   // 1 CTA / SM
-        opt_in_smem(k_color_rad_bwd<true>, kSmemR);
-        opt_in_smem(k_color_rad_bwd<false>, kSmemR);
-        if (g_opt_color_tma.load())
-            k_color_rad_bwd<true><<<tiles_grid(n, 1), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n,
-                                                                          dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, dn.a);
-        else
-            k_color_rad_bwd<false><<<tiles_grid(n, 1), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n,
-                                                                           dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, dn.a);
+        opt_in_smem(k_color_rad_bwd, kSmemR);
+        k_color_rad_bwd<<<persistent_grid(n_tiles(n), 1), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb,
+                                                                              g_rgb, n, dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, dn.a);
         if (int rc = check_launch("nsb_fused_color_bwd(radiance)")) return rc;
         dh = dh_scratch;
     }
     constexpr int kSmemS = 3 * kTileBytes + 2 * kTile * 48 * 2 + 2 * HW * NF * 2 + kTileBytes + kTile * tc::acc_stride(96 + 2 * 48) * 4 + 1024;   // 1 CTA / SM
-    opt_in_smem(k_color_sdf_bwd<true>, kSmemS);
-    opt_in_smem(k_color_sdf_bwd<false>, kSmemS);
-    PointSrc ps{x, rays_o, rays_d, t, ridx};
-    if (g_opt_color_tma.load() >= 2)
-        k_color_sdf_bwd<true><<<tiles_grid(n, 1), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
-                                                                      g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level, d_grid, d_W1, d_b1, d_W2, d_b2, dn.a);
-    else
-        k_color_sdf_bwd<false><<<tiles_grid(n, 1), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
-                                                                       g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level, d_grid, d_W1, d_b1, d_W2, d_b2, dn.a);
+    opt_in_smem(k_color_sdf_bwd, kSmemS);
+    const PointSrc ps{x, rays_o, rays_d, t, ridx};
+    k_color_sdf_bwd<<<persistent_grid(n_tiles(n), 1), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
+                                                                          g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level, d_grid, d_W1, d_b1, d_W2, d_b2, dn.a);
     return check_launch("nsb_fused_color_bwd(sdf)");
 }

@@ -19,7 +19,7 @@ void set_error(const char *fmt, ...) {
 }
 }  // namespace nsb
 
-namespace nsb { std::atomic<int> g_opt_sdf_simt{0}; std::atomic<int> g_opt_color_tma{2}; std::atomic<int> g_opt_asm_chunk{8}; }
+namespace nsb { std::atomic<int> g_opt_sdf_simt{0}; }
 
 namespace nsb {
 static thread_local DevCounts g_counts{nullptr, nullptr};
@@ -48,12 +48,10 @@ extern "C" int nsb_bind_device_counts(const int64_t *count0, const int64_t *coun
     return 0;
 }
 
-// Tunables / self-check switches.  "sdf_simt" = 1 routes nsb_fused_sdf* through the CUDA-core reference kernel of
-// csrc/fused.cu instead of the wgmma kernel (used by the tests to cross-check the two).
+// Self-check switch.  "sdf_simt" = 1 routes nsb_fused_sdf* through the CUDA-core reference kernel of csrc/fused.cu instead of
+// the wgmma kernel (used by the tests to cross-check the two).
 extern "C" int nsb_set_option(const char *key, int value) {
     if (key && !strcmp(key, "sdf_simt")) { nsb::g_opt_sdf_simt.store(value); return 0; }
-    if (key && !strcmp(key, "color_tma")) { nsb::g_opt_color_tma.store(value); return 0; }       // 0: plain 16-byte loads of the saved activation tiles (A/B)
-    if (key && !strcmp(key, "asm_chunk")) { nsb::g_opt_asm_chunk.store(value); return 0; }       // 1: every ray of nsb_assemble_boundary searches the hit list (A/B)
     nsb::set_error("nsb_set_option: unknown key '%s'", key ? key : "(null)");
     return 2;
 }

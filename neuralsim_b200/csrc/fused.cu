@@ -108,9 +108,8 @@ k_fused_sdf(const PLMeta m, const __half *__restrict__ grid, const DecoderDev de
 #pragma unroll
             for (int d = 0; d < D; ++d) xs[d] = x[i * D + d];
         }
-        // network space [-1,1] -> table space [0,1] (lotd_encoding.py:165), clamp (lotd.py:60)
 #pragma unroll
-        for (int d = 0; d < D; ++d) xs[d] = fminf(fmaxf(__fmaf_rn(xs[d], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
+        for (int d = 0; d < D; ++d) xs[d] = to_table_space(xs[d]);
         float h[NF];
         gather_row<D, F>(m, grid, xs, max_level, h);
         if (h_out) {

@@ -8,8 +8,6 @@
 //            dot product per row (16 hidden units per lane, summed over the lane quad) -> sdf[r]
 // The loop over levels is rolled on purpose (instruction cache: a fully unrolled gather is several thousand instructions).
 // W1 is staged once per persistent CTA.  Numerics: the fp16 rounding points of the reference's autocast graph (DESIGN.md).
-#include <stdlib.h>
-
 #include "fused_tc_common.cuh"
 
 namespace nsb {
@@ -19,7 +17,7 @@ namespace nsb {
 //         warp = sample ordinal.  For coherent rays (an image) the 32 lanes of a gather instruction then sit in neighbouring
 //         cells -> few 128 B lines per request; the L1 tag stage is what bounds this kernel.  sdf is written to the packed slot, so
 //         nothing downstream changes.  Incoherent rays (random training pixels) keep MODE 1: locality along the ray.
-template <int MODE, bool FAST_SP = false, int UNROLL = 2, bool PAIRED = false>
+template <int MODE>
 __global__ void __launch_bounds__(kTile)
 k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ x,
                const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
@@ -33,11 +31,7 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     stage_W1(dec, sB, tid);
-    if (tid < HW) {
-        sb1[tid] = tid < dec.width ? __half2float(dec.b1[tid]) : 0.f;
-        sW2[tid] = tid < dec.width ? __half2float(dec.W2[tid]) : 0.f;
-    }
-    if (tid == 0) sb2 = __half2float(dec.b2[0]);
+    stage_decoder_vectors(dec, sb1, sW2, &sb2, tid);
     tc::fence_async_smem();
     __syncthreads();
     const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
@@ -66,8 +60,8 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
                     for (int q = 0; q < 3; ++q) xs[q] = __fmaf_rn(d[q], tt, o[q]);
                 }
 #pragma unroll
-                for (int q = 0; q < 3; ++q) xs[q] = fminf(fmaxf(__fmaf_rn(xs[q], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
-                const float v = sdf_of_tile<FAST_SP, UNROLL, PAIRED>(ctx, xs, tid);
+                for (int q = 0; q < 3; ++q) xs[q] = to_table_space(xs[q]);
+                const float v = sdf_of_tile(ctx, xs, tid);
                 if (valid) {
                     sdf[first + k] = v;
                     if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -80,8 +74,8 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
             const int64_t i = tile * kTile + tid;
             const bool valid = i < n;
             float xs[3];
-            load_point(MODE == 1, x, rays_o, rays_d, ridx, t, i, valid, xs);
-            const float v = sdf_of_tile<FAST_SP, UNROLL, PAIRED>(ctx, xs, tid);
+            load_point(PointSrc{x, rays_o, rays_d, t, ridx}, MODE == 1, i, valid, xs);
+            const float v = sdf_of_tile(ctx, xs, tid);
             if (valid) {
                 sdf[i] = v;
                 if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -124,15 +118,8 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
 
     const int tid = threadIdx.x, lane = tid & 31;
     stage_W1(dec, sB, tid);
-    for (int e = tid; e < NF * HW; e += kTile) {              // W1^T: row = feature k, col = hidden j
-        const int k = e % NF, j = e / NF;
-        const __half v = j < dec.width ? dec.W1[j * NF + k] : __float2half_rn(0.f);
-        *reinterpret_cast<__half *>(sBT + (j / 8) * (NF * 16) + k * 16 + (j % 8) * 2) = v;
-    }
-    if (tid < HW) {
-        sb1[tid] = tid < dec.width ? __half2float(dec.b1[tid]) : 0.f;
-        sW2[tid] = tid < dec.width ? __half2float(dec.W2[tid]) : 0.f;
-    }
+    stage_W1T(dec, sBT, tid);
+    stage_decoder_vectors(dec, sb1, sW2, nullptr, tid);
     *reinterpret_cast<uint4 *>(sA + 4 * (kTile * 16) + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);   // constant chunk: [1,0,..]
     for (int c = HW; c < kCols; ++c) acc[tid * kS + c] = 0.f;
     if (tid == 0) sdb2 = 0.f;
@@ -148,7 +135,7 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         const bool valid = i_ < n;
         const int64_t i = (valid && keep) ? keep[i_] : i_;        // optional index list: the samples with a non-zero cotangent
         float xs[3];
-        load_point(FROM_RAYS, x, rays_o, rays_d, ridx, t, i, valid, xs);
+        load_point(PointSrc{x, rays_o, rays_d, t, ridx}, FROM_RAYS, i, valid, xs);
         const float dd = valid ? d_sdf[i] : 0.f;
         gather_row_to_tile<kTile>(m, grid, xs, max_level, sA, tid);
         tc::fence_async_smem();
@@ -162,10 +149,10 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
             tc::acc_ld8(acc, kS, tid, c * 8, z);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const float zz = __half2float(__float2half_rn(z[j] + sb1[c * 8 + j]));
+                const float zz = r16(z[j] + sb1[c * 8 + j]);
                 float a, s;
                 softplus_as(zz, spk, a, s);
-                da[j] = dd * __half2float(__float2half_rn(a));
+                da[j] = dd * r16(a);
                 dz[j] = dd * sW2[c * 8 + j] * s;
             }
             *reinterpret_cast<uint4 *>(sG + c * (kTile * 16) + tid * 16) = tc::pack8_f16(dz);
@@ -233,29 +220,8 @@ using namespace nsb;
 
 // CTAs of k_fused_sdf_tc per SM in the persistent grid.  5 would fit (90-101 registers, ~13 KB of shared memory), but the gather
 // is L1-bound and more warps gathering at once evict each other's lines: on an H100 (NVIDIA H100 80GB HBM3, 700 W) the boundary
-// query of an 800x600 frame took 5.8 ms per launch at 4 CTAs / SM, 7.3-7.4 ms at 5 and 6.5 ms at 6 (bench.py, NSB_SDF_CTAS, alternated).
+// query of an 800x600 frame took 5.8 ms per launch at 4 CTAs / SM, 7.3-7.4 ms at 5 and 6.5 ms at 6 (bench.py, alternated).
 constexpr int kSdfCtasPerSM = 4;
-
-static inline unsigned persistent_grid(int64_t n, int ctas_per_sm) {
-    const int64_t n_tiles = (n + kTile - 1) / kTile;
-    const int64_t wave = (int64_t)sm_count() * ctas_per_sm;
-    return (unsigned)(n_tiles < wave ? n_tiles : wave);
-}
-
-template <int MODE>
-static void launch_sdf(int variant, unsigned grid, cudaStream_t s, const PLMeta &m, const __half *g, const DecoderDevTC &d, const float *x, const float *ro,
-                       const float *rd, const int64_t *ridx, const float *t, int64_t n, int ml, float *sdf, const int64_t *pi, const int64_t *pr, int64_t np,
-                       const OccCollect &oc, const int64_t *nd) {
-    // default (variant 1): SFU softplus, two levels per gather trip (one level per trip thrashes L1 in ray-major order).
-    // variants: 0 libm / 2 levels per trip, 1 SFU / 2, 2 libm / 1, 3 SFU / 1, 4 SFU / 2 + paired corner loads (experiment, lotd_device.cuh)
-    if (variant < 0) variant = 1;                      // SFU softplus, two levels per trip
-    if (variant == 1) k_fused_sdf_tc<MODE, true, 2><<<grid, kTile, 0, s>>>(m, g, d, x, ro, rd, ridx, t, n, ml, sdf, pi, pr, np, oc, nd);
-    else if (variant == 2) k_fused_sdf_tc<MODE, false, 1><<<grid, kTile, 0, s>>>(m, g, d, x, ro, rd, ridx, t, n, ml, sdf, pi, pr, np, oc, nd);
-    else if (variant == 3) k_fused_sdf_tc<MODE, true, 1><<<grid, kTile, 0, s>>>(m, g, d, x, ro, rd, ridx, t, n, ml, sdf, pi, pr, np, oc, nd);
-    else if (variant == 5) k_fused_sdf_tc<MODE, true, 4><<<grid, kTile, 0, s>>>(m, g, d, x, ro, rd, ridx, t, n, ml, sdf, pi, pr, np, oc, nd);   // experiment: four levels (32 loads) per trip
-    else if (variant == 4 && plmeta_pairable(m, g)) k_fused_sdf_tc<MODE, true, 2, true><<<grid, kTile, 0, s>>>(m, g, d, x, ro, rd, ridx, t, n, ml, sdf, pi, pr, np, oc, nd);   // experiment: paired corner loads
-    else k_fused_sdf_tc<MODE, false, 2><<<grid, kTile, 0, s>>>(m, g, d, x, ro, rd, ridx, t, n, ml, sdf, pi, pr, np, oc, nd);
-}
 
 // mode 0: x[n,3];  1: (rays_o, rays_d, ridx, t)[n];  2: ray-tiled packs (pack_infos[n_packs,2], pack_ray[n_packs] or NULL, t, sdf packed)
 extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *x,
@@ -264,26 +230,20 @@ extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *pa
                                        const int64_t *pack_ray, int64_t n_packs, const nsb_occ_collect *collect) {
     const DevCounts dn = take_counts();
     PLMeta m;
-    if (make_plmeta(meta, &m)) return 2;
-    NSB_REQUIRE(m.n_pseudo == 16 && m.F == 2 && m.D == 3 && plmeta_two_feature_cells(m), "nsb_fused_sdf (tensor-core): built for 16 x 2 LoTD features in 3-D");
-    NSB_REQUIRE(dec->width >= 1 && dec->width <= 64, "nsb_fused_sdf (tensor-core): decoder width must be <= 64");
-    DecoderDevTC d{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2, dec->width,
-                   dec->beta};
-    // NSB_SDF_VARIANT / NSB_SDF_CTAS: profiling switches (profiles/ab_gather.py); see launch_sdf
-    // read per call on purpose: profiles/ab_gather.py flips them between launches (two getenv of short names, ~50 ns)
-    const char *ev = getenv("NSB_SDF_VARIANT"), *ec = getenv("NSB_SDF_CTAS");
-    const int variant = ev ? atoi(ev) : -1;
-    const int ctas = ec ? atoi(ec) : kSdfCtasPerSM;
+    DecoderDevTC d;
+    if (int rc = make_decoder(meta, dec, &m, &d, "nsb_fused_sdf (tensor-core)")) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     const int ml = max_level < 0 ? -1 : max_level;
     const __half *g = (const __half *)params_half;
-    OccCollect oc{nullptr, 1, 1, 1, 0.f};
-    if (collect && collect->grid_pcl) oc = OccCollect{collect->grid_pcl, collect->res[0], collect->res[1], collect->res[2], collect->inv_s};
-    if (mode == 2) {
-        const int64_t groups = (n_packs + 31) / 32, wave = (int64_t)sm_count() * ctas;
-        launch_sdf<2>(variant, (unsigned)(groups < wave ? groups : wave), s, m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf, pack_infos, pack_ray, n_packs, oc, dn.a);
-    } else if (mode == 1) launch_sdf<1>(variant, persistent_grid(n, ctas), s, m, g, d, nullptr, rays_o, rays_d, ridx, t, n, ml, sdf, nullptr, nullptr, 0, oc, dn.a);
-    else launch_sdf<0>(variant, persistent_grid(n, ctas), s, m, g, d, x, nullptr, nullptr, nullptr, nullptr, n, ml, sdf, nullptr, nullptr, 0, oc, dn.a);
+    const OccCollect oc = occ_collect_of(collect);
+    const unsigned tiles = persistent_grid((n + kTile - 1) / kTile, kSdfCtasPerSM);
+    if (mode == 2)            // a work unit of mode 2 is a group of 32 packs
+        k_fused_sdf_tc<2><<<persistent_grid((n_packs + 31) / 32, kSdfCtasPerSM), kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf,
+                                                                                                 pack_infos, pack_ray, n_packs, oc, dn.a);
+    else if (mode == 1)
+        k_fused_sdf_tc<1><<<tiles, kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, ridx, t, n, ml, sdf, nullptr, nullptr, 0, oc, dn.a);
+    else
+        k_fused_sdf_tc<0><<<tiles, kTile, 0, s>>>(m, g, d, x, nullptr, nullptr, nullptr, nullptr, n, ml, sdf, nullptr, nullptr, 0, oc, dn.a);
     return check_launch("nsb_fused_sdf(tc)");
 }
 
@@ -304,15 +264,12 @@ extern "C" int nsb_fused_sdf_bwd_indexed(const nsb_lotd_meta *meta, const void *
     NSB_REQUIRE(meta && params_half && dec && d_sdf && d_grid && d_W1 && d_b1 && d_W2 && d_b2, "nsb_fused_sdf_bwd: NULL argument");
     NSB_REQUIRE(x || (rays_o && rays_d && t), "nsb_fused_sdf_bwd: need x or (rays_o, rays_d, t)");
     PLMeta m;
-    if (make_plmeta(meta, &m)) return 2;
-    NSB_REQUIRE(m.n_pseudo == 16 && m.F == 2 && m.D == 3 && plmeta_two_feature_cells(m), "nsb_fused_sdf_bwd: built for 16 x 2 LoTD features in 3-D");
-    NSB_REQUIRE(dec->width >= 1 && dec->width <= 64, "nsb_fused_sdf_bwd: decoder width must be <= 64");
-    DecoderDevTC d{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2, dec->width,
-                   dec->beta};
+    DecoderDevTC d;
+    if (int rc = make_decoder(meta, dec, &m, &d, "nsb_fused_sdf_bwd")) return rc;
     constexpr int kBwdSmem = (128 * 40 + 128 * 128 + 64 * 32 + 32 * 64) * 2 + 128 * tc::acc_stride(64 + 40) * 4 + 128;
     opt_in_smem(k_sdf_bwd_tc<true>, kBwdSmem);
     opt_in_smem(k_sdf_bwd_tc<false>, kBwdSmem);
-    const unsigned grid = persistent_grid(n, 2);           // shared memory: 2 x 104 KB per SM
+    const unsigned grid = persistent_grid((n + kTile - 1) / kTile, 2);     // shared memory: 2 x 104 KB per SM
     cudaStream_t s = (cudaStream_t)stream;
     const int ml = max_level < 0 ? -1 : max_level;
     if (x == nullptr) k_sdf_bwd_tc<true><<<grid, kTile, kBwdSmem, s>>>(m, (const __half *)params_half, d, nullptr, rays_o, rays_d, ridx, t, d_sdf, n, ml,

@@ -1,5 +1,5 @@
-// Building blocks shared by the wgmma fused kernels (fused_tc.cu, color_tc.cu): tile constants, the per-thread
-// LoTD gather that writes straight into a core-matrix A tile, point loading and W1 staging.
+// Building blocks shared by the wgmma fused kernels (fused_tc.cu, color_tc.cu, ray_upsample.cu): tile constants, the per-thread
+// LoTD gather that writes straight into a core-matrix A tile, point loading, decoder staging and the host-side argument checks.
 #pragma once
 #include "lotd_device.cuh"
 #include "tc_util.cuh"
@@ -19,6 +19,10 @@ struct OccCollect {
     int rx, ry, rz;
     float inv_s;
 };
+inline OccCollect occ_collect_of(const nsb_occ_collect *c) {       // NULL or no grid: nothing is collected
+    if (c && c->grid_pcl) return OccCollect{c->grid_pcl, c->res[0], c->res[1], c->res[2], c->inv_s};
+    return OccCollect{nullptr, 1, 1, 1, 0.f};
+}
 __device__ __forceinline__ float r16(float v) { return __half2float(__float2half_rn(v)); }
 __device__ __forceinline__ void occ_collect_point(const OccCollect &oc, const float (&xs)[3], float sdf) {
     const int ix = min(max((int)__fmul_rn(xs[0], (float)oc.rx), 0), oc.rx - 1);
@@ -36,8 +40,9 @@ constexpr int NF = 32, HW = 64;           // features, hidden width (zero padded
 
 // the 16 levels of one point -> row `r` of a chunk-major [R x >=32] fp16 tile (4 bytes per level)
 // U levels per loop trip: the 8 U corner loads of a trip are independent, so U = 2 doubles the loads in flight per thread (the
-// latency-bound backward kernels run at 8-16 warps / SM); full unrolling is avoided on purpose (instruction cache, see fused_tc.cu).
-template <int R, int U = 2, bool PAIRED = false>
+// latency-bound backward kernels run at 8-16 warps / SM; one level per trip thrashes L1 in the ray-major order of k_fused_sdf_tc);
+// full unrolling is avoided on purpose (instruction cache, see fused_tc.cu).
+template <int R, int U = 2>
 __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half *__restrict__ grid, const float (&xs)[3],
                                                    int max_level, uint8_t *tile, int r) {
 #pragma unroll 1
@@ -48,9 +53,7 @@ __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half
 #pragma unroll
         for (int u = 0; u < U; ++u) level_cells3(m, p0 + u, xs, cell[u], w[u]);
 #pragma unroll
-        for (int u = 0; u < U; ++u)
-            packed[u] = PAIRED ? level_feat2_cells_paired(level_cells_ptr(m, p0 + u, grid), cell[u], w[u], (m.is_hash >> (p0 + u)) & 1u)
-                               : level_feat2_cells(level_cells_ptr(m, p0 + u, grid), cell[u], w[u]);
+        for (int u = 0; u < U; ++u) packed[u] = level_feat2_cells(level_cells_ptr(m, p0 + u, grid), cell[u], w[u]);
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             const uint32_t p = p0 + u;
@@ -59,24 +62,36 @@ __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half
     }
 }
 
-__device__ __forceinline__ void load_point(bool from_rays, const float *__restrict__ x, const float *__restrict__ rays_o,
-                                           const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
-                                           const float *__restrict__ t, int64_t i, bool valid, float (&xs)[3]) {
-    xs[0] = xs[1] = xs[2] = 0.f;
+// Where the points of a kernel come from: x[i] (network space), or rays_o/rays_d[ray] + t[i] rays_d[ray] with ray = ridx[i] (or i).
+struct PointSrc {
+    const float *x, *rays_o, *rays_d, *t;
+    const int64_t *ridx;
+};
+
+// point i: xn in network space, its ray, xs in table space; zeros for an invalid i
+__device__ __forceinline__ void load_point(const PointSrc &ps, bool from_rays, int64_t i, bool valid, float (&xn)[3], float (&xs)[3],
+                                           int64_t &ray) {
+    xn[0] = xn[1] = xn[2] = 0.f;
+    ray = 0;
     if (valid) {
         if (from_rays) {
-            const int64_t r = ridx ? ridx[i] : i;
-            const float tt = t[i];
+            ray = ps.ridx ? ps.ridx[i] : i;
+            const float tt = ps.t[i];
 #pragma unroll
-            for (int d = 0; d < 3; ++d) xs[d] = __fmaf_rn(rays_d[r * 3 + d], tt, rays_o[r * 3 + d]);
+            for (int d = 0; d < 3; ++d) xn[d] = __fmaf_rn(ps.rays_d[ray * 3 + d], tt, ps.rays_o[ray * 3 + d]);
         } else {
 #pragma unroll
-            for (int d = 0; d < 3; ++d) xs[d] = x[i * 3 + d];
+            for (int d = 0; d < 3; ++d) xn[d] = ps.x[i * 3 + d];
+            ray = ps.ridx ? ps.ridx[i] : i;
         }
     }
-    // network space [-1,1] -> table space [0,1] (lotd_encoding.py:165), clamp (lotd.py:60)
 #pragma unroll
-    for (int d = 0; d < 3; ++d) xs[d] = fminf(fmaxf(__fmaf_rn(xs[d], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
+    for (int d = 0; d < 3; ++d) xs[d] = to_table_space(xn[d]);
+}
+__device__ __forceinline__ void load_point(const PointSrc &ps, bool from_rays, int64_t i, bool valid, float (&xs)[3]) {
+    float xn[3];
+    int64_t ray;
+    load_point(ps, from_rays, i, valid, xn, xs, ray);
 }
 
 // Softplus(z; beta) with ATen's threshold (beta z > 20 -> identity) on the SFU: e = 2^(z beta log2 e), a = log2(1 + e) ln2 / beta.
@@ -118,6 +133,38 @@ __device__ __forceinline__ void stage_W1(const DecoderDevTC &dec, uint8_t *sB, i
     }
 }
 
+// W1^T [32 x 64] -> chunk-major B tile (row = feature k, column = hidden j), columns >= width zero
+__device__ __forceinline__ void stage_W1T(const DecoderDevTC &dec, uint8_t *sBT, int tid) {
+    for (int e = tid; e < NF * HW; e += kTile) {
+        const int k = e % NF, j = e / NF;
+        const __half v = j < dec.width ? dec.W1[j * NF + k] : __float2half_rn(0.f);
+        *reinterpret_cast<__half *>(sBT + (j / 8) * (NF * 16) + k * 16 + (j % 8) * 2) = v;
+    }
+}
+
+// b1 and W2 (zero past the decoder width) and b2 -> shared memory as fp32.  A kernel that does not read b1 or b2 passes nullptr for it;
+// that is decided by the argument's type, because the compiler cannot prove a shared-memory address non-null.
+template <typename B1, typename B2>
+__device__ __forceinline__ void stage_decoder_vectors(const DecoderDevTC &dec, B1 sb1, float *sW2, B2 sb2, int tid) {
+    constexpr bool kB1 = !std::is_same<B1, std::nullptr_t>::value, kB2 = !std::is_same<B2, std::nullptr_t>::value;
+    if (tid < HW) {
+        if constexpr (kB1) sb1[tid] = tid < dec.width ? __half2float(dec.b1[tid]) : 0.f;
+        sW2[tid] = tid < dec.width ? __half2float(dec.W2[tid]) : 0.f;
+    }
+    if constexpr (kB2) {
+        if (tid == 0) *sb2 = __half2float(dec.b2[0]);
+    }
+}
+
+// Host: the LoTD layout and decoder the wgmma kernels are built for -> their kernel arguments (0, or 2 with the error set).
+inline int make_decoder(const nsb_lotd_meta *meta, const nsb_sdf_decoder *dec, PLMeta *m, DecoderDevTC *d, const char *who) {
+    if (make_plmeta(meta, m)) return 2;
+    NSB_REQUIRE(m->n_pseudo == 16 && m->F == 2 && m->D == 3 && plmeta_two_feature_cells(*m), "%s: built for 16 x 2 LoTD features in 3-D", who);
+    NSB_REQUIRE(dec->width >= 1 && dec->width <= 64, "%s: decoder width must be <= 64", who);
+    *d = DecoderDevTC{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2, dec->width, dec->beta};
+    return 0;
+}
+
 // ---- one 128-point tile of the fused SDF query: gather -> wgmma -> SFU epilogue (used by k_fused_sdf_tc and by the per-ray kernels)
 struct SdfTile {
     const PLMeta &m;
@@ -134,9 +181,8 @@ struct SdfTile {
 // all 128 threads: my point's table coordinates -> my sdf (fp16-rounded, as fp32).  Ends with the CTA barrier that frees the tile.
 // The epilogue runs on the accumulator fragments: each lane folds its 16 of a row's 64 hidden units, the quad sums the four parts
 // in a fixed order (the same for every row, so a point's sdf does not depend on where it sits in the tile).
-template <bool FAST_SP, int UNROLL, bool PAIRED>
 __device__ __forceinline__ float sdf_of_tile(const SdfTile &c, const float (&xs)[3], int tid) {
-    gather_row_to_tile<kTile, UNROLL, PAIRED>(c.m, c.grid, xs, c.max_level, c.sA, tid);
+    gather_row_to_tile<kTile>(c.m, c.grid, xs, c.max_level, c.sA, tid);
     tc::fence_async_smem();                // generic-proxy smem writes -> visible to the tensor core (async proxy)
     __syncthreads();
     float z[2][HW / 2];
@@ -152,18 +198,15 @@ __device__ __forceinline__ float sdf_of_tile(const SdfTile &c, const float (&xs)
 #pragma unroll
                 for (int j = 0; j < 2; ++j) {
                     const int col = ch * 8 + 2 * q + j;
-                    const float zz = __half2float(__float2half_rn(z[h][4 * ch + 2 * i + j] + c.sb1[col]));
-                    float sp;
-                    if (FAST_SP) sp = softplus_a(zz, c.spk);
-                    else { const float zb = zz * c.spk.beta; sp = zb > 20.f ? zz : log1pf(expf(zb)) * (1.f / c.spk.beta); }
-                    out = fmaf(__half2float(__float2half_rn(sp)), c.sW2[col], out);
+                    const float zz = r16(z[h][4 * ch + 2 * i + j] + c.sb1[col]);
+                    out = fmaf(r16(softplus_a(zz, c.spk)), c.sW2[col], out);
                 }
             out += __shfl_xor_sync(0xffffffffu, out, 1);
             out += __shfl_xor_sync(0xffffffffu, out, 2);
             if (q == 0) c.srow[h * 64 + (tid >> 5) * 16 + (lane >> 2) + 8 * i] = out;
         }
     __syncthreads();
-    return __half2float(__float2half_rn(c.srow[tid] + c.sb2));
+    return r16(c.srow[tid] + c.sb2);
 }
 
 }  // namespace nsb

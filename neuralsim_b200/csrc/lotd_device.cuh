@@ -60,6 +60,9 @@ template <typename T> __device__ __forceinline__ T add_st(T a, T b);
 template <> __device__ __forceinline__ float add_st<float>(float a, float b) { return __fadd_rn(a, b); }
 template <> __device__ __forceinline__ __half add_st<__half>(__half a, __half b) { return __hadd(a, b); }
 
+// network space [-1,1] -> table space [0,1] (lotd_encoding.py:165), clamped (lotd.py:60)
+__device__ __forceinline__ float to_table_space(float x) { return fminf(fmaxf(__fmaf_rn(x, 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f); }
+
 // cell = floor(x*scale+0.5), frac = the remainder; scale = res-2 (lotd_hash_only.h:67).  One FMA, as nvcc emits
 // for the reference expression `positions[dim] * scale[dim] + 0.5f`.
 template <int D>
@@ -229,50 +232,6 @@ __device__ __forceinline__ uint32_t level_feat2_cells(const uint32_t *__restrict
     return *reinterpret_cast<uint32_t *>(&acc);
 }
 
-// ---- EXPERIMENT (off by default; NSB_SDF_VARIANT=4, profiles/ab_gather.py): paired corner loads.
-// Two corners of a level often sit in one aligned 8-byte pair of the fp16 image: on dense levels the z-neighbours (cell, cell + 1)
-// when `cell` is even; on hashed levels with a power-of-two table the x-neighbours, whose hashes differ only in bit 0 when x is even
-// ((x+1) ^ A == (x ^ A) ^ 1).  One 8-byte load then serves both and the second 4-byte load is predicated off: ~25 % fewer sectors on the
-// levels that dominate the L1 tag stage, for ~4 more integer instructions per pair.  Values and accumulation order are unchanged.
-__device__ __forceinline__ uint2 ld_nc_u64(const void *p) {
-    uint2 r;
-    asm volatile("ld.global.nc.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
-    return r;
-}
-template <int A, int B>
-__device__ __forceinline__ void load_corner_pair(const uint32_t *__restrict__ lp, const uint32_t (&cell)[8], uint32_t (&raw)[8]) {
-    const uint32_t ca = cell[A], cb = cell[B];
-    const uint2 pr = ld_nc_u64(lp + (ca & ~1u));
-    const bool odd = (ca & 1u) != 0u;
-    raw[A] = odd ? pr.y : pr.x;
-    uint32_t rb = odd ? pr.x : pr.y;
-    if ((ca ^ cb) != 1u) rb = ld_nc_u32(lp + cb);            // not the partner of A's pair: its own load
-    raw[B] = rb;
-}
-__device__ __forceinline__ uint32_t level_feat2_cells_paired(const uint32_t *__restrict__ lp, const uint32_t (&cell)[8], const float (&w)[8], bool hash_level) {
-    uint32_t raw[8];
-    if (hash_level) {                                            // x-neighbours: corners (0,1) (2,3) (4,5) (6,7)
-        load_corner_pair<0, 1>(lp, cell, raw); load_corner_pair<2, 3>(lp, cell, raw);
-        load_corner_pair<4, 5>(lp, cell, raw); load_corner_pair<6, 7>(lp, cell, raw);
-    } else {                                                     // z-neighbours: corners (0,4) (1,5) (2,6) (3,7)
-        load_corner_pair<0, 4>(lp, cell, raw); load_corner_pair<1, 5>(lp, cell, raw);
-        load_corner_pair<2, 6>(lp, cell, raw); load_corner_pair<3, 7>(lp, cell, raw);
-    }
-    __half2 acc = __floats2half2_rn(0.f, 0.f);
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        const float2 v = __half22float2(*reinterpret_cast<const __half2 *>(&raw[c]));
-        acc = __hadd2(acc, __floats2half2_rn(__fmul_rn(w[c], v.x), __fmul_rn(w[c], v.y)));
-    }
-    return *reinterpret_cast<uint32_t *>(&acc);
-}
-// precondition of the paired loads: every level has an even number of cells and starts 8-byte aligned in the fp16 image
-inline bool plmeta_pairable(const PLMeta &m, const void *params_half) {
-    for (uint32_t p = 0; p < m.n_pseudo; ++p)
-        if ((m.size[p] & 1u) || (((uintptr_t)params_half + 2ull * m.base[p]) & 7ull)) return false;
-    return true;
-}
-
 __device__ __forceinline__ void red_add2(float2 *dst, float a, float b) {
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(a), "f"(b) : "memory");
 }
@@ -323,20 +282,6 @@ inline bool plmeta_two_feature_cells(const PLMeta &m) {
     for (uint32_t p = 0; p < m.n_pseudo; ++p)
         if (m.nfeat[p] != 2u || (m.base[p] & 1u)) return false;
     return m.F == 2u;
-}
-
-// one level's two fp16 features of a point, accumulated in fp16 over the corners (reference semantics), as a packed half2
-__device__ __forceinline__ uint32_t level_feat2(const __half *__restrict__ grid, const uint32_t (&idx)[8], const float (&w)[8]) {
-    uint32_t raw[8];
-#pragma unroll
-    for (int c = 0; c < 8; ++c) raw[c] = ld_nc_u32(grid + idx[c]);
-    __half2 acc = __floats2half2_rn(0.f, 0.f);
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        const float2 v = __half22float2(*reinterpret_cast<const __half2 *>(&raw[c]));
-        acc = __hadd2(acc, __floats2half2_rn(__fmul_rn(w[c], v.x), __fmul_rn(w[c], v.y)));
-    }
-    return *reinterpret_cast<uint32_t *>(&acc);
 }
 
 // grad[dst .. dst+F) += g[f] * w, fp32, fire-and-forget vector reductions (8-byte aligned: F even, offsets even).

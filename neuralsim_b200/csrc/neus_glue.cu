@@ -206,35 +206,34 @@ __device__ __forceinline__ int count_less(const float *a, int n, float v, bool o
     return lo;
 }
 
-// CHUNK consecutive rays per warp trip: ONE search of the first ray in ridx_hit (18 dependent L2 loads on a frame -- half of the kernel's
-// time when every ray searched for itself, CHUNK = 1), the next CHUNK entries of the list in registers, a running rank for the rest.
-template <int CHUNK>
+// kAsmChunk consecutive rays per warp trip: ONE search of the first ray in ridx_hit (18 dependent L2 loads on a frame -- half of the
+// kernel's time when every ray searched for itself), the next kAsmChunk entries of the list in registers, a running rank for the rest.
 __global__ void __launch_bounds__(kAsmWarps * 32)
 k_assemble_boundary(const float *__restrict__ coarse, int64_t n_rays, int nc, const int64_t *__restrict__ ridx_hit, int64_t n_hit,
                     const float *__restrict__ fine, int nf, const AsmRuns runs, float *__restrict__ d1, float *__restrict__ mid,
                     int64_t *__restrict__ ridx_all, int64_t *__restrict__ pack_infos, const int64_t *__restrict__ n_rays_dev,
                     const int64_t *__restrict__ n_hit_dev) {
     extern __shared__ float s_v[];                        // [warps][2][nc + nf]
-    static_assert(CHUNK >= 1 && CHUNK <= 32, "one candidate per lane");
+    static_assert(kAsmChunk >= 1 && kAsmChunk <= 32, "one candidate per lane");
     n_rays = eff_n(n_rays, n_rays_dev);
     n_hit = eff_n(n_hit, n_hit_dev);
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, cap = nc + nf;
     float *raw = s_v + (size_t)w * 2 * cap, *srt = raw + cap;
-    const int64_t n_chunks = (n_rays + CHUNK - 1) / CHUNK;
+    const int64_t n_chunks = (n_rays + kAsmChunk - 1) / kAsmChunk;
     for (int64_t c = gwarp_(); c < n_chunks; c += nwarps_()) {
-        const int64_t r0 = c * CHUNK;
+        const int64_t r0 = c * kAsmChunk;
         int64_t lo0 = 0, cnt = n_hit;                     // lower bound of r0 in ridx_hit
         while (cnt > 0) {
             const int64_t step = cnt >> 1;
             if (ridx_hit[lo0 + step] < r0) { lo0 += step + 1; cnt -= step + 1; } else cnt = step;
         }
         long long cand = -1;                              // lane k: the k-th listed ray at or after r0
-        if (lane < CHUNK && lo0 + lane < n_hit) cand = ridx_hit[lo0 + lane];
+        if (lane < kAsmChunk && lo0 + lane < n_hit) cand = ridx_hit[lo0 + lane];
         int used = 0;                                     // listed rays among r0 .. r - 1
-        for (int j = 0; j < CHUNK; ++j) {
+        for (int j = 0; j < kAsmChunk; ++j) {
             const int64_t r = r0 + j;
             if (r >= n_rays) break;
-            const bool hit = __shfl_sync(0xffffffffu, cand, used) == r;      // used <= j < CHUNK
+            const bool hit = __shfl_sync(0xffffffffu, cand, used) == r;      // used <= j < kAsmChunk
             const int64_t lo = lo0 + used;
             const int n = nc + (hit ? nf : 0);
             const int64_t first = (int64_t)nc * r + (int64_t)nf * lo;
@@ -433,7 +432,6 @@ __global__ void k_query_counts(int64_t *__restrict__ c, int phase, int nc, int n
 
 }  // namespace nsb
 
-namespace nsb { extern std::atomic<int> g_opt_asm_chunk; }
 using namespace nsb;
 #define STREAM ((cudaStream_t)stream)
 
@@ -503,15 +501,9 @@ extern "C" int nsb_assemble_boundary(const float *coarse, int64_t n_rays, int32_
     runs.n = n_runs;
     NSB_REQUIRE(tot == n_fine, "nsb_assemble_boundary: run lengths must add up to n_fine");
     const unsigned grid = wave_grid(n_rays * 32, kAsmWarps * 32, 8);
-    if (g_opt_asm_chunk.load() > 1) {                     // rays per search of the hit list (nsb_set_option "asm_chunk": 1 = every ray searches, A/B)
-        opt_in_smem(k_assemble_boundary<kAsmChunk>, 96 * 1024);
-        k_assemble_boundary<kAsmChunk><<<grid, kAsmWarps * 32, smem, STREAM>>>(coarse, n_rays, n_coarse, ridx_hit, n_hit, fine, n_fine, runs, d1, mid, ridx_all,
-                                                                             pack_infos, dn.a, dn.b);
-    } else {
-        opt_in_smem(k_assemble_boundary<1>, 96 * 1024);
-        k_assemble_boundary<1><<<grid, kAsmWarps * 32, smem, STREAM>>>(coarse, n_rays, n_coarse, ridx_hit, n_hit, fine, n_fine, runs, d1, mid, ridx_all,
-                                                                     pack_infos, dn.a, dn.b);
-    }
+    opt_in_smem(k_assemble_boundary, 96 * 1024);
+    k_assemble_boundary<<<grid, kAsmWarps * 32, smem, STREAM>>>(coarse, n_rays, n_coarse, ridx_hit, n_hit, fine, n_fine, runs, d1, mid, ridx_all, pack_infos,
+                                                               dn.a, dn.b);
     return check_launch("nsb_assemble_boundary");
 }
 

@@ -81,6 +81,12 @@ inline unsigned wave_grid(int64_t work_items, int block, int ctas_per_sm) {
     return (unsigned)(waves * wave);
 }
 
+// Grid size for persistent kernels: one CTA per work unit, at most `ctas_per_sm` resident CTAs on every SM; each CTA loops over the rest.
+inline unsigned persistent_grid(int64_t work_units, int ctas_per_sm) {
+    const int64_t wave = (int64_t)sm_count() * ctas_per_sm;
+    return (unsigned)(work_units < wave ? work_units : wave);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

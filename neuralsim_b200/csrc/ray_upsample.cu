@@ -18,6 +18,7 @@ constexpr int kG = 4;            // rays per group = warps per CTA
 constexpr int kCap = 192;        // samples of one ray held in shared memory (marched + all merged stages but the last)
 constexpr int kMaxFine = 64;     // samples of one stage
 constexpr int kMaxStage = 4;
+constexpr int kCtasPerSM = 5;    // persistent grid; the scratch buffer holds one slice per CTA of that grid
 
 struct UpsampleArgs {
     int n_stage, use_estimate;
@@ -109,11 +110,7 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     stage_W1(dec, sB, tid);
-    if (tid < HW) {
-        sb1[tid] = tid < dec.width ? __half2float(dec.b1[tid]) : 0.f;
-        sW2[tid] = tid < dec.width ? __half2float(dec.W2[tid]) : 0.f;
-    }
-    if (tid == 0) sb2 = __half2float(dec.b2[0]);
+    stage_decoder_vectors(dec, sb1, sW2, &sb2, tid);
     tc::fence_async_smem();
     __syncthreads();
     const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
@@ -168,8 +165,8 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
                     for (int c = 0; c < 3; ++c) xs[c] = __fmaf_rn(s_d[q][c], tt, s_o[q][c]);
                 }
 #pragma unroll
-                for (int c = 0; c < 3; ++c) xs[c] = fminf(fmaxf(__fmaf_rn(xs[c], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
-                const float v = sdf_of_tile<true, 2, false>(ctx, xs, tid);
+                for (int c = 0; c < 3; ++c) xs[c] = to_table_space(xs[c]);
+                const float v = sdf_of_tile(ctx, xs, tid);
                 if (valid) {
                     p_sdf[0][q][r] = v;
                     if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -203,8 +200,8 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
                     for (int c = 0; c < 3; ++c) xs[c] = __fmaf_rn(s_d[q][c], tt, s_o[q][c]);
                 }
 #pragma unroll
-                for (int c = 0; c < 3; ++c) xs[c] = fminf(fmaxf(__fmaf_rn(xs[c], 0.5f, 0.5f), 1.0e-6f), 1.f - 1.0e-6f);
-                const float v = sdf_of_tile<true, 2, false>(ctx, xs, tid);
+                for (int c = 0; c < 3; ++c) xs[c] = to_table_space(xs[c]);
+                const float v = sdf_of_tile(ctx, xs, tid);
                 if (valid) {
                     s_fsdf[q][k] = v;
                     if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -236,9 +233,11 @@ extern "C" int nsb_upsample_persistent(const nsb_lotd_meta *meta, const void *pa
                              use_estimate_alpha, early_stop_eps, alpha_thre, fine_all, overflow, nullptr, 0, nullptr, stream);
 }
 
+static unsigned upsample_grid(int64_t n_hit) { return persistent_grid((n_hit + kG - 1) / kG, kCtasPerSM); }
+
+// per CTA of the grid: kG rays x 5 arrays (t, sdf of two generations, cdf) of long_cap floats
 extern "C" int64_t nsb_upsample_rays_scratch_floats(int64_t n_hit_cap, int32_t long_cap) {
-    const int64_t groups = (n_hit_cap + kG - 1) / kG, wave = (int64_t)sm_count() * 5;
-    return (groups < wave ? groups : wave) * kG * 5 * (int64_t)long_cap;
+    return (int64_t)upsample_grid(n_hit_cap) * kG * 5 * (int64_t)long_cap;
 }
 
 extern "C" int nsb_upsample_rays(const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *rays_o,
@@ -252,9 +251,8 @@ extern "C" int nsb_upsample_rays(const nsb_lotd_meta *meta, const void *params_h
                 "nsb_upsample_persistent: NULL argument");
     NSB_REQUIRE(n_stage >= 1 && n_stage <= kMaxStage, "nsb_upsample_persistent: 1..%d stages", kMaxStage);
     PLMeta m;
-    if (make_plmeta(meta, &m)) return 2;
-    NSB_REQUIRE(m.n_pseudo == 16 && m.F == 2 && m.D == 3 && plmeta_two_feature_cells(m), "nsb_upsample_persistent: built for 16 x 2 LoTD features in 3-D");
-    NSB_REQUIRE(dec->width >= 1 && dec->width <= 64, "nsb_upsample_persistent: decoder width must be <= 64");
+    DecoderDevTC d;
+    if (int rc = make_decoder(meta, dec, &m, &d, "nsb_upsample_persistent")) return rc;
     UpsampleArgs ua{};
     ua.n_stage = n_stage;
     ua.use_estimate = use_estimate_alpha;
@@ -270,13 +268,9 @@ extern "C" int nsb_upsample_rays(const nsb_lotd_meta *meta, const void *params_h
         if (i + 1 < n_stage) merged += n_fine[i];
     }
     NSB_REQUIRE(merged < kCap, "nsb_upsample_persistent: the merged stages alone exceed the per-ray capacity");
-    DecoderDevTC d{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2, dec->width, dec->beta};
-    const int64_t groups = (n_hit + kG - 1) / kG, wave = (int64_t)sm_count() * 5;
     NSB_REQUIRE(scratch == nullptr || long_cap > kCap, "nsb_upsample_rays: long_cap must exceed the shared-memory capacity (%d)", kCap);
-    OccCollect oc{nullptr, 1, 1, 1, 0.f};
-    if (collect && collect->grid_pcl) oc = OccCollect{collect->grid_pcl, collect->res[0], collect->res[1], collect->res[2], collect->inv_s};
-    k_upsample_persistent<<<(unsigned)(groups < wave ? groups : wave), kTile, 0, (cudaStream_t)stream>>>(
+    k_upsample_persistent<<<upsample_grid(n_hit), kTile, 0, (cudaStream_t)stream>>>(
         m, (const __half *)params_half, d, rays_o, rays_d, t_starts, pack_infos, ridx_hit, n_hit, max_level < 0 ? -1 : max_level, ua, fine_all, nf_total,
-        overflow, scratch, long_cap, oc, dn.a);
+        overflow, scratch, long_cap, occ_collect_of(collect), dn.a);
     return check_launch("nsb_upsample_rays");
 }

@@ -27,19 +27,16 @@ from . import neus_fused
 # True: the per-ray stages run as the fused kernels of csrc/neus_fused.cu; False: as the reference's chain of
 # pack_ops / elementwise calls (same maths; kept for the parity tests and as documentation of what is fused).
 FUSED_STAGES = True
-import os as _os
 # The no-grad half of the fused query (sdf of the marched samples + the up-sampling stages) as ONE persistent per-ray kernel
 # (csrc/ray_upsample.cu) or as one launch per stage -- same values either way (tests/test_ray_upsample_gpu.py).  The persistent kernel saves
 # launches on small batches (25 instead of 35 for 4096 random rays) and loses on large ones (its 128-point tiles are filled by 4 rays' 9-sample
 # stages to 28 %), so: True / False force it, "auto" (default) takes it below PERSISTENT_MAX_RAYS tested rays.  perturb=True always runs the stage kernels.
-_pu = _os.environ.get("NSB_PERSISTENT_UPSAMPLE", "auto")
-PERSISTENT_UPSAMPLE = "auto" if _pu == "auto" else (_pu != "0")
+PERSISTENT_UPSAMPLE = "auto"
 PERSISTENT_MAX_RAYS = 8192
 
 
 def use_persistent_upsample(n_rays: int) -> bool:
     return (n_rays < PERSISTENT_MAX_RAYS) if PERSISTENT_UPSAMPLE == "auto" else bool(PERSISTENT_UPSAMPLE)
-MARCHED_TILED = _os.environ.get("NSB_MARCHED_TILED", "0") != "0"     # ray-tiled traversal of the marched samples (off: ray-major was the faster order)
 
 __all__ = ["neus_cdf", "neus_ray_cdf_to_alpha", "neus_ray_sdf_to_alpha", "neus_ray_sdf_to_vw", "neus_packed_cdf_to_alpha",
            "neus_packed_sdf_to_alpha", "neus_packed_sdf_to_upsample_alpha", "neus_ray_sdf_to_upsample_alpha",
@@ -148,11 +145,10 @@ def _query_fused(model, ray_tested, view_dirs, rays_h_appear, *, perturb=False, 
         return _query_fused_tail(model, ray_tested, view_dirs, rays_h_appear, rays_o, rays_d, rays_inds, d1, mid, ridx_all, pinfo, pinfo_march, coherent, dtype,
                                  with_rgb=with_rgb, with_normal=with_normal, nablas_has_grad=nablas_has_grad, forward_inv_s=forward_inv_s)
     with torch.no_grad():
-        # marched packs are ragged (20-100 samples per ray): tiles of 32 rays are padded to the longest and the samples of one ray are
-        # already close together, so the ray-major order wins here (A/B switch MARCHED_TILED); the boundary and fine queries have
-        # uniform packs and are ray-tiled whenever the rays are image-ordered
-        tiled_m = coherent and MARCHED_TILED
-        sdf = model.forward_sdf_on_rays(ridx, depth_samples, rays_o, rays_d, packs=(pack_infos, ridx_hit) if tiled_m else None)["sdf"].to(dtype)
+        # marched packs are ragged (20-100 samples per ray): tiles of 32 rays would be padded to the longest and the samples of one ray
+        # are already close together, so they are queried in ray-major order (measured faster than ray-tiled); the boundary and fine
+        # queries have uniform packs and are ray-tiled whenever the rays are image-ordered
+        sdf = model.forward_sdf_on_rays(ridx, depth_samples, rays_o, rays_d)["sdf"].to(dtype)
         fine_stages = []
         for i, factor in enumerate(factors):
             cdf = neus_fused.upsample_cdf(sdf, depth_samples, pack_infos, upsample_inv_s * factor, use_estimate_alpha)

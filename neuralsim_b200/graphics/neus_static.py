@@ -15,7 +15,6 @@ tests/test_static_gpu.py: images bit-equal to the host-sized path, gradients equ
 from __future__ import annotations
 
 import ctypes
-import os
 
 import torch
 import torch.nn.functional as F
@@ -32,7 +31,7 @@ CNT_SLOTS = dict(n_rays=0, pairs=2, marched_raw=3, hit_raw=4, kept_raw=6, kept_r
 _NULL = ctypes.c_void_p(0)
 # "auto": small batches march once and copy (nsb_ray_marching_record + nsb_march_compact) when the per-ray record fits this many bytes;
 # "0": always the two-round march; "1": always the recorded march.  Same samples bit for bit either way.
-MARCH_ONEPASS = os.environ.get("NSB_MARCH_ONEPASS", "auto")
+MARCH_ONEPASS = "auto"
 MARCH_ONEPASS_MAX_BYTES = 64 << 20
 
 

@@ -1,11 +1,9 @@
-"""A/B of the step's glue on one GPU, one process, same model and poses (not a bench value; bench.py is):
-   asm_chunk   1 = every ray of nsb_assemble_boundary searches the hit list, 8 = one search per 8 consecutive rays
+"""A/B of the graph-captured step's march on one GPU, one process, same model and poses (not a bench value; bench.py is):
    onepass     0 = two-round march, 1 = march once recording the samples per ray + copy (auto: only when the record fits 64 MB)
 (r02j: the first version of this script captured its second frame with all-zero input rays and hung in the march until its timeout; only the
 first configuration of each run was recorded.  Fixed below.)
 Usage: python profiles/ab_glue.py [--rays 480000 | --rays 4096 --random-rays] [--steps 20] [--rounds 2]"""
 import argparse
-import ctypes
 import gc
 import json
 import os
@@ -25,7 +23,6 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=2)
     args = ap.parse_args()
-    from neuralsim_b200 import _lib
     from neuralsim_b200.graphics import neus_static as NS
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(0)
@@ -43,8 +40,7 @@ def main():
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
     caps = {}
 
-    def run(chunk, onepass):
-        _lib.lib().nsb_set_option(b"asm_chunk", ctypes.c_int(chunk))
+    def run(onepass):
         NS.MARCH_ONEPASS = onepass
         fr = NS.StaticFrame(model, args.rays, loss_fn=bench.loss_of, near=0.01, pre_hook=flat.zero_, **caps)
         if not caps:
@@ -70,12 +66,11 @@ def main():
         del fr
         gc.collect()
         torch.cuda.empty_cache()
-        return dict(asm_chunk=chunk, onepass=onepass, mean=sum(ts) / len(ts), median=ts[len(ts) // 2], min=ts[0], max=ts[-1], checksum=chk)
+        return dict(onepass=onepass, mean=sum(ts) / len(ts), median=ts[len(ts) // 2], min=ts[0], max=ts[-1], checksum=chk)
 
-    configs = [(1, "0"), (8, "0"), (8, "1")]
     for r in range(args.rounds):
-        for chunk, onepass in configs:
-            print(json.dumps(dict(rays=args.rays, round=r, **run(chunk, onepass))), flush=True)
+        for onepass in ("0", "1"):
+            print(json.dumps(dict(rays=args.rays, round=r, **run(onepass))), flush=True)
 
 
 if __name__ == "__main__":

@@ -53,17 +53,7 @@ def test_merge_sorted_vals_equals_aligned_merge():
         assert none is None and torch.equal(dep_m2, dep_ref)
 
 
-@pytest.fixture(params=[8, 1])
-def asm_chunk(request):
-    """both flavours of nsb_assemble_boundary: one search of the hit list per 8 rays (default) / per ray"""
-    import ctypes
-    from neuralsim_b200 import _lib as L
-    L.lib().nsb_set_option(b"asm_chunk", ctypes.c_int(request.param))
-    yield request.param
-    L.lib().nsb_set_option(b"asm_chunk", ctypes.c_int(8))
-
-
-def test_assemble_boundary_equals_reference_chain(asm_chunk):
+def test_assemble_boundary_equals_reference_chain():
     from neuralsim_b200.graphics import neus_fused as NF
     from neuralsim_b200.graphics.pack_ops import merge_two_batch_a_includes_b, packed_diff
     g = torch.Generator().manual_seed(2)

@@ -8,7 +8,6 @@ so a wrong tile shows up as 128 wrong rows.  Backward passes are compared with e
 restricted to one tile at a time while the kernel still runs over all points.  Bounds are about 3x the errors measured on an
 H100 80GB HBM3 (132 SMs, 400 W power limit); DESIGN.md §4 lists them."""
 import ctypes
-import os
 
 import numpy as np
 import pytest
@@ -19,8 +18,8 @@ from oracle import fused64, lotd as olotd
 pytestmark = pytest.mark.gpu
 
 TILE = 128
-# CTAs per SM of the persistent grids: kSdfCtasPerSM and persistent_grid(n, 2) in nsb_fused_sdf_bwd (csrc/fused_tc.cu);
-# tiles_grid(n, 2) for k_color_fwd and tiles_grid(n, 1) for both colour backward kernels (csrc/color_tc.cu)
+# CTAs per SM of the persistent grids: kSdfCtasPerSM and persistent_grid(tiles, 2) in nsb_fused_sdf_bwd (csrc/fused_tc.cu);
+# persistent_grid(tiles, 2) for k_color_fwd and persistent_grid(tiles, 1) for both colour backward kernels (csrc/color_tc.cu)
 CTAS_PER_SM = dict(sdf_fwd=4, sdf_bwd=2, color_fwd=2, color_bwd=1)
 
 # (decoder width, radiance width, n_appear), max_level; the first is the production configuration
@@ -38,7 +37,6 @@ RGB_FLIP_FRAC, RGB_MAX_ULP = 3e-3, 3.0              # measured <= 8.9e-4, 1.0
 NAB_MAX_REL, NAB_FRAC_1E5 = 2e-3, 1.5e-2            # measured <= 5.7e-4; fraction of elements above 1e-5 <= 4.2e-3
 BWD_REL = dict(grid=1e-4, W1=6e-5, b1=1e-4, W2=8e-5, b2=5e-6, R1=6e-3, rb1=6e-3, R2=6e-3, rb2=6e-3, R3=2e-4, rb3=6e-5)
 TILE_REL = {k: 1.5e-4 for k in BWD_REL}             # measured <= 4.6e-5
-TMA_REL = 1.5e-6                                    # measured <= 4.1e-7
 
 
 def _sms():
@@ -279,26 +277,3 @@ def test_sdf_backward_one_tile(which):
     want = ref.sdf_backward(inp["x"].numpy()[rows], c.numpy()[rows])
     _compare_grads(got, want, TILE_REL, f"sdf_bwd tile {which}={tile}")
 
-
-# ===================================================================================================================== color_tma
-@pytest.fixture
-def color_tma():
-    from neuralsim_b200 import _lib as L
-    yield lambda v: L.check(L.lib().nsb_set_option(b"color_tma", ctypes.c_int(v)))
-    L.check(L.lib().nsb_set_option(b"color_tma", ctypes.c_int(int(os.environ.get("NSB_COLOR_TMA", 2)))))   # the default, as _lib sets it
-
-
-def test_color_tma_variants_agree(color_tma):
-    """color_tma 0 (plain loads in both colour backward kernels), 1 (TMA in the radiance backward), 2 (TMA in both)"""
-    model, inp, _, _ = _case(PRODUCTION)
-    _assert_multi_tile("color_bwd", inp["x"].shape[0], 3)
-    out = _color_fwd(model, inp)
-    grads = {}
-    for v in (0, 1, 2):
-        color_tma(v)
-        grads[v] = _color_grads(model, out, inp["cot"], retain=True)
-    for v in (0, 1):
-        errs = {k: _rel(grads[v][k].cpu().numpy(), grads[2][k].cpu().numpy()) for k in grads[2]}
-        print(f"METRIC color_tma {v} vs 2 " + " ".join(f"{k}={e:.2e}" for k, e in errs.items()))
-        for k, e in errs.items():
-            assert e < TMA_REL, (v, k, e)
