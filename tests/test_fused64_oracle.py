@@ -127,3 +127,42 @@ def test_rounded_reference_forward_matches_autocast_restatement():
         assert frac < 1.5e-2 and worst <= 1.0, (k, frac, worst)
     err = np.abs(got["nablas"] - want["nablas"].detach().numpy()) / (got["nablas_scale"] + 1e-30)
     assert float(np.quantile(err, 0.99)) < 1e-5 and float(err.max()) < 2e-3, (np.quantile(err, 0.99), err.max())
+
+
+def test_merge_census_matches_reference_addressing_and_counts_heads():
+    """tests/util.py:merge_census, the model of the warp-merged table-gradient scatter that the GPU scatter tests use to assert which
+    (warp, level) pairs merge: its cells address the table as Fused64 does, and it counts run heads by the kernel's rule"""
+    from util import MERGE_MAX_HEADS, merge_census
+    cfg = olotd.gen_ngp_cfg()
+    g = torch.Generator().manual_seed(3)
+    x = (torch.rand(512, 3, generator=g) * 2 - 1).numpy()
+    x[:40] = 0.0                                                    # the point an invalid lane loads
+    for max_level in (None, 7):
+        ref = fused64.Fused64(np.zeros(olotd.LoDMeta(3, **cfg).n_params, dtype=np.float32), cfg, np.zeros((64, 32)), np.zeros(64),
+                              np.zeros((1, 64)), np.zeros(1), max_level=max_level)
+        c = merge_census(x, cfg, max_level=max_level)
+        levels = list(ref.levels(ref.xs_of(x)))
+        assert len(levels) == len(c["levels"]) == (16 if max_level is None else 8)
+        for (ooff, idx, w, dw), lvl, cell in zip(levels, c["levels"], c["cells"]):
+            loff = ref.meta.level_offsets[lvl]
+            assert np.array_equal(olotd.grid_index(ref.meta, lvl, cell) * 2 + loff, idx[0]), lvl
+        assert c["mergeable"].tolist() == [r <= 1024 for r in np.array(cfg["lod_res"])[c["levels"]]]
+    assert merge_census(x, cfg)["mergeable"].tolist() == [True] * 13 + [False] * 3      # levels 13..15 have more than 1024 cells per axis
+
+    # hand-built warps; level 0 has 14 cells per axis, cell k holds table-space k / 14 at its centre
+    cell0 = lambda kx, ky, kz, j=0: np.array([kx, ky, kz], dtype=np.float32) / 7.0 - 1.0 + np.float32(1e-5) * j
+    A, B = (3, 4, 5), (3, 4, 6)
+    pts = [cell0(*A, j) for j in range(10)] + [cell0(*B, j) for j in range(5)] + [cell0(*A, j) for j in range(9)]
+    pts += [cell0(j % 14, j // 14, 1) for j in range(32)]           # warp 1: 32 cells
+    pts += [cell0(*B, j) for j in range(32)]                        # warp 2: one cell
+    x = np.stack(pts)
+    order = np.concatenate([np.arange(24), np.full(8, -1), np.arange(24, 88)])
+    active = np.ones(order.shape[0], dtype=bool)
+    active[20] = False                                              # lane 20 (cell A): a zero cotangent in k_sdf_bwd_tc
+    c = merge_census(x, cfg, order=order, active=active)
+    # warp 0: A x10 | B x5 | A x5 | A (inactive) | A x3 | 8 invalid lanes -> 1 + 1 + 1 + 1 + 1 + 8 heads
+    assert c["heads"][:, 0].tolist() == [13, 32, 1]
+    assert c["heads"][0, 0] <= MERGE_MAX_HEADS < c["heads"][1, 0]
+    c = merge_census(x, cfg, order=order)                           # every valid lane active: lanes 15..23 are one run
+    assert c["heads"][:, 0].tolist() == [11, 32, 1]
+    assert c["valid"].tolist() == [True] * 24 + [False] * 8 + [True] * 64

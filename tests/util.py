@@ -58,3 +58,42 @@ def product_grads(model):
 def random_packs(rng, n_packs, lo, hi, device="cpu"):
     n = torch.from_numpy(rng.integers(lo, hi, n_packs)).long()
     return torch.stack([n.cumsum(0) - n, n], 1).to(device)
+
+
+MERGE_MAX_HEADS = 24        # warp_merge_updates (csrc/lotd_device.cuh): a warp with more run heads on a level issues every lane's own updates
+
+
+def merge_census(x, lotd_cfg, max_level=None, order=None, active=None):
+    """The run structure that the warp-merged table-gradient scatter (warp_merge_updates / cell_key3, csrc/lotd_device.cuh) sees.
+
+    x [N, 3]: network-space points.  order [W]: the point each work item (lane) loads, -1 for an invalid lane (it loads x = 0);
+    default: the N points in their order.  W is padded with invalid lanes to whole warps of 32.  active [W] bool: the lanes that carry
+    gradient (default: the valid ones; k_sdf_bwd_tc also makes a lane with a zero cotangent inactive).
+    A lane is a run head if it is inactive, if the previous lane is inactive or if its cell differs from the previous lane's.
+    -> dict(levels [L] (level of each contributing pseudo level), mergeable [L] (every axis resolution <= 1024), heads [W/32, L],
+            cells [L] of uint32 [W, 3] (cell coordinates per lane), valid [W])"""
+    from oracle import lotd as olotd
+    from oracle.fused64 import Fused64
+    meta = olotd.LoDMeta(3, **lotd_cfg)
+    x = np.asarray(x, dtype=np.float32)
+    order = np.arange(x.shape[0]) if order is None else np.asarray(order, dtype=np.int64)
+    W = -(-order.shape[0] // 32) * 32
+    order = np.concatenate([order, np.full(W - order.shape[0], -1, dtype=np.int64)])
+    valid = order >= 0
+    act = valid.copy() if active is None else np.concatenate([np.asarray(active, dtype=bool), np.zeros(W - len(active), dtype=bool)]) & valid
+    xs = Fused64.xs_of(np.where(valid[:, None], x[np.maximum(order, 0)], np.float32(0.0)))
+    prev_act = np.concatenate([[False], act[:-1]]).reshape(-1, 32)
+    prev_act[:, 0] = False
+    levels, mergeable, heads, cells = [], [], [], []
+    for psl, lvl, loff, foff, ooff in olotd._level_iter(meta, meta.n_levels if max_level is None else max_level):
+        res = np.array(meta.level_res_multidim[lvl], dtype=np.uint32)
+        cell, _ = olotd.pos_fract(xs, (res - 2).astype(np.float32))
+        c = cell.reshape(-1, 32, 3)
+        differs = np.ones(c.shape[:2], dtype=bool)
+        differs[:, 1:] = (c[:, 1:] != c[:, :-1]).any(-1)
+        head = ~act.reshape(-1, 32) | ~prev_act | differs
+        levels.append(lvl)
+        mergeable.append(bool((res <= 1024).all()))
+        heads.append(head.sum(1))
+        cells.append(cell)
+    return dict(levels=np.array(levels), mergeable=np.array(mergeable), heads=np.stack(heads, 1), cells=cells, valid=valid)
