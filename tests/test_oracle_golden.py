@@ -124,6 +124,40 @@ def test_lotd_gradcheck_style_properties():
     assert np.abs(z).sum() == 0                                   # lotd_torch_api.cu:294-297
 
 
+_CUBOID_3D = dict(lod_res=[[6, 11, 4], [10, 17, 6], [17, 29, 9], [29, 49, 15]], lod_n_feats=[2, 4, 2, 2], lod_types=["Dense"] * 2 + ["Hash"] * 2,
+                  hashmap_size=3001)
+_TABLE_4D = dict(lod_res=[[6, 6, 6, 4], [9, 9, 9, 6], [13, 13, 13, 8], [20, 20, 20, 12], [7, 11, 5, 4]], lod_n_feats=[2] * 5,
+                 lod_types=["Dense", "Dense", "Hash", "Hash", "Dense"], hashmap_size=2 ** 12)
+
+
+@pytest.mark.parametrize("D, cfg", [(3, _CUBOID_3D), (4, _TABLE_4D)], ids=["cuboid3d", "4d"])
+def test_lotd_adjoint_identities_cuboid_and_4d(D, cfg):
+    """The adjoint identities of test_lotd_gradcheck_style_properties on a cuboid 3-D table (with a 4-wide level and a hash size that is
+    not a power of two) and on the 4-D table of the distant model with a level that is cuboid in x / y / z.  A dense level also has to
+    address every cell of its [rx, ry, rz(, rw)] box exactly once."""
+    m = olotd.LoDMeta(D, **cfg)
+    rng = np.random.default_rng(1)
+    p = rng.uniform(-0.1, 0.1, m.n_params).astype(np.float32)
+    x = rng.uniform(1e-6, 1 - 1e-6, (3000, D)).astype(np.float32)
+    y, J = olotd.lod_fwd(m, x, p, need_input_grad=True)
+    g = rng.normal(size=y.shape).astype(np.float32)
+    gp = olotd.lod_bwd_grid(m, g, x, m.n_params)                  # <g, y(p)> == <dL_dp, p>
+    assert abs((gp * p).sum() - (g.astype(np.float64) * y).sum()) < 1e-6 * np.abs(gp * p).sum() + 1e-6
+    gin = rng.normal(size=x.shape).astype(np.float32)
+    a, b, _ = olotd.lod_bwd_bwd_input(m, gin, g, x, p, J)         # dL_dx = J^T g is bilinear in (g, p)
+    lhs = (gin.astype(np.float64) * olotd.lod_bwd_input(g, J)).sum()
+    assert abs(lhs - (b * p).sum()) < 1e-5 * abs(lhs) and abs(lhs - (a.astype(np.float64) * g).sum()) < 1e-5 * abs(lhs)
+    eps = 1e-4
+    for d in range(D):                                            # dy/dx along each axis by central differences
+        xp, xm = x.copy(), x.copy(); xp[:, d] += eps; xm[:, d] -= eps
+        fd = (olotd.lod_fwd(m, xp, p)[0].astype(np.float64) - olotd.lod_fwd(m, xm, p)[0]) / (xp[:, d] - xm[:, d])[:, None].astype(np.float64)
+        assert np.median(np.abs(fd - J[:, :, d])) < 2e-3, d
+    for lvl, res in enumerate(m.level_res_multidim):
+        if m.level_types[lvl] == olotd.DENSE:
+            cells = np.stack(np.meshgrid(*[np.arange(r, dtype=np.uint32) for r in res], indexing="ij"), -1).reshape(-1, D)
+            assert np.array_equal(np.sort(olotd.grid_index(m, lvl, cells)), np.arange(m.level_sizes[lvl]))
+
+
 def test_cfg1_sphere_pure_torch_cpu():
     """BASELINE.json configs[0]: analytic sphere, 64x64 rays, 32 samples -- the reference's pure-PyTorch CPU path."""
     from oracle import scene
