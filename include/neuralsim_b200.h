@@ -271,7 +271,8 @@ int nsb_query_counts(int64_t *counts, int32_t phase, int32_t n_coarse, const int
 int nsb_neus_upsample_cdf(const float *sdf, const float *depth, const int64_t *pack_infos, int64_t n_packs, float inv_s,
                           int use_estimate_alpha, float early_stop_eps, float alpha_thre, float *cdf, void *stream);
 /* packed_invert_cdf (pack_ops_cuda.cu:1634-1682) with ONE u[n_samples] row shared by every pack -> samples[n_packs, n_samples]
- * (what packed_sample_cdf(perturb=False) feeds it, graphics/raysample.py:38-61). */
+ * (what packed_sample_cdf(perturb=False) feeds it, graphics/raysample.py:38-61).  An empty pack's samples are NaN (bins / cdfs are
+ * not read for it; the reference's kernel reads bins[first], one past the pack). */
 int nsb_packed_invert_cdf_shared_u(const float *bins, const float *cdfs, const float *u, const int64_t *pack_infos, int64_t n_packs,
                                    int32_t n_samples, float *samples, void *stream);
 /* alpha[S] = neus_packed_sdf_to_alpha(sdf, *inv_s_dev) and, in the same pass, the compression selector / kept-count per pack

@@ -57,6 +57,7 @@ k_invert_cdf_shared_u(const float *__restrict__ bins, const float *__restrict__ 
         const int64_t p = t / n_s;
         const int64_t b = pi[2 * p];
         const uint32_t n = (uint32_t)pi[2 * p + 1];
+        if (n == 0) { samples[t] = __int_as_float(0x7fc00000); continue; }       // an empty pack has no bin to place u in: NaN, nothing read
         const float *bb = bins + b, *cc = cdfs + b;
         const float uu = u[t - p * n_s];
         uint32_t first = 0, count = n;                       // lower bound, clamped to n-1
@@ -64,7 +65,7 @@ k_invert_cdf_shared_u(const float *__restrict__ bins, const float *__restrict__ 
             const uint32_t step = count >> 1, it = first + step;
             if (cc[it] < uu) { first = it + 1; count -= step + 1; } else count = step;
         }
-        const uint32_t pos = n ? min(first, n - 1) : 0;
+        const uint32_t pos = min(first, n - 1);
         float r;
         if (pos == 0) r = bb[0];
         else {
