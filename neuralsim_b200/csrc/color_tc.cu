@@ -10,7 +10,7 @@
 //                    nablas = J^T g (J recomputed per level, never stored) -> radiance input row -> MMA -> relu -> MMA ->
 //                    relu -> 64->3 -> sigmoid.   Saves the fp16 activation tiles Z, X, Y1, Y2 in core-matrix layout.
 //   k_color_rad_bwd  radiance backward from the saved tiles: dZ2, dZ1 (MMA), dh (MMA), weight gradients accumulated in
-//                    shared memory over all tiles of the persistent CTA (MN-major MMAs contracting over the 128 points).
+//                    registers over all tiles of the persistent CTA (MN-major M64 MMAs contracting over the 128 points).
 //   k_color_sdf_bwd  gather pass for dg = J.dn, MMA du = dG.W1^T, MMA g = U.W1, dz (softplus'' term + sdf term),
 //                    MMA dh = dZ.W1, weight-gradient MMAs, one merged scatter (g (x) second-order weights + dh (x) trilinear
 //                    weights) into the fp32 table gradient.
@@ -90,6 +90,11 @@ __device__ __forceinline__ void unpack8(const uint4 &q, float (&v)[8]) {
 // The colour kernels run at 1-2 CTAs per SM (shared-memory bound), i.e. 4-8 warps: their gathers live on loads in flight PER THREAD, and
 // registers are plentiful -> four levels (32 corner loads) per gather trip instead of the two of k_fused_sdf_tc (which runs 24 warps per SM).
 constexpr int kColorGatherU = 4;
+
+// Resident CTAs per SM of the persistent grids of both colour backward kernels.  Their weight-gradient sums stay in registers (mma_m64)
+// and only the tiles the MMAs read live in shared memory (about 101 and 97 KB per CTA), so two CTAs fit an SM and the gather, MMA and
+// scatter phases of one overlap those of the other.  The launcher checks the occupancy calculator agrees (require_ctas_per_sm).
+constexpr int kColorBwdCtasPerSM = 2;
 
 // ===================================================================================================================== forward
 __global__ void __launch_bounds__(kTile)
@@ -278,12 +283,15 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 // T = [dZ2 | dZ1 | y2] (128 points x 192, three 16 KB blocks).  MMAs per tile:
 //   dY1 = dZ2 . R2                 (M128 N64 K64)    A = T block 0 (K-major),           B = R2^T tile
 //   dh  = dZ1 . R1[:, h columns]   (M128 N32 K64)    A = T block 1,                     B = R1h^T tile
-//   XA += [dZ2 | dZ1]^T . [Y1 | 1]           (M128 N72 K128, MN-major): rows 0..63  = [dR2 | drb2]
-//   XB += [dZ1 | y2 ]^T . [X | 1 gy3 0..]    (M128 N72 K128, MN-major): rows 0..63  = [dR1 | drb1], rows 64..127, cols 65..67 = dR3^T
+//   XA += dZ2^T . [Y1 | 1 | 0]               (M64 N80 K128, MN-major) = [dR2 | drb2]
+//   XB += dZ1^T . [X | 1 gy3 | 0]            (M64 N80 K128, MN-major) = [dR1 | drb1]
+//   X3 += y2^T  . [1 gy3 0..]                (M64 N8  K128, MN-major): cols 1..3 = dR3^T
+// XA, XB and X3 are register fragments carried over all tiles of the persistent CTA; the dY1 ReLU mask runs on the dY1 fragments, and
+// dh goes from its fragments straight to global memory, so the kernel stages no fp32 rows (~104 KB of shared memory: 2 CTAs / SM).
 // The three saved activation tiles of a point tile (X, Y1, Y2: 3 x 16 KB, each contiguous in global memory and in shared memory) are
 // fetched by the bulk async copy engine (cp.async.bulk -> mbarrier), issued by one thread; the fetch of the NEXT tile starts as soon
-// as the last MMA that reads the current tiles has completed, so it overlaps the epilogue, the dh store and the next prologue.
-__global__ void __launch_bounds__(kTile)
+// as the last MMA that reads the current tiles has completed, so it overlaps the dh store and the next prologue.
+__global__ void __launch_bounds__(kTile, kColorBwdCtasPerSM)
 k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uint8_t *__restrict__ Y1t, const uint8_t *__restrict__ Y2t,
                 const float *__restrict__ rgb, const float *__restrict__ g_rgb, int64_t n, float *__restrict__ dh_out,
                 float *__restrict__ dR1, float *__restrict__ drb1, float *__restrict__ dR2, float *__restrict__ drb2,
@@ -297,9 +305,6 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     uint8_t *sXe = sY1 + kTile * NE * 2;                       // 20 KB [X | 1 gy3 | 0]
     uint8_t *sR2T = sXe + kTile * NE * 2;                      //  8 KB (N = in i, K = out j) = R2[j][i]
     uint8_t *sR1h = sR2T + XW * XW * 2;                        //  4 KB (N = h column k, K = out j) = R1[j][22 + k]
-    constexpr uint32_t cDY1 = 0, cDH = 0, cXA = 64, cXB = 64 + NE;   // staged accumulator columns (dY1, then dh; XA, XB persist)
-    constexpr int kS = tc::acc_stride(64 + 2 * NE);
-    float *acc = reinterpret_cast<float *>(sR1h + NF * XW * 2); // 114 KB
     __shared__ float sR3[3][XW];
     __shared__ float sdb3[3];
     __shared__ __align__(8) uint64_t mbar_ld;
@@ -322,7 +327,11 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     *reinterpret_cast<uint4 *>(sY1 + 8 * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);       // [1, 0, ...]
     *reinterpret_cast<uint4 *>(sY1 + 9 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
     *reinterpret_cast<uint4 *>(sXe + 9 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
-    for (int c = cXA; c < cXB + NE; ++c) acc[tid * kS + c] = 0.f;
+    float xa[NE / 2], xb[NE / 2], x3[4];
+#pragma unroll
+    for (int k = 0; k < NE / 2; ++k) xa[k] = xb[k] = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) x3[k] = 0.f;
     if (tid == 0) {
         sdb3[0] = sdb3[1] = sdb3[2] = 0.f;
         tc::mbar_init(&mbar_ld, 1);
@@ -378,23 +387,29 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         }
         tc::fence_async_smem();
         __syncthreads();
-        tc::mma_to_rows<64, 0, 0, XW / 16>(acc, kS, cDY1, tc::kmajor(t_addr, kTile), tc::kmajor(r2t_addr, XW), false);   // dY1 = dZ2 . R2
-        __syncthreads();
-#pragma unroll 1
-        for (int c = 0; c < 8; ++c) {
-            float dy[8], y1[8];
-            tc::acc_ld8(acc, kS, tid, cDY1 + c * 8, dy);
-            unpack8(*reinterpret_cast<const uint4 *>(sY1 + c * kChunk + tid * 16), y1);
+        {
+            float dy[2][XW / 2];
+            tc::mma_m128<64, 0, 0, XW / 16>(dy, tc::kmajor(t_addr, kTile), tc::kmajor(r2t_addr, XW), false);   // dY1 = dZ2 . R2
+            // dZ1 = dY1 masked by Y1 > 0, on the fragments: T block 1 is read by no MMA in flight
 #pragma unroll
-            for (int j = 0; j < 8; ++j) dy[j] = y1[j] > 0.f ? dy[j] : 0.f;
-            *reinterpret_cast<uint4 *>(sT + kTileBytes + c * kChunk + tid * 16) = tc::pack8_f16(dy);
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int c = 0; c < XW / 8; ++c)
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        const uint32_t off = tc::pair_off<kTile>(h * 64 + tc::frag_row(r), tc::frag_col(c));
+                        const float2 y1 = tc::ld_pair_f16(sY1, off);
+                        tc::st_pair_f16(sT + kTileBytes, off, y1.x > 0.f ? dy[h][4 * c + 2 * r] : 0.f, y1.y > 0.f ? dy[h][4 * c + 2 * r + 1] : 0.f);
+                    }
         }
         tc::fence_async_smem();
         __syncthreads();
-        tc::mma_to_rows<32, 0, 0, XW / 16>(acc, kS, cDH, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(r1h_addr, NF), false);   // dh = dZ1 . R1[:, h]
+        float dh[2][NF / 2];
+        tc::mma_m128<32, 0, 0, XW / 16>(dh, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(r1h_addr, NF), false);   // dh = dZ1 . R1[:, h]
         // weight gradients: contract over the 128 points
-        tc::mma_to_rows<NE, 1, 1, kTile / 16>(acc, kS, cXA, tc::mnmajor(t_addr, kTile), tc::mnmajor(y1_addr, kTile), true);
-        tc::mma_to_rows<NE, 1, 1, kTile / 16>(acc, kS, cXB, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(xe_addr, kTile), true);
+        tc::mma_m64<NE, 1, 1, kTile / 16>(xa, tc::mnmajor(t_addr, kTile), tc::mnmajor(y1_addr, kTile), true);
+        tc::mma_m64<NE, 1, 1, kTile / 16>(xb, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(xe_addr, kTile), true);
+        tc::mma_m64<8, 1, 1, kTile / 16>(x3, tc::mnmajor(t_addr + 2 * kTileBytes, kTile), tc::mnmajor(xe_addr + 8 * kChunk, kTile), true);
         first_tile = false;
         __syncthreads();
         if (tid == 0 && tile + gridDim.x < n_tiles) {
@@ -403,39 +418,44 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
             tc::fence_async_smem();
             fetch(tile + gridDim.x);
         }
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-            float dh[8];
-            tc::acc_ld8(acc, kS, tid, cDH + c * 8, dh);
-            if (valid) {
-                *reinterpret_cast<float4 *>(dh_out + i * NF + c * 8) = make_float4(dh[0], dh[1], dh[2], dh[3]);
-                *reinterpret_cast<float4 *>(dh_out + i * NF + c * 8 + 4) = make_float4(dh[4], dh[5], dh[6], dh[7]);
+        // dh from the fragments: the four lanes of a row write its 32 contiguous bytes of a chunk.  No shared memory is read after the
+        // barrier above, so the next iteration may overwrite T right away.
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int64_t row = tile * kTile + h * 64 + tc::frag_row(r);
+                if (row < n) {
+#pragma unroll
+                    for (int c = 0; c < NF / 8; ++c)
+                        *reinterpret_cast<float2 *>(dh_out + row * NF + tc::frag_col(c)) = make_float2(dh[h][4 * c + 2 * r], dh[h][4 * c + 2 * r + 1]);
+                }
             }
-        }
-        __syncthreads();
     }
     if (!first_tile) {
-#pragma unroll 1
-        for (int c = 0; c < 9; ++c) {
-            float a[8], b[8];
-            tc::acc_ld8(acc, kS, tid, cXA + c * 8, a);
-            tc::acc_ld8(acc, kS, tid, cXB + c * 8, b);
-            if (tid < net.rw) {
-                if (c < 8) {
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) {
-                        const int col = c * 8 + k;
-                        if (col < net.rw) atomicAdd(dR2 + tid * net.rw + col, a[k]);
+        for (int r = 0; r < 2; ++r) {
+            const int row = tc::frag_row(r);
+            if (row >= net.rw) continue;
+#pragma unroll
+            for (int c = 0; c < NE / 8; ++c)
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const int col = tc::frag_col(c) + j;
+                    const float a = xa[4 * c + 2 * r + j], b = xb[4 * c + 2 * r + j];
+                    if (col < XW) {
+                        if (col < net.rw) atomicAdd(dR2 + row * net.rw + col, a);
                         const int rc = ref_col(col, net.n_appear);
-                        if (rc >= 0) atomicAdd(dR1 + tid * net.rin + rc, b[k]);
+                        if (rc >= 0) atomicAdd(dR1 + row * net.rin + rc, b);
+                    } else if (col == XW) {
+                        atomicAdd(drb2 + row, a);
+                        atomicAdd(drb1 + row, b);
                     }
-                } else {
-                    atomicAdd(drb2 + tid, a[0]);
-                    atomicAdd(drb1 + tid, b[0]);
                 }
-            } else if (tid >= XW && tid - XW < net.rw && c == 8) {
 #pragma unroll
-                for (int k = 0; k < 3; ++k) atomicAdd(dR3 + k * net.rw + (tid - XW), b[1 + k]);
+            for (int j = 0; j < 2; ++j) {
+                const int col = tc::frag_col(0) + j;
+                if (col >= 1 && col <= 3) atomicAdd(dR3 + (col - 1) * net.rw + row, x3[2 * r + j]);
             }
         }
         if (tid < 3) atomicAdd(drb3 + tid, sdb3[tid]);
@@ -448,13 +468,17 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
 //   du = dG . W1^T (M128 N64 K32);  g = U . W1 (M128 N32 K64)
 //   dz_j = fp16(du_j) w2_j beta s_j (1 - s_j) + dsdf w2_j s_j ;  v_j = fp16(du_j) s_j + dsdf a16_j
 //   dhz = dZ . W1 (M128 N32 K64)
-//   X1 += [dz | u]^T . [H | 1]   rows 0..63 = [dW1 (z part) | db1]
-//   X2 += [u | v]^T . [dG | 1]   rows 0..63, cols 0..31 = dW1 (second-order part);  rows 64..127, col 32 = dW2
+//   W  += dz^T . [H | 1 | 0]     (M64 N48 K128, MN-major) = [dW1 (z part) | db1]
+//   W[:, 0..31] += u^T . dG      (M64 N32 K128, MN-major): dW1 (second-order part); N = 32 keeps sum(u) out of db1
+//   V  += v^T . [1 0..]          (M64 N8  K128, MN-major): col 0 = dW2
 //   scatter per level / corner:  g_f * wsum_c(gin) + (dhz_f + dh_r_f) * w_c
+// W and V are register fragments carried over all tiles of the persistent CTA, dz and v are computed on the du fragments, and only g and
+// dhz -- the scatter needs a point's whole row of them -- are staged as fp32 rows, in T once its last MMA has completed (~97 KB of
+// shared memory: 2 CTAs / SM).
 // The saved Z tile (16 KB) and the H half of the saved X tile (8 KB) are fetched by the bulk async copy engine into shared memory, and
 // the NEXT tile's fetch is issued right after the last MMA of the current tile -- it runs behind the whole scatter phase.  (Reading Z
 // straight from global memory in the two epilogue loops costs 16 dependent round trips per tile at 8 warps per SM.)
-__global__ void __launch_bounds__(kTile)
+__global__ void __launch_bounds__(kTile, kColorBwdCtasPerSM)
 k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev net, const PointSrc ps, const uint8_t *__restrict__ Zt,
                 const uint8_t *__restrict__ Xt, const float *__restrict__ g_nab, const float *__restrict__ g_sdf, const float *__restrict__ dh_r,
                 int64_t n, int max_level, float *__restrict__ d_grid, float *__restrict__ d_W1, float *__restrict__ d_b1, float *__restrict__ d_W2,
@@ -469,10 +493,10 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
     uint8_t *sW1 = sGe + kTile * NX * 2;                       //  4 KB
     uint8_t *sW1T = sW1 + HW * NF * 2;                         //  4 KB
     uint8_t *sZ = sW1T + NF * HW * 2;                          // 16 KB saved pre-activations
-    constexpr uint32_t cDU = 0, cDHZ = 0, cG = 64, cX1 = 96, cX2 = 96 + NX;   // staged accumulator columns (du, then dhz; X1, X2 persist)
-    constexpr int kS = tc::acc_stride(96 + 2 * NX);
-    float *acc = reinterpret_cast<float *>(sZ + kTileBytes);   // 98 KB
-    __shared__ float sW2[HW];
+    constexpr int kS = tc::acc_stride(2 * NF);                 // staged rows [g | dhz] for the scatter: 34 KB, aliasing T
+    float *stage = reinterpret_cast<float *>(sT);
+    static_assert(kTile * kS * 4 <= 3 * kTileBytes, "the staged rows must fit in T");
+    __shared__ float sW2[HW], sdsdf[kTile];
     __shared__ float sdb2;
     __shared__ __align__(8) uint64_t mbar_ld;
 
@@ -484,7 +508,11 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
     *reinterpret_cast<uint4 *>(sGe + 4 * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);
     *reinterpret_cast<uint4 *>(sHe + 5 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
     *reinterpret_cast<uint4 *>(sGe + 5 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
-    for (int c = cX1; c < cX2 + NX; ++c) acc[tid * kS + c] = 0.f;
+    float wacc[NX / 2], vacc[4];
+#pragma unroll
+    for (int k = 0; k < NX / 2; ++k) wacc[k] = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) vacc[k] = 0.f;
     if (tid == 0) {
         sdb2 = 0.f;
         tc::mbar_init(&mbar_ld, 1);
@@ -517,6 +545,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
             for (int d = 0; d < 3; ++d) gin[d] = g_nab[i * 3 + d] * net.fac[d] * 0.5f;
         }
         const float dsdf = (valid && g_sdf) ? g_sdf[i] : 0.f;
+        sdsdf[tid] = dsdf;                                    // read by the fragment owners of my row
         tc::mbar_wait(&mbar_ld, ld_phase);                    // this tile's Z and H have landed
         ld_phase ^= 1;
         // u = fp16(w2 s)
@@ -549,31 +578,46 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         }
         tc::fence_async_smem();
         __syncthreads();
-        tc::mma_to_rows<64, 0, 0, NF / 16>(acc, kS, cDU, tc::kmajor(ge_addr, kTile), tc::kmajor(w1_addr, HW), false);                // du = dG . W1^T
-        tc::mma_to_rows<32, 0, 0, HW / 16>(acc, kS, cG, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(w1t_addr, NF), false);    // g = U . W1
-        __syncthreads();
-#pragma unroll 1
-        for (int c = 0; c < 8; ++c) {
-            float du[8], z[8], dz[8], vv[8];
-            tc::acc_ld8(acc, kS, tid, cDU + c * 8, du);
-            unpack8(*reinterpret_cast<const uint4 *>(sZ + c * kChunk + tid * 16), z);
+        float gfr[2][NF / 2];
+        {
+            float du[2][HW / 2];
+            tc::mma_m128<64, 0, 0, NF / 16>(du, tc::kmajor(ge_addr, kTile), tc::kmajor(w1_addr, HW), false);                  // du = dG . W1^T
+            tc::mma_m128<32, 0, 0, HW / 16>(gfr, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(w1t_addr, NF), false);   // g = U . W1
+            // dz -> T block 0, v -> T block 2, on the du fragments (no MMA in flight reads those blocks)
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                float a, s;
-                softplus_as(z[j], spk, a, s);
-                const float w2 = sW2[c * 8 + j], d = r16(du[j]);
-                const float curv = (z[j] * spk.k > spk.thr) ? 0.f : spk.beta * s * (1.f - s);
-                dz[j] = d * w2 * curv + dsdf * w2 * s;
-                vv[j] = d * s + dsdf * r16(a);
-            }
-            *reinterpret_cast<uint4 *>(sT + c * kChunk + tid * 16) = tc::pack8_f16(dz);
-            *reinterpret_cast<uint4 *>(sT + 2 * kTileBytes + c * kChunk + tid * 16) = tc::pack8_f16(vv);
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int row = h * 64 + tc::frag_row(r);
+                    const float ds = sdsdf[row];
+#pragma unroll
+                    for (int c = 0; c < HW / 8; ++c) {
+                        const int col = tc::frag_col(c);
+                        const uint32_t off = tc::pair_off<kTile>(row, col);
+                        const float2 z2 = tc::ld_pair_f16(sZ, off);
+                        float dz[2], vv[2];
+#pragma unroll
+                        for (int j = 0; j < 2; ++j) {
+                            const float z = j ? z2.y : z2.x;
+                            float a, s;
+                            softplus_as(z, spk, a, s);
+                            const float w2 = sW2[col + j], d = r16(du[h][4 * c + 2 * r + j]);
+                            const float curv = (z * spk.k > spk.thr) ? 0.f : spk.beta * s * (1.f - s);
+                            dz[j] = d * w2 * curv + ds * w2 * s;
+                            vv[j] = d * s + ds * r16(a);
+                        }
+                        tc::st_pair_f16(sT, off, dz[0], dz[1]);
+                        tc::st_pair_f16(sT + 2 * kTileBytes, off, vv[0], vv[1]);
+                    }
+                }
         }
         tc::fence_async_smem();
         __syncthreads();
-        tc::mma_to_rows<32, 0, 0, HW / 16>(acc, kS, cDHZ, tc::kmajor(t_addr, kTile), tc::kmajor(w1t_addr, NF), false);               // dhz = dZ . W1
-        tc::mma_to_rows<NX, 1, 1, kTile / 16>(acc, kS, cX1, tc::mnmajor(t_addr, kTile), tc::mnmajor(he_addr, kTile), true);
-        tc::mma_to_rows<NX, 1, 1, kTile / 16>(acc, kS, cX2, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(ge_addr, kTile), true);
+        float dhz[2][NF / 2];
+        tc::mma_m128<32, 0, 0, HW / 16>(dhz, tc::kmajor(t_addr, kTile), tc::kmajor(w1t_addr, NF), false);                        // dhz = dZ . W1
+        tc::mma_m64<NX, 1, 1, kTile / 16>(wacc, tc::mnmajor(t_addr, kTile), tc::mnmajor(he_addr, kTile), true);
+        tc::mma_m64<NF, 1, 1, kTile / 16>(*reinterpret_cast<float(*)[NF / 2]>(wacc), tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(ge_addr, kTile), true);
+        tc::mma_m64<8, 1, 1, kTile / 16>(vacc, tc::mnmajor(t_addr + 2 * kTileBytes, kTile), tc::mnmajor(ge_addr + 4 * kChunk, kTile), true);
         first_tile = false;
         const float dsum = warp_sum(dsdf);
         if (lane == 0 && dsum != 0.f) atomicAdd(&sdb2, dsum);
@@ -583,12 +627,16 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
             tc::fence_async_smem();
             fetch(tile + gridDim.x);
         }
+        // T is free (its MMAs have completed before the barrier above): stage the rows of g and dhz there for the scatter
+        tc::frag_store<NF>(gfr, stage, kS, 0);
+        tc::frag_store<NF>(dhz, stage, kS, NF);
+        __syncthreads();
         // ---- merged scatter
 #pragma unroll 1
         for (uint32_t g4 = 0; g4 < 4; ++g4) {
             float gg[8], hz[8];
-            tc::acc_ld8(acc, kS, tid, cG + g4 * 8, gg);
-            tc::acc_ld8(acc, kS, tid, cDHZ + g4 * 8, hz);
+            tc::acc_ld8(stage, kS, tid, g4 * 8, gg);
+            tc::acc_ld8(stage, kS, tid, NF + g4 * 8, hz);
             if (valid && dh_r) {
                 const float4 r0 = *reinterpret_cast<const float4 *>(dh_r + i * NF + g4 * 8), r1 = *reinterpret_cast<const float4 *>(dh_r + i * NF + g4 * 8 + 4);
                 hz[0] += r0.x; hz[1] += r0.y; hz[2] += r0.z; hz[3] += r0.w; hz[4] += r1.x; hz[5] += r1.y; hz[6] += r1.z; hz[7] += r1.w;
@@ -630,21 +678,20 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         __syncthreads();
     }
     if (!first_tile) {
-#pragma unroll 1
-        for (int c = 0; c < NF / 8; ++c) {
-            float a[8], b[8];
-            tc::acc_ld8(acc, kS, tid, cX1 + c * 8, a);
-            tc::acc_ld8(acc, kS, tid, cX2 + c * 8, b);
-            if (tid < net.dec.width) {
 #pragma unroll
-                for (int k = 0; k < 8; ++k) atomicAdd(d_W1 + tid * NF + c * 8 + k, a[k] + b[k]);
-            }
+        for (int r = 0; r < 2; ++r) {
+            const int row = tc::frag_row(r);
+            if (row >= net.dec.width) continue;
+#pragma unroll
+            for (int c = 0; c <= NF / 8; ++c)
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const int col = tc::frag_col(c) + j;
+                    if (col < NF) atomicAdd(d_W1 + row * NF + col, wacc[4 * c + 2 * r + j]);
+                    else if (col == NF) atomicAdd(d_b1 + row, wacc[4 * c + 2 * r + j]);
+                }
+            if (tc::frag_col(0) == 0) atomicAdd(d_W2 + row, vacc[2 * r]);
         }
-        float a1[8], b1[8];
-        tc::acc_ld8(acc, kS, tid, cX1 + 32, a1);
-        tc::acc_ld8(acc, kS, tid, cX2 + 32, b1);
-        if (tid < HW) { if (tid < net.dec.width) atomicAdd(d_b1 + tid, a1[0]); }
-        else if (tid - HW < net.dec.width) atomicAdd(d_W2 + (tid - HW), b1[0]);
         if (tid == 0) atomicAdd(d_b2, sdb2);
     }
 }
@@ -712,17 +759,20 @@ extern "C" int nsb_fused_color_bwd(const nsb_lotd_meta *meta, const void *params
     cudaStream_t s = (cudaStream_t)stream;
     const float *dh = nullptr;
     if (g_rgb) {
-        constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + kTile * tc::acc_stride(64 + 2 * 80) * 4 + 1024;   // 1 CTA / SM
+        constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + 1024;   // 101 KB
         opt_in_smem(k_color_rad_bwd, kSmemR);
-        k_color_rad_bwd<<<persistent_grid(n_tiles(n), 1), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb,
-                                                                              g_rgb, n, dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, dn.a);
+        if (int rc = require_ctas_per_sm(k_color_rad_bwd, kTile, kSmemR, kColorBwdCtasPerSM, "nsb_fused_color_bwd(radiance)")) return rc;
+        k_color_rad_bwd<<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1,
+                                                                                               (const uint8_t *)act_y2, rgb, g_rgb, n, dh_scratch, d_R1,
+                                                                                               d_rb1, d_R2, d_rb2, d_R3, d_rb3, dn.a);
         if (int rc = check_launch("nsb_fused_color_bwd(radiance)")) return rc;
         dh = dh_scratch;
     }
-    constexpr int kSmemS = 3 * kTileBytes + 2 * kTile * 48 * 2 + 2 * HW * NF * 2 + kTileBytes + kTile * tc::acc_stride(96 + 2 * 48) * 4 + 1024;   // 1 CTA / SM
+    constexpr int kSmemS = 3 * kTileBytes + 2 * kTile * 48 * 2 + 2 * HW * NF * 2 + kTileBytes + 1024;   // 97 KB
     opt_in_smem(k_color_sdf_bwd, kSmemS);
+    if (int rc = require_ctas_per_sm(k_color_sdf_bwd, kTile, kSmemS, kColorBwdCtasPerSM, "nsb_fused_color_bwd(sdf)")) return rc;
     const PointSrc ps{x, rays_o, rays_d, t, ridx};
-    k_color_sdf_bwd<<<persistent_grid(n_tiles(n), 1), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
+    k_color_sdf_bwd<<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
                                                                           g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level, d_grid, d_W1, d_b1, d_W2, d_b2, dn.a);
     return check_launch("nsb_fused_color_bwd(sdf)");
 }

@@ -3,6 +3,7 @@
 
 #include <map>
 #include <mutex>
+#include <tuple>
 #include <utility>
 
 #include "nsb_common.cuh"
@@ -39,6 +40,25 @@ bool smem_opt_in_needed(const void *kernel, int dev, int bytes) {
     if (g >= bytes) return false;
     g = bytes;
     return true;
+}
+
+int max_active_ctas(const void *kernel, int dev, int block, int smem_bytes) {
+    static std::mutex mu;
+    static std::map<std::tuple<const void *, int, int, int>, int> known;
+    const auto key = std::make_tuple(kernel, dev, block, smem_bytes);
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        const auto it = known.find(key);
+        if (it != known.end()) return it->second;
+    }
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, block, (size_t)smem_bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;                  // not cached: the caller reports it, and a later call asks again
+    }
+    std::lock_guard<std::mutex> lock(mu);
+    known[key] = n;
+    return n;
 }
 }  // namespace nsb
 

@@ -86,18 +86,24 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
 
 // =====================================================================================================================
 // Backward of forward_sdf wrt. the LoTD table and the decoder weights, one kernel, nothing saved by the forward.
-// Per tile of 128 points (thread r = point r = staged accumulator row r), d = dL/dsdf[r]:
-//   recompute  gather -> A tile [H | 1 | 0..];  MMA1: Z = H.W1^T (staged cols 0..63);  z = fp16(Z + b1); s = sigmoid(beta z), a = fp16(softplus)
-//   row r of the G tile [128 x 128] fp16 :=  [ dz_0..dz_63 | d*a_0..d*a_63 ],  dz_j = d * w2_j * s_j
+// Per tile of 128 points (thread r = point r for the gather and the scatter), d = dL/dsdf[r]:
+//   recompute  gather -> A tile [H | 1 | 0..];  MMA1: Z = H.W1^T (registers);  z = fp16(Z + b1); s = sigmoid(beta z), a = fp16(softplus)
+//   G tile [128 x 128] fp16 :=  [ dz_0..dz_63 | d*a_0..d*a_63 ],  dz_j = d * w2_j * s_j, written from the Z fragments
 //              (the reference rounds grad_z to fp16 at the same place, layers.py autocast backward)
-//   MMA2: dH[128 x 32]  = dZ . W1                 A = G cols 0..63 (K-major), B = W1^T tile          -> staged cols 0..31
-//   MMA3: X[128 x 40]  += G^T . [H | 1 | 0..]     both operands are the tiles above read MN-major, K = the 128 points;
-//              rows 0..63 of X = [ dW1 | db1 ], rows 64..127, column 32 = dW2; accumulated over all tiles of the
-//              persistent CTA in staged cols 64..103
-//   scatter dH into the fp32 table gradient (8 corners x 16 levels, red.global.add.v2.f32);  db2 via a warp sum.
+//   MMA2: dH[128 x 32]  = dZ . W1                 A = G cols 0..63 (K-major), B = W1^T tile          -> registers
+//   MMA3: X[64 x 40]   += dZ^T . [H | 1 | 0..]    both operands are the tiles above read MN-major, K = the 128 points: [ dW1 | db1 ]
+//   MMA4: V[64 x 8]    += (d*a)^T . [1 0..]       column 0 = dW2
+//              X and V are register fragments carried over all tiles of the persistent CTA
+//   dH staged as fp32 rows in G (free once the MMAs have completed) -> scatter into the fp32 table gradient (8 corners x 16 levels,
+//   red.global.add.v2.f32);  db2 via a warp sum.
 // =====================================================================================================================
+// Resident CTAs per SM of the persistent grid of k_sdf_bwd_tc: 51 KB of shared memory and 120 registers fit four.  On an H100
+// (NVIDIA H100 80GB HBM3, 400 W power limit) the kernel took 2.43 / 2.43 ms per bench step at 2 CTAs / SM, 2.24 / 2.19 ms at 3 and
+// 2.16 / 2.13 ms at 4 (profiles/bwd_kernels.py, the three builds alternated in one run; 2.48 ms before its sums moved to registers).
+constexpr int kSdfBwdCtasPerSM = 4;
+
 template <bool FROM_RAYS>
-__global__ void __launch_bounds__(kTile)
+__global__ void __launch_bounds__(kTile, kSdfBwdCtasPerSM)
 k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ x,
              const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
              const float *__restrict__ t, const float *__restrict__ d_sdf, int64_t n, int max_level, float *__restrict__ d_grid,
@@ -105,15 +111,16 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
              const int64_t *__restrict__ keep, const int64_t *__restrict__ n_dev) {
     n = eff_n(n, n_dev);
     constexpr int NX = 40, GW = 128;                          // NX: features + [1,0,..] chunk; GW: dz | d*a
-    constexpr int kCols = HW + NX, kS = tc::acc_stride(kCols);  // staged accumulators: Z / dH in cols 0..63, X in cols 64..103
-    extern __shared__ uint8_t dyn_smem[];                     // 104 KB of tiles and staged accumulators (> the 48 KB static limit)
+    constexpr int kS = tc::acc_stride(NF);                    // staged dH rows for the scatter: 18 KB, aliasing G
+    extern __shared__ uint8_t dyn_smem[];                     // 50 KB of tiles (> the 48 KB static limit)
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 127) & ~uintptr_t(127));
     uint8_t *sA = tiles;                                      // 10 KB : [H | 1 | 0..]
     uint8_t *sG = sA + kTile * NX * 2;                        // 32 KB : [dz | d*a]
     uint8_t *sB = sG + kTile * GW * 2;                        //  4 KB : W1   [64 x 32]  (B of MMA1)
     uint8_t *sBT = sB + HW * NF * 2;                          //  4 KB : W1^T [32 x 64]  (B of MMA2)
-    float *acc = reinterpret_cast<float *>(sBT + NF * HW * 2);   // 54 KB : [128 x kS] fp32
-    __shared__ float sb1[HW], sW2[HW];
+    float *stage = reinterpret_cast<float *>(sG);
+    static_assert(kTile * kS * 4 <= kTile * GW * 2, "the staged dH rows must fit in G");
+    __shared__ float sb1[HW], sW2[HW], sdd[kTile];
     __shared__ float sdb2;
 
     const int tid = threadIdx.x, lane = tid & 31;
@@ -121,7 +128,11 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
     stage_W1T(dec, sBT, tid);
     stage_decoder_vectors(dec, sb1, sW2, nullptr, tid);
     *reinterpret_cast<uint4 *>(sA + 4 * (kTile * 16) + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);   // constant chunk: [1,0,..]
-    for (int c = HW; c < kCols; ++c) acc[tid * kS + c] = 0.f;
+    float xacc[NX / 2], vacc[4];
+#pragma unroll
+    for (int k = 0; k < NX / 2; ++k) xacc[k] = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) vacc[k] = 0.f;
     if (tid == 0) sdb2 = 0.f;
     tc::fence_async_smem();
     __syncthreads();
@@ -137,34 +148,48 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         float xs[3];
         load_point(PointSrc{x, rays_o, rays_d, t, ridx}, FROM_RAYS, i, valid, xs);
         const float dd = valid ? d_sdf[i] : 0.f;
+        sdd[tid] = dd;                                           // read by the fragment owners of my row
         gather_row_to_tile<kTile>(m, grid, xs, max_level, sA, tid);
         tc::fence_async_smem();
         __syncthreads();
-        tc::mma_to_rows<HW, 0, 0, NF / 16>(acc, kS, 0, tc::kmajor(a_addr, kTile), tc::kmajor(b_addr, HW), false);   // Z = H . W1^T
-        __syncthreads();
-        // ---- my G row: dz (chunks 0..7) and d*a (chunks 8..15)
-#pragma unroll 1
-        for (int c = 0; c < HW / 8; ++c) {
-            float z[8], dz[8], da[8];
-            tc::acc_ld8(acc, kS, tid, c * 8, z);
+        {
+            float z[2][HW / 2];
+            tc::mma_m128<HW, 0, 0, NF / 16>(z, tc::kmajor(a_addr, kTile), tc::kmajor(b_addr, HW), false);   // Z = H . W1^T
+            // ---- G on the Z fragments: dz (chunks 0..7) and d*a (chunks 8..15); G is read by no MMA in flight
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float zz = r16(z[j] + sb1[c * 8 + j]);
-                float a, s;
-                softplus_as(zz, spk, a, s);
-                da[j] = dd * r16(a);
-                dz[j] = dd * sW2[c * 8 + j] * s;
-            }
-            *reinterpret_cast<uint4 *>(sG + c * (kTile * 16) + tid * 16) = tc::pack8_f16(dz);
-            *reinterpret_cast<uint4 *>(sG + (8 + c) * (kTile * 16) + tid * 16) = tc::pack8_f16(da);
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int row = h * 64 + tc::frag_row(r);
+                    const float d = sdd[row];
+#pragma unroll
+                    for (int c = 0; c < HW / 8; ++c) {
+                        const int col = tc::frag_col(c);
+                        float dz[2], da[2];
+#pragma unroll
+                        for (int j = 0; j < 2; ++j) {
+                            const float zz = r16(z[h][4 * c + 2 * r + j] + sb1[col + j]);
+                            float a, s;
+                            softplus_as(zz, spk, a, s);
+                            da[j] = d * r16(a);
+                            dz[j] = d * sW2[col + j] * s;
+                        }
+                        tc::st_pair_f16(sG, tc::pair_off<kTile>(row, col), dz[0], dz[1]);
+                        tc::st_pair_f16(sG, tc::pair_off<kTile>(row, HW + col), da[0], da[1]);
+                    }
+                }
         }
         tc::fence_async_smem();
-        __syncthreads();                                         // every thread has read Z and written its G row
-        tc::mma_to_rows<NF, 0, 0, HW / 16>(acc, kS, 0, tc::kmajor(g_addr, kTile), tc::kmajor(bt_addr, NF), false);          // dH = dZ . W1 : K = 64 hidden
-        tc::mma_to_rows<NX, 1, 1, kTile / 16>(acc, kS, HW, tc::mnmajor(g_addr, kTile), tc::mnmajor(a_addr, kTile), true);   // X += G^T . [H|1] : K = 128 points
+        __syncthreads();                                         // G is complete
+        float dh_fr[2][NF / 2];
+        tc::mma_m128<NF, 0, 0, HW / 16>(dh_fr, tc::kmajor(g_addr, kTile), tc::kmajor(bt_addr, NF), false);                          // dH = dZ . W1 : K = 64 hidden
+        tc::mma_m64<NX, 1, 1, kTile / 16>(xacc, tc::mnmajor(g_addr, kTile), tc::mnmajor(a_addr, kTile), true);                      // X += dZ^T . [H|1] : K = 128 points
+        tc::mma_m64<8, 1, 1, kTile / 16>(vacc, tc::mnmajor(g_addr + 8 * (kTile * 16), kTile), tc::mnmajor(a_addr + 4 * (kTile * 16), kTile), true);   // V += (d*a)^T . 1
         first_tile = false;
         const float dsum = warp_sum(dd);
         if (lane == 0 && dsum != 0.f) atomicAdd(&sdb2, dsum);
+        __syncthreads();                                         // the MMAs reading G have completed
+        tc::frag_store<NF>(dh_fr, stage, kS, 0);
         __syncthreads();
         // ---- my dH row -> scatter into the table gradient; only the reductions are predicated on "this point carries gradient".
         const bool active = valid && dd != 0.f;
@@ -172,7 +197,7 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
 #pragma unroll 1
         for (uint32_t g4 = 0; g4 < 4; ++g4) {
             float dh[8];
-            tc::acc_ld8(acc, kS, tid, g4 * 8, dh);                  // 4 levels x 2 features
+            tc::acc_ld8(stage, kS, tid, g4 * 8, dh);                // 4 levels x 2 features
             if (!warp_active) continue;
 #pragma unroll
             for (uint32_t q = 0; q < 4; ++q) {
@@ -195,21 +220,22 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         }
         __syncthreads();                                         // tiles + staged rows free for the next iteration
     }
-    // ---- flush the CTA's weight-gradient accumulators: X rows 0..63 = [dW1 | db1], rows 64..127 col 32 = dW2
+    // ---- flush the CTA's weight-gradient accumulators: X = [dW1 | db1], V column 0 = dW2
     if (!first_tile) {                                           // uniform per CTA
-#pragma unroll 1
-        for (int c = 0; c < NF / 8; ++c) {
-            float r[8];
-            tc::acc_ld8(acc, kS, tid, HW + c * 8, r);
-            if (tid < dec.width) {
 #pragma unroll
-                for (int k = 0; k < 8; ++k) atomicAdd(d_W1 + tid * NF + c * 8 + k, r[k]);
-            }
+        for (int r = 0; r < 2; ++r) {
+            const int row = tc::frag_row(r);
+            if (row >= dec.width) continue;
+#pragma unroll
+            for (int c = 0; c <= NF / 8; ++c)
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const int col = tc::frag_col(c) + j;
+                    if (col < NF) atomicAdd(d_W1 + row * NF + col, xacc[4 * c + 2 * r + j]);
+                    else if (col == NF) atomicAdd(d_b1 + row, xacc[4 * c + 2 * r + j]);
+                }
+            if (tc::frag_col(0) == 0) atomicAdd(d_W2 + row, vacc[2 * r]);
         }
-        float r1[8];
-        tc::acc_ld8(acc, kS, tid, HW + 32, r1);
-        if (tid < HW) { if (tid < dec.width) atomicAdd(d_b1 + tid, r1[0]); }
-        else if (tid - HW < dec.width) atomicAdd(d_W2 + (tid - HW), r1[0]);
         if (tid == 0) atomicAdd(d_b2, sdb2);
     }
 }
@@ -266,10 +292,12 @@ extern "C" int nsb_fused_sdf_bwd_indexed(const nsb_lotd_meta *meta, const void *
     PLMeta m;
     DecoderDevTC d;
     if (int rc = make_decoder(meta, dec, &m, &d, "nsb_fused_sdf_bwd")) return rc;
-    constexpr int kBwdSmem = (128 * 40 + 128 * 128 + 64 * 32 + 32 * 64) * 2 + 128 * tc::acc_stride(64 + 40) * 4 + 128;
+    constexpr int kBwdSmem = (128 * 40 + 128 * 128 + 64 * 32 + 32 * 64) * 2 + 128;       // 50 KB
     opt_in_smem(k_sdf_bwd_tc<true>, kBwdSmem);
     opt_in_smem(k_sdf_bwd_tc<false>, kBwdSmem);
-    const unsigned grid = persistent_grid((n + kTile - 1) / kTile, 2);     // shared memory: 2 x 104 KB per SM
+    if (int rc = require_ctas_per_sm(x == nullptr ? k_sdf_bwd_tc<true> : k_sdf_bwd_tc<false>, kTile, kBwdSmem, kSdfBwdCtasPerSM, "nsb_fused_sdf_bwd"))
+        return rc;
+    const unsigned grid = persistent_grid((n + kTile - 1) / kTile, kSdfBwdCtasPerSM);
     cudaStream_t s = (cudaStream_t)stream;
     const int ml = max_level < 0 ? -1 : max_level;
     if (x == nullptr) k_sdf_bwd_tc<true><<<grid, kTile, kBwdSmem, s>>>(m, (const __half *)params_half, d, nullptr, rays_o, rays_d, ridx, t, d_sdf, n, ml,

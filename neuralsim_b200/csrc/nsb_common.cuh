@@ -62,6 +62,18 @@ inline void opt_in_smem(K kernel, int bytes) {
         cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
 
+// Resident CTAs per SM of `kernel` at this block size and dynamic shared memory (cudaOccupancyMaxActiveBlocksPerMultiprocessor), computed
+// once per (kernel, device, block, bytes); common.cu.  Call it after opt_in_smem.
+int max_active_ctas(const void *kernel, int dev, int block, int smem_bytes);
+// A persistent grid sized for `ctas` resident CTAs per SM whose kernel fits fewer would run as serial waves, silently slower.  0 if the
+// occupancy calculator agrees, else 2 with the error set.
+template <typename K>
+inline int require_ctas_per_sm(K kernel, int block, int smem_bytes, int ctas, const char *who) {
+    const int got = max_active_ctas(reinterpret_cast<const void *>(kernel), current_device(), block, smem_bytes);
+    NSB_REQUIRE(got >= ctas, "%s: %d CTAs per SM fit with %d bytes of dynamic shared memory, the persistent grid assumes %d", who, got, smem_bytes, ctas);
+    return 0;
+}
+
 // Device-resident counts (nsb_bind_device_counts, include/neuralsim_b200.h): the entry points that support them take the binding of the
 // calling thread; the kernels then process min(n_arg, *count) items, n_arg being the capacity the launch was sized for.
 struct DevCounts { const int64_t *a, *b; };

@@ -15,7 +15,8 @@
 // A 128-row tile is two m64 wgmma row blocks.  The accumulator of rows [64h, 64h + 64) lives in d[h][] in the wgmma
 // fragment layout: warp w, lane l holds rows 64h + 16w + l/4 (+8) and columns 8c + 2(l%4) (+1).  Kernels whose
 // epilogue wants "thread r owns row r" stage the fragments in a padded fp32 row buffer in shared memory (frag_store,
-// then a CTA barrier, then acc_ld8 of the own row).
+// then a CTA barrier, then acc_ld8 of the own row); element-wise epilogues run on the fragments in place (frag_row,
+// frag_col, pair_off), and sums that persist over tiles stay in registers (mma_m64).
 #pragma once
 #include "nsb_common.cuh"
 
@@ -46,6 +47,16 @@ __device__ __forceinline__ Operand mnmajor(uint32_t addr, int rows) { return Ope
 // wgmma.mma_async m64nNk16, fp16 x fp16 -> fp32, A and B from shared memory; TA / TB = 1: the operand is MN-major.
 template <int N, int TA, int TB>
 struct Wgmma;
+template <int TA, int TB>
+struct Wgmma<8, TA, TB> {
+    __device__ __forceinline__ static void mma(float (&d)[4], uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, %7, %8;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+            : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
 template <int TA, int TB>
 struct Wgmma<32, TA, TB> {
     __device__ __forceinline__ static void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
@@ -124,6 +135,39 @@ __device__ __forceinline__ void mma_m128(float (&d)[2][N / 2], const Operand &a,
     for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int i = 0; i < N / 2; ++i) fence_operand(d[h][i]);
+}
+
+// D[64 x N] (+)= A[64 x 16 KSTEPS] . B[16 KSTEPS x N] by the whole warpgroup into fragments the caller keeps in registers
+// (the weight-gradient sums of the backward kernels, carried over all tiles of a persistent CTA); returns when the result is in d.
+// Same operand rules as mma_m128; only the first m64 row block of A is read.
+template <int N, int TA, int TB, int KSTEPS>
+__device__ __forceinline__ void mma_m64(float (&d)[N / 2], const Operand &a, const Operand &b, bool accumulate) {
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) fence_operand(d[i]);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < KSTEPS; ++ks)
+        Wgmma<N, TA, TB>::mma(d, make_desc(a.addr + ks * a.kstep, a.lbo, a.sbo), make_desc(b.addr + ks * b.kstep, b.lbo, b.sbo),
+                              (ks > 0 || accumulate) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait_all();
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) fence_operand(d[i]);
+}
+
+// Element-wise epilogues on the fragments, without staging rows: d[h][4c + 2i + j] of an m128 accumulator (d[4c + 2i + j] of an
+// m64 one) is row 64h + frag_row(i), column frag_col(c) + j.
+__device__ __forceinline__ int frag_row(int i) { return (threadIdx.x >> 5) * 16 + ((threadIdx.x & 31) >> 2) + 8 * i; }
+__device__ __forceinline__ int frag_col(int c) { return c * 8 + 2 * (threadIdx.x & 3); }
+// byte offset of the fp16 pair (row, col), (row, col + 1) of a chunk-major [R x K] tile, col even: the 32 lanes of a warp touch 128
+// contiguous bytes (8 rows x 16 bytes of one chunk), so the 4-byte accesses are free of bank conflicts
+template <int R>
+__device__ __forceinline__ uint32_t pair_off(int row, int col) { return (uint32_t)((col >> 3) * (R * 16) + row * 16 + (col & 7) * 2); }
+__device__ __forceinline__ float2 ld_pair_f16(const uint8_t *tile, uint32_t off) {
+    return __half22float2(*reinterpret_cast<const __half2 *>(tile + off));
+}
+__device__ __forceinline__ void st_pair_f16(uint8_t *tile, uint32_t off, float a, float b) {
+    *reinterpret_cast<__half2 *>(tile + off) = __floats2half2_rn(a, b);
 }
 
 // Row buffer of staged accumulators: row r at acc + r * stride (floats).  A stride = 4 (mod 8) keeps the row reads of
