@@ -204,8 +204,10 @@ int nsb_fused_sdf(const nsb_lotd_meta *meta_host, const void *params_half, const
 /* the three queries below with the occupancy-evidence side effect (collect may be NULL = the plain query) */
 int nsb_fused_sdf_collect(const nsb_lotd_meta *meta_host, const void *params_half, const nsb_sdf_decoder *dec_host, const float *x,
                           const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, int64_t n,
-                          const int64_t *pack_infos, const int64_t *pack_ray, int64_t n_packs, int32_t mode, int32_t max_level, float *sdf,
-                          const nsb_occ_collect *collect, void *stream);
+                          const int64_t *pack_infos, const int64_t *pack_ray, const int64_t *pack_order, int64_t n_packs, int32_t mode,
+                          int32_t max_level, float *sdf, const nsb_occ_collect *collect, void *stream);
+/* mode 2 (packs) walks the packs in groups of 32: pack_order[32 g .. 32 g + 32) (a permutation of the live packs, nsb_ray_block_order)
+ * or, with pack_order == NULL, packs 32 g .. 32 g + 32.  The order changes which samples share a gather instruction, not any value. */
 
 /* x = o[ridx] + d[ridx] * t, then forward_sdf.  ridx int64[N] indexes rays_o / rays_d [R,3]. */
 int nsb_fused_sdf_rays(const nsb_lotd_meta *meta_host, const void *params_half, const nsb_sdf_decoder *dec_host,
@@ -241,7 +243,7 @@ int nsb_fused_sdf_bwd_indexed(const nsb_lotd_meta *meta_host, const void *params
  * count-aware entry point of that thread consumes (and clears) the binding and its kernel processes min(n_arg, *c0) items -- n_arg
  * (the `n` / `n_packs` / `n_rays` / `n_list` argument) then is the CAPACITY the buffers and the grid were sized for.  c1 is the second
  * count of nsb_assemble_boundary (n_hit).  Count-aware: nsb_gather_rays, nsb_ray_marching_listed (first round: num_steps of the rays
- * in [*c0, n_rays) is written as 0; second round: the listed rays), nsb_ray_marching_record / nsb_march_compact (the same), nsb_fused_sdf_collect / _rays / _packs, nsb_fused_sdf_bwd(_indexed),
+ * in [*c0, n_rays) is written as 0; second round: the listed rays), nsb_ray_marching_record / nsb_march_compact (the same), nsb_fused_sdf_collect / _rays / _packs, nsb_ray_block_order, nsb_fused_sdf_bwd(_indexed),
  * nsb_neus_upsample_cdf, nsb_packed_invert_cdf_shared_u, nsb_merge_sorted_vals, nsb_assemble_boundary, nsb_neus_alpha_forward
  * (num_steps of the packs in [*c0, n_packs) is written as 0) / _backward, nsb_compact_samples, nsb_scatter_f32, nsb_flag_nonzero,
  * nsb_fused_color_fwd / _bwd, nsb_composite_forward / _backward.  With every size on the device a whole fwd+bwd step has no host
@@ -250,8 +252,9 @@ int nsb_bind_device_counts(const int64_t *count0, const int64_t *count1);
 /* flag[i] = (v[i] != 0) for i < live count, 0 up to n (count-aware). */
 int nsb_flag_nonzero(const float *v, int64_t n, int32_t *flag, void *stream);
 /* Derived sizes of one NeuS query in a device block `counts` of >= 32 int64 (zero-filled once per query):
+ *   written by nsb_ray_test_aabb: [2] coherent neighbour pairs, [27] image row length (-1: none found)
  *   written by nsb_scan_counts (totals = counts + 0 / + 3 / + 6 / + 9):
- *     [0] rays that pass the box test  [2] coherent neighbour pairs   [3] M marched samples  [4] n_hit rays with samples
+ *     [0] rays that pass the box test  [3] M marched samples  [4] n_hit rays with samples
  *     [6] K samples kept by the compression  [7] rays that keep samples   [9] samples with a non-zero cotangent (backward)
  *   written here, phase 0 (after the march scan):  [12] M and [13] n_hit (both 0 if the arena `march_cap` cannot hold the merged
  *     samples -- then bit 0 of [20] is set), [14+q] n_hit * n_fine[q], [22+q] samples in the merged buffer after stage q,
@@ -328,10 +331,19 @@ int nsb_compact_samples(const uint8_t *selector, const int64_t *pack_infos, cons
 int nsb_scatter_f32(const float *src, const int64_t *idx, int64_t n, float *dst, void *stream);
 /* AABBSpace.ray_test (nr3d_lib/models/spatial/aabb.py:71-99): normalised rays o_n, d_n [n,3], clamped slab interval near / far [n]
  * and flag[n] = the reference's validity mask.  center3 / radius3 are HOST pointers to 3 floats.  coherent_pairs (device, may be
- * NULL) is incremented by the number of rays i whose origin and direction are within 3 % of ray i-1's (image-ordered rays). */
+ * NULL) is incremented by the number of rays i whose origin and direction are within 3 % of ray i-1's (image-ordered rays).
+ * row_len (device, may be NULL) is set to the image row length W of image-ordered rays: the first i >= 2 at which the step
+ * d[i] - d[i-1] of the direction points against d[1] - d[0] (the return to the start of the next row); -1 if there is none. */
 int nsb_ray_test_aabb(const float *rays_o, const float *rays_d, int64_t n, const float *center3, const float *radius3, int has_near,
                       float near_clip, int has_far, float far_clip, float *o_n, float *d_n, float *near, float *far, int32_t *flag,
-                      int64_t *coherent_pairs, void *stream);
+                      int64_t *coherent_pairs, int64_t *row_len, void *stream);
+/* The 8 x 4 pixel-block order of packs for nsb_fused_sdf_collect's mode 2 (count-aware: n_packs live packs).  Pack p lies on pixel
+ * pix[via[p]] (via == NULL: pix[p]) of an image with row length *row_len, and the live packs are in ascending pixel order with no pixel
+ * twice (what the compactions produce).  order[n_packs] := the packs sorted by (py / 4, px / 8, (py % 4) 8 + px % 8), so that 32
+ * consecutive entries are one 8 x 4 block when the block is whole.  The identity if the n_rays rays the ray test saw are not
+ * image-ordered by its test (n_rays > 64 and *pairs >= 3/4 (n_rays - 1)), if *row_len < 2, or if a row is wider than 32768. */
+int nsb_ray_block_order(const int64_t *pix, const int64_t *via, int64_t n_packs, int64_t n_rays, const int64_t *pairs, const int64_t *row_len,
+                        int64_t *order, void *stream);
 /* rows idx[j] of (o_n, d_n, near, far) and of one optional per-ray fp32 payload extra[., extra_cols] (rays_h_appear) -> row j of
  * the compacted outputs. */
 int nsb_gather_rays(const int64_t *idx, int64_t n, const float *o_n, const float *d_n, const float *near, const float *far, float *o_c,

@@ -127,7 +127,7 @@ namespace nsb { extern std::atomic<int> g_opt_sdf_simt; }
 extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *x,
                                        const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, int64_t n,
                                        int32_t max_level, float *sdf, void *stream, int mode, const int64_t *pack_infos,
-                                       const int64_t *pack_ray, int64_t n_packs, const nsb_occ_collect *collect);
+                                       const int64_t *pack_ray, const int64_t *pack_order, int64_t n_packs, const nsb_occ_collect *collect);
 
 static int launch_fused_sdf(const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *x,
                             const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, int64_t n,
@@ -140,7 +140,7 @@ static int launch_fused_sdf(const nsb_lotd_meta *meta, const void *params_half, 
                 meta->n_feat_per_pseudo_lvl, meta->n_encoded_dims);
     NSB_REQUIRE(dec->width >= 1 && dec->width <= kMaxW, "nsb_fused_sdf: decoder width %d out of range (<= %d)", dec->width, kMaxW);
     if (!g_opt_sdf_simt.load() && h_out == nullptr && meta->n_pseudo_levels == 16)   // tensor-core kernel (csrc/fused_tc.cu)
-        return nsb_fused_sdf_tc_launch(meta, params_half, dec, x, rays_o, rays_d, ridx, t, n, max_level, sdf, stream, from_rays ? 1 : 0, nullptr, nullptr, 0, nullptr);
+        return nsb_fused_sdf_tc_launch(meta, params_half, dec, x, rays_o, rays_d, ridx, t, n, max_level, sdf, stream, from_rays ? 1 : 0, nullptr, nullptr, nullptr, 0, nullptr);
     PLMeta m;
     if (make_plmeta(meta, &m)) return 2;
     DecoderDev d{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2,
@@ -180,13 +180,13 @@ extern "C" int nsb_fused_sdf_packs(const nsb_lotd_meta *meta, const void *params
     NSB_REQUIRE(meta->n_dims_to_encode == 3 && meta->n_feat_per_pseudo_lvl == 2 && meta->n_encoded_dims == 32 && meta->n_pseudo_levels == 16,
                 "nsb_fused_sdf_packs: built for 3-D LoTD with 16 x 2 features");
     NSB_REQUIRE(dec->width >= 1 && dec->width <= kMaxW, "nsb_fused_sdf_packs: decoder width %d out of range (<= %d)", dec->width, kMaxW);
-    return nsb_fused_sdf_tc_launch(meta, params_half, dec, nullptr, rays_o, rays_d, nullptr, t, 0, max_level, sdf, stream, 2, pack_infos, pack_ray, n_packs, nullptr);
+    return nsb_fused_sdf_tc_launch(meta, params_half, dec, nullptr, rays_o, rays_d, nullptr, t, 0, max_level, sdf, stream, 2, pack_infos, pack_ray, nullptr, n_packs, nullptr);
 }
 
 extern "C" int nsb_fused_sdf_collect(const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *x, const float *rays_o,
                                      const float *rays_d, const int64_t *ridx, const float *t, int64_t n, const int64_t *pack_infos,
-                                     const int64_t *pack_ray, int64_t n_packs, int32_t mode, int32_t max_level, float *sdf,
-                                     const nsb_occ_collect *collect, void *stream) {
+                                     const int64_t *pack_ray, const int64_t *pack_order, int64_t n_packs, int32_t mode, int32_t max_level,
+                                     float *sdf, const nsb_occ_collect *collect, void *stream) {
     NSB_REQUIRE(meta && dec && params_half && dec->W1 && dec->b1 && dec->W2 && dec->b2, "nsb_fused_sdf_collect: NULL argument");
     NSB_REQUIRE(mode >= 0 && mode <= 2, "nsb_fused_sdf_collect: mode must be 0 (points), 1 (rays) or 2 (packs)");
     if ((mode == 2 && n_packs == 0) || (mode != 2 && n == 0)) return 0;
@@ -195,5 +195,5 @@ extern "C" int nsb_fused_sdf_collect(const nsb_lotd_meta *meta, const void *para
                 "nsb_fused_sdf_collect: built for 3-D LoTD with 16 x 2 features");
     NSB_REQUIRE(dec->width >= 1 && dec->width <= kMaxW, "nsb_fused_sdf_collect: decoder width %d out of range (<= %d)", dec->width, kMaxW);
     NSB_REQUIRE(!collect || !collect->grid_pcl || (collect->res[0] > 0 && collect->res[1] > 0 && collect->res[2] > 0), "nsb_fused_sdf_collect: bad grid resolution");
-    return nsb_fused_sdf_tc_launch(meta, params_half, dec, x, rays_o, rays_d, ridx, t, n, max_level, sdf, stream, mode, pack_infos, pack_ray, n_packs, collect);
+    return nsb_fused_sdf_tc_launch(meta, params_half, dec, x, rays_o, rays_d, ridx, t, n, max_level, sdf, stream, mode, pack_infos, pack_ray, pack_order, n_packs, collect);
 }

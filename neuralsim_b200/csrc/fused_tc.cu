@@ -13,16 +13,26 @@
 namespace nsb {
 
 // MODE 0: points x[n,3];  MODE 1: x = o[ridx[i]] + d[ridx[i]] t[i] in the given (ray-major) order;
-// MODE 2: the same packed samples traversed RAY-TILED: a tile = 32 consecutive packs (rays) x 4 consecutive samples, lane = ray,
-//         warp = sample ordinal.  For coherent rays (an image) the 32 lanes of a gather instruction then sit in neighbouring
-//         cells -> few 128 B lines per request; the L1 tag stage is what bounds this kernel.  sdf is written to the packed slot, so
-//         nothing downstream changes.  Incoherent rays (random training pixels) keep MODE 1: locality along the ray.
+// MODE 2: the same packed samples traversed RAY-TILED: a tile = 32 packs (rays) x 4 consecutive samples, lane = ray, warp = sample
+//         ordinal.  The 32 packs of group g are order[32 g .. 32 g + 32) -- nsb_ray_block_order puts an 8 x 4 pixel block of an image
+//         there -- or, with order == NULL, packs 32 g .. 32 g + 32 (a 32 x 1 strip of one image row).  For coherent rays the 32 lanes
+//         of a gather instruction then sit in neighbouring cells -> few 128 B lines per request; the L1 tag stage is what bounds this
+//         kernel, and a block touches fewer lines than a strip (DESIGN.md §5).  sdf is written to the packed slot, so nothing
+//         downstream changes.  Incoherent rays (random training pixels) keep MODE 1: locality along the ray.
+// CTAs of k_fused_sdf_tc per SM in the persistent grid, points / rays (modes 0, 1) and ray-tiled packs (mode 2).  5 would fit modes 0 and 1
+// (90 registers, ~13 KB of shared memory), but their gather is L1-bound and more warps gathering at once evict each other's lines: on an
+// H100 (NVIDIA H100 80GB HBM3, 700 W) the boundary query of an 800x600 frame, then walked in 32 x 1 strips, took 5.8 ms per launch at
+// 4 CTAs / SM, 7.3-7.4 ms at 5 and 6.5 ms at 6 (bench.py, alternated).  In 8 x 4 pixel blocks a warp touches fewer lines (DESIGN.md §5) and
+// 5 CTAs / SM are faster than 4; measured on an H100 80GB HBM3 at a 400 W power limit in DESIGN.md §6.
+constexpr int kSdfCtasPerSM = 4, kSdfPackCtasPerSM = 5;       // mode 2's register budget is set by __launch_bounds__ (0 = none for modes 0, 1)
+
 template <int MODE>
-__global__ void __launch_bounds__(kTile)
+__global__ void __launch_bounds__(kTile, MODE == 2 ? kSdfPackCtasPerSM : 0)
 k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ x,
                const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
                const float *__restrict__ t, int64_t n, int max_level, float *__restrict__ sdf, const int64_t *__restrict__ pack_infos,
-               const int64_t *__restrict__ pack_ray, int64_t n_packs, const OccCollect oc, const int64_t *__restrict__ n_dev) {
+               const int64_t *__restrict__ pack_ray, const int64_t *__restrict__ order, int64_t n_packs, const OccCollect oc,
+               const int64_t *__restrict__ n_dev) {
     if (MODE == 2) n_packs = eff_n(n_packs, n_dev); else n = eff_n(n, n_dev);       // device-resident count (nsb_bind_device_counts)
     __shared__ __align__(128) uint8_t sA[kTile * NF * 2];    // 8 KB : features, chunk-major core-matrix layout
     __shared__ __align__(128) uint8_t sB[HW * NF * 2];       // 4 KB : W1 [64 x 32], same layout
@@ -39,9 +49,12 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
     if (MODE == 2) {
         const int64_t n_groups = (n_packs + 31) / 32;
         for (int64_t g = blockIdx.x; g < n_groups; g += gridDim.x) {
-            const int64_t p = g * 32 + lane;
+            const int64_t slot = g * 32 + lane;
             int64_t first = 0, cnt = 0, ray = 0;
-            if (p < n_packs) { first = pack_infos[2 * p]; cnt = pack_infos[2 * p + 1]; ray = pack_ray ? pack_ray[p] : p; }
+            if (slot < n_packs) {
+                const int64_t p = order ? order[slot] : slot;
+                first = pack_infos[2 * p]; cnt = pack_infos[2 * p + 1]; ray = pack_ray ? pack_ray[p] : p;
+            }
             float o[3] = {0.f, 0.f, 0.f}, d[3] = {0.f, 0.f, 0.f};
             if (cnt > 0) {
 #pragma unroll
@@ -244,16 +257,12 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
 
 using namespace nsb;
 
-// CTAs of k_fused_sdf_tc per SM in the persistent grid.  5 would fit (90-101 registers, ~13 KB of shared memory), but the gather
-// is L1-bound and more warps gathering at once evict each other's lines: on an H100 (NVIDIA H100 80GB HBM3, 700 W) the boundary
-// query of an 800x600 frame took 5.8 ms per launch at 4 CTAs / SM, 7.3-7.4 ms at 5 and 6.5 ms at 6 (bench.py, alternated).
-constexpr int kSdfCtasPerSM = 4;
-
-// mode 0: x[n,3];  1: (rays_o, rays_d, ridx, t)[n];  2: ray-tiled packs (pack_infos[n_packs,2], pack_ray[n_packs] or NULL, t, sdf packed)
+// mode 0: x[n,3];  1: (rays_o, rays_d, ridx, t)[n];  2: ray-tiled packs (pack_infos[n_packs,2], pack_ray[n_packs] or NULL,
+// pack_order[n_packs] or NULL, t, sdf packed)
 extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *x,
                                        const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, int64_t n,
                                        int32_t max_level, float *sdf, void *stream, int mode, const int64_t *pack_infos,
-                                       const int64_t *pack_ray, int64_t n_packs, const nsb_occ_collect *collect) {
+                                       const int64_t *pack_ray, const int64_t *pack_order, int64_t n_packs, const nsb_occ_collect *collect) {
     const DevCounts dn = take_counts();
     PLMeta m;
     DecoderDevTC d;
@@ -263,13 +272,14 @@ extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *pa
     const __half *g = (const __half *)params_half;
     const OccCollect oc = occ_collect_of(collect);
     const unsigned tiles = persistent_grid((n + kTile - 1) / kTile, kSdfCtasPerSM);
+    if (mode == 2 && require_ctas_per_sm(k_fused_sdf_tc<2>, kTile, 0, kSdfPackCtasPerSM, "nsb_fused_sdf (packs)")) return 2;
     if (mode == 2)            // a work unit of mode 2 is a group of 32 packs
-        k_fused_sdf_tc<2><<<persistent_grid((n_packs + 31) / 32, kSdfCtasPerSM), kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf,
-                                                                                                 pack_infos, pack_ray, n_packs, oc, dn.a);
+        k_fused_sdf_tc<2><<<persistent_grid((n_packs + 31) / 32, kSdfPackCtasPerSM), kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf,
+                                                                                                 pack_infos, pack_ray, pack_order, n_packs, oc, dn.a);
     else if (mode == 1)
-        k_fused_sdf_tc<1><<<tiles, kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, ridx, t, n, ml, sdf, nullptr, nullptr, 0, oc, dn.a);
+        k_fused_sdf_tc<1><<<tiles, kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, ridx, t, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a);
     else
-        k_fused_sdf_tc<0><<<tiles, kTile, 0, s>>>(m, g, d, x, nullptr, nullptr, nullptr, nullptr, n, ml, sdf, nullptr, nullptr, 0, oc, dn.a);
+        k_fused_sdf_tc<0><<<tiles, kTile, 0, s>>>(m, g, d, x, nullptr, nullptr, nullptr, nullptr, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a);
     return check_launch("nsb_fused_sdf(tc)");
 }
 

@@ -336,10 +336,16 @@ struct RayTestArgs {
 __global__ void __launch_bounds__(256)
 k_ray_test_aabb(const float *__restrict__ rays_o, const float *__restrict__ rays_d, int64_t n, const RayTestArgs a, float *__restrict__ o_n,
                 float *__restrict__ d_n, float *__restrict__ near, float *__restrict__ far, int32_t *__restrict__ flag,
-                unsigned long long *__restrict__ coherent_pairs) {
+                unsigned long long *__restrict__ coherent_pairs, unsigned long long *__restrict__ row_len) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     unsigned int close = 0;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        if (row_len && i >= 2) {                         // image row length: the first i where the image-x step of the direction reverses
+            float rev = 0.f;
+#pragma unroll
+            for (int d = 0; d < 3; ++d) rev += (rays_d[i * 3 + d] - rays_d[(i - 1) * 3 + d]) * (rays_d[3 + d] - rays_d[d]);
+            if (rev < 0.f) atomicMin(row_len, (unsigned long long)i);
+        }
         if (coherent_pairs && i > 0) {                   // is ray i a neighbour of ray i-1 (image order)?  -> traversal order of the queries
             float dd = 0.f, od = 0.f;
 #pragma unroll
@@ -373,6 +379,85 @@ k_ray_test_aabb(const float *__restrict__ rays_o, const float *__restrict__ rays
     if (coherent_pairs) {
         close = __reduce_add_sync(0xffffffffu, close);
         if ((threadIdx.x & 31) == 0 && close) atomicAdd(coherent_pairs, (unsigned long long)close);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ 8 x 4 pixel-block order of the packs
+// order[j] = the pack in slot j when the live packs, in ascending pixel order, are re-sorted by (py / 4, px / 8, (py % 4) 8 + px % 8),
+// pixel = pix[via ? via[p] : p] = py W + px.  A block row (4 image rows) is a contiguous range of packs; one CTA per block row marks
+// the occupied pixels of each 8 x 4 block in a 32-bit mask, scans the popcounts over the blocks, and writes every pack to
+// range start + packs in earlier blocks + occupied pixels of its block before it.  Identity without row structure.
+constexpr int kOrdT = 256, kOrdMaxBx = 4096;              // blocks per block row: image rows up to 32768 pixels
+constexpr int kBlkW = 8, kBlkH = 4;                       // block shape: kBlkW x kBlkH = 32 pixels = one group of the ray-tiled query
+
+__device__ __forceinline__ int64_t pixel_of(const int64_t *__restrict__ pix, const int64_t *__restrict__ via, int64_t p) {
+    return pix[via ? via[p] : p];
+}
+
+__device__ int64_t lower_bound_pixel(const int64_t *__restrict__ pix, const int64_t *__restrict__ via, int64_t n, int64_t key) {
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (pixel_of(pix, via, mid) < key) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+
+__global__ void __launch_bounds__(kOrdT)
+k_ray_block_order(const int64_t *__restrict__ pix, const int64_t *__restrict__ via, int64_t n, int64_t n_rays, const int64_t *__restrict__ pairs,
+                  const int64_t *__restrict__ row_len, int64_t *__restrict__ order, const int64_t *__restrict__ n_dev) {
+    __shared__ uint32_t mask[kOrdMaxBx];
+    __shared__ int32_t offs[kOrdMaxBx];
+    __shared__ int32_t wsum[kOrdT / 32];
+    n = eff_n(n, n_dev);
+    const int64_t W = *row_len;
+    const bool coherent = n_rays > 64 && 4 * *pairs >= 3 * (n_rays - 1);   // the host-sized path's test (fields/space.py)
+    const int64_t nbx = (W + kBlkW - 1) / kBlkW;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (n == 0) return;
+    if (!coherent || W < 2 || nbx > kOrdMaxBx) {
+        for (int64_t j = (int64_t)blockIdx.x * kOrdT + tid; j < n; j += (int64_t)gridDim.x * kOrdT) order[j] = j;
+        return;
+    }
+    const int64_t rows = kBlkH * W, n_brows = pixel_of(pix, via, n - 1) / rows + 1;
+    constexpr int kPer = kOrdMaxBx / kOrdT;
+    for (int64_t by = blockIdx.x; by < n_brows; by += gridDim.x) {
+        const int64_t lo = lower_bound_pixel(pix, via, n, by * rows), hi = lower_bound_pixel(pix, via, n, (by + 1) * rows);
+        for (int64_t b = tid; b < nbx; b += kOrdT) mask[b] = 0u;
+        __syncthreads();
+        for (int64_t p = lo + tid; p < hi; p += kOrdT) {
+            const int64_t q = pixel_of(pix, via, p) - by * rows, py = q / W, px = q - py * W;
+            atomicOr(&mask[px / kBlkW], 1u << (py * kBlkW + px % kBlkW));
+        }
+        __syncthreads();
+        int loc = 0;                                          // exclusive scan of the block popcounts: kPer consecutive blocks per thread
+#pragma unroll
+        for (int k = 0; k < kPer; ++k) {
+            const int b = tid * kPer + k;
+            if (b < nbx) loc += __popc(mask[b]);
+        }
+        int incl = loc;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+        }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        int run = incl - loc;
+        for (int w = 0; w < warp; ++w) run += wsum[w];
+#pragma unroll
+        for (int k = 0; k < kPer; ++k) {
+            const int b = tid * kPer + k;
+            if (b < nbx) { offs[b] = run; run += __popc(mask[b]); }
+        }
+        __syncthreads();
+        for (int64_t p = lo + tid; p < hi; p += kOrdT) {
+            const int64_t q = pixel_of(pix, via, p) - by * rows, py = q / W, px = q - py * W;
+            const uint32_t bit = (uint32_t)(py * kBlkW + px % kBlkW);
+            order[lo + offs[px / kBlkW] + __popc(mask[px / kBlkW] & ((1u << bit) - 1u))] = p;
+        }
+        __syncthreads();                                      // mask / offs are rewritten for the next block row
     }
 }
 
@@ -529,12 +614,23 @@ extern "C" int nsb_scatter_f32(const float *src, const int64_t *idx, int64_t n, 
 
 extern "C" int nsb_ray_test_aabb(const float *rays_o, const float *rays_d, int64_t n, const float *center3, const float *radius3, int has_near,
                                  float near_clip, int has_far, float far_clip, float *o_n, float *d_n, float *near, float *far, int32_t *flag,
-                                 int64_t *coherent_pairs, void *stream) {
+                                 int64_t *coherent_pairs, int64_t *row_len, void *stream) {
     if (n == 0) return 0;
     NSB_REQUIRE(rays_o && rays_d && center3 && radius3 && o_n && d_n && near && far && flag, "nsb_ray_test_aabb: NULL argument");
     RayTestArgs a{{center3[0], center3[1], center3[2]}, {radius3[0], radius3[1], radius3[2]}, near_clip, far_clip, has_near, has_far};
-    k_ray_test_aabb<<<wave_grid(n, 256, 8), 256, 0, STREAM>>>(rays_o, rays_d, n, a, o_n, d_n, near, far, flag, (unsigned long long *)coherent_pairs);
+    if (row_len && cudaMemsetAsync(row_len, 0xff, sizeof(int64_t), STREAM) != cudaSuccess) return check_launch("nsb_ray_test_aabb (row length)");
+    k_ray_test_aabb<<<wave_grid(n, 256, 8), 256, 0, STREAM>>>(rays_o, rays_d, n, a, o_n, d_n, near, far, flag, (unsigned long long *)coherent_pairs,
+                                                           (unsigned long long *)row_len);
     return check_launch("nsb_ray_test_aabb");
+}
+
+extern "C" int nsb_ray_block_order(const int64_t *pix, const int64_t *via, int64_t n_packs, int64_t n_rays, const int64_t *pairs, const int64_t *row_len,
+                                   int64_t *order, void *stream) {
+    const DevCounts dn = take_counts();
+    if (n_packs == 0) return 0;
+    NSB_REQUIRE(pix && pairs && row_len && order, "nsb_ray_block_order: NULL argument");
+    k_ray_block_order<<<wave_grid(n_packs, 4 * 32 * 8, 1), kOrdT, 0, STREAM>>>(pix, via, n_packs, n_rays, pairs, row_len, order, dn.a);
+    return check_launch("nsb_ray_block_order");
 }
 
 extern "C" int nsb_gather_rays(const int64_t *idx, int64_t n, const float *o_n, const float *d_n, const float *near, const float *far, float *o_c,

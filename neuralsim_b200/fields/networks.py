@@ -237,12 +237,13 @@ class LoTDSDF(nn.Module):
                 meta.c_ref, L.ptr(grid16, "f16"), ctypes.byref(dec), None, L.ptr(rays_o, "f32"), L.ptr(rays_d, "f32"),
                 L.ptr(ridx, "i64", allow_none=(mode == 2)) if mode == 1 else None, L.ptr(t, "f32"), L.c_i64(t.numel()),
                 L.ptr(packs[0], "i64") if mode == 2 else None, L.ptr(packs[1], "i64", allow_none=True) if mode == 2 else None,
+                L.ptr(packs[2], "i64", allow_none=True) if mode == 2 and len(packs) > 2 else None,
                 L.c_i64(packs[0].shape[0] if mode == 2 else 0), L.c_i32(mode), L.c_i32(max_level), L.ptr(sdf),
                 ctypes.byref(collect) if collect is not None else None, L.stream_ptr()), "fused_sdf")
             return sdf
         sdf = torch.empty(pts.shape[0], dtype=torch.float32, device=pts.device)
         L.check(L.lib().nsb_fused_sdf_collect(meta.c_ref, L.ptr(grid16, "f16"), ctypes.byref(dec), L.ptr(pts, "f32"), None, None, None, None,
-                                              L.c_i64(pts.shape[0]), None, None, L.c_i64(0), L.c_i32(0), L.c_i32(max_level), L.ptr(sdf),
+                                              L.c_i64(pts.shape[0]), None, None, None, L.c_i64(0), L.c_i32(0), L.c_i32(max_level), L.ptr(sdf),
                                               ctypes.byref(self._collect) if getattr(self, "_collect", None) is not None else None, L.stream_ptr()),
                 "fused_sdf")
         return sdf

@@ -82,11 +82,11 @@ class AABBSpace(nn.Module):
         o_n, d_n = torch.empty(R, 3, device=dev), torch.empty(R, 3, device=dev)
         nr, fr = torch.empty(R, device=dev), torch.empty(R, device=dev)
         flag = torch.empty(R, dtype=torch.int32, device=dev)
-        pairs = torch.zeros(1, dtype=torch.int64, device=dev)
+        pairs = torch.zeros(2, dtype=torch.int64, device=dev)              # coherent neighbour pairs, image row length
         L.check(L.lib().nsb_ray_test_aabb(L.ptr(rays_o.contiguous(), "f32"), L.ptr(rays_d.contiguous(), "f32"), L.c_i64(R), c3, r3,
                                           ctypes.c_int(0 if near is None else 1), L.c_f32(0. if near is None else near),
                                           ctypes.c_int(0 if far is None else 1), L.c_f32(0. if far is None else far), L.ptr(o_n), L.ptr(d_n),
-                                          L.ptr(nr), L.ptr(fr), L.ptr(flag), L.ptr(pairs), L.stream_ptr()), "ray_test_aabb")
+                                          L.ptr(nr), L.ptr(fr), L.ptr(flag), L.ptr(pairs), L.ptr(pairs[1:]), L.stream_ptr()), "ray_test_aabb")
         sc = scan_counts(flag, want_index=True, extra=pairs)
         n, ridx = sc["n_nonzero"], sc["index"]
         o_c, d_c = torch.empty(n, 3, device=dev), torch.empty(n, 3, device=dev)
@@ -104,4 +104,6 @@ class AABBSpace(nn.Module):
         ret.update(rays_o=o_c, rays_d=d_c)
         # image-ordered rays (>= 3/4 of the rays neighbour their predecessor): the queries traverse samples ray-tiled (csrc/fused_tc.cu)
         ret["rays_coherent"] = R > 64 and sc["extra"][0] >= 0.75 * (R - 1)
+        if ret["rays_coherent"]:                       # what the queries need to walk the rays in 8 x 4 pixel blocks (graphics/neus.py)
+            ret["rays_row"] = (R, pairs)
         return ret

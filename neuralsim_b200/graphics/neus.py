@@ -131,6 +131,7 @@ def _query_fused(model, ray_tested, view_dirs, rays_h_appear, *, perturb=False, 
         torch.rand(depth_samples.shape, dtype=depth_samples.dtype, device=depth_samples.device)
     pack_infos = pinfo_march
     coherent = bool(ray_tested.get("rays_coherent", False))      # image-ordered rays: ray-tiled traversal inside the SDF kernel
+    rays_row = ray_tested.get("rays_row") if coherent else None   # ... in 8 x 4 pixel blocks
     surf = getattr(model, "implicit_surface", None)
     if use_persistent_upsample(rays_o.shape[0]) and not perturb and surf is not None and getattr(surf, "_fusable", lambda: False)():
         # the whole no-grad half in ONE persistent per-ray kernel (csrc/ray_upsample.cu); same values as the stage kernels below
@@ -150,6 +151,7 @@ def _query_fused(model, ray_tested, view_dirs, rays_h_appear, *, perturb=False, 
         # queries have uniform packs and are ray-tiled whenever the rays are image-ordered
         sdf = model.forward_sdf_on_rays(ridx, depth_samples, rays_o, rays_d)["sdf"].to(dtype)
         fine_stages = []
+        order_f = neus_fused.block_order(rays_inds, ridx_hit, rays_row) if rays_row is not None and n_stage > 1 else None
         for i, factor in enumerate(factors):
             cdf = neus_fused.upsample_cdf(sdf, depth_samples, pack_infos, upsample_inv_s * factor, use_estimate_alpha)
             if perturb:                  # one stratified u per pack and sample (raysample.py:38-61)
@@ -158,7 +160,7 @@ def _query_fused(model, ray_tested, view_dirs, rays_h_appear, *, perturb=False, 
                 fine = neus_fused.sample_cdf_uniform(depth_samples, cdf, pack_infos, num_fine[i])
             fine_stages.append(fine)
             if i < n_stage - 1:         # (the reference also merges after the last stage; nothing reads that result)
-                packs = (get_pack_infos_from_batch(ridx_hit.shape[0], fine.shape[1], device=fine.device), ridx_hit) if coherent else None
+                packs = (get_pack_infos_from_batch(ridx_hit.shape[0], fine.shape[1], device=fine.device), ridx_hit, order_f) if coherent else None
                 sdf_fine = model.forward_sdf_on_rays(ridx_hit, fine, rays_o, rays_d, packs=packs)["sdf"].to(dtype).contiguous()
                 depth_samples, sdf, pack_infos = neus_fused.merge_sorted_vals(depth_samples, sdf, pack_infos, fine, sdf_fine)
         fine_all = torch.cat(fine_stages, dim=-1) if n_stage > 1 else fine_stages[0]
@@ -170,7 +172,9 @@ def _query_fused(model, ray_tested, view_dirs, rays_h_appear, *, perturb=False, 
 def _query_fused_tail(model, ray_tested, view_dirs, rays_h_appear, rays_o, rays_d, rays_inds, d1, mid, ridx_all, pinfo, pinfo_march, coherent, dtype, *,
                       with_rgb, with_normal, nablas_has_grad, forward_inv_s):
     """boundary SDF (grad) -> alpha -> compression -> colour / normal query: the second half of `_query_fused`"""
-    sdf_b = model.forward_sdf_on_rays(ridx_all, d1, rays_o, rays_d, packs=(pinfo, None) if coherent else None)["sdf"].to(dtype)
+    rays_row = ray_tested.get("rays_row") if coherent else None
+    order_b = neus_fused.block_order(rays_inds, None, rays_row) if rays_row is not None else None
+    sdf_b = model.forward_sdf_on_rays(ridx_all, d1, rays_o, rays_d, packs=(pinfo, None, order_b) if coherent else None)["sdf"].to(dtype)
     comp = neus_fused.neus_alpha_compact(sdf_b, forward_inv_s, pinfo, ridx_all, mid, rays_inds)
     if comp is None:
         return dict(type="empty", rays_inds_hit=[]), {}

@@ -17,7 +17,7 @@ import torch
 from .. import _lib as L
 
 __all__ = ["upsample_cdf", "sample_cdf_uniform", "neus_alpha_compress", "neus_alpha_compact", "composite", "scan_counts", "merge_sorted_vals",
-           "assemble_boundary", "march_lean", "upsample_rays"]
+           "assemble_boundary", "march_lean", "upsample_rays", "block_order"]
 
 _U_CACHE = {}
 
@@ -163,6 +163,18 @@ def scan_counts(counts, *, want_first=False, want_info2=False, want_index=False,
     out["pack"] = pack[:nnz] if pack is not None else None
     out["src"] = nz_src[:nnz] if nz_src is not None else None
     return out
+
+
+@torch.no_grad()
+def block_order(pix, via, rays_row):
+    """order[P]: the packs on pixels pix[via[p]] (via None: pix[p]; ascending, unique) in 8 x 4 pixel blocks, for the ray-tiled SDF
+    query (csrc/neus_glue.cu: k_ray_block_order).  rays_row = (rays the ray test saw, its int64[2] (neighbour pairs, row length))."""
+    n = pix.shape[0] if via is None else via.shape[0]
+    order = torch.empty(n, dtype=torch.int64, device=pix.device)
+    n_rays, pr = rays_row
+    L.check(L.lib().nsb_ray_block_order(L.ptr(pix, "i64"), L.ptr(via, "i64", allow_none=True), L.c_i64(n), L.c_i64(n_rays), L.ptr(pr, "i64"),
+                                        L.ptr(pr[1:], "i64"), L.ptr(order), L.stream_ptr()), "ray_block_order")
+    return order
 
 
 @torch.no_grad()

@@ -27,7 +27,7 @@ from . import neus_fused as NF
 __all__ = ["render_static", "StaticFrame", "CNT_SLOTS"]
 
 CNT_SLOTS = dict(n_rays=0, pairs=2, marched_raw=3, hit_raw=4, kept_raw=6, kept_rays_raw=7, nonzero=9, marched=12, hit=13, fine0=14,
-                 boundary=18, kept=19, overflow=20, kept_rays=21, merged0=22, rays_if_kept_fits=26)
+                 boundary=18, kept=19, overflow=20, kept_rays=21, merged0=22, rays_if_kept_fits=26, row_len=27)
 _NULL = ctypes.c_void_p(0)
 # "auto": small batches march once and copy (nsb_ray_marching_record + nsb_march_compact) when the per-ray record fits this many bytes;
 # "0": always the two-round march; "1": always the recorded march.  Same samples bit for bit either way.
@@ -73,7 +73,8 @@ def _query_counts(cnt, phase, n_coarse1, num_fine, march_cap, kept_cap):
 
 
 def _sdf_launch(meta, grid16, dec, rays_o, rays_d, t, sdf, *, ridx=None, packs=None, ml, collect, cnt, slot, timer="lotd_gather"):
-    """the fused SDF query on rays with a device-resident count: mode 1 (ridx[n], count = samples) or mode 2 (packs, count = packs)"""
+    """the fused SDF query on rays with a device-resident count: mode 1 (ridx[n], count = samples) or mode 2 (packs = (pack_infos, pack_ray | None,
+    block order | None), count = packs)"""
     P = L.ptr
     mode = 2 if packs is not None else 1
     with L.KERNEL_TIMER.time(timer, t.numel()):
@@ -81,9 +82,20 @@ def _sdf_launch(meta, grid16, dec, rays_o, rays_d, t, sdf, *, ridx=None, packs=N
               meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), None, P(rays_o, "f32"), P(rays_d, "f32"),
               P(ridx, "i64") if mode == 1 else None, P(t, "f32"), L.c_i64(t.numel()),
               P(packs[0], "i64") if mode == 2 else None, P(packs[1], "i64", allow_none=True) if mode == 2 else None,
+              P(packs[2], "i64", allow_none=True) if mode == 2 and len(packs) > 2 else None,
               L.c_i64(packs[0].shape[0] if mode == 2 else 0), L.c_i32(mode), L.c_i32(ml), P(sdf),
               ctypes.byref(collect) if collect is not None else None, L.stream_ptr())
     return sdf
+
+
+def _block_order(rays_inds, via, n_rays, cnt, slot):
+    """the 8 x 4 pixel-block order of the cnt[slot] live packs on pixels rays_inds[via[p]] (nsb_ray_block_order; the row length and the
+    coherence test are the ray test's, in cnt)"""
+    n = rays_inds.shape[0] if via is None else via.shape[0]
+    order = torch.empty(n, dtype=torch.int64, device=rays_inds.device)
+    _call(L.lib().nsb_ray_block_order, "ray_block_order", cnt, slot, None, L.ptr(rays_inds, "i64"), L.ptr(via, "i64", allow_none=True), L.c_i64(n),
+          L.c_i64(n_rays), _slot(cnt, CNT_SLOTS["pairs"]), _slot(cnt, CNT_SLOTS["row_len"]), L.ptr(order), L.stream_ptr())
+    return order
 
 
 # ---------------------------------------------------------------------------------------------------------------- autograd pieces
@@ -360,9 +372,11 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         L.check(lib.nsb_ray_test_aabb(P(rays_o.contiguous(), "f32"), P(rays_d.contiguous(), "f32"), L.c_i64(R), sp._host_cr[1], sp._host_cr[2],
                                       ctypes.c_int(0 if near is None else 1), L.c_f32(0. if near is None else near),
                                       ctypes.c_int(0 if far is None else 1), L.c_f32(0. if far is None else far), P(o_n), P(d_n), P(nr), P(fr), P(flag),
-                                      _slot(cnt, CNT_SLOTS["pairs"]), L.stream_ptr()), "ray_test_aabb")
+                                      _slot(cnt, CNT_SLOTS["pairs"]), _slot(cnt, CNT_SLOTS["row_len"]), L.stream_ptr()), "ray_test_aabb")
         rays_inds = torch.empty(R, dtype=torch.int64, device=dev)
         _scan(flag, cnt, CNT_SLOTS["n_rays"], index=rays_inds, ws=st.ws[0])
+        # the boundary query walks its packs (the rays that passed) in 8 x 4 pixel blocks (csrc/neus_glue.cu: k_ray_block_order)
+        order_b = _block_order(rays_inds, None, R, cnt, CNT_SLOTS["n_rays"]) if coherent else None
         ha = rays_h_appear.detach().contiguous().float() if (rays_h_appear is not None and model.use_h_appear) else None
         if ha is None and model.use_h_appear:             # LiDAR-style rays carry no appearance code: the (dropped) radiance head reads zeros
             ha = torch.zeros(R, model.radiance_net.blocks.layers[0].in_features - 54, device=dev)
@@ -424,6 +438,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         sdf = torch.empty(march_cap if factors_loop else 1, dtype=torch.float32, device=dev)
         if factors_loop:
             fine_stages = []
+            order_f = _block_order(rays_inds, ridx_hit, R, cnt, CNT_SLOTS["hit"]) if coherent and n_stage > 1 else None
             _sdf_launch(st.meta, st.grid16, st.dec, o_c, d_c, depth, sdf, ridx=ridx, ml=st.ml, collect=st.collect, cnt=cnt, slot=CNT_SLOTS["marched"])
         for i, factor in enumerate(factors_loop):
             cdf = torch.empty(march_cap, dtype=torch.float32, device=dev)
@@ -440,7 +455,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
             if i < n_stage - 1:
                 sdf_fine = torch.empty(R * nf, dtype=torch.float32, device=dev)
                 if coherent:
-                    _sdf_launch(st.meta, st.grid16, st.dec, o_c, d_c, fine.view(-1), sdf_fine, packs=(get_pack_infos_from_batch(R, nf, device=dev), ridx_hit),
+                    _sdf_launch(st.meta, st.grid16, st.dec, o_c, d_c, fine.view(-1), sdf_fine, packs=(get_pack_infos_from_batch(R, nf, device=dev), ridx_hit, order_f),
                                 ml=st.ml, collect=st.collect, cnt=cnt, slot=CNT_SLOTS["hit"])
                 else:
                     _sdf_launch(st.meta, st.grid16, st.dec, o_c, d_c, fine.view(-1), sdf_fine, ridx=ridx_hit.unsqueeze(-1).expand(R, nf).reshape(-1).contiguous(),
@@ -463,7 +478,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     # ---------------- boundary SDF (grad) -> alpha -> compression
     s, b = model.implicit_surface, model.radiance_net.blocks.layers
     dl = s.decoder.layers
-    sdf_b = _StaticSDF.apply(st, ridx_all, d1, (pinfo, None) if coherent else None, CNT_SLOTS["n_rays"] if coherent else CNT_SLOTS["boundary"],
+    sdf_b = _StaticSDF.apply(st, ridx_all, d1, (pinfo, None, order_b) if coherent else None, CNT_SLOTS["n_rays"] if coherent else CNT_SLOTS["boundary"],
                              s.encoding.flattened_params, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
     inv_s = model.forward_inv_s()
     if not isinstance(inv_s, torch.Tensor):
