@@ -2,12 +2,20 @@
 // For every ray that marched into occupied voxels it replaces, per up-sampling stage, the launches
 //   k_fused_sdf_tc (sdf of the marched / new samples) -> k_upsample_cdf -> k_invert_cdf_shared_u -> k_merge_vals
 // (graphics/neus.py:_query_fused, reference neus_ray_query.py:861-905) and keeps the ray's samples in shared memory in between.
-// A CTA of 128 threads owns a group of 4 consecutive hit rays: warp w <-> ray w for the per-ray stages (the bodies are the stand-alone kernels'
-// own device functions, neus_device.cuh, so the results are bit-identical by construction); for the SDF evaluations the four rays' pending samples
-// are concatenated into 128-point tiles of the usual gather -> wgmma -> SFU pipeline (sdf_of_tile, fused_tc_common.cuh).
+// A CTA of 128 threads owns a group of 4 consecutive hit rays: warp w <-> ray w for the per-ray stages; for the SDF evaluations the four rays'
+// pending samples are concatenated into 128-point tiles of the usual gather -> wgmma -> SFU pipeline (sdf_of_tile, fused_tc_common.cuh).
+// Shared with the stand-alone kernels (neus_device.cuh): upsample_alpha_at, neus_alpha_at, replay_chunk and warp_scan_incl.  Restated here on
+// plain pointers: warp_upsample_cdf, invert_cdf_one and warp_merge are the statements of k_upsample_cdf, k_invert_cdf_shared_u and
+// k_merge_vals, so their bit-equality is not by construction; tests/test_ray_upsample_edges_gpu.py pins them (and the group-to-group state
+// below) to the stage kernels bit for bit and to float64 at their edges.
 // Output: fine[n_hit, sum(n_fine)] -- what `torch.cat(fine_stages, -1)` is on the multi-kernel path.  A ray whose samples do not fit the
 // per-ray shared-memory capacity (kCap) works on a slice of a global scratch buffer instead (same code: the stage bodies take plain
-// pointers); `overflow` is only raised for a ray longer than that slice (`long_cap`, sized from max_steps by the caller: cannot happen then).
+// pointers).  Overflow: overflow[j] is set to 1 (and nothing else is written to it) for a ray with more than long_cap - merged marched
+// samples (merged = the samples of every stage but the last), or, without scratch (nsb_upsample_persistent), more than kCap - merged; such
+// a ray is not processed: its row of `fine` is not written and none of its points is collected.  With long_cap sized from max_steps by the
+// caller (graphics/neus_fused.py: max_steps + merged + 64) a marched ray never overflows.
+// An empty pack (n = 0) is skipped the same way: its row is not written and nothing is collected for it (the stage kernels write NaN
+// samples for it instead).  Production never passes one: the hit rays of the march hold >= 1 sample.
 // Training-time sample collection (accel.collect_samples on every SDF query, renderer_mixin.py:154-164) is done in-kernel as in k_fused_sdf_tc.
 #include "fused_tc_common.cuh"
 #include "neus_device.cuh"
@@ -128,7 +136,7 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
             n = (int)pack_infos[2 * j + 1];
         }
         bool in_smem = n <= room;
-        if (!in_smem && (scratch == nullptr || n > long_cap - (kCap - room))) {      // longer than the scratch slice: flagged, row left undefined
+        if (!in_smem && (scratch == nullptr || n > long_cap - (kCap - room))) {      // longer than the scratch slice: flagged, row not written
             if (lane == 0) overflow[j] = 1;
             n = 0;
             in_smem = true;

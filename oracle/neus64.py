@@ -209,9 +209,10 @@ def lower_bound(cc, u):
     return first
 
 
-def invert_cdf(bins, cdf32, u, pack_infos):
+def invert_cdf(bins, cdf32, u, pack_infos, return_pos=False):
     """k_invert_cdf_shared_u: u [n_s] shared by all packs; cdf32 the fp32 cdf the kernel reads (decisions on it are exact).
-    -> (samples [P, n_s] float64 (NaN for an empty pack), scale [P, n_s]: |b0| + |b1 - b0|, pos [P, n_s])"""
+    -> (samples [P, n_s] float64 (NaN for an empty pack), scale [P, n_s]: |b0| + |b1 - b0|), and with return_pos also pos [P, n_s]: the
+    bin each sample took (the lower bound clamped to n - 1; 0 for an empty pack)"""
     b32, c32, u32 = np.asarray(bins, F32), np.asarray(cdf32, F32), np.asarray(u, F32)
     pi = np.asarray(pack_infos, dtype=np.int64).reshape(-1, 2)
     P, ns = pi.shape[0], u32.shape[0]
@@ -231,7 +232,7 @@ def invert_cdf(bins, cdf32, u, pack_infos):
             r = np.where(q == 0, bb[0], np.where(pmf < F32(1e-5), b0, interp))
         out[p] = r
         scale[p] = np.abs(b0) + np.abs(b1 - b0)
-    return out, scale
+    return (out, scale, pos) if return_pos else (out, scale)
 
 
 def composite_forward(w, t, pack_infos, rgb=None, nablas=None, normalize_depth=True):
