@@ -415,6 +415,34 @@ int nsb_upsample_persistent(const nsb_lotd_meta *meta_host, const void *params_h
                             int32_t max_level, int32_t n_stage, const int32_t *n_fine, const float *inv_s_stage, const float *const *u_stage,
                             int32_t use_estimate_alpha, float early_stop_eps, float alpha_thre, float *fine_all, int32_t *overflow, void *stream);
 
+/* ---------------------------------------------------------------- marching cubes (csrc/mesh.cu)
+ * The stages of nr3d_lib.graphics.trianglemesh.extract_mesh (trianglemesh.py:134-254: lattice, SDF volume, skimage marching cubes) on a
+ * lattice of n0 x n1 x n2 points (point (i, j, k) at flat index (i n1 + j) n2 + k, k fastest: meshgrid(indexing="ij")) streamed in slabs of
+ * whole planes along axis 0.  A slab owns planes [p0, p1): the vertices on the edges (+x, +y, +z) their points own and the cells
+ * (p0 - 1 .. p1 - 2).  Slot l in [0, (p1 - p0) n1 n2) of every per-slab array is point (p0 + l / (n1 n2), j, k) and cell (p0 - 1 + l / (n1 n2), j, k).
+ * sdf_win: fp32 planes [w0, w0 + n_win) of the volume, holding at least planes [p0 - 1, p1 + 1) (count) / [p0 - 1, p1 + 2) (vertices), clipped
+ * to [0, n0).  A point is inside when sdf < level.  The case table (csrc/mc_table.cuh) is generated by oracle/mc_table.py.
+ *
+ * nsb_mc_lattice_points: x[n, 3] = (lin0[i], lin1[j], lin2[k]) of the flat indices start .. start + n - 1 (the query points).
+ * nsb_mc_count: flags[l] = bits (x, y, z) of the owned edges whose ends differ in sign, vcount[l] = their number; cases[l] = case index of
+ *   the cell of slot l (0 if it does not exist), tcount[l] = its triangle count.  Scan both counts (nsb_scan_counts) for vfirst / tfirst.
+ * nsb_mc_vertices: the vertices of slot l at vfirst[l] + 0, 1, 2 in axis order: position bmin + spacing (idx + t), t = (level - s0) / (s1 - s0),
+ *   normal = normalise(g0 + t (g1 - g0)) of the lattice gradients g (central differences, one-sided at the volume border, over the spacing);
+ *   fp64 arithmetic, fp32 outputs verts[., 3], normals[., 3].  bmin3_host / spacing3_host: HOST arrays of 3 doubles.
+ * nsb_mc_triangles: faces[tfirst[l] + q] (int32 [., 3]) = triangle q of the cell of slot l, as global vertex ids: vbase + vfirst + rank of the
+ *   edge among its owner's flags, or, for an owner on plane p0 - 1, carry_base + carry_first[jk] + rank among carry_flags[jk] (that plane's
+ *   flags and scanned offsets, kept from the previous slab; may be NULL when p0 == 0).  The caller makes sure the ids fit in int32. */
+int nsb_mc_lattice_points(const float *lin0, const float *lin1, const float *lin2, int32_t n1, int32_t n2, int64_t start, int64_t n, float *x,
+                          void *stream);
+int nsb_mc_count(const float *sdf_win, int32_t w0, int32_t n_win, int32_t n0, int32_t n1, int32_t n2, int32_t p0, int32_t p1, double level,
+                 uint8_t *flags, int32_t *vcount, uint8_t *cases, int32_t *tcount, void *stream);
+int nsb_mc_vertices(const float *sdf_win, int32_t w0, int32_t n_win, int32_t n0, int32_t n1, int32_t n2, int32_t p0, int32_t p1, double level,
+                    const double *bmin3_host, const double *spacing3_host, const uint8_t *flags, const int32_t *vfirst, float *verts, float *normals,
+                    void *stream);
+int nsb_mc_triangles(int32_t n0, int32_t n1, int32_t n2, int32_t p0, int32_t p1, const uint8_t *cases, const int32_t *tcount, const int32_t *tfirst,
+                     const uint8_t *flags, const int32_t *vfirst, int64_t vbase, const uint8_t *carry_flags, const int32_t *carry_first,
+                     int64_t carry_base, int32_t *faces, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -57,6 +57,12 @@ def lib():
         _lib.nsb_last_error.restype = ctypes.c_char_p
         _lib.nsb_launch_count.restype = ctypes.c_uint64
         _lib.nsb_color_tile_bytes.restype = ctypes.c_int64
+        # marching cubes (csrc/mesh.cu): `level` is a double, which an undeclared ctypes call would not pass
+        vp, i32, i64, f64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_double
+        _lib.nsb_mc_lattice_points.argtypes = [vp, vp, vp, i32, i32, i64, i64, vp, vp]
+        _lib.nsb_mc_count.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, f64, vp, vp, vp, vp, vp]
+        _lib.nsb_mc_vertices.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, f64, vp, vp, vp, vp, vp, vp, vp]
+        _lib.nsb_mc_triangles.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp, vp, i64, vp, vp]
     return _lib
 
 
