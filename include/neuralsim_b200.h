@@ -245,7 +245,7 @@ int nsb_fused_sdf_bwd_indexed(const nsb_lotd_meta *meta_host, const void *params
  * count of nsb_assemble_boundary (n_hit).  Count-aware: nsb_gather_rays, nsb_ray_marching_listed (first round: num_steps of the rays
  * in [*c0, n_rays) is written as 0; second round: the listed rays), nsb_ray_marching_record / nsb_march_compact (the same), nsb_fused_sdf_collect / _rays / _packs, nsb_ray_block_order, nsb_fused_sdf_bwd(_indexed),
  * nsb_neus_upsample_cdf, nsb_packed_invert_cdf_shared_u, nsb_merge_sorted_vals, nsb_assemble_boundary, nsb_neus_alpha_forward
- * (num_steps of the packs in [*c0, n_packs) is written as 0) / _backward, nsb_compact_samples, nsb_scatter_f32, nsb_flag_nonzero,
+ * (num_steps of the packs in [*c0, n_packs) is written as 0) / _backward / _backward_kept / _backward_kept_list, nsb_compact_samples, nsb_scatter_f32, nsb_flag_nonzero,
  * nsb_fused_color_fwd / _bwd, nsb_composite_forward / _backward.  With every size on the device a whole fwd+bwd step has no host
  * read and can be captured in a CUDA graph (neuralsim_b200/graphics/neus_static.py). */
 int nsb_bind_device_counts(const int64_t *count0, const int64_t *count1);
@@ -285,6 +285,19 @@ int nsb_neus_alpha_forward(const float *sdf, const int64_t *pack_infos, int64_t 
 /* adjoint of the above: d_sdf[S] (written), d_inv_s[1] (accumulated; caller zero-fills). */
 int nsb_neus_alpha_backward(const float *sdf, const int64_t *pack_infos, int64_t n_packs, const float *inv_s_dev, const float *d_alpha,
                             float *d_sdf, float *d_inv_s, void *stream);
+/* The same adjoint over the kept samples only, for a d_alpha that is zero outside them (the cotangent of the compression's gather).
+ * Inputs are nsb_scan_counts' outputs over the kept counts: nidx[j] = the pack of the j-th ray that keeps samples, pack_infos_kept[j] =
+ * its range in kept order, pidx[K] = the sample index of every kept sample, d_alpha[K] in kept order.  Pass 1 writes d_sdf[S] ONLY at
+ * the samples next to a kept interval with a non-zero cotangent (nothing else of d_sdf is touched), counts[j] = the non-zero d_sdf of
+ * ray j (0 for j in [live, n_packs)), and accumulates d_inv_s[1].  d_sdf equals nsb_neus_alpha_backward's bit for bit.  Pass 2, after
+ * offsets = exclusive scan of counts: list[offsets[j] + ..] = the sample indices with non-zero d_sdf, ascending (= flag(d_sdf != 0) +
+ * scan over all S samples), and ray[i] = the pack of every listed sample i.  Both count-aware (the rays that keep samples). */
+int nsb_neus_alpha_backward_kept(const float *sdf, const int64_t *pack_infos, const int64_t *nidx, const int64_t *pack_infos_kept,
+                                 const int64_t *pidx, int64_t n_packs, const float *inv_s_dev, const float *d_alpha, float *d_sdf,
+                                 int32_t *counts, float *d_inv_s, void *stream);
+int nsb_neus_alpha_backward_kept_list(const int64_t *pack_infos, const int64_t *nidx, const int64_t *pack_infos_kept, const int64_t *pidx,
+                                      const float *d_alpha, const float *d_sdf, const int32_t *offsets, int64_t n_packs, int64_t *list,
+                                      int64_t *ray, void *stream);
 /* Volume integration of one packed buffer (app/renderers/single_volume_renderer.py:73-102): vw = alpha_to_vw(alpha);
  * mask = sum vw; depth = sum vw t / (mask + 1e-10) (or sum vw t); rgb_out = sum vw rgb; nablas_out = sum vw nablas.
  * rgb / nablas ([K,3]) may be NULL.  ray_index[n_packs] (or NULL = identity): the per-ray outputs of pack p are written at
@@ -319,14 +332,17 @@ int nsb_merge_sorted_vals(const float *dep_a, const float *sdf_a, const int64_t 
 /* sort(cat(fine stages)) + merge_two_batch_a_includes_b with the coarse samples + ray ids + interval mid-points
  * (neus_ray_query.py:907-976): coarse[n_rays, n_coarse] sorted rows; fine[n_hit, n_fine] rows of the rays ridx_hit (sorted,
  * unique), each a concatenation of n_runs sorted runs of run_len_host[q] samples (one per up-sampling stage; HOST array, <= 8 runs).
- * -> d1, mid [S], ridx_all [S], pack_infos [n_rays, 2], S = n_rays n_coarse + n_hit n_fine. */
+ * -> d1, mid [S], ridx_all [S], pack_infos [n_rays, 2], S = n_rays n_coarse + n_hit n_fine.  mid and ridx_all may be NULL
+ * (not written: nsb_compact_samples can derive both at the kept samples). */
 int nsb_assemble_boundary(const float *coarse, int64_t n_rays, int32_t n_coarse, const int64_t *ridx_hit, int64_t n_hit, const float *fine,
                           int32_t n_fine, const int32_t *run_len_host, int32_t n_runs, float *d1, float *mid, int64_t *ridx_all,
                           int64_t *pack_infos, void *stream);
-/* gather of the samples packed_volume_render_compression keeps (pack_ops.py:286-291): slot = first_out[p] + rank inside the pack. */
+/* gather of the samples packed_volume_render_compression keeps (pack_ops.py:286-291): slot = first_out[p] + rank inside the pack.
+ * ridx_all == NULL: ridx_c = the pack index.  t == NULL: t_c = the interval mid-point of nsb_assemble_boundary computed from `d1`
+ * (the same value bit for bit); otherwise t_c = t[sample] and d1 is unused. */
 int nsb_compact_samples(const uint8_t *selector, const int64_t *pack_infos, const int32_t *first_out, const int32_t *kept, int64_t n_packs,
-                        const int64_t *ridx_all, const float *t, const float *alpha, int64_t *pidx, int64_t *ridx_c, float *t_c,
-                        float *alpha_c, void *stream);
+                        const int64_t *ridx_all, const float *t, const float *d1, const float *alpha, int64_t *pidx, int64_t *ridx_c,
+                        float *t_c, float *alpha_c, void *stream);
 /* dst[idx[j]] = src[j] (unique idx; adjoint of the gather above). */
 int nsb_scatter_f32(const float *src, const int64_t *idx, int64_t n, float *dst, void *stream);
 /* AABBSpace.ray_test (nr3d_lib/models/spatial/aabb.py:71-99): normalised rays o_n, d_n [n,3], clamped slab interval near / far [n]

@@ -107,6 +107,28 @@ k_neus_alpha_fwd(const float *__restrict__ sdf, const int64_t *__restrict__ pi, 
 
 // adjoint: alpha_i = max(0, (c_i - c_{i+1}) / (c_i + e)), c = sigmoid(s * inv_s)
 //   d alpha_i / d c_i = (c_{i+1} + e) / (c_i + e)^2 ,  d alpha_i / d c_{i+1} = -1 / (c_i + e)   (where the clamp is inactive: raw >= 0)
+// d_sdf of sample k of pack (b, n) from the cotangents of the two intervals it bounds (g_own: interval k, g_prev: interval k - 1, not
+// both 0); adds the sample's d_inv_s term to acc_invs.  Shared by the full-width and the kept-interval backward: the same value bit for bit.
+__device__ __forceinline__ float alpha_bwd_at(const float *__restrict__ sdf, int64_t b, int64_t n, int64_t k, float inv_s, float g_own,
+                                              float g_prev, float &acc_invs) {
+    const float s = sdf[b + k];
+    const float c = sigmoidf_(s * inv_s);
+    float gc = 0.f;                                             // dL/dc_k
+    if (k < n - 1) {                                            // as c_i of interval k
+        const float c1 = sigmoidf_(sdf[b + k + 1] * inv_s);
+        const float den = c + 1e-5f;
+        if ((c - c1) / den >= 0.f) gc += g_own * (c1 + 1e-5f) / (den * den);
+    }
+    if (k > 0) {                                                // as c_{i+1} of interval k-1
+        const float cp = sigmoidf_(sdf[b + k - 1] * inv_s);
+        const float den = cp + 1e-5f;
+        if ((cp - c) / den >= 0.f) gc -= g_prev / den;
+    }
+    const float dc = c * (1.f - c);
+    acc_invs += gc * dc * s;
+    return gc * dc * inv_s;
+}
+
 __global__ void __launch_bounds__(kNB)
 k_neus_alpha_bwd(const float *__restrict__ sdf, const int64_t *__restrict__ pi, int64_t n_packs, const float *__restrict__ inv_s_p,
                  const float *__restrict__ d_alpha, float *__restrict__ d_sdf, float *__restrict__ d_inv_s, const int64_t *__restrict__ n_dev) {
@@ -119,26 +141,98 @@ k_neus_alpha_bwd(const float *__restrict__ sdf, const int64_t *__restrict__ pi, 
         for (int64_t k = lane; k < n; k += 32) {
             const float g_own = (k < n - 1) ? d_alpha[b + k] : 0.f, g_prev = (k > 0) ? d_alpha[b + k - 1] : 0.f;
             if (g_own == 0.f && g_prev == 0.f) { d_sdf[b + k] = 0.f; continue; }     // most samples: compressed away / empty space
-            const float s = sdf[b + k];
-            const float c = sigmoidf_(s * inv_s);
-            float gc = 0.f;                                             // dL/dc_k
-            if (k < n - 1) {                                            // as c_i of interval k
-                const float c1 = sigmoidf_(sdf[b + k + 1] * inv_s);
-                const float den = c + 1e-5f;
-                if ((c - c1) / den >= 0.f) gc += g_own * (c1 + 1e-5f) / (den * den);
-            }
-            if (k > 0) {                                                // as c_{i+1} of interval k-1
-                const float cp = sigmoidf_(sdf[b + k - 1] * inv_s);
-                const float den = cp + 1e-5f;
-                if ((cp - c) / den >= 0.f) gc -= g_prev / den;
-            }
-            const float dc = c * (1.f - c);
-            d_sdf[b + k] = gc * dc * inv_s;
-            acc_invs += gc * dc * s;
+            d_sdf[b + k] = alpha_bwd_at(sdf, b, n, k, inv_s, g_own, g_prev, acc_invs);
         }
     }
     acc_invs = warp_sum(acc_invs);
     if (lane == 0 && acc_invs != 0.f) atomicAdd(d_inv_s, acc_invs);
+}
+
+// ------------------------------------------------------------------------------------------------ kept-interval alpha backward
+// The same adjoint driven by the compression's outputs: d_alpha is non-zero only at the K kept samples, so d_sdf can only be non-zero at
+// a kept sample k < n - 1 (g_own) or right after one (g_prev).  One warp per ray that keeps samples (j < live count): p = nidx[j] is its
+// boundary pack, its kept samples are pidx[o0 .. o0 + m) (ascending), (o0, m) = pinfo_kept[j], their cotangents d_alpha[o0 .. o0 + m).
+// Lane l of a 32-sample chunk owns kept sample k_l and -- unless it is kept too -- k_l + 1: ascending candidates across the lanes.
+struct KeptCand {
+    int64_t k[2];           // [0]: the kept sample itself, [1]: the sample after it
+    float g_own[2], g_prev[2];
+    bool live[2];           // a candidate with a non-zero cotangent on one of its intervals
+};
+
+__device__ __forceinline__ KeptCand kept_candidates(const int64_t *__restrict__ pidx, const float *__restrict__ d_alpha, int64_t o0, int64_t m,
+                                                    int64_t q, int64_t b, int64_t n) {
+    KeptCand c;
+    c.live[0] = c.live[1] = false;
+    if (q >= m) return c;
+    const int64_t k = pidx[o0 + q] - b;
+    const float g = d_alpha[o0 + q];
+    const bool prev_kept = q > 0 && pidx[o0 + q - 1] - b == k - 1;
+    const bool next_kept = q + 1 < m && pidx[o0 + q + 1] - b == k + 1;
+    c.k[0] = k;
+    c.g_own[0] = (k < n - 1) ? g : 0.f;
+    c.g_prev[0] = prev_kept ? d_alpha[o0 + q - 1] : 0.f;
+    c.live[0] = !(c.g_own[0] == 0.f && c.g_prev[0] == 0.f);
+    c.k[1] = k + 1;
+    c.g_own[1] = 0.f;
+    c.g_prev[1] = g;
+    c.live[1] = k < n - 1 && !next_kept && g != 0.f;
+    return c;
+}
+
+// pass 1: d_sdf at every live candidate (into the boundary-wide buffer, nothing else of it is written), the per-ray count of non-zero
+// d_sdf (0 for the rays in [live, n_cap)), d_inv_s
+__global__ void __launch_bounds__(kNB)
+k_neus_alpha_bwd_kept(const float *__restrict__ sdf, const int64_t *__restrict__ pi, const int64_t *__restrict__ nidx,
+                      const int64_t *__restrict__ pinfo_kept, const int64_t *__restrict__ pidx, int64_t n_cap, const float *__restrict__ inv_s_p,
+                      const float *__restrict__ d_alpha, float *__restrict__ d_sdf, int32_t *__restrict__ counts, float *__restrict__ d_inv_s,
+                      const int64_t *__restrict__ n_dev) {
+    const int lane = threadIdx.x & 31;
+    const float inv_s = inv_s_p[0];
+    const int64_t live = eff_n(n_cap, n_dev);
+    for (int64_t j = live + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n_cap; j += (int64_t)gridDim.x * blockDim.x) counts[j] = 0;
+    float acc_invs = 0.f;
+    for (int64_t j = gwarp(); j < live; j += nwarps()) {
+        const int64_t p = nidx[j], b = pi[2 * p], n = pi[2 * p + 1], o0 = pinfo_kept[2 * j], m = pinfo_kept[2 * j + 1];
+        int nz = 0;
+        for (int64_t q = lane; q - lane < m; q += 32) {
+            const KeptCand c = kept_candidates(pidx, d_alpha, o0, m, q, b, n);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                if (!c.live[e]) continue;
+                const float d = alpha_bwd_at(sdf, b, n, c.k[e], inv_s, c.g_own[e], c.g_prev[e], acc_invs);
+                d_sdf[b + c.k[e]] = d;
+                nz += d != 0.f;
+            }
+        }
+        nz = __reduce_add_sync(0xffffffffu, nz);
+        if (lane == 0) counts[j] = nz;
+    }
+    acc_invs = warp_sum(acc_invs);
+    if (lane == 0 && acc_invs != 0.f) atomicAdd(d_inv_s, acc_invs);
+}
+
+// pass 2: list[offs[j] + ...] = the boundary indices of ray j's non-zero d_sdf, ascending (what a flag + scan over the boundary-wide
+// d_sdf gives); ray[i] = the ray (pack) of listed index i
+__global__ void __launch_bounds__(kNB)
+k_neus_alpha_bwd_kept_list(const int64_t *__restrict__ pi, const int64_t *__restrict__ nidx, const int64_t *__restrict__ pinfo_kept,
+                           const int64_t *__restrict__ pidx, const float *__restrict__ d_alpha, const float *__restrict__ d_sdf,
+                           const int32_t *__restrict__ offs, int64_t n_packs, int64_t *__restrict__ list, int64_t *__restrict__ ray,
+                           const int64_t *__restrict__ n_dev) {
+    const int lane = threadIdx.x & 31;
+    n_packs = eff_n(n_packs, n_dev);
+    for (int64_t j = gwarp(); j < n_packs; j += nwarps()) {
+        const int64_t p = nidx[j], b = pi[2 * p], n = pi[2 * p + 1], o0 = pinfo_kept[2 * j], m = pinfo_kept[2 * j + 1];
+        int64_t out = offs[j];
+        for (int64_t q = lane; q - lane < m; q += 32) {
+            const KeptCand c = kept_candidates(pidx, d_alpha, o0, m, q, b, n);
+            const bool f0 = c.live[0] && d_sdf[b + c.k[0]] != 0.f, f1 = c.live[1] && d_sdf[b + c.k[1]] != 0.f;
+            const uint32_t m0 = __ballot_sync(0xffffffffu, f0), m1 = __ballot_sync(0xffffffffu, f1), lt = (1u << lane) - 1u;
+            const int64_t o = out + __popc(m0 & lt) + __popc(m1 & lt);
+            if (f0) { list[o] = b + c.k[0]; ray[b + c.k[0]] = p; }
+            if (f1) { list[o + f0] = b + c.k[1]; ray[b + c.k[1]] = p; }
+            out += __popc(m0) + __popc(m1);
+        }
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ compositing
@@ -284,6 +378,30 @@ extern "C" int nsb_neus_alpha_backward(const float *sdf, const int64_t *pack_inf
     NSB_REQUIRE(sdf && pack_infos && inv_s_dev && d_alpha && d_sdf && d_inv_s, "nsb_neus_alpha_backward: NULL argument");
     k_neus_alpha_bwd<<<pack_grid(n_packs), kNB, 0, STREAM>>>(sdf, pack_infos, n_packs, inv_s_dev, d_alpha, d_sdf, d_inv_s, dn.a);
     return check_launch("nsb_neus_alpha_backward");
+}
+
+extern "C" int nsb_neus_alpha_backward_kept(const float *sdf, const int64_t *pack_infos, const int64_t *nidx, const int64_t *pack_infos_kept,
+                                            const int64_t *pidx, int64_t n_packs, const float *inv_s_dev, const float *d_alpha, float *d_sdf,
+                                            int32_t *counts, float *d_inv_s, void *stream) {
+    const DevCounts dn = take_counts();
+    if (n_packs == 0) return 0;
+    NSB_REQUIRE(sdf && pack_infos && nidx && pack_infos_kept && pidx && inv_s_dev && d_alpha && d_sdf && counts && d_inv_s,
+                "nsb_neus_alpha_backward_kept: NULL argument");
+    k_neus_alpha_bwd_kept<<<pack_grid(n_packs), kNB, 0, STREAM>>>(sdf, pack_infos, nidx, pack_infos_kept, pidx, n_packs, inv_s_dev, d_alpha, d_sdf,
+                                                                  counts, d_inv_s, dn.a);
+    return check_launch("nsb_neus_alpha_backward_kept");
+}
+
+extern "C" int nsb_neus_alpha_backward_kept_list(const int64_t *pack_infos, const int64_t *nidx, const int64_t *pack_infos_kept, const int64_t *pidx,
+                                                 const float *d_alpha, const float *d_sdf, const int32_t *offsets, int64_t n_packs, int64_t *list,
+                                                 int64_t *ray, void *stream) {
+    const DevCounts dn = take_counts();
+    if (n_packs == 0) return 0;
+    NSB_REQUIRE(pack_infos && nidx && pack_infos_kept && pidx && d_alpha && d_sdf && offsets && list && ray,
+                "nsb_neus_alpha_backward_kept_list: NULL argument");
+    k_neus_alpha_bwd_kept_list<<<pack_grid(n_packs), kNB, 0, STREAM>>>(pack_infos, nidx, pack_infos_kept, pidx, d_alpha, d_sdf, offsets, n_packs, list,
+                                                                       ray, dn.a);
+    return check_launch("nsb_neus_alpha_backward_kept_list");
 }
 
 extern "C" int nsb_composite_forward(const float *alpha, const float *t, const float *rgb, const float *nablas, const int64_t *pack_infos,

@@ -196,6 +196,12 @@ k_merge_vals(const float *__restrict__ dep_a, const float *__restrict__ sdf_a, c
 constexpr int kAsmWarps = 8, kAsmMaxRuns = 8, kAsmChunk = 8;
 struct AsmRuns { int n, len[kAsmMaxRuns]; };              // the fine row is a concatenation of `n` sorted runs (one per up-sampling stage)
 
+// mid[k] of a sorted pack: d_k + (d_{k+1} - d_k) / 2, the last sample's own depth + 0 (k_assemble_boundary, k_compact_samples)
+__device__ __forceinline__ float interval_mid(float v, float next, bool last) {
+    const float diff = last ? 0.f : __fsub_rn(next, v);
+    return __fadd_rn(v, __fmul_rn(diff, 0.5f));
+}
+
 __device__ __forceinline__ int count_less(const float *a, int n, float v, bool or_equal) {   // #{a_i < v} or #{a_i <= v}, a sorted
     int lo = 0, cnt = n;
     while (cnt > 0) {
@@ -241,10 +247,9 @@ k_assemble_boundary(const float *__restrict__ coarse, int64_t n_rays, int nc, co
             if (!hit) {                                   // the coarse row is already sorted: straight copy
                 for (int k = lane; k < nc; k += 32) {
                     const float v = coarse[r * nc + k];
-                    const float diff = (k < nc - 1) ? __fsub_rn(coarse[r * nc + k + 1], v) : 0.f;
                     d1[first + k] = v;
-                    mid[first + k] = __fadd_rn(v, __fmul_rn(diff, 0.5f));
-                    ridx_all[first + k] = r;
+                    if (mid) mid[first + k] = interval_mid(v, k < nc - 1 ? coarse[r * nc + k + 1] : 0.f, k == nc - 1);
+                    if (ridx_all) ridx_all[first + k] = r;
                 }
                 continue;
             }
@@ -268,10 +273,9 @@ k_assemble_boundary(const float *__restrict__ coarse, int64_t n_rays, int nc, co
             __syncwarp();
             for (int k = lane; k < n; k += 32) {
                 const float v = srt[k];
-                const float diff = (k < n - 1) ? __fsub_rn(srt[k + 1], v) : 0.f;
                 d1[first + k] = v;
-                mid[first + k] = __fadd_rn(v, __fmul_rn(diff, 0.5f));
-                ridx_all[first + k] = r;
+                if (mid) mid[first + k] = interval_mid(v, k < n - 1 ? srt[k + 1] : 0.f, k == n - 1);
+                if (ridx_all) ridx_all[first + k] = r;
             }
         }
     }
@@ -279,11 +283,12 @@ k_assemble_boundary(const float *__restrict__ coarse, int64_t n_rays, int nc, co
 
 // ------------------------------------------------------------------------------------------------ compaction of the kept samples
 // selector[S] marks the samples packed_volume_render_compression keeps; first_out[p] = exclusive scan of the kept counts.
-// Kept sample s of pack p -> slot first_out[p] + (number of kept samples before s in the pack).
+// Kept sample s of pack p -> slot first_out[p] + (number of kept samples before s in the pack).  Without ridx_all the ray is the pack;
+// without t the depth is the mid-point of the sample's interval in d1 (what k_assemble_boundary writes to `mid`).
 __global__ void __launch_bounds__(256)
 k_compact_samples(const uint8_t *__restrict__ selector, const int64_t *__restrict__ pi, const int32_t *__restrict__ first_out,
                   const int32_t *__restrict__ kept, int64_t n_packs, const int64_t *__restrict__ ridx_all, const float *__restrict__ t,
-                  const float *__restrict__ alpha, int64_t *__restrict__ pidx, int64_t *__restrict__ ridx_c, float *__restrict__ t_c,
+                  const float *__restrict__ d1, const float *__restrict__ alpha, int64_t *__restrict__ pidx, int64_t *__restrict__ ridx_c, float *__restrict__ t_c,
                   float *__restrict__ alpha_c, const int64_t *__restrict__ n_dev) {
     const int lane = threadIdx.x & 31;
     n_packs = eff_n(n_packs, n_dev);
@@ -300,8 +305,8 @@ k_compact_samples(const uint8_t *__restrict__ selector, const int64_t *__restric
             if (sel) {
                 const int64_t o = out + __popc(m & ((1u << lane) - 1u));
                 pidx[o] = b + k;
-                ridx_c[o] = ridx_all[b + k];
-                t_c[o] = t[b + k];
+                ridx_c[o] = ridx_all ? ridx_all[b + k] : p;
+                t_c[o] = t ? t[b + k] : interval_mid(d1[b + k], k < n - 1 ? d1[b + k + 1] : 0.f, k == n - 1);
                 alpha_c[o] = alpha[b + k];
             }
             const int c = __popc(m);
@@ -574,7 +579,7 @@ extern "C" int nsb_assemble_boundary(const float *coarse, int64_t n_rays, int32_
                                      int64_t *pack_infos, void *stream) {
     const DevCounts dn = take_counts();
     if (n_rays == 0) return 0;
-    NSB_REQUIRE(coarse && d1 && mid && ridx_all && pack_infos, "nsb_assemble_boundary: NULL argument");
+    NSB_REQUIRE(coarse && d1 && pack_infos, "nsb_assemble_boundary: NULL argument");
     NSB_REQUIRE(n_hit == 0 || (ridx_hit && fine), "nsb_assemble_boundary: hit rays need ridx_hit and fine");
     NSB_REQUIRE(n_coarse > 0 && n_fine >= 0 && n_coarse + n_fine <= 1024, "nsb_assemble_boundary: n_coarse + n_fine must be <= 1024");
     const size_t smem = (size_t)kAsmWarps * 2 * (n_coarse + n_fine) * sizeof(float);
@@ -593,14 +598,14 @@ extern "C" int nsb_assemble_boundary(const float *coarse, int64_t n_rays, int32_
 }
 
 extern "C" int nsb_compact_samples(const uint8_t *selector, const int64_t *pack_infos, const int32_t *first_out, const int32_t *kept, int64_t n_packs,
-                                   const int64_t *ridx_all, const float *t, const float *alpha, int64_t *pidx, int64_t *ridx_c, float *t_c,
-                                   float *alpha_c, void *stream) {
+                                   const int64_t *ridx_all, const float *t, const float *d1, const float *alpha, int64_t *pidx, int64_t *ridx_c,
+                                   float *t_c, float *alpha_c, void *stream) {
     const DevCounts dn = take_counts();
     if (n_packs == 0) return 0;
-    NSB_REQUIRE(selector && pack_infos && first_out && kept && ridx_all && t && alpha && pidx && ridx_c && t_c && alpha_c,
+    NSB_REQUIRE(selector && pack_infos && first_out && kept && (t || d1) && alpha && pidx && ridx_c && t_c && alpha_c,
                 "nsb_compact_samples: NULL argument");
-    k_compact_samples<<<wave_grid(n_packs * 32, 256, 8), 256, 0, STREAM>>>(selector, pack_infos, first_out, kept, n_packs, ridx_all, t, alpha, pidx, ridx_c,
-                                                                          t_c, alpha_c, dn.a);
+    k_compact_samples<<<wave_grid(n_packs * 32, 256, 8), 256, 0, STREAM>>>(selector, pack_infos, first_out, kept, n_packs, ridx_all, t, d1, alpha, pidx,
+                                                                          ridx_c, t_c, alpha_c, dn.a);
     return check_launch("nsb_compact_samples");
 }
 

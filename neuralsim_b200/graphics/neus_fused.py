@@ -225,7 +225,7 @@ def neus_alpha_compact(sdf, inv_s, pack_infos, ridx_all, t_mid, rays_inds, early
         pidx, ridx_c = torch.empty(K, dtype=torch.int64, device=dev), torch.empty(K, dtype=torch.int64, device=dev)
         t_c, alpha_c = torch.empty(K, dtype=torch.float32, device=dev), torch.empty(K, dtype=torch.float32, device=dev)
         L.check(L.lib().nsb_compact_samples(L.ptr(sel.view(torch.uint8), "u8"), L.ptr(pack_infos, "i64"), L.ptr(sc["first"], "i32"), L.ptr(steps, "i32"),
-                                            L.c_i64(pack_infos.shape[0]), L.ptr(ridx_all, "i64"), L.ptr(t_mid, "f32"), L.ptr(alpha.detach(), "f32"),
+                                            L.c_i64(pack_infos.shape[0]), L.ptr(ridx_all, "i64"), L.ptr(t_mid, "f32"), None, L.ptr(alpha.detach(), "f32"),
                                             L.ptr(pidx), L.ptr(ridx_c), L.ptr(t_c), L.ptr(alpha_c), L.stream_ptr()), "compact_samples")
     alpha_k = _GatherUnique.apply(alpha, pidx, alpha_c) if alpha.requires_grad else alpha_c
     return dict(alpha=alpha_k, ridx=ridx_c, t=t_c, pack_infos=sc["pack"], nidx=sc["index"], rays_inds_hit=sc["src"], pidx=pidx)

@@ -99,91 +99,75 @@ def _block_order(rays_inds, via, n_rays, cnt, slot):
 
 
 # ---------------------------------------------------------------------------------------------------------------- autograd pieces
-class _StaticSDF(torch.autograd.Function):
-    """boundary SDF query with grad (fields/networks.py:_FusedSDF with device-resident sizes): the backward compacts the samples with a
-    non-zero cotangent by flag -> scan -> index list, all on the device, and runs k_sdf_bwd_tc over that list."""
+class _StaticBoundary(torch.autograd.Function):
+    """boundary SDF query -> alpha -> compression -> gather of the kept samples (fields/networks.py:_FusedSDF + graphics/neus_fused.py:
+    neus_alpha_compact with device-resident sizes).  -> alpha of the K kept samples (differentiable in inv_s and the SDF parameters) and
+    their depth, ray, the kept packs and their pixels.  The backward runs over the kept samples only: d_alpha is zero everywhere else, so
+    the kept-interval adjoint (nsb_neus_alpha_backward_kept) lists the boundary samples with a non-zero d_sdf -- per-ray counts, a scan
+    over the rays, the list -- and k_sdf_bwd_tc walks that list; nothing boundary-wide is filled, scattered, flagged or scanned."""
 
     @staticmethod
-    def forward(ctx, st, ridx, t, packs, count_slot, grid, W1, b1, W2, b2):
-        sdf = torch.empty(t.numel(), dtype=torch.float32, device=t.device)
-        _sdf_launch(st.meta, st.grid16, st.dec, st.rays_o, st.rays_d, t, sdf, ridx=ridx if packs is None else None, packs=packs, ml=st.ml,
-                    collect=st.collect, cnt=st.cnt, slot=count_slot, timer="fused_sdf_fwd")
-        ctx.st, ctx.ridx, ctx.t = st, ridx, t
-        ctx.shapes = (grid.shape, W1.shape, b1.shape, W2.shape, b2.shape)
-        return sdf
+    def forward(ctx, st, d1, pinfo, ridx_all, order_b, rays_inds, kept_cap, qc, inv_s, grid, W1, b1, W2, b2):
+        """ridx_all None: coherent rays, the query walks the packs in the 8 x 4 pixel-block order order_b; else sample by sample"""
+        R, dev, cnt, P, lib = pinfo.shape[0], d1.device, st.cnt, L.ptr, L.lib()
+        sdf = torch.empty(d1.numel(), dtype=torch.float32, device=dev)
+        _sdf_launch(st.meta, st.grid16, st.dec, st.rays_o, st.rays_d, d1, sdf, ridx=ridx_all, packs=(pinfo, None, order_b) if ridx_all is None else None,
+                    ml=st.ml, collect=st.collect, cnt=cnt, slot=CNT_SLOTS["n_rays"] if ridx_all is None else CNT_SLOTS["boundary"], timer="fused_sdf_fwd")
+        inv_c = inv_s.detach().contiguous().float().reshape(1)
+        alpha = torch.empty_like(sdf)
+        sel = torch.empty(sdf.shape[0], dtype=torch.bool, device=dev)
+        steps = torch.empty(R, dtype=torch.int32, device=dev)
+        _call(lib.nsb_neus_alpha_forward, "neus_alpha_forward", cnt, CNT_SLOTS["n_rays"], None, P(sdf, "f32"), P(pinfo, "i64"), L.c_i64(R),
+              P(inv_c, "f32"), L.c_f32(1e-4), L.c_f32(0.0), P(alpha), P(sel), P(steps), L.stream_ptr())
+        first = torch.empty(R, dtype=torch.int32, device=dev)
+        nidx = torch.empty(R, dtype=torch.int64, device=dev)
+        pinfo_kept = torch.empty(R, 2, dtype=torch.int64, device=dev)
+        rays_inds_hit = torch.empty(R, dtype=torch.int64, device=dev)
+        _scan(steps, cnt, CNT_SLOTS["kept_raw"], first=first, index=nidx, pack=pinfo_kept, src=rays_inds, nz_src=rays_inds_hit, ws=st.ws[2])
+        _query_counts(cnt, 1, *qc)
+        pidx, ridx_k = torch.empty(kept_cap, dtype=torch.int64, device=dev), torch.empty(kept_cap, dtype=torch.int64, device=dev)
+        t_k, alpha_k = torch.empty(kept_cap, dtype=torch.float32, device=dev), torch.empty(kept_cap, dtype=torch.float32, device=dev)
+        _call(lib.nsb_compact_samples, "compact_samples", cnt, CNT_SLOTS["rays_if_kept_fits"], None, P(sel.view(torch.uint8), "u8"), P(pinfo, "i64"),
+              P(first, "i32"), P(steps, "i32"), L.c_i64(R), None, None, P(d1, "f32"), P(alpha, "f32"), P(pidx), P(ridx_k), P(t_k), P(alpha_k), L.stream_ptr())
+        ctx.st, ctx.saved = st, (d1, sdf, inv_c, pinfo, nidx, pinfo_kept, pidx)
+        ctx.shapes = (inv_s.shape, grid.shape, W1.shape, b1.shape, W2.shape, b2.shape)
+        ctx.mark_non_differentiable(t_k, ridx_k, pinfo_kept, rays_inds_hit)
+        return alpha_k, t_k, ridx_k, pinfo_kept, rays_inds_hit
 
     @staticmethod
     @torch.autograd.function.once_differentiable
-    def backward(ctx, d_sdf):
-        st, dev = ctx.st, d_sdf.device
-        gs, w1s, b1s, w2s, b2s = ctx.shapes
+    def backward(ctx, g_alpha, _gt, _gr, _gp, _gi):
+        st, (d1, sdf, inv_c, pinfo, nidx, pinfo_kept, pidx) = ctx.st, ctx.saved
+        dev, R, S, K = sdf.device, pinfo.shape[0], sdf.numel(), pidx.numel()
+        inv_shape, gs, w1s, b1s, w2s, b2s = ctx.shapes
         d_grid = torch.zeros(gs, dtype=torch.float32, device=dev)
         ks = [int(torch.Size(x).numel()) for x in (w1s, b1s, w2s, b2s)]
-        small = torch.zeros(sum(ks), dtype=torch.float32, device=dev)
-        d_W1, d_b1 = small[:ks[0]].view(w1s), small[ks[0]:ks[0] + ks[1]].view(b1s)
-        d_W2, d_b2 = small[ks[0] + ks[1]:ks[0] + ks[1] + ks[2]].view(w2s), small[ks[0] + ks[1] + ks[2]:].view(b2s)
-        d_sdf = d_sdf.contiguous().float()
-        n = d_sdf.numel()
-        P, cnt = L.ptr, st.cnt
-        flag = torch.empty(n, dtype=torch.int32, device=dev)
-        _call(L.lib().nsb_flag_nonzero, "flag_nonzero", cnt, CNT_SLOTS["boundary"], None, P(d_sdf, "f32"), L.c_i64(n), P(flag), L.stream_ptr())
-        keep = torch.empty(n, dtype=torch.int64, device=dev)
-        _scan(flag, cnt, CNT_SLOTS["nonzero"], index=keep, ws=st.ws[3])
-        with L.KERNEL_TIMER.time("fused_sdf_bwd", n):
-            _call(L.lib().nsb_fused_sdf_bwd_indexed, "fused_sdf_bwd", cnt, CNT_SLOTS["nonzero"], None,
-                  st.meta.c_ref, P(st.grid16, "f16"), ctypes.byref(st.dec), None, P(st.rays_o, "f32"), P(st.rays_d, "f32"), P(ctx.ridx, "i64"),
-                  P(ctx.t, "f32"), P(d_sdf, "f32"), P(keep, "i64"), L.c_i64(n), L.c_i32(st.ml), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2),
-                  L.stream_ptr())
-        return None, None, None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2
-
-
-class _StaticAlpha(torch.autograd.Function):
-    """graphics/neus_fused.py:_NeusAlpha over the live packs cnt[0]"""
-
-    @staticmethod
-    def forward(ctx, sdf, inv_s, pack_infos, cnt, early_stop_eps, alpha_thre):
-        sdf_c, inv_c = sdf.detach().contiguous().float(), inv_s.detach().contiguous().float().reshape(1)
-        Pn, dev = pack_infos.shape[0], sdf_c.device
-        alpha = torch.empty_like(sdf_c)
-        sel = torch.empty(sdf_c.shape[0], dtype=torch.bool, device=dev)
-        steps = torch.empty(Pn, dtype=torch.int32, device=dev)
-        P = L.ptr
-        _call(L.lib().nsb_neus_alpha_forward, "neus_alpha_forward", cnt, CNT_SLOTS["n_rays"], None, P(sdf_c, "f32"), P(pack_infos, "i64"), L.c_i64(Pn),
-              P(inv_c, "f32"), L.c_f32(early_stop_eps), L.c_f32(alpha_thre), P(alpha), P(sel), P(steps), L.stream_ptr())
-        ctx.save_for_backward(sdf_c, inv_c, pack_infos)
-        ctx.cnt, ctx.inv_shape = cnt, inv_s.shape
-        ctx.mark_non_differentiable(sel, steps)
-        return alpha, sel, steps
-
-    @staticmethod
-    def backward(ctx, g_alpha, _gs, _gn):
-        sdf_c, inv_c, pack_infos = ctx.saved_tensors
-        g = g_alpha.contiguous().float()
-        d_sdf = torch.empty_like(sdf_c)
-        d_inv = torch.zeros(1, device=sdf_c.device, dtype=torch.float32)
-        P = L.ptr
-        _call(L.lib().nsb_neus_alpha_backward, "neus_alpha_backward", ctx.cnt, CNT_SLOTS["n_rays"], None, P(sdf_c, "f32"), P(pack_infos, "i64"),
-              L.c_i64(pack_infos.shape[0]), P(inv_c, "f32"), P(g, "f32"), P(d_sdf), P(d_inv), L.stream_ptr())
-        return (d_sdf if ctx.needs_input_grad[0] else None, d_inv.reshape(ctx.inv_shape) if ctx.needs_input_grad[1] else None, None, None, None, None)
-
-
-class _StaticGather(torch.autograd.Function):
-    """out = the kernel-made gather src[pidx[:K]]; backward scatters the K live rows into zeros"""
-
-    @staticmethod
-    def forward(ctx, src, pidx, gathered, cnt):
-        ctx.save_for_backward(pidx)
-        ctx.n, ctx.cnt = src.shape[0], cnt
-        return gathered
-
-    @staticmethod
-    def backward(ctx, g):
-        pidx, = ctx.saved_tensors
-        g = g.contiguous().float()
-        d = torch.zeros(ctx.n, dtype=torch.float32, device=g.device)
-        P = L.ptr
-        _call(L.lib().nsb_scatter_f32, "scatter_f32", ctx.cnt, CNT_SLOTS["kept"], None, P(g, "f32"), P(pidx, "i64"), L.c_i64(pidx.shape[0]), P(d), L.stream_ptr())
-        return d, None, None, None
+        small = torch.zeros(1 + sum(ks), dtype=torch.float32, device=dev)
+        d_inv, o = small[:1], 1
+        d_W1, d_b1 = small[o:o + ks[0]].view(w1s), small[o + ks[0]:o + ks[0] + ks[1]].view(b1s)
+        o += ks[0] + ks[1]
+        d_W2, d_b2 = small[o:o + ks[2]].view(w2s), small[o + ks[2]:].view(b2s)
+        P, cnt, lib = L.ptr, st.cnt, L.lib()
+        if g_alpha is not None:
+            g = g_alpha.contiguous().float()
+            d_sdf = torch.empty(S, dtype=torch.float32, device=dev)            # written at the listed samples only
+            ray = torch.empty(S, dtype=torch.int64, device=dev)                # (the same)
+            counts = torch.empty(R, dtype=torch.int32, device=dev)
+            a = (P(pinfo, "i64"), P(nidx, "i64"), P(pinfo_kept, "i64"), P(pidx, "i64"))
+            _call(lib.nsb_neus_alpha_backward_kept, "neus_alpha_backward_kept", cnt, CNT_SLOTS["kept_rays"], None, P(sdf, "f32"), *a, L.c_i64(R),
+                  P(inv_c, "f32"), P(g, "f32"), P(d_sdf), P(counts), P(d_inv), L.stream_ptr())
+            offs = torch.empty(R, dtype=torch.int32, device=dev)
+            _scan(counts, cnt, CNT_SLOTS["nonzero"], first=offs, ws=st.ws[3])
+            n_list = min(S, 2 * K)                         # at most a kept sample and the one after it per kept sample
+            keep = torch.empty(n_list, dtype=torch.int64, device=dev)
+            _call(lib.nsb_neus_alpha_backward_kept_list, "neus_alpha_backward_kept_list", cnt, CNT_SLOTS["kept_rays"], None, *a, P(g, "f32"), P(d_sdf, "f32"),
+                  P(offs, "i32"), L.c_i64(R), P(keep), P(ray), L.stream_ptr())
+            with L.KERNEL_TIMER.time("fused_sdf_bwd", n_list):
+                _call(lib.nsb_fused_sdf_bwd_indexed, "fused_sdf_bwd", cnt, CNT_SLOTS["nonzero"], None,
+                      st.meta.c_ref, P(st.grid16, "f16"), ctypes.byref(st.dec), None, P(st.rays_o, "f32"), P(st.rays_d, "f32"), P(ray, "i64"),
+                      P(d1, "f32"), P(d_sdf, "f32"), P(keep, "i64"), L.c_i64(n_list), L.c_i32(st.ml), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2),
+                      L.stream_ptr())
+        return (None,) * 8 + (d_inv.reshape(inv_shape), d_grid, d_W1, d_b1, d_W2, d_b2)
 
 
 class _StaticColor(torch.autograd.Function):
@@ -469,33 +453,22 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         if fine_stages is not None:
             fine_all = (torch.cat(fine_stages, dim=-1) if n_stage > 1 else fine_stages[0]).contiguous()
         d1 = torch.empty(S_cap, dtype=torch.float32, device=dev)
-        mid = torch.empty(S_cap, dtype=torch.float32, device=dev)
-        ridx_all = torch.empty(S_cap, dtype=torch.int64, device=dev)
+        # the ray of every boundary sample: only the incoherent boundary query (one sample per row) reads it; everything else derives it
+        ridx_all = None if coherent else torch.empty(S_cap, dtype=torch.int64, device=dev)
         pinfo = torch.empty(R, 2, dtype=torch.int64, device=dev)
         rl = (ctypes.c_int32 * n_stage)(*num_fine)
         _call(lib.nsb_assemble_boundary, "assemble_boundary", cnt, CNT_SLOTS["n_rays"], CNT_SLOTS["hit"], P(coarse, "f32"), L.c_i64(R), L.c_i32(nc1),
-              P(ridx_hit, "i64"), L.c_i64(R), P(fine_all, "f32"), L.c_i32(nf_tot), rl, L.c_i32(n_stage), P(d1), P(mid), P(ridx_all), P(pinfo), L.stream_ptr())
+              P(ridx_hit, "i64"), L.c_i64(R), P(fine_all, "f32"), L.c_i32(nf_tot), rl, L.c_i32(n_stage), P(d1), None, P(ridx_all, "i64", allow_none=True), P(pinfo),
+              L.stream_ptr())
     # ---------------- boundary SDF (grad) -> alpha -> compression
     s, b = model.implicit_surface, model.radiance_net.blocks.layers
     dl = s.decoder.layers
-    sdf_b = _StaticSDF.apply(st, ridx_all, d1, (pinfo, None, order_b) if coherent else None, CNT_SLOTS["n_rays"] if coherent else CNT_SLOTS["boundary"],
-                             s.encoding.flattened_params, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
     inv_s = model.forward_inv_s()
     if not isinstance(inv_s, torch.Tensor):
         inv_s = torch.tensor(float(inv_s), device=dev)
-    alpha, sel, steps = _StaticAlpha.apply(sdf_b, inv_s, pinfo, cnt, 1e-4, 0.0)
-    with torch.no_grad():
-        first = torch.empty(R, dtype=torch.int32, device=dev)
-        nidx = torch.empty(R, dtype=torch.int64, device=dev)
-        pinfo_kept = torch.empty(R, 2, dtype=torch.int64, device=dev)
-        rays_inds_hit = torch.empty(R, dtype=torch.int64, device=dev)
-        _scan(steps, cnt, CNT_SLOTS["kept_raw"], first=first, index=nidx, pack=pinfo_kept, src=rays_inds, nz_src=rays_inds_hit, ws=st.ws[2])
-        _query_counts(cnt, 1, nc1, num_fine, march_cap, kept_cap)
-        pidx, ridx_k = torch.empty(kept_cap, dtype=torch.int64, device=dev), torch.empty(kept_cap, dtype=torch.int64, device=dev)
-        t_k, alpha_c = torch.empty(kept_cap, dtype=torch.float32, device=dev), torch.empty(kept_cap, dtype=torch.float32, device=dev)
-        _call(lib.nsb_compact_samples, "compact_samples", cnt, CNT_SLOTS["rays_if_kept_fits"], None, P(sel.view(torch.uint8), "u8"), P(pinfo, "i64"), P(first, "i32"),
-              P(steps, "i32"), L.c_i64(R), P(ridx_all, "i64"), P(mid, "f32"), P(alpha.detach(), "f32"), P(pidx), P(ridx_k), P(t_k), P(alpha_c), L.stream_ptr())
-    alpha_k = _StaticGather.apply(alpha, pidx, alpha_c, cnt) if alpha.requires_grad else alpha_c
+    alpha_k, t_k, ridx_k, pinfo_kept, rays_inds_hit = _StaticBoundary.apply(
+        st, d1, pinfo, ridx_all, order_b, rays_inds, kept_cap,
+        (nc1, num_fine, march_cap, kept_cap), inv_s, s.encoding.flattened_params, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
     # ---------------- colour / normal query on the kept samples
     params = (s.encoding.flattened_params, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias, b[0].weight, b[0].bias, b[1].weight, b[1].bias,
               b[2].weight, b[2].bias)
