@@ -317,6 +317,7 @@ int nsb_composite_backward(const float *alpha, const float *t, const float *rgb,
  *   pack_ops.py:286-291): first[n] = exclusive prefix sum of counts; info2[n,2] = (first, count) int32 (`packed_info`);
  *   for the non-zero entries in order: nz_index[j] = i, nz_pack[j] = (first_i, count_i), nz_src[j] = src[i];
  *   totals[2] = (sum of counts, number of non-zero entries), on the device.  Outputs other than totals may be NULL.
+ *   first / info2 are int32 and valid only while the sum of counts is below 2^31; totals and nz_pack are int64 and always exact.
  *   workspace_zeroed: nsb_scan_workspace_bytes() of device memory, zero-filled before every call.
  *   Host hand-off without a driver call: `totals` may point to mapped pinned host memory of >= 4 int64; with ticket != 0 the kernel
  *   writes totals[2] = *extra_src (if given) and, after a system-scope fence, totals[3] = ticket, which the host polls. */
@@ -330,8 +331,8 @@ int64_t nsb_scan_workspace_bytes(void);
 int nsb_merge_sorted_vals(const float *dep_a, const float *sdf_a, const int64_t *pack_infos_a, const float *dep_b, const float *sdf_b,
                           int64_t n_packs, int32_t n_b, float *dep_m, float *sdf_m, int64_t *pack_infos_m, void *stream);
 /* sort(cat(fine stages)) + merge_two_batch_a_includes_b with the coarse samples + ray ids + interval mid-points
- * (neus_ray_query.py:907-976): coarse[n_rays, n_coarse] sorted rows; fine[n_hit, n_fine] rows of the rays ridx_hit (sorted,
- * unique), each a concatenation of n_runs sorted runs of run_len_host[q] samples (one per up-sampling stage; HOST array, <= 8 runs).
+ * (neus_ray_query.py:907-976): coarse[n_rays, n_coarse] sorted rows; fine[n_hit, n_fine] rows of the rays ridx_hit (which must be
+ * ascending and unique: the kernel finds a ray in the list by binary search), each a concatenation of n_runs sorted runs of run_len_host[q] samples (one per up-sampling stage; HOST array, <= 8 runs).
  * -> d1, mid [S], ridx_all [S], pack_infos [n_rays, 2], S = n_rays n_coarse + n_hit n_fine.  mid and ridx_all may be NULL
  * (not written: nsb_compact_samples can derive both at the kept samples). */
 int nsb_assemble_boundary(const float *coarse, int64_t n_rays, int32_t n_coarse, const int64_t *ridx_hit, int64_t n_hit, const float *fine,

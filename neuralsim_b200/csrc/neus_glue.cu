@@ -10,8 +10,9 @@
 //                        mid-points  (neus_ray_query.py:907-976)
 //   k_compact_samples    packed_volume_render_compression's gather of the kept samples (pack_ops.py:286-291 + :1010-1030)
 //
-// All outputs are the reference's values (same fp32 roundings; ties between equal depths carry equal payloads, so the order
-// inside a tie is immaterial).
+// All outputs are the reference's values (same fp32 roundings).  Equal depths keep a fixed order: in the merge a b goes before an equal
+// a, in the boundary assembly the order is (coarse, run 0, run 1, ...).  The step's ties carry equal payloads, so only the sign bit
+// of a +0.0 / -0.0 tie shows it (tests/test_glue_edges_gpu.py pins it).
 #include "nsb_common.cuh"
 
 namespace nsb {

@@ -1,5 +1,6 @@
-"""Glue kernels of the per-ray query (csrc/neus_glue.cu) against the chains of reference-API calls they replace
-(pack_ops / raymarch / raysample wrappers of this package, themselves pinned against the reference's kernels and the oracle)."""
+"""Glue kernels of the per-ray query (csrc/neus_glue.cu): agreement with the chains of reference-API calls they replace (the pack_ops /
+raymarch / raysample wrappers of this package, themselves pinned against the reference's kernels and the oracle), at one small shape per
+kernel.  The kernels against a serial oracle of their own, at the sizes where they loop and at their edges: tests/test_glue_edges_gpu.py."""
 import numpy as np
 import pytest
 import torch
