@@ -395,13 +395,18 @@ int64_t nsb_color_tile_bytes(int64_t n);
 /* Points are x[n,3] or rays_o/rays_d[R,3] + ridx[n] (NULL = identity) + t[n]; view_dirs[R,3] and h_appear[R,n_appear] are
  * indexed by ridx (by the point index when ridx is NULL).  Outputs fp32: sdf[n], nablas[n,3], rgb[n,3], x_out[n,3] (optional).
  * act_* : four buffers of nsb_color_tile_bytes(n) each kept for the backward, or all NULL for inference.
- * collect: NULL or the occupancy-evidence side effect of forward_sdf_nablas (see nsb_occ_collect). */
+ * collect: NULL or the occupancy-evidence side effect of forward_sdf_nablas (see nsb_occ_collect).
+ * rgb == NULL selects the geometry-only form (LoTDSDF.forward_sdf_nablas alone): sdf, nablas, x_out, act_z and the h half of act_x are
+ * written exactly as with rgb, nothing of the radiance net is read, view_dirs, h_appear, act_y1 and act_y2 may be NULL (act_z and act_x
+ * both or neither), and net_host may have rad_width == 0 with NULL radiance pointers (a model without a radiance net). */
 int nsb_fused_color_fwd(const nsb_lotd_meta *meta_host, const void *params_half, const nsb_color_net *net_host, const float *x,
                         const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, const float *view_dirs,
                         const float *h_appear, int64_t n, int32_t max_level, float *sdf, float *nablas, float *rgb, float *x_out,
                         void *act_z, void *act_x, void *act_y1, void *act_y2, const nsb_occ_collect *collect, void *stream);
 /* Cotangents g_sdf[n], g_nablas[n,3], g_rgb[n,3] (each may be NULL = zero); dh_scratch[n,32] fp32 workspace.
- * All gradient outputs are fp32 and ACCUMULATED into (caller zero-fills); d_R* use the reference's column order. */
+ * All gradient outputs are fp32 and ACCUMULATED into (caller zero-fills); d_R* use the reference's column order.
+ * With g_rgb == NULL the radiance backward does not run: act_y1, act_y2, rgb, dh_scratch and d_R* / d_rb* may then be NULL, and net_host
+ * may have rad_width == 0 with NULL radiance pointers (the activations of a geometry-only forward are enough). */
 int nsb_fused_color_bwd(const nsb_lotd_meta *meta_host, const void *params_half, const nsb_color_net *net_host, const float *x,
                         const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, int64_t n, int32_t max_level,
                         const void *act_z, const void *act_x, const void *act_y1, const void *act_y2, const float *rgb,

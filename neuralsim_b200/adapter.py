@@ -14,7 +14,9 @@ the renderers call (`ray_test`, `ray_query`, `forward_sdf_nablas` stays the refe
 
 Only attribute names are used (duck typing), because the reference's model classes cannot be imported in the build container (addict, kornia, ...
 are not installable there, SURVEY.md §8c); tests/test_adapter_gpu.py drives it with a stand-in that exposes exactly the reference's attributes.
-Anything outside the built envelope raises instead of silently keeping the slow path.
+Anything outside the built envelope raises instead of silently keeping the slow path.  A reference model without a radiance net
+(`radiance_cfg: null`, e.g. the LiDAR-only StreetSurf configuration: `radiance_net is None`) becomes a geometry-only LoTDNeuSModel
+(`radiance_cfg=False`) that shares the table, the decoder, `ln_inv_s`, the occupancy buffers and `radius3d_original`.
 """
 from __future__ import annotations
 
@@ -52,17 +54,21 @@ def describe(ref_model) -> dict:
         raise RuntimeError(f"adapter: decoder activation {type(act).__name__} is outside the built envelope (Softplus)")
     space = getattr(ref_model, "space", None) or enc.space
     aabb = space.aabb.detach().cpu().tolist()
-    blocks = rad.blocks
-    in_rad = blocks.layers[0].in_features
-    n_appear = in_rad - (3 + 16 + 3 + enc.out_features)
-    if n_appear < 0:
-        raise RuntimeError("adapter: radiance net input width does not match [x, SH4(v), n, h, h_appear]")
+    if rad is None:                                          # geometry only (lotd_neus.py:71-85)
+        radiance_cfg = False
+    else:
+        blocks = rad.blocks
+        in_rad = blocks.layers[0].in_features
+        n_appear = in_rad - (3 + 16 + 3 + enc.out_features)
+        if n_appear < 0:
+            raise RuntimeError("adapter: radiance net input width does not match [x, SH4(v), n, h, h_appear]")
+        radiance_cfg = dict(n_appear_embedding=int(n_appear), dir_embed_cfg=dict(type="spherical", degree=4), **_mlp_shape(blocks))
     occ = ref_model.accel.occ
     rq = ref_model.ray_query_cfg
     return dict(
         surface_cfg=dict(aabb=aabb, sdf_scale=float(getattr(surf, "sdf_scale", 1.0)), encoding_cfg=dict(lotd_cfg=_lotd_cfg_of(enc)),
                          decoder_cfg=dict(**_mlp_shape(dec), activation=dict(type="softplus", beta=float(act.beta)))),
-        radiance_cfg=dict(n_appear_embedding=int(n_appear), dir_embed_cfg=dict(type="spherical", degree=4), **_mlp_shape(blocks)),
+        radiance_cfg=radiance_cfg,
         var_ctrl_cfg=dict(ln_inv_s_init=float(ref_model.ctrl_var.ln_inv_s.detach().reshape(-1)[0]),
                           ln_inv_s_factor=float(getattr(ref_model.ctrl_var, "ln_inv_s_factor", 10.0)),
                           start_it=getattr(ref_model.ctrl_var, "start_it", 0), stop_it=getattr(ref_model.ctrl_var, "stop_it", 1),
@@ -92,7 +98,10 @@ def accelerate(ref_model, *, patch=True) -> LoTDNeuSModel:
         raise RuntimeError(f"adapter: table sizes differ ({tuple(os_.encoding.flattened_params.shape)} here, {tuple(rs.encoding.flattened_params.shape)} in the "
                            "reference): level types outside Dense / Hash?")
     _share(os_.encoding, "flattened_params", rs.encoding.flattened_params)
-    for mine, theirs in ((os_.decoder.layers, rs.decoder.layers), (ours.radiance_net.blocks.layers, ref_model.radiance_net.blocks.layers)):
+    pairs = [(os_.decoder.layers, rs.decoder.layers)]
+    if ours.radiance_net is not None:
+        pairs.append((ours.radiance_net.blocks.layers, ref_model.radiance_net.blocks.layers))
+    for mine, theirs in pairs:
         for a, b in zip(mine, theirs):
             if a.weight.shape != b.weight.shape:
                 raise RuntimeError(f"adapter: layer shapes differ ({tuple(a.weight.shape)} vs {tuple(b.weight.shape)})")

@@ -96,7 +96,21 @@ constexpr int kColorGatherU = 4;
 // scatter phases of one overlap those of the other.  The launcher checks the occupancy calculator agrees (require_ctas_per_sm).
 constexpr int kColorBwdCtasPerSM = 2;
 
+// Resident CTAs per SM of the geometry-only forward (k_color_fwd<false>): without R1 / R2 and with the X tile cut to its h half it needs
+// about 67 KB of shared memory instead of 91 KB, which would fit three CTAs on an SM.  The launcher asks for the shared-memory carve-out of
+// exactly this many CTAs, because what is not carved out is L1, which the table gathers (ld.global.nc) hit: three CTAs leave about 28 KB of
+// L1, two about 92 KB.  DESIGN.md §6 has the measurement of 2 against 3 (profiles/lidar_geometry_step.py builds the other residency with
+// -DNSB_COLOR_GEO_CTAS_PER_SM).
+#ifndef NSB_COLOR_GEO_CTAS_PER_SM
+#define NSB_COLOR_GEO_CTAS_PER_SM 2
+#endif
+constexpr int kColorGeoCtasPerSM = NSB_COLOR_GEO_CTAS_PER_SM;
+
 // ===================================================================================================================== forward
+// kRad = false is the geometry-only form (models without a radiance net, and rays that render no rgb): it stops after nablas, writes the
+// Z tile and the h half of the X tile (at the X tile's 16 KB stride, so k_color_sdf_bwd reads them unchanged) and never reads the
+// radiance weights, view_dirs, h_appear, rgb_out, Y1t or Y2t.
+template <bool kRad>
 __global__ void __launch_bounds__(kTile)
 k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev net, const PointSrc ps, const float *__restrict__ view_dirs,
             const float *__restrict__ h_appear, int64_t n, int max_level, float *__restrict__ sdf_out, float *__restrict__ nab_out,
@@ -105,37 +119,41 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
     n = eff_n(n, n_dev);
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
-    uint8_t *sX = tiles;                                       // 16 KB [h | x sh n ha 0]
-    uint8_t *sU = sX + kTileBytes;                             // 16 KB u, later relu(y1)
+    uint8_t *sX = tiles;                                       // 16 KB [h | x sh n ha 0] (geometry-only: 8 KB, the h half)
+    uint8_t *sU = sX + (kRad ? kTileBytes : 4 * kChunk);       // 16 KB u, later relu(y1)
     uint8_t *sW1 = sU + kTileBytes;                            //  4 KB W1   [64 x 32]
     uint8_t *sW1T = sW1 + HW * NF * 2;                         //  4 KB W1^T [32 x 64]
-    uint8_t *sR1 = sW1T + HW * NF * 2;                         //  8 KB R1 [64 x 64] (internal column order)
-    uint8_t *sR2 = sR1 + XW * XW * 2;                          //  8 KB R2 [64 x 64]
+    uint8_t *sR1 = sW1T + HW * NF * 2;                         //  8 KB R1 [64 x 64] (internal column order; radiance only)
+    uint8_t *sR2 = sR1 + XW * XW * 2;                          //  8 KB R2 [64 x 64] (radiance only)
     constexpr int kS = tc::acc_stride(64);
-    float *acc = reinterpret_cast<float *>(sR2 + XW * XW * 2); // 34 KB staged accumulator rows (Z, g, Y1, Y2 in turn)
+    float *acc = reinterpret_cast<float *>(kRad ? sR2 + XW * XW * 2 : sR1);   // 34 KB staged accumulator rows (Z, g, Y1, Y2 in turn)
     __shared__ float sb1[HW], sW2[HW], srb1[XW], srb2[XW], sR3[3][XW];
     __shared__ float sb2, srb3[3];
 
     const int tid = threadIdx.x;
     stage_W1(net.dec, sW1, tid);
     stage_W1T(net.dec, sW1T, tid);
-    for (int e = tid; e < XW * XW; e += kTile) {
-        const int j = e % XW, k = e / XW;                      // (out j, in k)
-        const int rc = ref_col(k, net.n_appear);
-        const __half v1 = (j < net.rw && rc >= 0) ? net.R1[j * net.rin + rc] : __float2half_rn(0.f);
-        const __half v2 = (j < net.rw && k < net.rw) ? net.R2[j * net.rw + k] : __float2half_rn(0.f);
-        *reinterpret_cast<__half *>(sR1 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v1;
-        *reinterpret_cast<__half *>(sR2 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v2;
+    if constexpr (kRad) {
+        for (int e = tid; e < XW * XW; e += kTile) {
+            const int j = e % XW, k = e / XW;                  // (out j, in k)
+            const int rc = ref_col(k, net.n_appear);
+            const __half v1 = (j < net.rw && rc >= 0) ? net.R1[j * net.rin + rc] : __float2half_rn(0.f);
+            const __half v2 = (j < net.rw && k < net.rw) ? net.R2[j * net.rw + k] : __float2half_rn(0.f);
+            *reinterpret_cast<__half *>(sR1 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v1;
+            *reinterpret_cast<__half *>(sR2 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v2;
+        }
     }
     stage_decoder_vectors(net.dec, sb1, sW2, &sb2, tid);
-    if (tid < XW) {
-        srb1[tid] = tid < net.rw ? __half2float(net.rb1[tid]) : 0.f;
-        srb2[tid] = tid < net.rw ? __half2float(net.rb2[tid]) : 0.f;
+    if constexpr (kRad) {
+        if (tid < XW) {
+            srb1[tid] = tid < net.rw ? __half2float(net.rb1[tid]) : 0.f;
+            srb2[tid] = tid < net.rw ? __half2float(net.rb2[tid]) : 0.f;
 #pragma unroll
-        for (int k = 0; k < 3; ++k) sR3[k][tid] = tid < net.rw ? __half2float(net.R3[k * net.rw + tid]) : 0.f;
-    }
-    if (tid == 0) {
-        for (int k = 0; k < 3; ++k) srb3[k] = __half2float(net.rb3[k]);
+            for (int k = 0; k < 3; ++k) sR3[k][tid] = tid < net.rw ? __half2float(net.R3[k * net.rw + tid]) : 0.f;
+        }
+        if (tid == 0) {
+            for (int k = 0; k < 3; ++k) srb3[k] = __half2float(net.rb3[k]);
+        }
     }
     tc::fence_async_smem();
     __syncthreads();
@@ -201,68 +219,75 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         float nab[3];
 #pragma unroll
         for (int d = 0; d < 3; ++d) nab[d] = __fmul_rn(__fmul_rn(nacc[d], 0.5f), net.fac[d]);
-        // ---- radiance input, columns 32..63: [x | SH(v) | clamp(n) | h_appear | 0]
-        {
-            float xr[32];
-#pragma unroll
-            for (int k = 0; k < 32; ++k) xr[k] = 0.f;
-            xr[0] = xn[0]; xr[1] = xn[1]; xr[2] = xn[2];
-            if (valid) {
-                sh_basis(view_dirs[ray * 3], view_dirs[ray * 3 + 1], view_dirs[ray * 3 + 2], 4, xr + 3);
-                if (h_appear) {
-#pragma unroll
-                    for (int k = 0; k < 8; ++k)
-                        if (k < net.n_appear) xr[22 + k] = h_appear[ray * net.n_appear + k];
-                }
-            }
-#pragma unroll
-            for (int d = 0; d < 3; ++d) xr[19 + d] = fminf(fmaxf(nab[d], -1.f), 1.f);
-            uint8_t *xt = Xt ? Xt + tile * kTileBytes : nullptr;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                float v8[8];
-#pragma unroll
-                for (int k = 0; k < 8; ++k) v8[k] = xr[c * 8 + k];
-                const uint4 q = tc::pack8_f16(v8);
-                *reinterpret_cast<uint4 *>(sX + (4 + c) * kChunk + tid * 16) = q;
-                if (xt) {
-                    *reinterpret_cast<uint4 *>(xt + (4 + c) * kChunk + tid * 16) = q;
-                    *reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16) = *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16);
-                }
-            }
-        }
-        tc::fence_async_smem();
-        __syncthreads();
-        tc::mma_to_rows<64, 0, 0, XW / 16>(acc, kS, 0, tc::kmajor(x_addr, kTile), tc::kmajor(r1_addr, XW), false);   // Y1 = X . R1^T
-        __syncthreads();
-        uint8_t *y1t = Y1t ? Y1t + tile * kTileBytes : nullptr;
-#pragma unroll 1
-        for (int c = 0; c < XW / 8; ++c) {
-            float y[8];
-            tc::acc_ld8(acc, kS, tid, c * 8, y);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) y[j] = fmaxf(r16(y[j] + srb1[c * 8 + j]), 0.f);
-            const uint4 q = tc::pack8_f16(y);
-            *reinterpret_cast<uint4 *>(sU + c * kChunk + tid * 16) = q;
-            if (y1t) *reinterpret_cast<uint4 *>(y1t + c * kChunk + tid * 16) = q;
-        }
-        tc::fence_async_smem();
-        __syncthreads();
-        tc::mma_to_rows<64, 0, 0, XW / 16>(acc, kS, 0, tc::kmajor(u_addr, kTile), tc::kmajor(r2_addr, XW), false);   // Y2 = relu(Y1) . R2^T
-        __syncthreads();
         float o3[3] = {0.f, 0.f, 0.f};
-        uint8_t *y2t = Y2t ? Y2t + tile * kTileBytes : nullptr;
-#pragma unroll 1
-        for (int c = 0; c < XW / 8; ++c) {
-            float y[8];
-            tc::acc_ld8(acc, kS, tid, c * 8, y);
+        if constexpr (kRad) {
+            // ---- radiance input, columns 32..63: [x | SH(v) | clamp(n) | h_appear | 0]
+            {
+                float xr[32];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                y[j] = fmaxf(r16(y[j] + srb2[c * 8 + j]), 0.f);
+                for (int k = 0; k < 32; ++k) xr[k] = 0.f;
+                xr[0] = xn[0]; xr[1] = xn[1]; xr[2] = xn[2];
+                if (valid) {
+                    sh_basis(view_dirs[ray * 3], view_dirs[ray * 3 + 1], view_dirs[ray * 3 + 2], 4, xr + 3);
+                    if (h_appear) {
 #pragma unroll
-                for (int k = 0; k < 3; ++k) o3[k] = fmaf(y[j], sR3[k][c * 8 + j], o3[k]);
+                        for (int k = 0; k < 8; ++k)
+                            if (k < net.n_appear) xr[22 + k] = h_appear[ray * net.n_appear + k];
+                    }
+                }
+#pragma unroll
+                for (int d = 0; d < 3; ++d) xr[19 + d] = fminf(fmaxf(nab[d], -1.f), 1.f);
+                uint8_t *xt = Xt ? Xt + tile * kTileBytes : nullptr;
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    float v8[8];
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) v8[k] = xr[c * 8 + k];
+                    const uint4 q = tc::pack8_f16(v8);
+                    *reinterpret_cast<uint4 *>(sX + (4 + c) * kChunk + tid * 16) = q;
+                    if (xt) {
+                        *reinterpret_cast<uint4 *>(xt + (4 + c) * kChunk + tid * 16) = q;
+                        *reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16) = *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16);
+                    }
+                }
             }
-            if (y2t) *reinterpret_cast<uint4 *>(y2t + c * kChunk + tid * 16) = tc::pack8_f16(y);
+            tc::fence_async_smem();
+            __syncthreads();
+            tc::mma_to_rows<64, 0, 0, XW / 16>(acc, kS, 0, tc::kmajor(x_addr, kTile), tc::kmajor(r1_addr, XW), false);   // Y1 = X . R1^T
+            __syncthreads();
+            uint8_t *y1t = Y1t ? Y1t + tile * kTileBytes : nullptr;
+#pragma unroll 1
+            for (int c = 0; c < XW / 8; ++c) {
+                float y[8];
+                tc::acc_ld8(acc, kS, tid, c * 8, y);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) y[j] = fmaxf(r16(y[j] + srb1[c * 8 + j]), 0.f);
+                const uint4 q = tc::pack8_f16(y);
+                *reinterpret_cast<uint4 *>(sU + c * kChunk + tid * 16) = q;
+                if (y1t) *reinterpret_cast<uint4 *>(y1t + c * kChunk + tid * 16) = q;
+            }
+            tc::fence_async_smem();
+            __syncthreads();
+            tc::mma_to_rows<64, 0, 0, XW / 16>(acc, kS, 0, tc::kmajor(u_addr, kTile), tc::kmajor(r2_addr, XW), false);   // Y2 = relu(Y1) . R2^T
+            __syncthreads();
+            uint8_t *y2t = Y2t ? Y2t + tile * kTileBytes : nullptr;
+#pragma unroll 1
+            for (int c = 0; c < XW / 8; ++c) {
+                float y[8];
+                tc::acc_ld8(acc, kS, tid, c * 8, y);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    y[j] = fmaxf(r16(y[j] + srb2[c * 8 + j]), 0.f);
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) o3[k] = fmaf(y[j], sR3[k][c * 8 + j], o3[k]);
+                }
+                if (y2t) *reinterpret_cast<uint4 *>(y2t + c * kChunk + tid * 16) = tc::pack8_f16(y);
+            }
+        } else if (Xt) {                                       // the h half of the saved X tile (what k_color_sdf_bwd fetches)
+            uint8_t *xt = Xt + tile * kTileBytes;
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                *reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16) = *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16);
         }
         if (valid) {
             sdf_out[i] = sdf;
@@ -270,8 +295,10 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 #pragma unroll
             for (int d = 0; d < 3; ++d) {
                 nab_out[i * 3 + d] = nab[d];
-                const float y3 = r16(o3[d] + srb3[d]);
-                rgb_out[i * 3 + d] = r16(1.f / (1.f + expf(-y3)));
+                if constexpr (kRad) {
+                    const float y3 = r16(o3[d] + srb3[d]);
+                    rgb_out[i * 3 + d] = r16(1.f / (1.f + expf(-y3)));
+                }
                 if (x_out) x_out[i * 3 + d] = xn[d];
             }
         }
@@ -701,12 +728,18 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
 using namespace nsb;
 
 namespace {
-int make_net(const nsb_color_net *c, const nsb_lotd_meta *meta, PLMeta *m, ColorNetDev *d, const char *who) {
+// radiance: the launch runs the radiance net (rgb asked for).  Otherwise rad_width == 0 with NULL radiance pointers (a geometry-only
+// model) is accepted as well as a whole radiance net, which is then not read.
+int make_net(const nsb_color_net *c, const nsb_lotd_meta *meta, PLMeta *m, ColorNetDev *d, const char *who, bool radiance) {
     const nsb_sdf_decoder dec{c->W1, c->b1, c->W2, c->b2, c->width, c->beta};
     if (int rc = make_decoder(meta, &dec, m, &d->dec, who)) return rc;
-    NSB_REQUIRE(c->rad_width >= 1 && c->rad_width <= 64, "%s: radiance width must be <= 64", who);
-    NSB_REQUIRE(c->n_appear >= 0 && c->n_appear <= 8 && c->rad_in == 54 + c->n_appear,
-                "%s: radiance input must be [x(3), SH deg 4 (16), n(3), h(32), h_appear(<=8)]", who);
+    if (radiance || c->rad_width != 0) {
+        NSB_REQUIRE(c->rad_width >= 1 && c->rad_width <= 64, "%s: radiance width must be <= 64", who);
+        NSB_REQUIRE(c->n_appear >= 0 && c->n_appear <= 8 && c->rad_in == 54 + c->n_appear,
+                    "%s: radiance input must be [x(3), SH deg 4 (16), n(3), h(32), h_appear(<=8)]", who);
+    } else {
+        NSB_REQUIRE(!c->R1 && !c->rb1 && !c->R2 && !c->rb2 && !c->R3 && !c->rb3, "%s: rad_width 0 (no radiance net) needs NULL radiance pointers", who);
+    }
     d->R1 = (const __half *)c->R1; d->rb1 = (const __half *)c->rb1; d->R2 = (const __half *)c->R2; d->rb2 = (const __half *)c->rb2;
     d->R3 = (const __half *)c->R3; d->rb3 = (const __half *)c->rb3;
     d->rw = c->rad_width; d->rin = c->rad_in; d->n_appear = c->n_appear;
@@ -725,20 +758,40 @@ extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params
                                    void *act_y1, void *act_y2, const nsb_occ_collect *collect, void *stream) {
     const DevCounts dn = take_counts();
     if (n == 0) return 0;
-    NSB_REQUIRE(meta && params_half && net && sdf && nablas && rgb && view_dirs, "nsb_fused_color_fwd: NULL argument");
+    const bool rad = rgb != nullptr;
+    NSB_REQUIRE(meta && params_half && net && sdf && nablas && (view_dirs || !rad), "nsb_fused_color_fwd: NULL argument");
     NSB_REQUIRE(x || (rays_o && rays_d && t), "nsb_fused_color_fwd: need x or (rays_o, rays_d, t)");
-    NSB_REQUIRE((act_z && act_x && act_y1 && act_y2) || (!act_z && !act_x && !act_y1 && !act_y2), "nsb_fused_color_fwd: pass all four activation buffers or none");
+    if (rad)
+        NSB_REQUIRE((act_z && act_x && act_y1 && act_y2) || (!act_z && !act_x && !act_y1 && !act_y2), "nsb_fused_color_fwd: pass all four activation buffers or none");
+    else
+        NSB_REQUIRE((act_z && act_x) || (!act_z && !act_x), "nsb_fused_color_fwd: without rgb, pass act_z and act_x or neither");
     PLMeta m;
     ColorNetDev d;
-    if (int rc = make_net(net, meta, &m, &d, "nsb_fused_color_fwd")) return rc;
-    NSB_REQUIRE(d.n_appear == 0 || h_appear, "nsb_fused_color_fwd: h_appear is NULL but the net has %d appearance channels", d.n_appear);
-    constexpr int kSmem = 2 * kTileBytes + 2 * HW * NF * 2 + 2 * XW * XW * 2 + kTile * tc::acc_stride(64) * 4 + 1024;
-    opt_in_smem(k_color_fwd, kSmem);
+    if (int rc = make_net(net, meta, &m, &d, "nsb_fused_color_fwd", rad)) return rc;
     const PointSrc ps{x, rays_o, rays_d, t, ridx};
-    k_color_fwd<<<persistent_grid(n_tiles(n), 2), kTile, kSmem, (cudaStream_t)stream>>>(m, (const __half *)params_half, d, ps, view_dirs, h_appear, n,
-                                                                                        max_level < 0 ? -1 : max_level, sdf, nablas, rgb, x_out, (uint8_t *)act_z,
-                                                                                        (uint8_t *)act_x, (uint8_t *)act_y1, (uint8_t *)act_y2,
-                                                                                        occ_collect_of(collect), dn.a);
+    const int ml = max_level < 0 ? -1 : max_level;
+    if (!rad) {                                                // geometry only: sdf, nablas, x, Z and the h half of X
+        constexpr int kSmemG = 4 * kChunk + kTileBytes + 2 * HW * NF * 2 + kTile * tc::acc_stride(64) * 4 + 1024;   // 67 KB
+        // carve-out for kColorGeoCtasPerSM CTAs (dynamic + static shared memory + the 1 KB the hardware reserves per CTA), in % of 228 KB;
+        // the driver rounds it up to the next configuration it supports
+        constexpr int kCarveout = (100 * kColorGeoCtasPerSM * (kSmemG + 2 * 1024) + 228 * 1024 - 1) / (228 * 1024);
+        if (smem_opt_in_needed(reinterpret_cast<const void *>(k_color_fwd<false>), current_device(), kSmemG)) {
+            cudaFuncSetAttribute(k_color_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemG);
+            cudaFuncSetAttribute(k_color_fwd<false>, cudaFuncAttributePreferredSharedMemoryCarveout, kCarveout);
+        }
+        if (int rc = require_ctas_per_sm(k_color_fwd<false>, kTile, kSmemG, kColorGeoCtasPerSM, "nsb_fused_color_fwd(geometry)")) return rc;
+        k_color_fwd<false><<<persistent_grid(n_tiles(n), kColorGeoCtasPerSM), kTile, kSmemG, (cudaStream_t)stream>>>(
+            m, (const __half *)params_half, d, ps, nullptr, nullptr, n, ml, sdf, nablas, nullptr, x_out, (uint8_t *)act_z, (uint8_t *)act_x,
+            nullptr, nullptr, occ_collect_of(collect), dn.a);
+        return check_launch("nsb_fused_color_fwd");
+    }
+    NSB_REQUIRE(d.n_appear == 0 || h_appear, "nsb_fused_color_fwd: h_appear is NULL but the net has %d appearance channels", d.n_appear);
+    constexpr int kSmem = 2 * kTileBytes + 2 * HW * NF * 2 + 2 * XW * XW * 2 + kTile * tc::acc_stride(64) * 4 + 1024;   // 91 KB: 2 CTAs / SM
+    opt_in_smem(k_color_fwd<true>, kSmem);
+    k_color_fwd<true><<<persistent_grid(n_tiles(n), 2), kTile, kSmem, (cudaStream_t)stream>>>(m, (const __half *)params_half, d, ps, view_dirs, h_appear, n,
+                                                                                             ml, sdf, nablas, rgb, x_out, (uint8_t *)act_z,
+                                                                                             (uint8_t *)act_x, (uint8_t *)act_y1, (uint8_t *)act_y2,
+                                                                                             occ_collect_of(collect), dn.a);
     return check_launch("nsb_fused_color_fwd");
 }
 
@@ -750,12 +803,16 @@ extern "C" int nsb_fused_color_bwd(const nsb_lotd_meta *meta, const void *params
                                    void *stream) {
     const DevCounts dn = take_counts();
     if (n == 0) return 0;
-    NSB_REQUIRE(meta && params_half && net && act_z && act_x && act_y1 && act_y2 && rgb && dh_scratch, "nsb_fused_color_bwd: NULL argument");
-    NSB_REQUIRE(d_grid && d_W1 && d_b1 && d_W2 && d_b2 && d_R1 && d_rb1 && d_R2 && d_rb2 && d_R3 && d_rb3, "nsb_fused_color_bwd: NULL gradient buffer");
+    NSB_REQUIRE(meta && params_half && net && act_z && act_x, "nsb_fused_color_bwd: NULL argument");
+    NSB_REQUIRE(d_grid && d_W1 && d_b1 && d_W2 && d_b2, "nsb_fused_color_bwd: NULL gradient buffer");
+    if (g_rgb) {                                               // the radiance backward's inputs and outputs
+        NSB_REQUIRE(act_y1 && act_y2 && rgb && dh_scratch, "nsb_fused_color_bwd: NULL argument (g_rgb given)");
+        NSB_REQUIRE(d_R1 && d_rb1 && d_R2 && d_rb2 && d_R3 && d_rb3, "nsb_fused_color_bwd: NULL radiance gradient buffer (g_rgb given)");
+    }
     NSB_REQUIRE(x || (rays_o && rays_d && t), "nsb_fused_color_bwd: need x or (rays_o, rays_d, t)");
     PLMeta m;
     ColorNetDev d;
-    if (int rc = make_net(net, meta, &m, &d, "nsb_fused_color_bwd")) return rc;
+    if (int rc = make_net(net, meta, &m, &d, "nsb_fused_color_bwd", g_rgb != nullptr)) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     const float *dh = nullptr;
     if (g_rgb) {

@@ -4,6 +4,7 @@
 State-dict names follow the reference so checkpoints keep loading (SURVEY.md §9):
   implicit_surface.encoding.flattened_params, implicit_surface.decoder.layers.{0,1}.{weight,bias},
   radiance_net.blocks.layers.{0,1,2}.{weight,bias}, ctrl_var.ln_inv_s, accel.occ.{is_initialized,occ_grid,occ_val_grid}.
+A geometry-only model (`radiance_cfg=False`, the reference's `radiance_cfg: null`) has no `radiance_net.*` keys.
 """
 from __future__ import annotations
 
@@ -30,7 +31,11 @@ class _Cfg(dict):
 
 
 class LoTDNeuS(nn.Module):
-    def __init__(self, surface_cfg: dict = None, radiance_cfg: dict = None, var_ctrl_cfg: dict = None, dtype=torch.half, device=None,
+    """radiance_cfg: a dict of RadianceNet arguments over the defaults; None builds the default radiance net; False builds none -- a
+    geometry-only model (the reference's `radiance_cfg: null`, lotd_neus.py:71-85, e.g. the LiDAR-only StreetSurf configuration): then
+    `radiance_net` is None, use_view_dirs = use_nablas = use_h_appear = False, and only sdf / nablas can be queried."""
+
+    def __init__(self, surface_cfg: dict = None, radiance_cfg=None, var_ctrl_cfg: dict = None, dtype=torch.half, device=None,
                  generator=None, n_appear_embedding: int = None):
         super().__init__()
         self.dtype = dtype
@@ -41,17 +46,21 @@ class LoTDNeuS(nn.Module):
         self.implicit_surface = LoTDSDF(encoding_cfg=sc.get("encoding_cfg"), decoder_cfg=sc.get("decoder_cfg"), dtype=dtype, device=device,
                                         generator=generator, sdf_scale=sc.get("sdf_scale", 1.0), aabb=self.space.aabb.cpu(),
                                         radius3d_original=(self.space.radius3d_original.cpu() if aabb is not None else bounding_size / 2.))
-        rc = dict(use_pos=True, use_view_dirs=True, use_nablas=True, D=2, W=64)
-        rc.update(radiance_cfg or {})
-        if n_appear_embedding is not None:
-            rc["n_appear_embedding"] = n_appear_embedding
-        self.radiance_net = RadianceNet(n_extra_feat=self.implicit_surface.encoding.out_features, dtype=dtype, device=device, generator=generator, **rc)
+        if radiance_cfg is False:
+            self.radiance_net = None
+        else:
+            rc = dict(use_pos=True, use_view_dirs=True, use_nablas=True, D=2, W=64)
+            rc.update(radiance_cfg or {})
+            if n_appear_embedding is not None:
+                rc["n_appear_embedding"] = n_appear_embedding
+            self.radiance_net = RadianceNet(n_extra_feat=self.implicit_surface.encoding.out_features, dtype=dtype, device=device, generator=generator, **rc)
         vc = dict(ln_inv_s_init=0.3, ln_inv_s_factor=10.0, stop_it=1, start_it=0, final_inv_s=2048.)
         vc.update({k: v for k, v in (var_ctrl_cfg or {}).items() if k != "ctrl_type"})
         self.ctrl_var = VarSingleMixLinear(**vc, device=device)
-        self.use_view_dirs = self.radiance_net.use_view_dirs
-        self.use_nablas = self.radiance_net.use_nablas
-        self.use_h_appear = self.radiance_net.use_h_appear
+        r = self.radiance_net
+        self.use_view_dirs = r is not None and r.use_view_dirs
+        self.use_nablas = r is not None and r.use_nablas
+        self.use_h_appear = r is not None and r.use_h_appear
         self.max_level = None
 
     @property
@@ -82,8 +91,14 @@ class LoTDNeuS(nn.Module):
         return self.forward_sdf(torch.addcmul(rays_o[ridx], rays_d[ridx], t.unsqueeze(-1)))
 
     # ---- fused colour query (csrc/color_tc.cu)
+    def _geometry_fusable(self):
+        """the preconditions of the geometry-only colour op (sdf + nablas, csrc/color_tc.cu k_color_fwd<false>): those of the fused SDF query"""
+        return self.implicit_surface._fusable()
+
     def _color_fusable(self):
         from .networks import SHEncoder
+        if self.radiance_net is None:
+            return False
         r, b = self.radiance_net, self.radiance_net.blocks
         return (self.implicit_surface._fusable() and r.use_pos and r.use_view_dirs and r.use_nablas and r.use_extra_feat
                 and isinstance(r.embed_fn_view, SHEncoder) and r.embed_fn_view.degree == 4 and b.D == 2 and not b.skips and b.dtype == torch.half
@@ -101,22 +116,42 @@ class LoTDNeuS(nn.Module):
         cache = getattr(self, "_color_cache", None)
         if cache is None or cache[0] != key:
             t = [p.detach().to(torch.half).contiguous() for p in ps]
-            r3 = s.radius3d_original                      # a buffer: read back once, not at every parameter update (a host sync)
-            fk = (r3.data_ptr(), r3._version, float(s.sdf_scale))
-            if getattr(self, "_fac_cache", (None,))[0] != fk:
-                self._fac_cache = (fk, (s.sdf_scale / r3).float().tolist())
-            fac = self._fac_cache[1]
+            fac = self._nablas_fac()
             net = L.ColorNetC(*[x.data_ptr() for x in t], s.decoder.layers[0].out_features, b[0].out_features, b[0].in_features,
                               b[0].in_features - 54, float(s.decoder.layers[0].activation.beta), (ctypes.c_float * 3)(*fac))
             cache = self._color_cache = (key, t, net)
         return grid16, cache[2], cache[1]
 
-    def forward_on_rays(self, ridx, t, rays_o, rays_d, view_dirs, rays_h_appear=None, *, nablas_has_grad=True):
-        """LoTDNeuS.forward at x = o[ridx] + d[ridx] t with per-ray view_dirs / h_appear, as one fused op (fields/fused_color.py)."""
+    def _nablas_fac(self):
+        """sdf_scale / radius3d_original per axis as host floats"""
+        s = self.implicit_surface
+        r3 = s.radius3d_original                          # a buffer: read back once, not at every parameter update (a host sync)
+        fk = (r3.data_ptr(), r3._version, float(s.sdf_scale))
+        if getattr(self, "_fac_cache", (None,))[0] != fk:
+            self._fac_cache = (fk, (s.sdf_scale / r3).float().tolist())
+        return self._fac_cache[1]
+
+    def _fused_geometry_state(self):
+        """(fp16 table, nsb_color_net with rad_width = 0, the fp16 tensors it points at) for the geometry-only op; the fp16 images are
+        the fused SDF query's (LoTDSDF._fused_state)"""
+        s = self.implicit_surface
+        grid16, _dec = s._fused_state()
+        t, fac = s._fused_cache[1], self._nablas_fac()
+        cache = getattr(self, "_geo_cache", None)
+        if cache is None or cache[0] is not t or cache[1] != fac:
+            d = s.decoder.layers
+            net = L.ColorNetC(*[x.data_ptr() for x in t[1:]], *([None] * 6), d[0].out_features, 0, 0, 0, float(d[0].activation.beta),
+                              (ctypes.c_float * 3)(*fac))
+            cache = self._geo_cache = (t, list(fac), net)
+        return grid16, cache[2], t
+
+    def forward_on_rays(self, ridx, t, rays_o, rays_d, view_dirs=None, rays_h_appear=None, *, nablas_has_grad=True, with_rgb=True):
+        """LoTDNeuS.forward at x = o[ridx] + d[ridx] t with per-ray view_dirs / h_appear, as one fused op (fields/fused_color.py).
+        with_rgb=False: sdf and nablas only (no view_dirs / h_appear; any model, with or without a radiance net)."""
         accel = getattr(self, "accel", None)
         collect = accel.occ.collect_struct() if (self.training and accel is not None) else None
         return fused_color(self, ridx, t, rays_o, rays_d, view_dirs, rays_h_appear if self.use_h_appear else None,
-                           nablas_has_grad=nablas_has_grad, collect=collect)
+                           nablas_has_grad=nablas_has_grad, collect=collect, with_rgb=with_rgb)
 
     @torch.no_grad()
     def query_sdf(self, x):
@@ -127,6 +162,8 @@ class LoTDNeuS(nn.Module):
                                                         grad_guard=grad_guard)
 
     def forward(self, x, *, v=None, h_appear=None, has_grad: bool = None, nablas_has_grad: bool = None, with_rgb=True, with_normal=True):
+        if with_rgb and self.radiance_net is None:
+            raise RuntimeError("LoTDNeuS.forward(with_rgb=True): this model has no radiance net (radiance_cfg=False); query it with with_rgb=False")
         prefix = x.shape[:-1]
         if with_normal or (with_rgb and self.use_nablas):
             ret = self.forward_sdf_nablas(x, has_grad=has_grad, nablas_has_grad=nablas_has_grad)

@@ -189,21 +189,22 @@ def _query_fused_tail(model, ray_tested, view_dirs, rays_h_appear, rays_o, rays_
 
 def _net_forward_into(volume_buffer, model, rays_o, rays_d, view_dirs, rays_h_appear, ridx_all, depths, *, nablas_has_grad,
                       with_rgb, with_normal, dtype, cond_kw=None):
-    if view_dirs is None and cond_kw is None and not with_rgb and with_normal and FUSED_STAGES and getattr(model, "use_view_dirs", False) and not rays_d.requires_grad:
-        # LiDAR-style rays (with_rgb=False, with_normal=True: code_single/tools/train.py:900): sdf + second-order nablas are what is needed; the
-        # fused op computes them (its radiance head runs too and is dropped; no gradient reaches the radiance net)
-        view_dirs = rays_d / rays_d.detach().norm(dim=-1).clamp_min(1.0e-10).unsqueeze(-1)
-        if rays_h_appear is None and getattr(model, "use_h_appear", False):
-            rays_h_appear = rays_d.new_zeros(rays_d.shape[0], model.radiance_net.blocks.layers[0].in_features - 54)
-    if (FUSED_STAGES and cond_kw is None and (with_rgb or with_normal) and view_dirs is not None and getattr(model, "_color_fusable", lambda: False)()
-            and not (rays_h_appear is not None and rays_h_appear.requires_grad) and not depths.requires_grad
-            # learnable rays (pose refinement): the reference's model.forward(x = o + d t) carries d(loss)/d(rays); the fused op detaches them
-            and not (rays_o.requires_grad or rays_d.requires_grad or view_dirs.requires_grad)):
+    fused = (FUSED_STAGES and cond_kw is None and not depths.requires_grad
+             # learnable rays (pose refinement): the reference's model.forward(x = o + d t) carries d(loss)/d(rays); the fused op detaches them
+             and not (rays_o.requires_grad or rays_d.requires_grad))
+    if fused and not with_rgb and with_normal and getattr(model, "_geometry_fusable", lambda: False)():
+        # LiDAR-style rays (with_rgb=False, with_normal=True: code_single/tools/train.py:900) and models without a radiance net: sdf +
+        # second-order nablas from the geometry-only fused op; no radiance head runs and nothing reaches a radiance net
+        out = model.forward_on_rays(ridx_all, depths, rays_o, rays_d, nablas_has_grad=nablas_has_grad, with_rgb=False)
+        volume_buffer["net_x"] = out["x"]
+        volume_buffer["nablas"] = out["nablas"].to(dtype)
+        return
+    if (fused and with_rgb and view_dirs is not None and getattr(model, "_color_fusable", lambda: False)()
+            and not (rays_h_appear is not None and rays_h_appear.requires_grad) and not view_dirs.requires_grad):
         out = model.forward_on_rays(ridx_all, depths, rays_o, rays_d, view_dirs, rays_h_appear, nablas_has_grad=nablas_has_grad)
         volume_buffer["net_x"] = out["x"]
         volume_buffer["nablas"] = out["nablas"].to(dtype)
-        if with_rgb:
-            volume_buffer["rgb"] = out["rgb"].to(dtype)
+        volume_buffer["rgb"] = out["rgb"].to(dtype)
         return
     x = torch.addcmul(rays_o[ridx_all], rays_d[ridx_all], depths.unsqueeze(-1))
     kw = dict(x=x, nablas_has_grad=nablas_has_grad, with_rgb=with_rgb, with_normal=with_normal)

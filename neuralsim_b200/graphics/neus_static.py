@@ -171,37 +171,41 @@ class _StaticBoundary(torch.autograd.Function):
 
 
 class _StaticColor(torch.autograd.Function):
-    """fields/fused_color.py:_FusedColor over the K = cnt[19] kept samples (buffers sized kept_cap)"""
+    """fields/fused_color.py:_FusedColor over the K = cnt[19] kept samples (buffers sized kept_cap); params: the five SDF parameters, then the
+    six radiance parameters when rgb is computed (without them: the geometry-only form, no rgb output)"""
 
     @staticmethod
     def forward(ctx, st, ridx, t, view_dirs, h_appear, keep_acts, *params):
+        rad = len(params) > 5
         n, dev = t.numel(), t.device
         sdf = torch.empty(n, dtype=torch.float32, device=dev)
         nab = torch.empty(n, 3, dtype=torch.float32, device=dev)
-        rgb = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        rgb = torch.empty(n, 3, dtype=torch.float32, device=dev) if rad else None
         x = torch.empty(n, 3, dtype=torch.float32, device=dev)
-        acts = torch.empty(4, int(L.lib().nsb_color_tile_bytes(L.c_i64(n))), dtype=torch.uint8, device=dev) if keep_acts else None
-        ap = [L.ptr(acts[k]) if keep_acts else None for k in range(4)]
+        n_act = 4 if rad else 2                                  # Z, X (+ Y1, Y2)
+        acts = torch.empty(n_act, int(L.lib().nsb_color_tile_bytes(L.c_i64(n))), dtype=torch.uint8, device=dev) if keep_acts else None
+        ap = [L.ptr(acts[k]) if keep_acts and k < n_act else None for k in range(4)]
         P = L.ptr
         with L.KERNEL_TIMER.time("fused_color_fwd", n):
             _call(L.lib().nsb_fused_color_fwd, "fused_color_fwd", st.cnt, CNT_SLOTS["kept"], None,
                   st.meta.c_ref, P(st.grid16, "f16"), ctypes.byref(st.net), None, P(st.rays_o, "f32"), P(st.rays_d, "f32"), P(ridx, "i64"), P(t, "f32"),
-                  P(view_dirs, "f32"), P(h_appear, "f32", allow_none=True), L.c_i64(n), L.c_i32(st.ml), P(sdf), P(nab), P(rgb), P(x), *ap,
-                  ctypes.byref(st.collect) if st.collect is not None else None, L.stream_ptr())
-        ctx.st, ctx.ridx, ctx.t, ctx.n = st, ridx, t, n
+                  P(view_dirs, "f32", allow_none=not rad), P(h_appear, "f32", allow_none=True), L.c_i64(n), L.c_i32(st.ml), P(sdf), P(nab),
+                  P(rgb, allow_none=not rad), P(x), *ap, ctypes.byref(st.collect) if st.collect is not None else None, L.stream_ptr())
+        ctx.st, ctx.ridx, ctx.t, ctx.n, ctx.rad = st, ridx, t, n, rad
         ctx.held = (acts, rgb)
         ctx.shapes = [p.shape for p in params]
         ctx.set_materialize_grads(False)
         ctx.mark_non_differentiable(x)
-        return sdf, nab, rgb, x
+        return (sdf, nab, rgb, x) if rad else (sdf, nab, x)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
-    def backward(ctx, g_sdf, g_nab, g_rgb, _gx):
+    def backward(ctx, *g_out):
         acts, rgb = ctx.held
         if acts is None:
             raise RuntimeError("static colour query: backward through a forward that ran without grad")
-        st, dev, n = ctx.st, rgb.device, ctx.n
+        st, dev, n = ctx.st, acts.device, ctx.n
+        g_sdf, g_nab, g_rgb = g_out[0], g_out[1], (g_out[2] if ctx.rad else None)
         sizes = [int(torch.Size(s).numel()) for s in ctx.shapes[1:]]
         small = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
         grads, o = [torch.zeros(ctx.shapes[0], dtype=torch.float32, device=dev)], 0
@@ -212,13 +216,15 @@ class _StaticColor(torch.autograd.Function):
             return (None,) * 6 + tuple(grads)
         c = lambda g: None if g is None else g.contiguous().float()
         g_sdf, g_nab, g_rgb = c(g_sdf), c(g_nab), c(g_rgb)
-        dh = torch.empty(n, 32, dtype=torch.float32, device=dev)
+        dh = torch.empty(n, 32, dtype=torch.float32, device=dev) if g_rgb is not None else None
         P = L.ptr
+        ag = [P(g) for g in grads] + [None] * (11 - len(grads))          # d_R* / d_rb*: NULL without the radiance net's parameters
         with L.KERNEL_TIMER.time("fused_color_bwd", n):
             _call(L.lib().nsb_fused_color_bwd, "fused_color_bwd", st.cnt, CNT_SLOTS["kept"], None,
                   st.meta.c_ref, P(st.grid16, "f16"), ctypes.byref(st.net), None, P(st.rays_o, "f32"), P(st.rays_d, "f32"), P(ctx.ridx, "i64"),
-                  P(ctx.t, "f32"), L.c_i64(n), L.c_i32(st.ml), P(acts[0]), P(acts[1]), P(acts[2]), P(acts[3]), P(rgb), P(g_sdf, allow_none=True),
-                  P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh), *[P(g) for g in grads], L.stream_ptr())
+                  P(ctx.t, "f32"), L.c_i64(n), L.c_i32(st.ml), P(acts[0]), P(acts[1]), *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]),
+                  P(rgb, allow_none=True), P(g_sdf, allow_none=True), P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh, allow_none=True),
+                  *ag, L.stream_ptr())
         return (None,) * 6 + tuple(grads)
 
 
@@ -275,12 +281,16 @@ class _State:
     __slots__ = ("meta", "grid16", "dec", "net", "held", "rays_o", "rays_d", "ml", "collect", "cnt", "ws")
 
 
-def _fp16_images(model):
-    """fp16 images of the masters, re-cast INSIDE the step (a captured graph must not rely on a host-side version check)"""
-    s, b = model.implicit_surface, model.radiance_net.blocks.layers
+def _fp16_images(model, radiance=True):
+    """fp16 images of the masters, re-cast INSIDE the step (a captured graph must not rely on a host-side version check).  radiance=False:
+    the table and the decoder only, and a net struct without a radiance net (rad_width = 0) for the geometry-only colour query"""
+    s = model.implicit_surface
     d = s.decoder.layers
-    ps = [s.encoding.flattened_params, d[0].weight, d[0].bias, d[1].weight, d[1].bias, b[0].weight, b[0].bias, b[1].weight, b[1].bias, b[2].weight, b[2].bias]
-    # one multi-tensor cast for the ten small tensors (a launch each otherwise: at 4096 rays per step the step is launch-bound), one for the table
+    ps = [s.encoding.flattened_params, d[0].weight, d[0].bias, d[1].weight, d[1].bias]
+    if radiance:
+        b = model.radiance_net.blocks.layers
+        ps += [b[0].weight, b[0].bias, b[1].weight, b[1].bias, b[2].weight, b[2].bias]
+    # one multi-tensor cast for the small tensors (a launch each otherwise: at 4096 rays per step the step is launch-bound), one for the table
     t = [torch.empty(p.shape, dtype=torch.half, device=p.device) for p in ps]
     with torch.no_grad():
         t[0].copy_(ps[0].detach())
@@ -290,17 +300,25 @@ def _fp16_images(model):
     fk = (r3.data_ptr(), r3._version, float(s.sdf_scale))
     if getattr(model, "_fac_cache", (None,))[0] != fk:
         model._fac_cache = (fk, (s.sdf_scale / r3).float().tolist())
-    net = L.ColorNetC(*[x.data_ptr() for x in t[1:]], d[0].out_features, b[0].out_features, b[0].in_features, b[0].in_features - 54,
-                      float(d[0].activation.beta), (ctypes.c_float * 3)(*model._fac_cache[1]))
+    fac = (ctypes.c_float * 3)(*model._fac_cache[1])
+    if radiance:
+        net = L.ColorNetC(*[x.data_ptr() for x in t[1:]], d[0].out_features, b[0].out_features, b[0].in_features, b[0].in_features - 54,
+                          float(d[0].activation.beta), fac)
+    else:
+        net = L.ColorNetC(*[x.data_ptr() for x in t[1:]], *([None] * 6), d[0].out_features, 0, 0, 0, float(d[0].activation.beta), fac)
     return t, dec, net, ps
 
 
 def static_supported(model, cfg):
     qp = dict(model.ray_query_cfg.get("query_param", {}) or {})
     occ = getattr(getattr(model, "accel", None), "occ", None)
-    return (getattr(model, "_color_fusable", lambda: False)() and model.use_view_dirs and occ is not None and occ.occ_grid.dim() == 3
+    if cfg.get("with_rgb", True):
+        net_ok = getattr(model, "_color_fusable", lambda: False)() and model.use_view_dirs
+    else:                                                    # sdf / nablas only (or alpha only): the geometry-only colour query, if any
+        net_ok = getattr(model, "_geometry_fusable", lambda: False)()
+    return (net_ok and occ is not None and occ.occ_grid.dim() == 3
             and occ.occ_grid.numel() * 4 // 32 <= 96 * 1024 and qp.get("num_coarse", 0) > 0 and len(qp.get("upsample_inv_s_factors", (1, 4, 16))) <= 4
-            and qp.get("coarse_step_cfg", {}).get("step_mode", "linear") == "linear" and (cfg.get("with_rgb", True) or cfg.get("with_normal", True)))
+            and qp.get("coarse_step_cfg", {}).get("step_mode", "linear") == "linear")
 
 
 def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=None, march_cap, kept_cap, coherent=False, with_rgb=True, with_normal=True,
@@ -309,6 +327,8 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     `coherent`: image-ordered rays (the boundary / fine queries then walk the samples ray-tiled) -- a host decision here (the host-sized
     path measures it in the ray-test kernel)."""
     P, lib = L.ptr, L.lib()
+    if with_rgb and getattr(model, "radiance_net", None) is None:
+        raise RuntimeError("render_static(with_rgb=True): the model has no radiance net (radiance_cfg=False); render it with with_rgb=False")
     if perturb:
         raise RuntimeError("render_static: perturb=True is not built (random streams of capacity-sized draws differ from the reference's); "
                            "use the host-sized path (SingleVolumeRenderer.render)")
@@ -340,7 +360,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     wsb = (NF._scan_ws_bytes() + 255) // 256 * 256
     st.ws = torch.zeros(4, wsb, dtype=torch.uint8, device=dev)          # the zeroed workspaces of the step's four scans, one fill
     with torch.no_grad():
-        t16, st.dec, st.net, masters = _fp16_images(model)
+        t16, st.dec, st.net, masters = _fp16_images(model, radiance=with_rgb)
         st.held, st.grid16 = t16, t16[0]
         st.meta = model.implicit_surface.encoding.meta
         st.ml = model.implicit_surface._ml(model.max_level)
@@ -361,8 +381,9 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         _scan(flag, cnt, CNT_SLOTS["n_rays"], index=rays_inds, ws=st.ws[0])
         # the boundary query walks its packs (the rays that passed) in 8 x 4 pixel blocks (csrc/neus_glue.cu: k_ray_block_order)
         order_b = _block_order(rays_inds, None, R, cnt, CNT_SLOTS["n_rays"]) if coherent else None
-        ha = rays_h_appear.detach().contiguous().float() if (rays_h_appear is not None and model.use_h_appear) else None
-        if ha is None and model.use_h_appear:             # LiDAR-style rays carry no appearance code: the (dropped) radiance head reads zeros
+        # only the radiance head reads appearance codes: rays that render no rgb gather none
+        ha = rays_h_appear.detach().contiguous().float() if (with_rgb and rays_h_appear is not None and model.use_h_appear) else None
+        if ha is None and with_rgb and model.use_h_appear:
             ha = torch.zeros(R, model.radiance_net.blocks.layers[0].in_features - 54, device=dev)
         n_ha = ha.shape[1] if ha is not None else 0
         rbuf = torch.zeros(R * (8 + n_ha), device=dev)     # the compacted rays in ONE zero-filled allocation (rows beyond the live count stay 0)
@@ -372,7 +393,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         _call(lib.nsb_gather_rays, "gather_rays", cnt, CNT_SLOTS["n_rays"], None, P(rays_inds, "i64"), L.c_i64(R), P(o_n), P(d_n), P(nr), P(fr), P(o_c), P(d_c),
               P(n_c), P(f_c), P(ha, allow_none=True), P(ha_c, allow_none=True), L.c_i32(0 if ha is None else ha.shape[1]), L.stream_ptr())
         st.rays_o, st.rays_d = o_c, d_c
-        view_dirs = (d_c / d_c.norm(dim=-1).clamp_min(1.0e-10).unsqueeze(-1)).contiguous()
+        view_dirs = (d_c / d_c.norm(dim=-1).clamp_min(1.0e-10).unsqueeze(-1)).contiguous() if with_rgb else None
         # ---------------- coarse samples + march
         coarse = batch_sample_step_linear(n_c, f_c, nc1, prefix_shape=[R], perturb=perturb).contiguous()
         occ_grid = model.accel.occ.occ_grid
@@ -461,7 +482,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
               P(ridx_hit, "i64"), L.c_i64(R), P(fine_all, "f32"), L.c_i32(nf_tot), rl, L.c_i32(n_stage), P(d1), None, P(ridx_all, "i64", allow_none=True), P(pinfo),
               L.stream_ptr())
     # ---------------- boundary SDF (grad) -> alpha -> compression
-    s, b = model.implicit_surface, model.radiance_net.blocks.layers
+    s = model.implicit_surface
     dl = s.decoder.layers
     inv_s = model.forward_inv_s()
     if not isinstance(inv_s, torch.Tensor):
@@ -469,17 +490,23 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     alpha_k, t_k, ridx_k, pinfo_kept, rays_inds_hit = _StaticBoundary.apply(
         st, d1, pinfo, ridx_all, order_b, rays_inds, kept_cap,
         (nc1, num_fine, march_cap, kept_cap), inv_s, s.encoding.flattened_params, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
-    # ---------------- colour / normal query on the kept samples
-    params = (s.encoding.flattened_params, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias, b[0].weight, b[0].bias, b[1].weight, b[1].bias,
-              b[2].weight, b[2].bias)
-    keep_acts = torch.is_grad_enabled() and any(p.requires_grad for p in params)
-    _sdf_k, nab, rgb, x = _StaticColor.apply(st, ridx_k, t_k, view_dirs, ha_c, keep_acts, *params)
-    if not nablas_has_grad:
-        nab = nab.detach()
+    # ---------------- colour / normal query on the kept samples (none when neither is rendered: depth and mask need alpha alone)
+    rgb = nab = x = None
+    if with_rgb or with_normal:
+        params = (s.encoding.flattened_params, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
+        if with_rgb:
+            b = model.radiance_net.blocks.layers
+            params += (b[0].weight, b[0].bias, b[1].weight, b[1].bias, b[2].weight, b[2].bias)
+        keep_acts = torch.is_grad_enabled() and any(p.requires_grad for p in params)
+        out = _StaticColor.apply(st, ridx_k, t_k, view_dirs, ha_c, keep_acts, *params)
+        nab, x = out[1], out[-1]
+        rgb = out[2] if with_rgb else None
+        if not nablas_has_grad:
+            nab = nab.detach()
     nab_i = nab if with_normal else None
     if nab_i is not None and not training:
         nab_i = F.normalize(nab_i.clamp(-1, 1), dim=-1)
-    vw, m, d, c, nn_ = _StaticComposite.apply(alpha_k, t_k, rgb if with_rgb else None, nab_i, pinfo_kept, rays_inds_hit, R, cnt,
+    vw, m, d, c, nn_ = _StaticComposite.apply(alpha_k, t_k, rgb, nab_i, pinfo_kept, rays_inds_hit, R, cnt,
                                               bool(depth_use_normalized_vw), 1e-4, 0.0)
     rendered = dict(mask_volume=m, depth_volume=d)
     if with_rgb:
@@ -502,7 +529,8 @@ def sliced_volume_buffer(buffers, cnt):
         return dict(type="empty", rays_inds_hit=[])
     vb = dict(type="packed", rays_inds_hit=buffers["rays_inds_hit"][:Pu], pack_infos_hit=buffers["pack_infos_hit"][:Pu])
     for k in ("opacity_alpha", "t", "rgb", "nablas", "net_x", "vw"):
-        vb[k] = buffers[k][:K]
+        if buffers[k] is not None:                           # rgb / nablas / net_x: None when the step did not query them
+            vb[k] = buffers[k][:K]
     return vb
 
 
