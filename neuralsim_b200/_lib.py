@@ -57,6 +57,7 @@ def lib():
         _lib.nsb_last_error.restype = ctypes.c_char_p
         _lib.nsb_launch_count.restype = ctypes.c_uint64
         _lib.nsb_color_tile_bytes.restype = ctypes.c_int64
+        _lib.nsb_upsample_rays_scratch_floats.restype = ctypes.c_int64
         # marching cubes (csrc/mesh.cu): `level` is a double, which an undeclared ctypes call would not pass
         vp, i32, i64, f64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_double
         _lib.nsb_mc_lattice_points.argtypes = [vp, vp, vp, i32, i32, i64, i64, vp, vp]
@@ -70,6 +71,26 @@ def check(rc, what=""):
     if rc != 0:
         msg = lib().nsb_last_error().decode("utf-8", "replace")
         raise RuntimeError(f"{what}: {msg}" if what else msg)
+
+
+def slot(cnt, k):
+    """device pointer of cnt[k] (an int64 device count block)"""
+    return ctypes.c_void_p(cnt.data_ptr() + 8 * k)
+
+
+def call(fn, what, *args, count=None):
+    """fn(*args) checked.  count = (cnt, k0[, k1]): the launch processes the device-resident counts cnt[k0] (and cnt[k1]) instead of
+    its size arguments, which then are the capacities (nsb_bind_device_counts: bound to this thread for the one call, then cleared)."""
+    if count is None:
+        check(fn(*args), what)
+        return
+    l = lib()
+    l.nsb_bind_device_counts(slot(count[0], count[1]), slot(count[0], count[2]) if len(count) > 2 else _NULL)
+    try:
+        rc = fn(*args)
+    finally:
+        l.nsb_bind_device_counts(_NULL, _NULL)
+    check(rc, what)
 
 
 def launch_count() -> int:

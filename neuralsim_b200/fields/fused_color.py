@@ -17,16 +17,31 @@ from torch import autograd
 from .. import _lib as L
 
 
+def color_net_c(t16, dec, rad, fac):
+    """nsb_color_net over the fp16 images t16 = (W1, b1, W2, b2[, R1, rb1, R2, rb2, R3, rb3]) of the decoder layers `dec` and the radiance
+    layers `rad` (None: the geometry-only net, rad_width = 0); fac: sdf_scale / radius3d_original per axis"""
+    ptrs = [x.data_ptr() for x in t16] + [None] * (10 - len(t16))
+    rw, ri, na = (rad[0].out_features, rad[0].in_features, rad[0].in_features - 54) if rad is not None else (0, 0, 0)
+    return L.ColorNetC(*ptrs, dec[0].out_features, rw, ri, na, float(dec[0].activation.beta), (ctypes.c_float * 3)(*fac))
+
+
+class ColorQuery:
+    """what the forward and backward launches of one colour query share: the table's meta and fp16 image, the net struct and the fp16
+    tensors it points at, the rays, max level, the occupancy collection and the device count (_lib.call's count=, None: host-sized)"""
+    __slots__ = ("meta", "grid16", "net", "held", "rays_o", "rays_d", "ml", "collect", "count")
+
+    def __init__(self, meta, grid16, net, held, rays_o, rays_d, ml, collect, count):
+        self.meta, self.grid16, self.net, self.held = meta, grid16, net, held
+        self.rays_o, self.rays_d, self.ml, self.collect, self.count = rays_o, rays_d, ml, collect, count
+
+
 class _FusedColor(autograd.Function):
-    """params: the five SDF parameters (table, W1, b1, W2, b2), then the six radiance parameters when rgb is computed"""
+    """q: ColorQuery; params: the five SDF parameters (table, W1, b1, W2, b2), then the six radiance parameters when rgb is computed"""
 
     @staticmethod
-    def forward(ctx, model, pts, view_dirs, h_appear, max_level, keep, collect, *params):
+    def forward(ctx, q, ridx, t, view_dirs, h_appear, keep, *params):
         rad = len(params) > 5
-        grid16, net, _held = model._fused_color_state() if rad else model._fused_geometry_state()
-        ridx, t, rays_o, rays_d = pts
         n, dev = t.numel(), t.device
-        meta = model.implicit_surface.encoding.meta
         sdf = torch.empty(n, dtype=torch.float32, device=dev)
         nab = torch.empty(n, 3, dtype=torch.float32, device=dev)
         rgb = torch.empty(n, 3, dtype=torch.float32, device=dev) if rad else None
@@ -36,15 +51,14 @@ class _FusedColor(autograd.Function):
         if keep:
             acts = torch.empty(n_act, int(L.lib().nsb_color_tile_bytes(L.c_i64(n))), dtype=torch.uint8, device=dev)
         ap = [L.ptr(acts[k]) if keep and k < n_act else None for k in range(4)]
+        P = L.ptr
         with L.KERNEL_TIMER.time("fused_color_fwd", n):
-            L.check(L.lib().nsb_fused_color_fwd(meta.c_ref, L.ptr(grid16, "f16"), ctypes.byref(net), None, L.ptr(rays_o, "f32"), L.ptr(rays_d, "f32"),
-                                                L.ptr(ridx, "i64"), L.ptr(t, "f32"), L.ptr(view_dirs, "f32", allow_none=not rad),
-                                                L.ptr(h_appear, "f32", allow_none=True), L.c_i64(n), L.c_i32(max_level), L.ptr(sdf), L.ptr(nab),
-                                                L.ptr(rgb, allow_none=not rad), L.ptr(x), *ap, ctypes.byref(collect) if collect is not None else None,
-                                                L.stream_ptr()),
-                    "fused_color_fwd")
-        ctx.model, ctx.pts, ctx.max_level, ctx.n, ctx.rad = model, pts, max_level, n, rad
-        ctx.held = (grid16, net, _held, acts, rgb)
+            L.call(L.lib().nsb_fused_color_fwd, "fused_color_fwd", q.meta.c_ref, P(q.grid16, "f16"), ctypes.byref(q.net), None, P(q.rays_o, "f32"),
+                   P(q.rays_d, "f32"), P(ridx, "i64"), P(t, "f32"), P(view_dirs, "f32", allow_none=not rad), P(h_appear, "f32", allow_none=True),
+                   L.c_i64(n), L.c_i32(q.ml), P(sdf), P(nab), P(rgb, allow_none=not rad), P(x), *ap,
+                   ctypes.byref(q.collect) if q.collect is not None else None, L.stream_ptr(), count=q.count)
+        ctx.q, ctx.ridx, ctx.t, ctx.n, ctx.rad = q, ridx, t, n, rad
+        ctx.held = (acts, rgb)
         ctx.shapes = [p.shape for p in params]
         ctx.set_materialize_grads(False)
         ctx.mark_non_differentiable(x)
@@ -53,12 +67,11 @@ class _FusedColor(autograd.Function):
     @staticmethod
     @autograd.function.once_differentiable
     def backward(ctx, *g_out):
-        grid16, net, _held, acts, rgb = ctx.held
+        acts, rgb = ctx.held
         if acts is None:
             raise RuntimeError("fused_color: backward through a forward that ran without grad")
+        q, dev, n = ctx.q, acts.device, ctx.n
         g_sdf, g_nab, g_rgb = g_out[0], g_out[1], (g_out[2] if ctx.rad else None)
-        dev, n = acts.device, ctx.n
-        meta = ctx.model.implicit_surface.encoding.meta
         # one zero-fill for the table gradient, one for the small tensors (views of a flat buffer)
         sizes = [int(torch.Size(s).numel()) for s in ctx.shapes[1:]]
         small = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
@@ -67,20 +80,18 @@ class _FusedColor(autograd.Function):
             grads.append(small[o:o + k].view(sh))
             o += k
         if g_sdf is None and g_nab is None and g_rgb is None:
-            return (None,) * 7 + tuple(grads)
-        ridx, t, rays_o, rays_d = ctx.pts
+            return (None,) * 6 + tuple(grads)
         c = lambda g: None if g is None else g.contiguous().float()
         g_sdf, g_nab, g_rgb = c(g_sdf), c(g_nab), c(g_rgb)
         dh = torch.empty(n, 32, dtype=torch.float32, device=dev) if g_rgb is not None else None
-        ag = [L.ptr(g) for g in grads] + [None] * (11 - len(grads))          # d_R* / d_rb*: NULL without the radiance net's parameters
+        P = L.ptr
+        ag = [P(g) for g in grads] + [None] * (11 - len(grads))          # d_R* / d_rb*: NULL without the radiance net's parameters
         with L.KERNEL_TIMER.time("fused_color_bwd", n):
-            L.check(L.lib().nsb_fused_color_bwd(meta.c_ref, L.ptr(grid16, "f16"), ctypes.byref(net), None, L.ptr(rays_o, "f32"), L.ptr(rays_d, "f32"),
-                                                L.ptr(ridx, "i64"), L.ptr(t, "f32"), L.c_i64(n), L.c_i32(ctx.max_level), L.ptr(acts[0]), L.ptr(acts[1]),
-                                                *([L.ptr(acts[2]), L.ptr(acts[3])] if ctx.rad else [None, None]), L.ptr(rgb, allow_none=True),
-                                                L.ptr(g_sdf, allow_none=True), L.ptr(g_nab, allow_none=True), L.ptr(g_rgb, allow_none=True),
-                                                L.ptr(dh, allow_none=True), *ag, L.stream_ptr()),
-                    "fused_color_bwd")
-        return (None,) * 7 + tuple(grads)
+            L.call(L.lib().nsb_fused_color_bwd, "fused_color_bwd", q.meta.c_ref, P(q.grid16, "f16"), ctypes.byref(q.net), None, P(q.rays_o, "f32"),
+                   P(q.rays_d, "f32"), P(ctx.ridx, "i64"), P(ctx.t, "f32"), L.c_i64(n), L.c_i32(q.ml), P(acts[0]), P(acts[1]),
+                   *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]), P(rgb, allow_none=True), P(g_sdf, allow_none=True),
+                   P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh, allow_none=True), *ag, L.stream_ptr(), count=q.count)
+        return (None,) * 6 + tuple(grads)
 
 
 def fused_color(model, ridx, t, rays_o, rays_d, view_dirs=None, h_appear=None, *, nablas_has_grad=True, collect=None, with_rgb=True):
@@ -92,12 +103,13 @@ def fused_color(model, ridx, t, rays_o, rays_d, view_dirs=None, h_appear=None, *
     if with_rgb:
         r = model.radiance_net.blocks.layers
         params += (r[0].weight, r[0].bias, r[1].weight, r[1].bias, r[2].weight, r[2].bias)
-    pts = (ridx.reshape(-1).contiguous().long(), t.detach().reshape(-1).contiguous().float(), rays_o.detach().contiguous().float(),
-           rays_d.detach().contiguous().float())
+    grid16, net, held = model._fused_color_state() if with_rgb else model._fused_geometry_state()
+    q = ColorQuery(s.encoding.meta, grid16, net, held, rays_o.detach().contiguous().float(), rays_d.detach().contiguous().float(), s._ml(model.max_level),
+                   collect, None)
     keep = torch.is_grad_enabled() and any(p.requires_grad for p in params)
     ha = None if (h_appear is None or not with_rgb) else h_appear.detach().contiguous().float()
     vd = view_dirs.detach().contiguous().float() if with_rgb else None
-    out = _FusedColor.apply(model, pts, vd, ha, s._ml(model.max_level), keep, collect, *params)
+    out = _FusedColor.apply(q, ridx.reshape(-1).contiguous().long(), t.detach().reshape(-1).contiguous().float(), vd, ha, keep, *params)
     sdf, nab, x = out[0], out[1], out[-1]
     if not nablas_has_grad:
         nab = nab.detach()

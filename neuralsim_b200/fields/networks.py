@@ -5,8 +5,8 @@ fields/nerf/mlp_nerf.py:188-289, embedders/spherical_harmonics/sphere_harmonics.
 
 fp32 master weights, fp16 autocast evaluation -- the numerics contract of the reference.  The modules below are the
 reference's layers (torch autocast, cuBLAS) and remain the specification; the hot path replaces them by fused wgmma
-kernels with the same rounding points: SDF queries (with or without grad) by `nsb_fused_sdf*` + `nsb_fused_sdf_bwd`
-(`_FusedSDF`, csrc/fused_tc.cu), the colour / normal query by `nsb_fused_color_*` (fields/fused_color.py, csrc/color_tc.cu).
+kernels with the same rounding points: SDF queries (with or without grad) by `nsb_fused_sdf_collect` + `nsb_fused_sdf_bwd_indexed`
+(`sdf_fwd`, `sdf_bwd`, `_FusedSDF`, csrc/fused_tc.cu), the colour / normal query by `nsb_fused_color_*` (fields/fused_color.py, csrc/color_tc.cu).
 """
 from __future__ import annotations
 
@@ -135,18 +135,58 @@ class SHEncoder(nn.Module):
         return _sh_encoder.apply(flat, self.degree, flat.requires_grad).unflatten(0, prefix)
 
 
+def sdf_decoder_c(t16, layers):
+    """nsb_sdf_decoder over the fp16 images t16 = (W1, b1, W2, b2) of the decoder layers"""
+    return L.SdfDecoderC(t16[0].data_ptr(), t16[1].data_ptr(), t16[2].data_ptr(), t16[3].data_ptr(), layers[0].out_features,
+                         float(layers[0].activation.beta))
+
+
+def sdf_fwd(meta, grid16, dec, sdf, max_level, *, x=None, rays_o=None, rays_d=None, t=None, ridx=None, packs=None, collect=None, count=None):
+    """one launch of the fused SDF query (nsb_fused_sdf_collect) into sdf: points x [n,3], or samples t [n] of rays ridx [n], or, with
+    packs = (pack_infos, pack ray | None[, block order | None]), the packs of t (ray-tiled; ridx unused)"""
+    P = L.ptr
+    if x is not None:
+        pts = (P(x, "f32"), None, None, None, None, L.c_i64(x.shape[0]), None, None, None, L.c_i64(0), L.c_i32(0))
+    elif packs is None:
+        pts = (None, P(rays_o, "f32"), P(rays_d, "f32"), P(ridx, "i64"), P(t, "f32"), L.c_i64(t.numel()), None, None, None, L.c_i64(0), L.c_i32(1))
+    else:
+        pts = (None, P(rays_o, "f32"), P(rays_d, "f32"), None, P(t, "f32"), L.c_i64(t.numel()), P(packs[0], "i64"), P(packs[1], "i64", allow_none=True),
+               P(packs[2], "i64", allow_none=True) if len(packs) > 2 else None, L.c_i64(packs[0].shape[0]), L.c_i32(2))
+    L.call(L.lib().nsb_fused_sdf_collect, "fused_sdf", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), *pts, L.c_i32(max_level), P(sdf),
+           ctypes.byref(collect) if collect is not None else None, L.stream_ptr(), count=count)
+    return sdf
+
+
+def sdf_bwd(meta, grid16, dec, d_sdf, n, max_level, grads, *, x=None, rays=None, keep=None, count=None):
+    """one launch of the fused SDF backward (nsb_fused_sdf_bwd_indexed), accumulated into grads = (d_grid, d_W1, d_b1, d_W2, d_b2): row i of
+    the n rows is sample keep[i] (keep None: i) of the points x or of rays = (rays_o, rays_d, ridx, t)"""
+    P = L.ptr
+    pts = (P(x, "f32"), None, None, None, None) if x is not None else (None, P(rays[0], "f32"), P(rays[1], "f32"), P(rays[2], "i64"), P(rays[3], "f32"))
+    d_grid, d_W1, d_b1, d_W2, d_b2 = grads
+    L.call(L.lib().nsb_fused_sdf_bwd_indexed, "fused_sdf_bwd", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), *pts, P(d_sdf, "f32"),
+           P(keep, "i64", allow_none=True), L.c_i64(n), L.c_i32(max_level), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2), L.stream_ptr(), count=count)
+
+
 class _FusedSDF(autograd.Function):
     """sdf = decoder(LoTD(x)) as ONE op with a hand-written backward (csrc/fused_tc.cu): forward keeps nothing but its
     inputs, backward recomputes features / pre-activations and accumulates straight into fp32 gradients of the table and
-    the four decoder tensors.  `x` is either points [N,3] or a (ridx, t, rays_o, rays_d) tuple (x = o[ridx] + d[ridx] t)."""
+    the four decoder tensors.  `x` is either points [N,3] or a (ridx, t, rays_o, rays_d, packs | None) tuple (x = o[ridx] + d[ridx] t)."""
 
     @staticmethod
-    def forward(ctx, owner, pts, max_level, grid, W1, b1, W2, b2):
+    def forward(ctx, owner, pts, max_level, collect, grid, W1, b1, W2, b2):
         grid16, dec = owner._fused_state()
-        with L.KERNEL_TIMER.time("fused_sdf_fwd", (pts[1] if isinstance(pts, tuple) else pts).shape[0]):
-            sdf = owner._launch_sdf(grid16, dec, pts, max_level)
+        meta = owner.encoding.meta
+        if isinstance(pts, tuple):
+            ridx, t, rays_o, rays_d, packs = pts
+            sdf = torch.empty(t.numel(), dtype=torch.float32, device=t.device)
+            with L.KERNEL_TIMER.time("fused_sdf_fwd", t.shape[0]):
+                sdf_fwd(meta, grid16, dec, sdf, max_level, rays_o=rays_o, rays_d=rays_d, t=t, ridx=ridx, packs=packs, collect=collect)
+        else:
+            sdf = torch.empty(pts.shape[0], dtype=torch.float32, device=pts.device)
+            with L.KERNEL_TIMER.time("fused_sdf_fwd", pts.shape[0]):
+                sdf_fwd(meta, grid16, dec, sdf, max_level, x=pts, collect=collect)
         n = sdf.shape[0]
-        ctx.owner, ctx.pts, ctx.max_level, ctx.n = owner, pts[:5] if isinstance(pts, tuple) else pts, max_level, n
+        ctx.owner, ctx.pts, ctx.max_level, ctx.n = owner, pts, max_level, n
         ctx.held = (grid16, dec, owner._fused_cache[1])          # the fp16 images the forward used (the tensors `dec` points into stay alive)
         ctx.shapes = (grid.shape, W1.shape, b1.shape, W2.shape, b2.shape)
         return sdf
@@ -169,24 +209,21 @@ class _FusedSDF(autograd.Function):
         keep = scan_counts(d_sdf.ne(0).to(torch.int32), want_index=True)["index"]
         n = keep.numel()
         if n == 0:
-            return None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2
+            return None, None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2
         sparse = n < 0.9 * ctx.n
         if sparse:
             d_sdf = d_sdf[keep]
         if isinstance(ctx.pts, tuple):
-            ridx, t, rays_o, rays_d, _packs = ctx.pts[:5]
+            ridx, t, rays_o, rays_d, _packs = ctx.pts
             if sparse:
                 ridx, t = ridx[keep], t[keep]
-            args = (None, L.ptr(rays_o, "f32"), L.ptr(rays_d, "f32"), L.ptr(ridx, "i64"), L.ptr(t, "f32"))
+            x, rays = None, (rays_o, rays_d, ridx, t)
         else:
-            pts = ctx.pts[keep] if sparse else ctx.pts
-            args = (L.ptr(pts, "f32"), None, None, None, None)
+            x, rays = (ctx.pts[keep] if sparse else ctx.pts), None
         n = n if sparse else ctx.n
         with L.KERNEL_TIMER.time("fused_sdf_bwd", n):
-            L.check(L.lib().nsb_fused_sdf_bwd(meta.c_ref, L.ptr(grid16, "f16"), ctypes.byref(dec), *args, L.ptr(d_sdf, "f32"), L.c_i64(n),
-                                              L.c_i32(ctx.max_level), L.ptr(d_grid), L.ptr(d_W1), L.ptr(d_b1), L.ptr(d_W2), L.ptr(d_b2),
-                                              L.stream_ptr()), "fused_sdf_bwd")
-        return None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2
+            sdf_bwd(meta, grid16, dec, d_sdf, n, ctx.max_level, (d_grid, d_W1, d_b1, d_W2, d_b2), x=x, rays=rays)
+        return None, None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2
 
 
 class LoTDSDF(nn.Module):
@@ -225,39 +262,12 @@ class LoTDSDF(nn.Module):
         ml = max_level or self.encoding.max_level
         return self.encoding.meta.n_levels if ml is None else int(ml)
 
-    def _launch_sdf(self, grid16, dec, pts, max_level):
-        """one launch of the fused query.  pts: x [n,3]  |  (ridx, t, rays_o, rays_d, packs | None[, collect | None])"""
-        meta = self.encoding.meta
-        if isinstance(pts, tuple):
-            ridx, t, rays_o, rays_d, packs = pts[:5]
-            collect = pts[5] if len(pts) > 5 else None
-            sdf = torch.empty(t.numel(), dtype=torch.float32, device=t.device)
-            mode = 2 if packs is not None else 1
-            L.check(L.lib().nsb_fused_sdf_collect(
-                meta.c_ref, L.ptr(grid16, "f16"), ctypes.byref(dec), None, L.ptr(rays_o, "f32"), L.ptr(rays_d, "f32"),
-                L.ptr(ridx, "i64", allow_none=(mode == 2)) if mode == 1 else None, L.ptr(t, "f32"), L.c_i64(t.numel()),
-                L.ptr(packs[0], "i64") if mode == 2 else None, L.ptr(packs[1], "i64", allow_none=True) if mode == 2 else None,
-                L.ptr(packs[2], "i64", allow_none=True) if mode == 2 and len(packs) > 2 else None,
-                L.c_i64(packs[0].shape[0] if mode == 2 else 0), L.c_i32(mode), L.c_i32(max_level), L.ptr(sdf),
-                ctypes.byref(collect) if collect is not None else None, L.stream_ptr()), "fused_sdf")
-            return sdf
-        sdf = torch.empty(pts.shape[0], dtype=torch.float32, device=pts.device)
-        L.check(L.lib().nsb_fused_sdf_collect(meta.c_ref, L.ptr(grid16, "f16"), ctypes.byref(dec), L.ptr(pts, "f32"), None, None, None, None,
-                                              L.c_i64(pts.shape[0]), None, None, None, L.c_i64(0), L.c_i32(0), L.c_i32(max_level), L.ptr(sdf),
-                                              ctypes.byref(self._collect) if getattr(self, "_collect", None) is not None else None, L.stream_ptr()),
-                "fused_sdf")
-        return sdf
-
     def fused_sdf_autograd(self, x, max_level: int = None, collect=None):
         """differentiable (wrt. table + decoder) fused query on points [...,3]"""
         d = self.decoder.layers
         prefix = x.shape[:-1]
-        self._collect = collect
-        try:
-            sdf = _FusedSDF.apply(self, x.detach().reshape(-1, 3).contiguous().float(), self._ml(max_level), self.encoding.flattened_params,
-                                  d[0].weight, d[0].bias, d[1].weight, d[1].bias)
-        finally:
-            self._collect = None
+        sdf = _FusedSDF.apply(self, x.detach().reshape(-1, 3).contiguous().float(), self._ml(max_level), collect, self.encoding.flattened_params,
+                              d[0].weight, d[0].bias, d[1].weight, d[1].bias)
         return sdf.view(prefix)
 
     def fused_sdf_rays_autograd(self, ridx, t, rays_o, rays_d, max_level: int = None, packs=None, collect=None):
@@ -266,8 +276,8 @@ class LoTDSDF(nn.Module):
         if t.dim() == 2:
             ridx = ridx.unsqueeze(-1).expand(shape)
         pts = (ridx.reshape(-1).contiguous().long(), t.detach().reshape(-1).contiguous().float(), rays_o.detach().contiguous(),
-               rays_d.detach().contiguous(), packs, collect)
-        sdf = _FusedSDF.apply(self, pts, self._ml(max_level), self.encoding.flattened_params, d[0].weight, d[0].bias, d[1].weight, d[1].bias)
+               rays_d.detach().contiguous(), packs)
+        sdf = _FusedSDF.apply(self, pts, self._ml(max_level), collect, self.encoding.flattened_params, d[0].weight, d[0].bias, d[1].weight, d[1].bias)
         return sdf.view(shape)
 
     def forward_sdf_nablas(self, x, *, has_grad: bool = None, nablas_has_grad: bool = None, max_level: int = None, grad_guard=None):
@@ -305,9 +315,7 @@ class LoTDSDF(nn.Module):
         key = tuple((p.data_ptr(), p._version) for p in ps)
         if self._fused_cache is None or self._fused_cache[0] != key:
             t = [p.detach().to(torch.half).contiguous() for p in ps]
-            dec = L.SdfDecoderC(t[1].data_ptr(), t[2].data_ptr(), t[3].data_ptr(), t[4].data_ptr(), self.decoder.layers[0].out_features,
-                                float(self.decoder.layers[0].activation.beta))
-            self._fused_cache = (key, t, dec)
+            self._fused_cache = (key, t, sdf_decoder_c(t[1:], self.decoder.layers))
         return self._fused_cache[1][0], self._fused_cache[2]
 
     @torch.no_grad()
@@ -315,35 +323,24 @@ class LoTDSDF(nn.Module):
         grid16, dec = self._fused_state()
         prefix = x.shape[:-1]
         xf = x.reshape(-1, 3).contiguous().float()
-        self._collect = collect
-        try:
-            with L.KERNEL_TIMER.time("lotd_gather", xf.shape[0]):
-                sdf = self._launch_sdf(grid16, dec, xf, self._ml(max_level))
-        finally:
-            self._collect = None
+        sdf = torch.empty(xf.shape[0], dtype=torch.float32, device=xf.device)
+        with L.KERNEL_TIMER.time("lotd_gather", xf.shape[0]):
+            sdf_fwd(self.encoding.meta, grid16, dec, sdf, self._ml(max_level), x=xf, collect=collect)
         return sdf.view(prefix)
 
     @torch.no_grad()
     def fused_sdf_rays(self, ridx, t, rays_o, rays_d, max_level: int = None, packs=None, collect=None):
         grid16, dec = self._fused_state()
         shape = t.shape
-        if packs is not None or collect is not None:
-            if packs is None and t.dim() == 2:
+        if packs is None:
+            if t.dim() == 2:
                 ridx = ridx.unsqueeze(-1).expand(shape)
-            tf = t.reshape(-1).contiguous().float()
-            pts = (ridx.reshape(-1).contiguous().long() if packs is None else None, tf, rays_o.contiguous(), rays_d.contiguous(), packs, collect)
-            with L.KERNEL_TIMER.time("lotd_gather", tf.shape[0]):
-                sdf = self._launch_sdf(grid16, dec, pts, self._ml(max_level))
-            return sdf.view(shape)
-        if t.dim() == 2:
-            ridx = ridx.unsqueeze(-1).expand(shape)
-        ridx, tf = ridx.reshape(-1).contiguous().long(), t.reshape(-1).contiguous().float()
+            ridx = ridx.reshape(-1).contiguous().long()
+        tf = t.reshape(-1).contiguous().float()
         sdf = torch.empty(tf.shape[0], dtype=torch.float32, device=tf.device)
-        ml = self.encoding.meta.n_levels if (max_level or self.encoding.max_level) is None else int(max_level or self.encoding.max_level)
         with L.KERNEL_TIMER.time("lotd_gather", tf.shape[0]):
-          L.check(L.lib().nsb_fused_sdf_rays(self.encoding.meta.c_ref, L.ptr(grid16, "f16"), ctypes.byref(dec), L.ptr(rays_o.contiguous(), "f32"),
-                                           L.ptr(rays_d.contiguous(), "f32"), L.ptr(ridx, "i64"), L.ptr(tf, "f32"), L.c_i64(tf.shape[0]),
-                                           L.c_i32(ml), L.ptr(sdf), L.stream_ptr()), "fused_sdf_rays")
+            sdf_fwd(self.encoding.meta, grid16, dec, sdf, self._ml(max_level), rays_o=rays_o.contiguous(), rays_d=rays_d.contiguous(), t=tf, ridx=ridx,
+                    packs=packs, collect=collect)
         return sdf.view(shape)
 
 

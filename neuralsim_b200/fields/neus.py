@@ -8,8 +8,6 @@ A geometry-only model (`radiance_cfg=False`, the reference's `radiance_cfg: null
 """
 from __future__ import annotations
 
-import ctypes
-
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -18,9 +16,8 @@ from ..graphics import neus as neus_graphics, neus_fused
 from ..graphics.neus import neus_ray_query_march_occ_multi_upsample_compressed
 from ..graphics.nerf import packed_alpha_to_vw, ray_alpha_to_vw
 from ..graphics.pack_ops import packed_div, packed_sum
-from .. import _lib as L
 from .accel import OccGridAccel
-from .fused_color import fused_color
+from .fused_color import color_net_c, fused_color
 from .networks import LoTDSDF, RadianceNet, VarSingleMixLinear
 from .space import AABBSpace
 
@@ -116,10 +113,7 @@ class LoTDNeuS(nn.Module):
         cache = getattr(self, "_color_cache", None)
         if cache is None or cache[0] != key:
             t = [p.detach().to(torch.half).contiguous() for p in ps]
-            fac = self._nablas_fac()
-            net = L.ColorNetC(*[x.data_ptr() for x in t], s.decoder.layers[0].out_features, b[0].out_features, b[0].in_features,
-                              b[0].in_features - 54, float(s.decoder.layers[0].activation.beta), (ctypes.c_float * 3)(*fac))
-            cache = self._color_cache = (key, t, net)
+            cache = self._color_cache = (key, t, color_net_c(t, s.decoder.layers, b, self._nablas_fac()))
         return grid16, cache[2], cache[1]
 
     def _nablas_fac(self):
@@ -139,10 +133,7 @@ class LoTDNeuS(nn.Module):
         t, fac = s._fused_cache[1], self._nablas_fac()
         cache = getattr(self, "_geo_cache", None)
         if cache is None or cache[0] is not t or cache[1] != fac:
-            d = s.decoder.layers
-            net = L.ColorNetC(*[x.data_ptr() for x in t[1:]], *([None] * 6), d[0].out_features, 0, 0, 0, float(d[0].activation.beta),
-                              (ctypes.c_float * 3)(*fac))
-            cache = self._geo_cache = (t, list(fac), net)
+            cache = self._geo_cache = (t, list(fac), color_net_c(t[1:], s.decoder.layers, None, fac))
         return grid16, cache[2], t
 
     def forward_on_rays(self, ridx, t, rays_o, rays_d, view_dirs=None, rays_h_appear=None, *, nablas_has_grad=True, with_rgb=True):

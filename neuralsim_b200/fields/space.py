@@ -1,6 +1,8 @@
 """Axis-aligned bounding space -- API of `nr3d_lib.models.spatial.AABBSpace` (reference: models/spatial/aabb.py:20-99)."""
 from __future__ import annotations
 
+import ctypes
+
 import torch
 import torch.nn as nn
 
@@ -67,27 +69,25 @@ class AABBSpace(nn.Module):
             ret.update(rays_o=rays_o[ridx], rays_d=rays_d[ridx])
         return ret
 
-    @torch.no_grad()
-    def _ray_test_fused(self, rays_o, rays_d, near, far, normalized, extra_ray_data):
-        """The same test as below in three launches and one host read (csrc/neus_glue.cu: k_ray_test_aabb, k_scan_counts, k_gather_rays)."""
-        from ..graphics.neus_fused import scan_counts
-        import ctypes
-        R, dev = rays_o.shape[0], rays_o.device
+    def _center_radius_c(self):
+        """the box's centre and half-size as host float[3] arrays, read back only when the aabb changed"""
         if getattr(self, "_host_cr", None) is None or self._host_cr[0] != (self.aabb.data_ptr(), self.aabb._version):
             c, r = self.center.tolist(), self.radius3d.tolist()
             self._host_cr = ((self.aabb.data_ptr(), self.aabb._version), (ctypes.c_float * 3)(*c), (ctypes.c_float * 3)(*r))
-        c3, r3 = self._host_cr[1], self._host_cr[2]
+        return self._host_cr[1], self._host_cr[2]
+
+    @torch.no_grad()
+    def _ray_test_fused(self, rays_o, rays_d, near, far, normalized, extra_ray_data):
+        """The same test as below in three launches and one host read (csrc/neus_glue.cu: k_ray_test_aabb, k_scan_counts, k_gather_rays)."""
+        from ..graphics import neus_fused as NF
+        R, dev = rays_o.shape[0], rays_o.device
         if normalized:
             c3, r3 = (ctypes.c_float * 3)(0., 0., 0.), (ctypes.c_float * 3)(1., 1., 1.)
-        o_n, d_n = torch.empty(R, 3, device=dev), torch.empty(R, 3, device=dev)
-        nr, fr = torch.empty(R, device=dev), torch.empty(R, device=dev)
-        flag = torch.empty(R, dtype=torch.int32, device=dev)
+        else:
+            c3, r3 = self._center_radius_c()
         pairs = torch.zeros(2, dtype=torch.int64, device=dev)              # coherent neighbour pairs, image row length
-        L.check(L.lib().nsb_ray_test_aabb(L.ptr(rays_o.contiguous(), "f32"), L.ptr(rays_d.contiguous(), "f32"), L.c_i64(R), c3, r3,
-                                          ctypes.c_int(0 if near is None else 1), L.c_f32(0. if near is None else near),
-                                          ctypes.c_int(0 if far is None else 1), L.c_f32(0. if far is None else far), L.ptr(o_n), L.ptr(d_n),
-                                          L.ptr(nr), L.ptr(fr), L.ptr(flag), L.ptr(pairs), L.ptr(pairs[1:]), L.stream_ptr()), "ray_test_aabb")
-        sc = scan_counts(flag, want_index=True, extra=pairs)
+        tested = NF.ray_test_aabb(rays_o, rays_d, c3, r3, near, far, L.ptr(pairs), L.ptr(pairs[1:]))
+        sc = NF.scan_counts(tested[4], want_index=True, extra=pairs)
         n, ridx = sc["n_nonzero"], sc["index"]
         o_c, d_c = torch.empty(n, 3, device=dev), torch.empty(n, 3, device=dev)
         n_c, f_c = torch.empty(n, device=dev), torch.empty(n, device=dev)
@@ -96,9 +96,7 @@ class AABBSpace(nn.Module):
                           and v.shape[0] == R and v.is_contiguous() and not v.requires_grad), None)
         ex = extra_ray_data[fused_key] if fused_key is not None else None
         ex_c = torch.empty(n, ex.shape[1], device=dev) if ex is not None else None
-        L.check(L.lib().nsb_gather_rays(L.ptr(ridx, "i64"), L.c_i64(n), L.ptr(o_n), L.ptr(d_n), L.ptr(nr), L.ptr(fr), L.ptr(o_c), L.ptr(d_c),
-                                        L.ptr(n_c), L.ptr(f_c), L.ptr(ex, allow_none=True), L.ptr(ex_c, allow_none=True),
-                                        L.c_i32(0 if ex is None else ex.shape[1]), L.stream_ptr()), "gather_rays")
+        NF.gather_rays(ridx, n, tested[:4], (o_c, d_c, n_c, f_c), ex, ex_c)
         ret = dict(num_rays=n, rays_inds=ridx, near=n_c, far=f_c)
         ret.update({k: (ex_c if k == fused_key else (v[ridx] if isinstance(v, torch.Tensor) else v)) for k, v in extra_ray_data.items()})
         ret.update(rays_o=o_c, rays_d=d_c)

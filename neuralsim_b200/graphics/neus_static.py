@@ -20,6 +20,8 @@ import torch
 import torch.nn.functional as F
 
 from .. import _lib as L
+from ..fields.fused_color import ColorQuery, _FusedColor, color_net_c
+from ..fields.networks import sdf_bwd, sdf_decoder_c, sdf_fwd
 from .raysample import batch_sample_step_linear
 from .pack_ops import get_pack_infos_from_batch
 from . import neus_fused as NF
@@ -28,7 +30,6 @@ __all__ = ["render_static", "StaticFrame", "CNT_SLOTS"]
 
 CNT_SLOTS = dict(n_rays=0, pairs=2, marched_raw=3, hit_raw=4, kept_raw=6, kept_rays_raw=7, nonzero=9, marched=12, hit=13, fine0=14,
                  boundary=18, kept=19, overflow=20, kept_rays=21, merged0=22, rays_if_kept_fits=26, row_len=27)
-_NULL = ctypes.c_void_p(0)
 # "auto": small batches march once and copy (nsb_ray_marching_record + nsb_march_compact) when the per-ray record fits this many bytes;
 # "0": always the two-round march; "1": always the recorded march.  Same samples bit for bit either way.
 MARCH_ONEPASS = "auto"
@@ -41,61 +42,29 @@ def march_onepass(n_rays, max_steps):
     return MARCH_ONEPASS == "1" or 4 * int(n_rays) * int(max_steps) <= MARCH_ONEPASS_MAX_BYTES
 
 
-def _slot(cnt, k):
-    return ctypes.c_void_p(cnt.data_ptr() + 8 * k)
+_slot = L.slot
 
 
 def _call(fn, what, cnt, k0, k1, *args):
-    """one count-aware launch: bind cnt[k0] (and cnt[k1]) to this thread, launch, clear"""
-    lib = L.lib()
-    lib.nsb_bind_device_counts(_slot(cnt, k0), _slot(cnt, k1) if k1 is not None else _NULL)
-    try:
-        rc = fn(*args)
-    finally:
-        lib.nsb_bind_device_counts(_NULL, _NULL)
-    L.check(rc, what)
+    """one launch with the counts cnt[k0] (and cnt[k1]) of the step's count block (_lib.call)"""
+    L.call(fn, what, *args, count=(cnt, k0) if k1 is None else (cnt, k0, k1))
 
 
 def _scan(counts, cnt, slot, *, first=None, info2=None, index=None, pack=None, src=None, nz_src=None, ws=None):
-    """nsb_scan_counts with the totals left in cnt[slot], cnt[slot + 1] (no host hand-off)"""
-    if ws is None:
-        ws = torch.zeros(NF._scan_ws_bytes(), dtype=torch.uint8, device=counts.device)
-    P = L.ptr
-    L.check(L.lib().nsb_scan_counts(P(counts, "i32"), L.c_i64(counts.shape[0]), P(first, allow_none=True), P(info2, allow_none=True),
-                                    P(index, allow_none=True), P(pack, allow_none=True), P(src, "i64", allow_none=True), P(nz_src, allow_none=True),
-                                    _slot(cnt, slot), None, L.c_i64(0), P(ws), L.stream_ptr()), "scan_counts")
+    """neus_fused.scan_launch with the totals left in cnt[slot], cnt[slot + 1] (no host hand-off)"""
+    NF.scan_launch(counts, _slot(cnt, slot), first=first, info2=info2, index=index, pack=pack, src=src, nz_src=nz_src, ws=ws)
+
+
+def _block_order(rays_inds, via, n_rays, cnt, slot):
+    """the 8 x 4 pixel-block order of the cnt[slot] live packs on pixels rays_inds[via[p]] (neus_fused.ray_block_order; the row length and
+    the coherence test are the ray test's, in cnt)"""
+    return NF.ray_block_order(rays_inds, via, n_rays, _slot(cnt, CNT_SLOTS["pairs"]), _slot(cnt, CNT_SLOTS["row_len"]), count=(cnt, slot))
 
 
 def _query_counts(cnt, phase, n_coarse1, num_fine, march_cap, kept_cap):
     nf = (ctypes.c_int32 * max(len(num_fine), 1))(*[int(n) for n in num_fine])
     L.check(L.lib().nsb_query_counts(ctypes.c_void_p(cnt.data_ptr()), L.c_i32(phase), L.c_i32(n_coarse1), nf, L.c_i32(len(num_fine)),
                                      L.c_i64(march_cap), L.c_i64(kept_cap), L.stream_ptr()), "query_counts")
-
-
-def _sdf_launch(meta, grid16, dec, rays_o, rays_d, t, sdf, *, ridx=None, packs=None, ml, collect, cnt, slot, timer="lotd_gather"):
-    """the fused SDF query on rays with a device-resident count: mode 1 (ridx[n], count = samples) or mode 2 (packs = (pack_infos, pack_ray | None,
-    block order | None), count = packs)"""
-    P = L.ptr
-    mode = 2 if packs is not None else 1
-    with L.KERNEL_TIMER.time(timer, t.numel()):
-        _call(L.lib().nsb_fused_sdf_collect, "fused_sdf", cnt, slot, None,
-              meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), None, P(rays_o, "f32"), P(rays_d, "f32"),
-              P(ridx, "i64") if mode == 1 else None, P(t, "f32"), L.c_i64(t.numel()),
-              P(packs[0], "i64") if mode == 2 else None, P(packs[1], "i64", allow_none=True) if mode == 2 else None,
-              P(packs[2], "i64", allow_none=True) if mode == 2 and len(packs) > 2 else None,
-              L.c_i64(packs[0].shape[0] if mode == 2 else 0), L.c_i32(mode), L.c_i32(ml), P(sdf),
-              ctypes.byref(collect) if collect is not None else None, L.stream_ptr())
-    return sdf
-
-
-def _block_order(rays_inds, via, n_rays, cnt, slot):
-    """the 8 x 4 pixel-block order of the cnt[slot] live packs on pixels rays_inds[via[p]] (nsb_ray_block_order; the row length and the
-    coherence test are the ray test's, in cnt)"""
-    n = rays_inds.shape[0] if via is None else via.shape[0]
-    order = torch.empty(n, dtype=torch.int64, device=rays_inds.device)
-    _call(L.lib().nsb_ray_block_order, "ray_block_order", cnt, slot, None, L.ptr(rays_inds, "i64"), L.ptr(via, "i64", allow_none=True), L.c_i64(n),
-          L.c_i64(n_rays), _slot(cnt, CNT_SLOTS["pairs"]), _slot(cnt, CNT_SLOTS["row_len"]), L.ptr(order), L.stream_ptr())
-    return order
 
 
 # ---------------------------------------------------------------------------------------------------------------- autograd pieces
@@ -109,26 +78,24 @@ class _StaticBoundary(torch.autograd.Function):
     @staticmethod
     def forward(ctx, st, d1, pinfo, ridx_all, order_b, rays_inds, kept_cap, qc, inv_s, grid, W1, b1, W2, b2):
         """ridx_all None: coherent rays, the query walks the packs in the 8 x 4 pixel-block order order_b; else sample by sample"""
-        R, dev, cnt, P, lib = pinfo.shape[0], d1.device, st.cnt, L.ptr, L.lib()
+        R, dev, cnt = pinfo.shape[0], d1.device, st.cnt
         sdf = torch.empty(d1.numel(), dtype=torch.float32, device=dev)
-        _sdf_launch(st.meta, st.grid16, st.dec, st.rays_o, st.rays_d, d1, sdf, ridx=ridx_all, packs=(pinfo, None, order_b) if ridx_all is None else None,
-                    ml=st.ml, collect=st.collect, cnt=cnt, slot=CNT_SLOTS["n_rays"] if ridx_all is None else CNT_SLOTS["boundary"], timer="fused_sdf_fwd")
+        with L.KERNEL_TIMER.time("fused_sdf_fwd", d1.numel()):
+            if ridx_all is None:
+                sdf_fwd(st.meta, st.grid16, st.dec, sdf, st.ml, rays_o=st.rays_o, rays_d=st.rays_d, t=d1, packs=(pinfo, None, order_b), collect=st.collect,
+                        count=(cnt, CNT_SLOTS["n_rays"]))
+            else:
+                sdf_fwd(st.meta, st.grid16, st.dec, sdf, st.ml, rays_o=st.rays_o, rays_d=st.rays_d, t=d1, ridx=ridx_all, collect=st.collect,
+                        count=(cnt, CNT_SLOTS["boundary"]))
         inv_c = inv_s.detach().contiguous().float().reshape(1)
-        alpha = torch.empty_like(sdf)
-        sel = torch.empty(sdf.shape[0], dtype=torch.bool, device=dev)
-        steps = torch.empty(R, dtype=torch.int32, device=dev)
-        _call(lib.nsb_neus_alpha_forward, "neus_alpha_forward", cnt, CNT_SLOTS["n_rays"], None, P(sdf, "f32"), P(pinfo, "i64"), L.c_i64(R),
-              P(inv_c, "f32"), L.c_f32(1e-4), L.c_f32(0.0), P(alpha), P(sel), P(steps), L.stream_ptr())
+        alpha, sel, steps = NF.alpha_forward(sdf, pinfo, inv_c, 1e-4, 0.0, count=(cnt, CNT_SLOTS["n_rays"]))
         first = torch.empty(R, dtype=torch.int32, device=dev)
         nidx = torch.empty(R, dtype=torch.int64, device=dev)
         pinfo_kept = torch.empty(R, 2, dtype=torch.int64, device=dev)
         rays_inds_hit = torch.empty(R, dtype=torch.int64, device=dev)
         _scan(steps, cnt, CNT_SLOTS["kept_raw"], first=first, index=nidx, pack=pinfo_kept, src=rays_inds, nz_src=rays_inds_hit, ws=st.ws[2])
         _query_counts(cnt, 1, *qc)
-        pidx, ridx_k = torch.empty(kept_cap, dtype=torch.int64, device=dev), torch.empty(kept_cap, dtype=torch.int64, device=dev)
-        t_k, alpha_k = torch.empty(kept_cap, dtype=torch.float32, device=dev), torch.empty(kept_cap, dtype=torch.float32, device=dev)
-        _call(lib.nsb_compact_samples, "compact_samples", cnt, CNT_SLOTS["rays_if_kept_fits"], None, P(sel.view(torch.uint8), "u8"), P(pinfo, "i64"),
-              P(first, "i32"), P(steps, "i32"), L.c_i64(R), None, None, P(d1, "f32"), P(alpha, "f32"), P(pidx), P(ridx_k), P(t_k), P(alpha_k), L.stream_ptr())
+        pidx, ridx_k, t_k, alpha_k = NF.compact_samples(sel, pinfo, first, steps, alpha, kept_cap, d1=d1, count=(cnt, CNT_SLOTS["rays_if_kept_fits"]))
         ctx.st, ctx.saved = st, (d1, sdf, inv_c, pinfo, nidx, pinfo_kept, pidx)
         ctx.shapes = (inv_s.shape, grid.shape, W1.shape, b1.shape, W2.shape, b2.shape)
         ctx.mark_non_differentiable(t_k, ridx_k, pinfo_kept, rays_inds_hit)
@@ -160,120 +127,12 @@ class _StaticBoundary(torch.autograd.Function):
             _scan(counts, cnt, CNT_SLOTS["nonzero"], first=offs, ws=st.ws[3])
             n_list = min(S, 2 * K)                         # at most a kept sample and the one after it per kept sample
             keep = torch.empty(n_list, dtype=torch.int64, device=dev)
-            _call(lib.nsb_neus_alpha_backward_kept_list, "neus_alpha_backward_kept_list", cnt, CNT_SLOTS["kept_rays"], None, *a, P(g, "f32"), P(d_sdf, "f32"),
-                  P(offs, "i32"), L.c_i64(R), P(keep), P(ray), L.stream_ptr())
+            _call(lib.nsb_neus_alpha_backward_kept_list, "neus_alpha_backward_kept_list", cnt, CNT_SLOTS["kept_rays"], None, *a, P(g, "f32"),
+                  P(d_sdf, "f32"), P(offs, "i32"), L.c_i64(R), P(keep), P(ray), L.stream_ptr())
             with L.KERNEL_TIMER.time("fused_sdf_bwd", n_list):
-                _call(lib.nsb_fused_sdf_bwd_indexed, "fused_sdf_bwd", cnt, CNT_SLOTS["nonzero"], None,
-                      st.meta.c_ref, P(st.grid16, "f16"), ctypes.byref(st.dec), None, P(st.rays_o, "f32"), P(st.rays_d, "f32"), P(ray, "i64"),
-                      P(d1, "f32"), P(d_sdf, "f32"), P(keep, "i64"), L.c_i64(n_list), L.c_i32(st.ml), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2),
-                      L.stream_ptr())
+                sdf_bwd(st.meta, st.grid16, st.dec, d_sdf, n_list, st.ml, (d_grid, d_W1, d_b1, d_W2, d_b2), rays=(st.rays_o, st.rays_d, ray, d1), keep=keep,
+                        count=(cnt, CNT_SLOTS["nonzero"]))
         return (None,) * 8 + (d_inv.reshape(inv_shape), d_grid, d_W1, d_b1, d_W2, d_b2)
-
-
-class _StaticColor(torch.autograd.Function):
-    """fields/fused_color.py:_FusedColor over the K = cnt[19] kept samples (buffers sized kept_cap); params: the five SDF parameters, then the
-    six radiance parameters when rgb is computed (without them: the geometry-only form, no rgb output)"""
-
-    @staticmethod
-    def forward(ctx, st, ridx, t, view_dirs, h_appear, keep_acts, *params):
-        rad = len(params) > 5
-        n, dev = t.numel(), t.device
-        sdf = torch.empty(n, dtype=torch.float32, device=dev)
-        nab = torch.empty(n, 3, dtype=torch.float32, device=dev)
-        rgb = torch.empty(n, 3, dtype=torch.float32, device=dev) if rad else None
-        x = torch.empty(n, 3, dtype=torch.float32, device=dev)
-        n_act = 4 if rad else 2                                  # Z, X (+ Y1, Y2)
-        acts = torch.empty(n_act, int(L.lib().nsb_color_tile_bytes(L.c_i64(n))), dtype=torch.uint8, device=dev) if keep_acts else None
-        ap = [L.ptr(acts[k]) if keep_acts and k < n_act else None for k in range(4)]
-        P = L.ptr
-        with L.KERNEL_TIMER.time("fused_color_fwd", n):
-            _call(L.lib().nsb_fused_color_fwd, "fused_color_fwd", st.cnt, CNT_SLOTS["kept"], None,
-                  st.meta.c_ref, P(st.grid16, "f16"), ctypes.byref(st.net), None, P(st.rays_o, "f32"), P(st.rays_d, "f32"), P(ridx, "i64"), P(t, "f32"),
-                  P(view_dirs, "f32", allow_none=not rad), P(h_appear, "f32", allow_none=True), L.c_i64(n), L.c_i32(st.ml), P(sdf), P(nab),
-                  P(rgb, allow_none=not rad), P(x), *ap, ctypes.byref(st.collect) if st.collect is not None else None, L.stream_ptr())
-        ctx.st, ctx.ridx, ctx.t, ctx.n, ctx.rad = st, ridx, t, n, rad
-        ctx.held = (acts, rgb)
-        ctx.shapes = [p.shape for p in params]
-        ctx.set_materialize_grads(False)
-        ctx.mark_non_differentiable(x)
-        return (sdf, nab, rgb, x) if rad else (sdf, nab, x)
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, *g_out):
-        acts, rgb = ctx.held
-        if acts is None:
-            raise RuntimeError("static colour query: backward through a forward that ran without grad")
-        st, dev, n = ctx.st, acts.device, ctx.n
-        g_sdf, g_nab, g_rgb = g_out[0], g_out[1], (g_out[2] if ctx.rad else None)
-        sizes = [int(torch.Size(s).numel()) for s in ctx.shapes[1:]]
-        small = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
-        grads, o = [torch.zeros(ctx.shapes[0], dtype=torch.float32, device=dev)], 0
-        for sh, k in zip(ctx.shapes[1:], sizes):
-            grads.append(small[o:o + k].view(sh))
-            o += k
-        if g_sdf is None and g_nab is None and g_rgb is None:
-            return (None,) * 6 + tuple(grads)
-        c = lambda g: None if g is None else g.contiguous().float()
-        g_sdf, g_nab, g_rgb = c(g_sdf), c(g_nab), c(g_rgb)
-        dh = torch.empty(n, 32, dtype=torch.float32, device=dev) if g_rgb is not None else None
-        P = L.ptr
-        ag = [P(g) for g in grads] + [None] * (11 - len(grads))          # d_R* / d_rb*: NULL without the radiance net's parameters
-        with L.KERNEL_TIMER.time("fused_color_bwd", n):
-            _call(L.lib().nsb_fused_color_bwd, "fused_color_bwd", st.cnt, CNT_SLOTS["kept"], None,
-                  st.meta.c_ref, P(st.grid16, "f16"), ctypes.byref(st.net), None, P(st.rays_o, "f32"), P(st.rays_d, "f32"), P(ctx.ridx, "i64"),
-                  P(ctx.t, "f32"), L.c_i64(n), L.c_i32(st.ml), P(acts[0]), P(acts[1]), *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]),
-                  P(rgb, allow_none=True), P(g_sdf, allow_none=True), P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh, allow_none=True),
-                  *ag, L.stream_ptr())
-        return (None,) * 6 + tuple(grads)
-
-
-class _StaticComposite(torch.autograd.Function):
-    """graphics/neus_fused.py:_Composite over the cnt[21] rays that keep samples, written straight into whole-image buffers"""
-
-    @staticmethod
-    def forward(ctx, alpha, t, rgb, nablas, pack_infos, ray_index, n_rays, cnt, normalize_depth, early_stop_eps, alpha_thre):
-        a, tt = alpha.detach().contiguous().float(), t.detach().contiguous().float()
-        r = None if rgb is None else rgb.detach().contiguous().float()
-        nb = None if nablas is None else nablas.detach().contiguous().float()
-        Pn, dev = pack_infos.shape[0], a.device
-        vw = torch.empty_like(a)
-        cols = 2 + (3 if r is not None else 0) + (3 if nb is not None else 0)
-        buf = torch.zeros(cols * n_rays, device=dev)
-        mask, depth = buf[:n_rays], buf[n_rays:2 * n_rays]
-        rgb_o = buf[2 * n_rays:5 * n_rays].view(n_rays, 3) if r is not None else None
-        o3 = 5 * n_rays if r is not None else 2 * n_rays
-        nab_o = buf[o3:o3 + 3 * n_rays].view(n_rays, 3) if nb is not None else None
-        P = L.ptr
-        _call(L.lib().nsb_composite_forward, "composite_forward", cnt, CNT_SLOTS["kept_rays"], None, P(a, "f32"), P(tt, "f32"), P(r, "f32", allow_none=True),
-              P(nb, "f32", allow_none=True), P(pack_infos, "i64"), L.c_i64(Pn), L.c_f32(early_stop_eps), L.c_f32(alpha_thre),
-              ctypes.c_int(1 if normalize_depth else 0), P(ray_index, "i64"), P(vw), P(mask), P(depth), P(rgb_o, allow_none=True),
-              P(nab_o, allow_none=True), L.stream_ptr())
-        ctx.save_for_backward(a, tt, r, nb, vw, pack_infos, mask, depth, ray_index)
-        ctx.cfg = (normalize_depth, early_stop_eps, alpha_thre, cnt)
-        ctx.set_materialize_grads(False)
-        empty = a.new_empty(0)
-        return vw, mask, depth, (rgb_o if rgb_o is not None else empty), (nab_o if nab_o is not None else empty)
-
-    @staticmethod
-    def backward(ctx, g_vw, g_mask, g_depth, g_rgb, g_nab):
-        a, tt, r, nb, vw, pack_infos, mask, depth, ray_index = ctx.saved_tensors
-        normalize_depth, eps, thre, cnt = ctx.cfg
-
-        def opt(g, present=True):
-            return None if (g is None or not present) else g.contiguous().float()
-        g_vw, g_mask, g_depth = opt(g_vw), opt(g_mask), opt(g_depth)
-        g_rgb, g_nab = opt(g_rgb, r is not None), opt(g_nab, nb is not None)
-        d_alpha = torch.empty_like(a)
-        d_rgb = torch.empty_like(r) if r is not None else None
-        d_nab = torch.empty_like(nb) if nb is not None else None
-        P = L.ptr
-        _call(L.lib().nsb_composite_backward, "composite_backward", cnt, CNT_SLOTS["kept_rays"], None,
-              P(a, "f32"), P(tt, "f32"), P(r, allow_none=True), P(nb, allow_none=True), P(vw, "f32"), P(pack_infos, "i64"), L.c_i64(pack_infos.shape[0]),
-              L.c_f32(eps), L.c_f32(thre), ctypes.c_int(1 if normalize_depth else 0), P(mask), P(depth), P(g_mask, allow_none=True),
-              P(g_depth, allow_none=True), P(g_rgb, allow_none=True), P(g_nab, allow_none=True), P(g_vw, allow_none=True), P(ray_index, "i64"),
-              P(d_alpha), P(d_rgb, allow_none=True), P(d_nab, allow_none=True), L.stream_ptr())
-        return (d_alpha, None, d_rgb, d_nab) + (None,) * 7
 
 
 class _State:
@@ -287,26 +146,15 @@ def _fp16_images(model, radiance=True):
     s = model.implicit_surface
     d = s.decoder.layers
     ps = [s.encoding.flattened_params, d[0].weight, d[0].bias, d[1].weight, d[1].bias]
+    b = model.radiance_net.blocks.layers if radiance else None
     if radiance:
-        b = model.radiance_net.blocks.layers
         ps += [b[0].weight, b[0].bias, b[1].weight, b[1].bias, b[2].weight, b[2].bias]
     # one multi-tensor cast for the small tensors (a launch each otherwise: at 4096 rays per step the step is launch-bound), one for the table
     t = [torch.empty(p.shape, dtype=torch.half, device=p.device) for p in ps]
     with torch.no_grad():
         t[0].copy_(ps[0].detach())
         torch._foreach_copy_(t[1:], [p.detach() for p in ps[1:]])
-    dec = L.SdfDecoderC(t[1].data_ptr(), t[2].data_ptr(), t[3].data_ptr(), t[4].data_ptr(), d[0].out_features, float(d[0].activation.beta))
-    r3 = s.radius3d_original
-    fk = (r3.data_ptr(), r3._version, float(s.sdf_scale))
-    if getattr(model, "_fac_cache", (None,))[0] != fk:
-        model._fac_cache = (fk, (s.sdf_scale / r3).float().tolist())
-    fac = (ctypes.c_float * 3)(*model._fac_cache[1])
-    if radiance:
-        net = L.ColorNetC(*[x.data_ptr() for x in t[1:]], d[0].out_features, b[0].out_features, b[0].in_features, b[0].in_features - 54,
-                          float(d[0].activation.beta), fac)
-    else:
-        net = L.ColorNetC(*[x.data_ptr() for x in t[1:]], *([None] * 6), d[0].out_features, 0, 0, 0, float(d[0].activation.beta), fac)
-    return t, dec, net, ps
+    return t, sdf_decoder_c(t[1:5], d), color_net_c(t[1:], d, b, model._nablas_fac()), ps
 
 
 def static_supported(model, cfg):
@@ -341,7 +189,6 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     num_fine = qp.get("num_fine", 8)
     num_fine = [num_fine] * n_stage if isinstance(num_fine, int) else list(num_fine)
     num_fine = [n // 2 * 2 + 1 for n in num_fine]
-    nf_tot = int(sum(num_fine))
     upsample_inv_s = qp.get("upsample_inv_s", 64.) / model.upsample_s_divisor
     use_est = bool(qp.get("upsample_use_estimate_alpha", False))
     nablas_has_grad = bool(qp.get("nablas_has_grad", False))
@@ -350,7 +197,6 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     step_size, dt_gamma = mc.get("step_size", 1e-3) * fac, mc.get("dt_gamma", 0.0) * fac
     max_steps, max_step_size = int(mc.get("max_steps", 512)), mc.get("max_step_size", 1e10)
     march_cap, kept_cap = int(march_cap), int(kept_cap)
-    S_cap = R * (nc1 + nf_tot)
     if cnt is None:
         cnt = torch.zeros(32, dtype=torch.int64, device=dev)
     else:
@@ -366,19 +212,10 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         st.ml = model.implicit_surface._ml(model.max_level)
         st.collect = model.accel.occ.collect_struct() if training else None
         # ---------------- ray test (fields/space.py:_ray_test_fused without the host read)
-        sp = model.space
-        if getattr(sp, "_host_cr", None) is None or sp._host_cr[0] != (sp.aabb.data_ptr(), sp.aabb._version):
-            c, r = sp.center.tolist(), sp.radius3d.tolist()
-            sp._host_cr = ((sp.aabb.data_ptr(), sp.aabb._version), (ctypes.c_float * 3)(*c), (ctypes.c_float * 3)(*r))
-        o_n, d_n = torch.empty(R, 3, device=dev), torch.empty(R, 3, device=dev)
-        nr, fr = torch.empty(R, device=dev), torch.empty(R, device=dev)
-        flag = torch.empty(R, dtype=torch.int32, device=dev)
-        L.check(lib.nsb_ray_test_aabb(P(rays_o.contiguous(), "f32"), P(rays_d.contiguous(), "f32"), L.c_i64(R), sp._host_cr[1], sp._host_cr[2],
-                                      ctypes.c_int(0 if near is None else 1), L.c_f32(0. if near is None else near),
-                                      ctypes.c_int(0 if far is None else 1), L.c_f32(0. if far is None else far), P(o_n), P(d_n), P(nr), P(fr), P(flag),
-                                      _slot(cnt, CNT_SLOTS["pairs"]), _slot(cnt, CNT_SLOTS["row_len"]), L.stream_ptr()), "ray_test_aabb")
+        c3, r3 = model.space._center_radius_c()
+        tested = NF.ray_test_aabb(rays_o, rays_d, c3, r3, near, far, _slot(cnt, CNT_SLOTS["pairs"]), _slot(cnt, CNT_SLOTS["row_len"]))
         rays_inds = torch.empty(R, dtype=torch.int64, device=dev)
-        _scan(flag, cnt, CNT_SLOTS["n_rays"], index=rays_inds, ws=st.ws[0])
+        _scan(tested[4], cnt, CNT_SLOTS["n_rays"], index=rays_inds, ws=st.ws[0])
         # the boundary query walks its packs (the rays that passed) in 8 x 4 pixel blocks (csrc/neus_glue.cu: k_ray_block_order)
         order_b = _block_order(rays_inds, None, R, cnt, CNT_SLOTS["n_rays"]) if coherent else None
         # only the radiance head reads appearance codes: rays that render no rgb gather none
@@ -390,8 +227,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         o_c, d_c = rbuf[:3 * R].view(R, 3), rbuf[3 * R:6 * R].view(R, 3)
         n_c, f_c = rbuf[6 * R:7 * R], rbuf[7 * R:8 * R]
         ha_c = rbuf[8 * R:].view(R, n_ha) if ha is not None else None
-        _call(lib.nsb_gather_rays, "gather_rays", cnt, CNT_SLOTS["n_rays"], None, P(rays_inds, "i64"), L.c_i64(R), P(o_n), P(d_n), P(nr), P(fr), P(o_c), P(d_c),
-              P(n_c), P(f_c), P(ha, allow_none=True), P(ha_c, allow_none=True), L.c_i32(0 if ha is None else ha.shape[1]), L.stream_ptr())
+        NF.gather_rays(rays_inds, R, tested[:4], (o_c, d_c, n_c, f_c), ha, ha_c, count=(cnt, CNT_SLOTS["n_rays"]))
         st.rays_o, st.rays_d = o_c, d_c
         view_dirs = (d_c / d_c.norm(dim=-1).clamp_min(1.0e-10).unsqueeze(-1)).contiguous() if with_rgb else None
         # ---------------- coarse samples + march
@@ -399,12 +235,10 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         occ_grid = model.accel.occ.occ_grid
         res = occ_grid.shape[-3:]
         g8 = occ_grid.contiguous().view(torch.uint8)
-        bits = torch.empty((occ_grid.numel() + 31) // 32, dtype=torch.int32, device=dev)
-        L.check(lib.nsb_pack_occ_bits(P(g8, "u8"), L.c_i64(occ_grid.numel()), P(bits), L.stream_ptr()), "pack_occ_bits")
+        bits = NF.pack_occ_bits(occ_grid)
         roi = torch.tensor([-1, -1, -1, 1, 1, 1], dtype=torch.float32, device=dev) if getattr(model, "_static_roi", None) is None else model._static_roi
         model._static_roi = roi
-        margs = (L.c_i64(R), P(o_c, "f32"), P(d_c, "f32"), P(n_c, "f32"), P(f_c, "f32"), P(roi, "f32"), None, L.c_i32(res[0]), L.c_i32(res[1]), L.c_i32(res[2]),
-                 P(g8, "u8"), L.c_f32(step_size), L.c_f32(max_step_size), L.c_f32(dt_gamma), ctypes.c_uint32(max_steps))
+        margs = NF.march_args(o_c, d_c, n_c, f_c, roi, occ_grid, step_size, max_step_size, dt_gamma, max_steps)
         num_steps = torch.empty(R, dtype=torch.int32, device=dev)
         # small batches: a march costs the latency of its longest ray -> march ONCE, recording the samples per ray, and copy (csrc/march.cu)
         rec_t = torch.empty(R * max_steps, dtype=torch.float32, device=dev) if march_onepass(R, max_steps) else None
@@ -414,8 +248,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
                       P(f_c, "f32"), P(roi, "f32"), L.c_i32(res[0]), L.c_i32(res[1]), L.c_i32(res[2]), P(g8, "u8"), L.c_f32(step_size), L.c_f32(max_step_size),
                       L.c_f32(dt_gamma), ctypes.c_uint32(max_steps), P(num_steps), P(rec_t), P(bits), L.stream_ptr())
             else:
-                _call(lib.nsb_ray_marching_listed, "ray_marching", cnt, CNT_SLOTS["n_rays"], None, *margs, None, P(num_steps), None, None, None, None, None, None,
-                      L.c_i64(0), P(bits), L.stream_ptr())
+                NF.march_listed(margs, bits, num_steps=num_steps, count=(cnt, CNT_SLOTS["n_rays"]))
         info2 = torch.empty(R, 2, dtype=torch.int32, device=dev)
         ridx_hit = torch.empty(R, dtype=torch.int64, device=dev)
         pack_infos = torch.empty(R, 2, dtype=torch.int64, device=dev)
@@ -428,59 +261,39 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
                 _call(lib.nsb_march_compact, "march_compact", cnt, CNT_SLOTS["hit"], None, P(rec_t, "f32"), ctypes.c_uint32(max_steps), P(info2, "i32"),
                       P(ridx_hit, "i64"), L.c_i64(R), P(depth), P(ridx32), L.stream_ptr())
             else:
-                _call(lib.nsb_ray_marching_listed, "ray_marching", cnt, CNT_SLOTS["hit"], None, *margs, P(info2), None, P(depth), None, P(ridx32), None, None,
-                      P(ridx_hit, "i64"), L.c_i64(R), P(bits), L.stream_ptr())
+                NF.march_listed(margs, bits, info2=info2, t_starts=depth, ridx=ridx32, ray_list=ridx_hit, n_list=R, count=(cnt, CNT_SLOTS["hit"]))
         ridx = ridx32.long()
         # ---------------- up-sampling (no grad)
         from . import neus as GN
-        fine_stages = None
+        hit = (cnt, CNT_SLOTS["hit"])
         if GN.use_persistent_upsample(R):                    # ONE persistent per-ray kernel (csrc/ray_upsample.cu): small batches (graphics/neus.py)
             fine_all, _ovf = NF.upsample_rays(st.meta, st.grid16, st.dec, ridx_hit, pack_infos, depth, o_c, d_c, [upsample_inv_s * f for f in factors], num_fine,
-                                              max_level=st.ml, max_steps=max_steps, use_estimate_alpha=use_est, collect=st.collect, count=(cnt, CNT_SLOTS["hit"]))
-            factors_loop = []
+                                              max_level=st.ml, max_steps=max_steps, use_estimate_alpha=use_est, collect=st.collect, count=hit)
         else:
-            factors_loop = factors
-        sdf = torch.empty(march_cap if factors_loop else 1, dtype=torch.float32, device=dev)
-        if factors_loop:
             fine_stages = []
             order_f = _block_order(rays_inds, ridx_hit, R, cnt, CNT_SLOTS["hit"]) if coherent and n_stage > 1 else None
-            _sdf_launch(st.meta, st.grid16, st.dec, o_c, d_c, depth, sdf, ridx=ridx, ml=st.ml, collect=st.collect, cnt=cnt, slot=CNT_SLOTS["marched"])
-        for i, factor in enumerate(factors_loop):
-            cdf = torch.empty(march_cap, dtype=torch.float32, device=dev)
-            _call(lib.nsb_neus_upsample_cdf, "neus_upsample_cdf", cnt, CNT_SLOTS["hit"], None, P(sdf, "f32"), P(depth, "f32"), P(pack_infos, "i64"), L.c_i64(R),
-                  L.c_f32(upsample_inv_s * factor), ctypes.c_int(1 if use_est else 0), L.c_f32(1e-4), L.c_f32(0.0), P(cdf), L.stream_ptr())
-            nf = num_fine[i]
-            fine = torch.empty(R, nf, dtype=torch.float32, device=dev)
-            u = NF._U_CACHE.get((nf, dev))
-            if u is None:
-                u = NF._U_CACHE[(nf, dev)] = torch.linspace(0., 1., nf + 2, device=dev, dtype=torch.float32)[1:-1].contiguous()
-            _call(lib.nsb_packed_invert_cdf_shared_u, "packed_invert_cdf_shared_u", cnt, CNT_SLOTS["hit"], None, P(depth, "f32"), P(cdf, "f32"), P(u, "f32"),
-                  P(pack_infos, "i64"), L.c_i64(R), L.c_i32(nf), P(fine), L.stream_ptr())
-            fine_stages.append(fine)
-            if i < n_stage - 1:
-                sdf_fine = torch.empty(R * nf, dtype=torch.float32, device=dev)
-                if coherent:
-                    _sdf_launch(st.meta, st.grid16, st.dec, o_c, d_c, fine.view(-1), sdf_fine, packs=(get_pack_infos_from_batch(R, nf, device=dev), ridx_hit, order_f),
-                                ml=st.ml, collect=st.collect, cnt=cnt, slot=CNT_SLOTS["hit"])
-                else:
-                    _sdf_launch(st.meta, st.grid16, st.dec, o_c, d_c, fine.view(-1), sdf_fine, ridx=ridx_hit.unsqueeze(-1).expand(R, nf).reshape(-1).contiguous(),
-                                ml=st.ml, collect=st.collect, cnt=cnt, slot=CNT_SLOTS["fine0"] + i)
-                dep_m = torch.empty(march_cap, dtype=torch.float32, device=dev)
-                sdf_m = torch.empty(march_cap, dtype=torch.float32, device=dev)
-                pim = torch.empty_like(pack_infos)
-                _call(lib.nsb_merge_sorted_vals, "merge_sorted_vals", cnt, CNT_SLOTS["hit"], None, P(depth, "f32"), P(sdf, "f32"), P(pack_infos, "i64"),
-                      P(fine, "f32"), P(sdf_fine, "f32"), L.c_i64(R), L.c_i32(nf), P(dep_m), P(sdf_m), P(pim), L.stream_ptr())
-                depth, sdf, pack_infos = dep_m, sdf_m, pim
-        if fine_stages is not None:
+            sdf = torch.empty(march_cap, dtype=torch.float32, device=dev)
+            with L.KERNEL_TIMER.time("lotd_gather", march_cap):
+                sdf_fwd(st.meta, st.grid16, st.dec, sdf, st.ml, rays_o=o_c, rays_d=d_c, t=depth, ridx=ridx, collect=st.collect, count=(cnt, CNT_SLOTS["marched"]))
+            for i, factor in enumerate(factors):
+                cdf = NF.upsample_cdf(sdf, depth, pack_infos, upsample_inv_s * factor, use_est, count=hit)
+                nf = num_fine[i]
+                fine = NF.sample_cdf_uniform(depth, cdf, pack_infos, nf, count=hit)
+                fine_stages.append(fine)
+                if i < n_stage - 1:
+                    sdf_fine = torch.empty(R * nf, dtype=torch.float32, device=dev)
+                    with L.KERNEL_TIMER.time("lotd_gather", R * nf):
+                        if coherent:
+                            sdf_fwd(st.meta, st.grid16, st.dec, sdf_fine, st.ml, rays_o=o_c, rays_d=d_c, t=fine.view(-1),
+                                    packs=(get_pack_infos_from_batch(R, nf, device=dev), ridx_hit, order_f), collect=st.collect, count=hit)
+                        else:
+                            sdf_fwd(st.meta, st.grid16, st.dec, sdf_fine, st.ml, rays_o=o_c, rays_d=d_c, t=fine.view(-1),
+                                    ridx=ridx_hit.unsqueeze(-1).expand(R, nf).reshape(-1).contiguous(), collect=st.collect, count=(cnt, CNT_SLOTS["fine0"] + i))
+                    depth, sdf, pack_infos = NF.merge_sorted_vals(depth, sdf, pack_infos, fine, sdf_fine, n_out=march_cap, count=hit)
             fine_all = (torch.cat(fine_stages, dim=-1) if n_stage > 1 else fine_stages[0]).contiguous()
-        d1 = torch.empty(S_cap, dtype=torch.float32, device=dev)
         # the ray of every boundary sample: only the incoherent boundary query (one sample per row) reads it; everything else derives it
-        ridx_all = None if coherent else torch.empty(S_cap, dtype=torch.int64, device=dev)
-        pinfo = torch.empty(R, 2, dtype=torch.int64, device=dev)
-        rl = (ctypes.c_int32 * n_stage)(*num_fine)
-        _call(lib.nsb_assemble_boundary, "assemble_boundary", cnt, CNT_SLOTS["n_rays"], CNT_SLOTS["hit"], P(coarse, "f32"), L.c_i64(R), L.c_i32(nc1),
-              P(ridx_hit, "i64"), L.c_i64(R), P(fine_all, "f32"), L.c_i32(nf_tot), rl, L.c_i32(n_stage), P(d1), None, P(ridx_all, "i64", allow_none=True), P(pinfo),
-              L.stream_ptr())
+        d1, _mid, ridx_all, pinfo = NF.assemble_boundary(coarse, ridx_hit, fine_all, num_fine, want_mid=False, want_ridx=not coherent,
+                                                         count=(cnt, CNT_SLOTS["n_rays"], CNT_SLOTS["hit"]))
     # ---------------- boundary SDF (grad) -> alpha -> compression
     s = model.implicit_surface
     dl = s.decoder.layers
@@ -498,7 +311,8 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
             b = model.radiance_net.blocks.layers
             params += (b[0].weight, b[0].bias, b[1].weight, b[1].bias, b[2].weight, b[2].bias)
         keep_acts = torch.is_grad_enabled() and any(p.requires_grad for p in params)
-        out = _StaticColor.apply(st, ridx_k, t_k, view_dirs, ha_c, keep_acts, *params)
+        q = ColorQuery(st.meta, st.grid16, st.net, st.held, st.rays_o, st.rays_d, st.ml, st.collect, (cnt, CNT_SLOTS["kept"]))
+        out = _FusedColor.apply(q, ridx_k, t_k, view_dirs, ha_c, keep_acts, *params)
         nab, x = out[1], out[-1]
         rgb = out[2] if with_rgb else None
         if not nablas_has_grad:
@@ -506,8 +320,8 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     nab_i = nab if with_normal else None
     if nab_i is not None and not training:
         nab_i = F.normalize(nab_i.clamp(-1, 1), dim=-1)
-    vw, m, d, c, nn_ = _StaticComposite.apply(alpha_k, t_k, rgb, nab_i, pinfo_kept, rays_inds_hit, R, cnt,
-                                              bool(depth_use_normalized_vw), 1e-4, 0.0)
+    vw, m, d, c, nn_ = NF.composite(alpha_k, t_k, pinfo_kept, rgb=rgb, nablas=nab_i, normalize_depth=bool(depth_use_normalized_vw), ray_index=rays_inds_hit,
+                                    n_rays=R, count=(cnt, CNT_SLOTS["kept_rays"]))
     rendered = dict(mask_volume=m, depth_volume=d)
     if with_rgb:
         rendered["rgb_volume"] = c

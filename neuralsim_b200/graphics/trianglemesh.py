@@ -21,7 +21,7 @@ import numpy as np
 import torch
 
 from .. import _lib as L
-from .neus_fused import _scan_ws_bytes, scan_counts
+from .neus_fused import _scan_ws_bytes, scan_counts, scan_launch
 
 __all__ = ["extract_mesh", "write_ply"]
 
@@ -159,8 +159,7 @@ def extract_mesh(
         L.check(lib.nsb_mc_count(L.ptr(win), w0, w1 - w0, n0, n1, n2, p0, p1, float(level), L.ptr(flags), L.ptr(vcount), L.ptr(cases),
                                  L.ptr(tcount), stream), "mc_count")
         ws = torch.zeros(ws_bytes, dtype=torch.uint8, device=dev)
-        L.check(lib.nsb_scan_counts(L.ptr(vcount, "i32"), L.c_i64(n), L.ptr(vfirst), None, None, None, None, None, L.ptr(vtot), None,
-                                    L.c_i64(0), L.ptr(ws), stream), "mc vertex scan")
+        scan_launch(vcount, L.ptr(vtot), first=vfirst, ws=ws)
         sc = scan_counts(tcount, want_first=True, extra=vtot[:1])        # the slab's one host read: triangle and vertex totals
         nt, nv = sc["total"], sc["extra"][0]
         if vbase + nv > _I32_MAX:

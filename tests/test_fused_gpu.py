@@ -1,5 +1,7 @@
 """Fused forward_sdf kernel (csrc/fused.cu) against (i) the CPU oracle and (ii) the reference's actual code path on the
 GPU: LoTD feature kernel + torch.autocast(fp16) MLP (what nr3d_lib's DenseLayer executes)."""
+import ctypes
+
 import numpy as np
 import pytest
 import torch
@@ -52,17 +54,27 @@ def test_fused_sdf_rays_matches_points(cuda):
 
 
 def test_tensor_core_kernel_matches_cuda_core_kernel(cuda):
-    """csrc/fused_tc.cu (wgmma) against csrc/fused.cu (CUDA cores): same rounding points, fp32 accumulation order differs."""
+    """csrc/fused_tc.cu (wgmma, what LoTDSDF.fused_sdf runs) against csrc/fused.cu's k_fused_sdf (CUDA cores): same rounding points, fp32
+    accumulation order differs.  The reference comes from nsb_fused_sdf with sdf_simt = 1 and the feature output h_out_half, which only
+    k_fused_sdf writes: its sentinels must be gone."""
     from neuralsim_b200 import _lib
     P, model = make_pair(cuda)
+    s = model.implicit_surface
+    grid16, dec = s._fused_state()
     g = torch.Generator().manual_seed(11)
     for n in (1, 127, 128, 129, 5000, 200001):
         x = (torch.rand(n, 3, generator=g) * 2 - 1).to(cuda)
-        with torch.no_grad():
-            _lib.check(_lib.lib().nsb_set_option(b"sdf_simt", 1))
-            ref = model.implicit_surface.fused_sdf(x)
+        ref = torch.empty(n, device=cuda)
+        h = torch.full((n, 32), float("nan"), dtype=torch.half, device=cuda)
+        _lib.check(_lib.lib().nsb_set_option(b"sdf_simt", 1))
+        try:
+            _lib.check(_lib.lib().nsb_fused_sdf(s.encoding.meta.c_ref, _lib.ptr(grid16, "f16"), ctypes.byref(dec), _lib.ptr(x, "f32"), _lib.c_i64(n),
+                                                _lib.c_i32(s._ml(None)), _lib.ptr(ref), _lib.ptr(h), _lib.stream_ptr()), "fused_sdf")
+        finally:
             _lib.check(_lib.lib().nsb_set_option(b"sdf_simt", 0))
-            got = model.implicit_surface.fused_sdf(x)
+        assert not bool(torch.isnan(h).any()), n                     # k_fused_sdf ran
+        with torch.no_grad():
+            got = s.fused_sdf(x)
         frac, worst = _ulp16_mismatch(got, ref)
         assert frac < 2e-2 and worst <= 2.0, (n, frac, worst)
 
