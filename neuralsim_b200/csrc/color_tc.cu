@@ -6,9 +6,9 @@
 // and its autograd backward (LoTDFunctionBwdDydx.backward = lod_bwd_bwd_input, lotd.py:193-268; the autocast MLP
 // double-backward) with three kernels:
 //
-//   k_color_fwd      gather h -> MMA Z=H.W1^T -> z,a,sdf,u=fp16(w2 s) -> MMA g=U.W1 (= dsdf/dh) -> second gather pass
-//                    nablas = J^T g (J recomputed per level, never stored) -> radiance input row -> MMA -> relu -> MMA ->
-//                    relu -> 64->3 -> sigmoid.   Saves the fp16 activation tiles Z, X, Y1, Y2 in core-matrix layout.
+//   k_color_fwd      one gather: h and the per-level Jacobian J from the same corner loads (J kept in registers, never stored)
+//                    -> MMA Z=H.W1^T -> z,a,sdf,u=fp16(w2 s) -> MMA g=U.W1 (= dsdf/dh) -> nablas = J^T g -> radiance input row
+//                    -> MMA -> relu -> MMA -> relu -> 64->3 -> sigmoid.   Saves the fp16 activation tiles Z, X, Y1, Y2 in core-matrix layout.
 //   k_color_rad_bwd  radiance backward from the saved tiles: dZ2, dZ1 (MMA), dh (MMA), weight gradients accumulated in
 //                    registers over all tiles of the persistent CTA (MN-major M64 MMAs contracting over the 128 points).
 //   k_color_sdf_bwd  gather pass for dg = J.dn, MMA du = dG.W1^T, MMA g = U.W1, dz (softplus'' term + sdf term),
@@ -46,19 +46,12 @@ __host__ __device__ inline int ref_col(int k, int n_appear) {
 }
 
 
-// d(y_f)/d(x_d) of one level (both features), exactly as k_lotd_fwd<3,2,true,true> computes dy_dx
-__device__ __forceinline__ void level_jacobian(const PLMeta &m, uint32_t p, const float (&xs)[3], const __half *__restrict__ grid,
-                                               float (&J0)[3], float (&J1)[3]) {
-    uint32_t cell[8];
-    float w[8], fr[3], scale[3];
-    level_cells3(m, p, xs, cell, w, fr, scale);
-    const uint32_t *lp = level_cells_ptr(m, p, grid);
+// d(y_f)/d(x_d) of one level (both features) from its 8 corner cells as loaded, exactly as k_lotd_fwd<3,2,true,true> computes dy_dx
+__device__ __forceinline__ void jacobian_from_raw(const uint32_t (&raw)[8], const float (&fr)[3], const float (&scale)[3], float (&J0)[3],
+                                                  float (&J1)[3]) {
     float2 v[8];
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        const uint32_t raw = ld_nc_u32(lp + cell[c]);
-        v[c] = __half22float2(*reinterpret_cast<const __half2 *>(&raw));
-    }
+    for (int c = 0; c < 8; ++c) v[c] = __half22float2(*reinterpret_cast<const __half2 *>(&raw[c]));
 #pragma unroll
     for (int gd = 0; gd < 3; ++gd) {
         float a0 = 0.f, a1 = 0.f;
@@ -81,6 +74,17 @@ __device__ __forceinline__ void level_jacobian(const PLMeta &m, uint32_t p, cons
     }
 }
 
+__device__ __forceinline__ void level_jacobian(const PLMeta &m, uint32_t p, const float (&xs)[3], const __half *__restrict__ grid,
+                                               float (&J0)[3], float (&J1)[3]) {
+    uint32_t cell[8], raw[8];
+    float w[8], fr[3], scale[3];
+    level_cells3(m, p, xs, cell, w, fr, scale);
+    const uint32_t *lp = level_cells_ptr(m, p, grid);
+#pragma unroll
+    for (int c = 0; c < 8; ++c) raw[c] = ld_nc_u32(lp + cell[c]);
+    jacobian_from_raw(raw, fr, scale, J0, J1);
+}
+
 __device__ __forceinline__ void unpack8(const uint4 &q, float (&v)[8]) {
     const __half2 *h = reinterpret_cast<const __half2 *>(&q);
 #pragma unroll
@@ -91,6 +95,35 @@ __device__ __forceinline__ void unpack8(const uint4 &q, float (&v)[8]) {
 // registers are plentiful -> four levels (32 corner loads) per gather trip instead of the two of k_fused_sdf_tc (which runs 24 warps per SM).
 constexpr int kColorGatherU = 4;
 
+// The one table gather of the colour forward: each level's 8 corners are loaded once and give both its fp16 feature pair (-> row r of the
+// chunk-major X tile, zero above max_level, as gather_row_to_tile writes it) and its Jacobian J0[p], J1[p], which stay in registers until
+// g = U.W1 is known.  Fully unrolled, unlike the rolled gathers of the 16-24-warp kernels, so that J (96 floats) is statically indexed:
+// k_color_fwd runs 8 warps per SM and has no min-blocks bound, so it may use the registers.  The corner loads of kColorGatherU levels are
+// issued before any of them is consumed.
+__device__ __forceinline__ void gather_row_and_jacobian(const PLMeta &m, const __half *__restrict__ grid, const float (&xs)[3], int max_level,
+                                                        uint8_t *tile, int r, float (&J0)[16][3], float (&J1)[16][3]) {
+#pragma unroll
+    for (uint32_t p0 = 0; p0 < 16; p0 += kColorGatherU) {
+        uint32_t cell[kColorGatherU][8], raw[kColorGatherU][8];
+        float w[kColorGatherU][8], fr[kColorGatherU][3], sc[kColorGatherU][3];
+#pragma unroll
+        for (int u = 0; u < kColorGatherU; ++u) level_cells3(m, p0 + u, xs, cell[u], w[u], fr[u], sc[u]);
+#pragma unroll
+        for (int u = 0; u < kColorGatherU; ++u) {
+            const uint32_t *lp = level_cells_ptr(m, p0 + u, grid);
+#pragma unroll
+            for (int c = 0; c < 8; ++c) raw[u][c] = ld_nc_u32(lp + cell[u][c]);
+        }
+#pragma unroll
+        for (int u = 0; u < kColorGatherU; ++u) {
+            const uint32_t p = p0 + u;
+            const uint32_t packed = feat2_from_raw(raw[u], w[u]);
+            *reinterpret_cast<uint32_t *>(tile + (p >> 2) * (kTile * 16) + r * 16 + (p & 3) * 4) = ((int)m.level[p] <= max_level) ? packed : 0u;
+            jacobian_from_raw(raw[u], fr[u], sc[u], J0[p], J1[p]);
+        }
+    }
+}
+
 // Resident CTAs per SM of the persistent grids of both colour backward kernels.  Their weight-gradient sums stay in registers (mma_m64)
 // and only the tiles the MMAs read live in shared memory (about 101 and 97 KB per CTA), so two CTAs fit an SM and the gather, MMA and
 // scatter phases of one overlap those of the other.  The launcher checks the occupancy calculator agrees (require_ctas_per_sm).
@@ -99,12 +132,9 @@ constexpr int kColorBwdCtasPerSM = 2;
 // Resident CTAs per SM of the geometry-only forward (k_color_fwd<false>): without R1 / R2 and with the X tile cut to its h half it needs
 // about 67 KB of shared memory instead of 91 KB, which would fit three CTAs on an SM.  The launcher asks for the shared-memory carve-out of
 // exactly this many CTAs, because what is not carved out is L1, which the table gathers (ld.global.nc) hit: three CTAs leave about 28 KB of
-// L1, two about 92 KB.  DESIGN.md §6 has the measurement of 2 against 3 (profiles/lidar_geometry_step.py builds the other residency with
-// -DNSB_COLOR_GEO_CTAS_PER_SM).
-#ifndef NSB_COLOR_GEO_CTAS_PER_SM
-#define NSB_COLOR_GEO_CTAS_PER_SM 2
-#endif
-constexpr int kColorGeoCtasPerSM = NSB_COLOR_GEO_CTAS_PER_SM;
+// L1, two about 92 KB.  Three CTAs measured 2x slower (DESIGN.md §6), and with the Jacobian held in registers through the MMAs (about 250
+// registers per thread) the register file holds two.
+constexpr int kColorGeoCtasPerSM = 2;
 
 // ===================================================================================================================== forward
 // kRad = false is the geometry-only form (models without a radiance net, and rays that render no rgb): it stops after nablas, writes the
@@ -168,13 +198,16 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         float xn[3], xs[3];
         int64_t ray;
         load_point(ps, ps.x == nullptr, i, valid, xn, xs, ray);
-        gather_row_to_tile<kTile, kColorGatherU>(m, grid, xs, max_level, sX, tid);          // h -> chunks 0..3 of X
+        float J0[16][3], J1[16][3];
+        gather_row_and_jacobian(m, grid, xs, max_level, sX, tid, J0, J1);                  // h -> chunks 0..3 of X, J -> registers
         tc::fence_async_smem();
         __syncthreads();
         tc::mma_to_rows<64, 0, 0, NF / 16>(acc, kS, 0, tc::kmajor(x_addr, kTile), tc::kmajor(w1_addr, HW), false);   // Z = H . W1^T
         __syncthreads();
         // ---- decoder epilogue: z, a -> sdf ; u = fp16(w2 * s) (first-order cotangent at z)
         float out = 0.f;
+        // the saved tiles (512 B per point, written once and read once by the backward) are stored evict-first (st.global.cs), so that
+        // the stream does not push the L2-resident table out of L2 while this kernel gathers from it
         uint8_t *zt = Zt ? Zt + tile * kTileBytes : nullptr;
 #pragma unroll 1
         for (int c = 0; c < HW / 8; ++c) {
@@ -189,16 +222,16 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
                 uu[j] = sW2[c * 8 + j] * s;
             }
             *reinterpret_cast<uint4 *>(sU + c * kChunk + tid * 16) = tc::pack8_f16(uu);
-            if (zt) *reinterpret_cast<uint4 *>(zt + c * kChunk + tid * 16) = tc::pack8_f16(z);
+            if (zt) __stcs(reinterpret_cast<uint4 *>(zt + c * kChunk + tid * 16), tc::pack8_f16(z));
         }
         const float sdf = r16(out + sb2);
         tc::fence_async_smem();
         __syncthreads();
         tc::mma_to_rows<32, 0, 0, HW / 16>(acc, kS, 0, tc::kmajor(u_addr, kTile), tc::kmajor(w1t_addr, NF), false);   // g = U . W1
         __syncthreads();
-        // ---- second gather pass: nablas01 = J^T g, f ascending (k_lotd_bwd_input order)
+        // ---- nablas01 = J^T g, f ascending (k_lotd_bwd_input order), J from the gather
         float nacc[3] = {0.f, 0.f, 0.f};
-#pragma unroll 1
+#pragma unroll
         for (uint32_t g4 = 0; g4 < 4; ++g4) {
             float gg[8];
             tc::acc_ld8(acc, kS, tid, g4 * 8, gg);
@@ -206,13 +239,11 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
             for (uint32_t q = 0; q < 4; ++q) {
                 const uint32_t p = g4 * 4 + q;
                 if ((int)m.level[p] <= max_level) {
-                    float J0[3], J1[3];
-                    level_jacobian(m, p, xs, grid, J0, J1);
                     const float g0 = r16(gg[2 * q]), g1 = r16(gg[2 * q + 1]);
 #pragma unroll
-                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g0, J0[d], nacc[d]);
+                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g0, J0[p][d], nacc[d]);
 #pragma unroll
-                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g1, J1[d], nacc[d]);
+                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g1, J1[p][d], nacc[d]);
                 }
             }
         }
@@ -246,8 +277,8 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
                     const uint4 q = tc::pack8_f16(v8);
                     *reinterpret_cast<uint4 *>(sX + (4 + c) * kChunk + tid * 16) = q;
                     if (xt) {
-                        *reinterpret_cast<uint4 *>(xt + (4 + c) * kChunk + tid * 16) = q;
-                        *reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16) = *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16);
+                        __stcs(reinterpret_cast<uint4 *>(xt + (4 + c) * kChunk + tid * 16), q);
+                        __stcs(reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16), *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16));
                     }
                 }
             }
@@ -264,7 +295,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
                 for (int j = 0; j < 8; ++j) y[j] = fmaxf(r16(y[j] + srb1[c * 8 + j]), 0.f);
                 const uint4 q = tc::pack8_f16(y);
                 *reinterpret_cast<uint4 *>(sU + c * kChunk + tid * 16) = q;
-                if (y1t) *reinterpret_cast<uint4 *>(y1t + c * kChunk + tid * 16) = q;
+                if (y1t) __stcs(reinterpret_cast<uint4 *>(y1t + c * kChunk + tid * 16), q);
             }
             tc::fence_async_smem();
             __syncthreads();
@@ -281,13 +312,13 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 #pragma unroll
                     for (int k = 0; k < 3; ++k) o3[k] = fmaf(y[j], sR3[k][c * 8 + j], o3[k]);
                 }
-                if (y2t) *reinterpret_cast<uint4 *>(y2t + c * kChunk + tid * 16) = tc::pack8_f16(y);
+                if (y2t) __stcs(reinterpret_cast<uint4 *>(y2t + c * kChunk + tid * 16), tc::pack8_f16(y));
             }
         } else if (Xt) {                                       // the h half of the saved X tile (what k_color_sdf_bwd fetches)
             uint8_t *xt = Xt + tile * kTileBytes;
 #pragma unroll
             for (int c = 0; c < 4; ++c)
-                *reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16) = *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16);
+                __stcs(reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16), *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16));
         }
         if (valid) {
             sdf_out[i] = sdf;

@@ -219,10 +219,8 @@ __device__ __forceinline__ float2 *level_grad_ptr(const PLMeta &m, uint32_t p, f
     return q;
 }
 
-__device__ __forceinline__ uint32_t level_feat2_cells(const uint32_t *__restrict__ lp, const uint32_t (&cell)[8], const float (&w)[8]) {
-    uint32_t raw[8];
-#pragma unroll
-    for (int c = 0; c < 8; ++c) raw[c] = ld_nc_u32(lp + cell[c]);
+// the fp16 feature pair of one level from its 8 corner cells as loaded (two fp16 features per 32-bit word) and their trilinear weights
+__device__ __forceinline__ uint32_t feat2_from_raw(const uint32_t (&raw)[8], const float (&w)[8]) {
     __half2 acc = __floats2half2_rn(0.f, 0.f);
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
@@ -230,6 +228,13 @@ __device__ __forceinline__ uint32_t level_feat2_cells(const uint32_t *__restrict
         acc = __hadd2(acc, __floats2half2_rn(__fmul_rn(w[c], v.x), __fmul_rn(w[c], v.y)));
     }
     return *reinterpret_cast<uint32_t *>(&acc);
+}
+
+__device__ __forceinline__ uint32_t level_feat2_cells(const uint32_t *__restrict__ lp, const uint32_t (&cell)[8], const float (&w)[8]) {
+    uint32_t raw[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) raw[c] = ld_nc_u32(lp + cell[c]);
+    return feat2_from_raw(raw, w);
 }
 
 __device__ __forceinline__ void red_add2(float2 *dst, float a, float b) {

@@ -242,9 +242,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+// The source is read once (the saved activation tiles of the colour query, hundreds of MB per step): its L2 lines are marked evict-first,
+// so that the stream does not push the L2-resident LoTD table and its gradient out of L2.
 __device__ __forceinline__ void tma_load_bulk(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)), "l"(gmem_src),
-                 "r"(bytes), "r"(smem_u32(bar))
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
                  : "memory");
 }
 

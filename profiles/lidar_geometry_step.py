@@ -2,8 +2,8 @@
 
   (a) a geometry-only cfg3 model (radiance_cfg=False, the LiDAR-only StreetSurf configuration) at 8192 rays and at one 64 x 2048 sweep
       (131 072 rays): the host-sized step (SingleVolumeRenderer + loss + backward), the graph step (StaticFrame) and the same model on the
-      module path (forward_sdf_nablas + autograd); with the library as built (2 CTAs per SM for k_color_fwd<false>) and, alternated with it,
-      a library built with -DNSB_COLOR_GEO_CTAS_PER_SM=3 (--alt-lib, built into a temporary directory when not given);
+      module path (forward_sdf_nablas + autograd); with the library as built and, alternated with it, another build of this checkout's
+      library (--alt-lib PATH, geometry-only arms only; DESIGN.md §6's 3-CTA residency was such a build);
   (b) the cfg3 colour model's LiDAR arm (8192 rays, host-sized and graph) against another checkout (--parent ROOT, its library built),
       alternated with this one; the rendered buffers of one fixed batch are compared bit for bit;
   (c) torch.profiler runs (a process per library) with the device time per step of each colour kernel.
@@ -145,19 +145,6 @@ def profile_worker(args):
 
 
 # ------------------------------------------------------------------------------------------------------------ driver
-def _build_alt(dst):
-    sys.path.insert(0, ROOT)
-    from neuralsim_b200 import build as B
-    B.build_library()
-    obj = os.path.join(dst, "color_tc.o")
-    subprocess.run([B.NVCC, *B.FLAGS, "-DNSB_COLOR_GEO_CTAS_PER_SM=3", "-c", os.path.join(B.CSRC, "color_tc.cu"), "-o", obj], check=True,
-                   capture_output=True)
-    objs = [os.path.join(B.OBJ, s.replace(".cu", ".o")) for s in B.SOURCES if s != "color_tc.cu"] + [obj]
-    lib = os.path.join(dst, "libneuralsim_b200.so")
-    subprocess.run([B.NVCC, "-shared", "-o", lib, *objs, *B.ARCH, "-cudart", "static"], check=True, capture_output=True)
-    return lib
-
-
 def _run(cmd):
     p = subprocess.run(cmd, capture_output=True, text=True)
     if p.returncode != 0:
@@ -191,10 +178,11 @@ def main():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"], capture_output=True, text=True)
     print(json.dumps(dict(gpu=q.stdout.strip())), flush=True)
     tmp = tempfile.mkdtemp(prefix="nsb_lidar_geo_")
-    alt = args.alt_lib or _build_alt(tmp)
     me = os.path.abspath(__file__)
     common = ["--steps", str(args.steps), "--warmup", str(args.warmup), "--dump", tmp]
-    configs = [("built", ROOT, None, "geo:host,geo:graph,geo_module:host,colour:host,colour:graph"), ("alt3", ROOT, alt, "geo:host,geo:graph")]
+    configs = [("built", ROOT, None, "geo:host,geo:graph,geo_module:host,colour:host,colour:graph")]
+    if args.alt_lib:
+        configs.append(("alt", ROOT, os.path.abspath(args.alt_lib), "geo:host,geo:graph"))
     if args.parent:
         configs.append(("parent", os.path.abspath(args.parent), None, "colour:host,colour:graph"))
     results = []
