@@ -724,9 +724,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
                     ua[c] = g0 * wsum + h0 * w[c];
                     ub[c] = g1 * wsum + h1 * w[c];
                 }
-                bool issue = valid;
-                if (level_mergeable(m, p)) issue = warp_merge_updates(cell_key3(m, p, xs), valid, ua, ub, lane);   // neighbouring samples, same cell
-                if (issue) {
+                if (warp_merge_updates(cell_key3(m, p, xs), valid, ua, ub, lane)) {   // neighbouring samples, same cell
                     float2 *gp = level_grad_ptr(m, p, d_grid);
 #pragma unroll
                     for (int c = 0; c < 8; ++c) red_add2(gp + cell[c], ua[c], ub[c]);

@@ -222,9 +222,7 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
                 const float g0 = active ? dh[2 * q] : 0.f, g1 = active ? dh[2 * q + 1] : 0.f;
 #pragma unroll
                 for (int c = 0; c < 8; ++c) { a[c] = g0 * w[c]; b[c] = g1 * w[c]; }
-                bool issue = active;
-                if (level_mergeable(m, p)) issue = warp_merge_updates(cell_key3(m, p, xs), active, a, b, lane);   // neighbouring samples, same cell
-                if (issue) {
+                if (warp_merge_updates(cell_key3(m, p, xs), active, a, b, lane)) {   // neighbouring samples, same cell
                     float2 *gp = level_grad_ptr(m, p, d_grid);
 #pragma unroll
                     for (int c = 0; c < 8; ++c) red_add2(gp + cell[c], a[c], b[c]);

@@ -160,6 +160,7 @@ __device__ __forceinline__ void stage_decoder_vectors(const DecoderDevTC &dec, B
 inline int make_decoder(const nsb_lotd_meta *meta, const nsb_sdf_decoder *dec, PLMeta *m, DecoderDevTC *d, const char *who) {
     if (make_plmeta(meta, m)) return 2;
     NSB_REQUIRE(m->n_pseudo == 16 && m->F == 2 && m->D == 3 && plmeta_two_feature_cells(*m), "%s: built for 16 x 2 LoTD features in 3-D", who);
+    NSB_REQUIRE(plmeta_cell_key_fits(*m), "%s: a level resolution exceeds %u cells per axis (the backward's merge key)", who, 1u << kCellKeyBits);
     NSB_REQUIRE(dec->width >= 1 && dec->width <= 64, "%s: decoder width must be <= 64", who);
     *d = DecoderDevTC{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2, dec->width, dec->beta};
     return 0;

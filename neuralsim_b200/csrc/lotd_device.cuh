@@ -243,27 +243,33 @@ __device__ __forceinline__ void red_add2(float2 *dst, float a, float b) {
 
 // ---- warp-merged table-gradient updates.  The fp32 atomics themselves bound the table
 // backward (the same rate whether the points are ordered or shuffled, at any occupancy), so the lever is FEWER atomics.
-// The lanes of a warp are consecutive samples of a ray; on the coarse / middle levels neighbouring samples fall into the same cell
-// and update the same 8 corners.  Runs of lanes with equal integer cell coordinates are summed with shuffles (segmented reduction
-// over contiguous runs; the run structure is one ballot) and only the run's first lane issues the 8 reductions.
+// The lanes of a warp are consecutive samples of a ray; neighbouring samples fall into the same cell on the coarse and middle levels,
+// and on the finest levels too where the up-sampled samples crowd around the surface.  Runs of lanes with equal integer cell
+// coordinates are summed with shuffles (segmented reduction over contiguous runs; the run structure is one ballot) and only the run's
+// first lane issues the 8 reductions.
 // `key` must identify the cell exactly (not its hash); lanes that carry no gradient pass active = false.
-__device__ __forceinline__ uint32_t cell_key3(const PLMeta &m, uint32_t p, const float (&xs)[3]) {      // res <= 1024 per axis
-    uint32_t k = 0;
+constexpr uint32_t kCellKeyBits = 21;                  // per axis: the three cell coordinates of any level with res <= 2^21 per axis
+__device__ __forceinline__ uint64_t cell_key3(const PLMeta &m, uint32_t p, const float (&xs)[3]) {
+    uint64_t k = 0;
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
         const float v = __fmaf_rn(xs[d], (float)(m.res[p][d] - 2u), 0.5f);
-        k |= (__float_as_uint(__fadd_rd(v, 8388608.f)) - 0x4B000000u) << (10 * d);
+        k |= (uint64_t)(__float_as_uint(__fadd_rd(v, 8388608.f)) - 0x4B000000u) << (kCellKeyBits * d);
     }
     return k;
 }
-__device__ __forceinline__ bool level_mergeable(const PLMeta &m, uint32_t p) {
-    return m.res[p][0] <= 1024u && m.res[p][1] <= 1024u && m.res[p][2] <= 1024u;
+// host: every axis of every pseudo level fits the key (a cell coordinate is < res)
+inline bool plmeta_cell_key_fits(const PLMeta &m) {
+    for (uint32_t p = 0; p < m.n_pseudo; ++p)
+        for (uint32_t d = 0; d < m.D; ++d)
+            if (m.res[p][d] > (1u << kCellKeyBits)) return false;
+    return true;
 }
 
 // a[c], b[c]: this lane's updates of corner c (feature 0 / 1).  On return the lanes for which the result is true hold the sums of
 // their run and must issue them; the others are done.  Every lane of the warp must call (shuffles).
-__device__ __forceinline__ bool warp_merge_updates(uint32_t key, bool active, float (&a)[8], float (&b)[8], int lane) {
-    const uint32_t prev = __shfl_up_sync(0xffffffffu, key, 1);
+__device__ __forceinline__ bool warp_merge_updates(uint64_t key, bool active, float (&a)[8], float (&b)[8], int lane) {
+    const uint64_t prev = __shfl_up_sync(0xffffffffu, key, 1);
     const uint32_t act = __ballot_sync(0xffffffffu, active);
     const bool prev_act = lane > 0 && ((act >> (lane - 1)) & 1u);
     const bool head = !active || !prev_act || key != prev;       // inactive lanes are runs of their own

@@ -25,14 +25,56 @@ def color_net_c(t16, dec, rad, fac):
     return L.ColorNetC(*ptrs, dec[0].out_features, rw, ri, na, float(dec[0].activation.beta), (ctypes.c_float * 3)(*fac))
 
 
+class SharedTableGrad:
+    """One zero-filled fp32 table gradient that several backward nodes of a step scatter into, instead of a buffer each that autograd
+    then adds up.  The nodes take the table through `route(table)`, an identity node created before them: each node's backward adds its
+    part into `take()` and returns None for the table, and the identity node -- which autograd runs only after every node that consumes
+    its output -- hands the finished buffer on and empties the holder.  So autograd sees the buffer only once all parts are in it,
+    whatever else contributes to the table's gradient, and the next backward pass (a retained graph) starts from a fresh zeroed buffer."""
+    __slots__ = ("buf",)
+
+    def __init__(self):
+        self.buf = None
+
+    def route(self, table):
+        """-> the table as the input of the nodes that scatter into this holder"""
+        return _TableGradSink.apply(self, table)
+
+    def take(self, shape, device):
+        """(inside a backward) -> the buffer, zero-filled by the first caller of this backward pass"""
+        if self.buf is None:
+            self.buf = torch.zeros(shape, dtype=torch.float32, device=device)
+        return self.buf
+
+
+class _TableGradSink(autograd.Function):
+    """identity on the table; its backward passes the holder's buffer on (see SharedTableGrad)"""
+
+    @staticmethod
+    def forward(ctx, holder, table):
+        ctx.holder = holder
+        ctx.set_materialize_grads(False)
+        return table.view_as(table)
+
+    @staticmethod
+    @autograd.function.once_differentiable
+    def backward(ctx, g):
+        buf, ctx.holder.buf = ctx.holder.buf, None
+        if g is not None:                          # a consumer that returned its own table gradient
+            buf = g if buf is None else buf.add_(g)
+        return None, buf
+
+
 class ColorQuery:
     """what the forward and backward launches of one colour query share: the table's meta and fp16 image, the net struct and the fp16
-    tensors it points at, the rays, max level, the occupancy collection and the device count (_lib.call's count=, None: host-sized)"""
-    __slots__ = ("meta", "grid16", "net", "held", "rays_o", "rays_d", "ml", "collect", "count")
+    tensors it points at, the rays, max level, the occupancy collection, the device count (_lib.call's count=, None: host-sized) and
+    the step's shared table gradient (a SharedTableGrad, None: the backward fills its own)"""
+    __slots__ = ("meta", "grid16", "net", "held", "rays_o", "rays_d", "ml", "collect", "count", "table_grad")
 
-    def __init__(self, meta, grid16, net, held, rays_o, rays_d, ml, collect, count):
+    def __init__(self, meta, grid16, net, held, rays_o, rays_d, ml, collect, count, table_grad=None):
         self.meta, self.grid16, self.net, self.held = meta, grid16, net, held
         self.rays_o, self.rays_d, self.ml, self.collect, self.count = rays_o, rays_d, ml, collect, count
+        self.table_grad = table_grad
 
 
 class _FusedColor(autograd.Function):
@@ -72,15 +114,20 @@ class _FusedColor(autograd.Function):
             raise RuntimeError("fused_color: backward through a forward that ran without grad")
         q, dev, n = ctx.q, acts.device, ctx.n
         g_sdf, g_nab, g_rgb = g_out[0], g_out[1], (g_out[2] if ctx.rad else None)
-        # one zero-fill for the table gradient, one for the small tensors (views of a flat buffer)
+        # one zero-fill for the table gradient (or the step's shared one), one for the small tensors (views of a flat buffer)
         sizes = [int(torch.Size(s).numel()) for s in ctx.shapes[1:]]
         small = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
-        grads, o = [torch.zeros(ctx.shapes[0], dtype=torch.float32, device=dev)], 0
+        if q.table_grad is None:
+            d_grid = torch.zeros(ctx.shapes[0], dtype=torch.float32, device=dev)
+        else:
+            d_grid = q.table_grad.take(ctx.shapes[0], dev)            # handed on by the table's SharedTableGrad.route node
+        grads, o = [d_grid], 0
         for sh, k in zip(ctx.shapes[1:], sizes):
             grads.append(small[o:o + k].view(sh))
             o += k
+        ret = (None,) * 6 + ((d_grid if q.table_grad is None else None),) + tuple(grads[1:])
         if g_sdf is None and g_nab is None and g_rgb is None:
-            return (None,) * 6 + tuple(grads)
+            return ret
         c = lambda g: None if g is None else g.contiguous().float()
         g_sdf, g_nab, g_rgb = c(g_sdf), c(g_nab), c(g_rgb)
         dh = torch.empty(n, 32, dtype=torch.float32, device=dev) if g_rgb is not None else None
@@ -91,7 +138,7 @@ class _FusedColor(autograd.Function):
                    P(q.rays_d, "f32"), P(ctx.ridx, "i64"), P(ctx.t, "f32"), L.c_i64(n), L.c_i32(q.ml), P(acts[0]), P(acts[1]),
                    *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]), P(rgb, allow_none=True), P(g_sdf, allow_none=True),
                    P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh, allow_none=True), *ag, L.stream_ptr(), count=q.count)
-        return (None,) * 6 + tuple(grads)
+        return ret
 
 
 def fused_color(model, ridx, t, rays_o, rays_d, view_dirs=None, h_appear=None, *, nablas_has_grad=True, collect=None, with_rgb=True):

@@ -20,7 +20,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import _lib as L
-from ..fields.fused_color import ColorQuery, _FusedColor, color_net_c
+from ..fields.fused_color import ColorQuery, SharedTableGrad, _FusedColor, color_net_c
 from ..fields.networks import sdf_bwd, sdf_decoder_c, sdf_fwd
 from .raysample import batch_sample_step_linear
 from .pack_ops import get_pack_infos_from_batch
@@ -107,7 +107,7 @@ class _StaticBoundary(torch.autograd.Function):
         st, (d1, sdf, inv_c, pinfo, nidx, pinfo_kept, pidx) = ctx.st, ctx.saved
         dev, R, S, K = sdf.device, pinfo.shape[0], sdf.numel(), pidx.numel()
         inv_shape, gs, w1s, b1s, w2s, b2s = ctx.shapes
-        d_grid = torch.zeros(gs, dtype=torch.float32, device=dev)
+        d_grid = st.table_grad.take(gs, dev)           # shared with the colour query's backward, handed on by SharedTableGrad.route
         ks = [int(torch.Size(x).numel()) for x in (w1s, b1s, w2s, b2s)]
         small = torch.zeros(1 + sum(ks), dtype=torch.float32, device=dev)
         d_inv, o = small[:1], 1
@@ -132,12 +132,12 @@ class _StaticBoundary(torch.autograd.Function):
             with L.KERNEL_TIMER.time("fused_sdf_bwd", n_list):
                 sdf_bwd(st.meta, st.grid16, st.dec, d_sdf, n_list, st.ml, (d_grid, d_W1, d_b1, d_W2, d_b2), rays=(st.rays_o, st.rays_d, ray, d1), keep=keep,
                         count=(cnt, CNT_SLOTS["nonzero"]))
-        return (None,) * 8 + (d_inv.reshape(inv_shape), d_grid, d_W1, d_b1, d_W2, d_b2)
+        return (None,) * 8 + (d_inv.reshape(inv_shape), None, d_W1, d_b1, d_W2, d_b2)
 
 
 class _State:
     """what the kernels of one static step share"""
-    __slots__ = ("meta", "grid16", "dec", "net", "held", "rays_o", "rays_d", "ml", "collect", "cnt", "ws")
+    __slots__ = ("meta", "grid16", "dec", "net", "held", "rays_o", "rays_d", "ml", "collect", "cnt", "ws", "table_grad")
 
 
 def _fp16_images(model, radiance=True):
@@ -205,6 +205,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     st.cnt = cnt
     wsb = (NF._scan_ws_bytes() + 255) // 256 * 256
     st.ws = torch.zeros(4, wsb, dtype=torch.uint8, device=dev)          # the zeroed workspaces of the step's four scans, one fill
+    st.table_grad = SharedTableGrad()          # the boundary and colour backward nodes scatter into one table gradient
     with torch.no_grad():
         t16, st.dec, st.net, masters = _fp16_images(model, radiance=with_rgb)
         st.held, st.grid16 = t16, t16[0]
@@ -298,20 +299,21 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     s = model.implicit_surface
     dl = s.decoder.layers
     inv_s = model.forward_inv_s()
+    table = st.table_grad.route(s.encoding.flattened_params)            # the table as both backward nodes' input
     if not isinstance(inv_s, torch.Tensor):
         inv_s = torch.tensor(float(inv_s), device=dev)
     alpha_k, t_k, ridx_k, pinfo_kept, rays_inds_hit = _StaticBoundary.apply(
         st, d1, pinfo, ridx_all, order_b, rays_inds, kept_cap,
-        (nc1, num_fine, march_cap, kept_cap), inv_s, s.encoding.flattened_params, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
+        (nc1, num_fine, march_cap, kept_cap), inv_s, table, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
     # ---------------- colour / normal query on the kept samples (none when neither is rendered: depth and mask need alpha alone)
     rgb = nab = x = None
     if with_rgb or with_normal:
-        params = (s.encoding.flattened_params, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
+        params = (table, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
         if with_rgb:
             b = model.radiance_net.blocks.layers
             params += (b[0].weight, b[0].bias, b[1].weight, b[1].bias, b[2].weight, b[2].bias)
         keep_acts = torch.is_grad_enabled() and any(p.requires_grad for p in params)
-        q = ColorQuery(st.meta, st.grid16, st.net, st.held, st.rays_o, st.rays_d, st.ml, st.collect, (cnt, CNT_SLOTS["kept"]))
+        q = ColorQuery(st.meta, st.grid16, st.net, st.held, st.rays_o, st.rays_d, st.ml, st.collect, (cnt, CNT_SLOTS["kept"]), st.table_grad)
         out = _FusedColor.apply(q, ridx_k, t_k, view_dirs, ha_c, keep_acts, *params)
         nab, x = out[1], out[-1]
         rgb = out[2] if with_rgb else None
