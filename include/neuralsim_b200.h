@@ -90,6 +90,33 @@ int nsb_lotd_bwd_bwd_input(const nsb_lotd_meta *meta_host, const float *dL_ddLdx
                            int dL_dy_is_half, const float *input, const float *dy_dx, int64_t n,
                            int32_t max_level, float scale, float *dL_ddLdy, float *dL_dparam, void *stream);
 
+/* Batched tables (lotd_hash_only.h:44-55, lotd_torch_api.cu:263-290): `params` holds several tables of n_params elements.
+ * Point i reads the table of batch b = inds[i] if inds is set (a negative inds[i] skips the point: zero y / dy_dx / dL_dx /
+ * dL_ddLdy rows, no table gradient), else b = i / data_size if data_size is non-zero, else b = 0.  The table starts at element
+ * offsets[b] if offsets is set, else at b * n_params; the start is formed in 64 bits.  Batches may share a table: their
+ * gradients add up.  Offsets must be even (feature pairs are read and reduced as one access); index and offset values are not
+ * range-checked here (bindings/_lotd.py checks them).  A NULL batch, or one with all three fields empty, is the unbatched
+ * call; a non-zero data_size must divide n. */
+typedef struct nsb_lotd_batch {
+    const int64_t *inds;        /* [N] int64, or NULL */
+    const int64_t *offsets;     /* [B] int64 element offsets, or NULL */
+    uint32_t data_size;         /* points per batch (consecutive), or 0 */
+} nsb_lotd_batch;
+
+/* The four entries above with a batch argument (batch_host: host pointer, may be NULL); the entries above are these with
+ * batch_host = NULL.  For nsb_lotd_bwd_input_batched only `inds` matters (it has no table). */
+int nsb_lotd_fwd_batched(const nsb_lotd_meta *meta_host, const float *input, const void *params, int params_is_half,
+                         int64_t n, int32_t max_level, const nsb_lotd_batch *batch_host, void *y, float *dy_dx, void *stream);
+int nsb_lotd_bwd_grid_batched(const nsb_lotd_meta *meta_host, const void *dL_dy, int dL_dy_is_half, const float *input,
+                              int64_t n, int32_t max_level, const nsb_lotd_batch *batch_host, float scale, float *dL_dparam,
+                              void *stream);
+int nsb_lotd_bwd_input_batched(const void *dL_dy, int dL_dy_is_half, const float *dy_dx, int64_t n, int32_t n_feat,
+                               int32_t n_dims, const nsb_lotd_batch *batch_host, float scale, float *dL_dx, void *stream);
+int nsb_lotd_bwd_bwd_input_batched(const nsb_lotd_meta *meta_host, const float *dL_ddLdx, const void *dL_dy,
+                                   int dL_dy_is_half, const float *input, const float *dy_dx, int64_t n, int32_t max_level,
+                                   const nsb_lotd_batch *batch_host, float scale, float *dL_ddLdy, float *dL_dparam,
+                                   void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * _occ_grid  (csrc/occ_grid/src/occ_grid.cpp:21-33, include/occ_grid/cpp_api.h:14-65)
  * ray_marching / batched_ray_marching, AABB contraction.  Two calls, as the reference's two kernel

@@ -28,6 +28,10 @@ class LotdMetaC(ctypes.Structure):
     ]
 
 
+class LotdBatchC(ctypes.Structure):
+    _fields_ = [("inds", ctypes.c_void_p), ("offsets", ctypes.c_void_p), ("data_size", ctypes.c_uint32)]
+
+
 class SdfDecoderC(ctypes.Structure):
     _fields_ = [("W1", ctypes.c_void_p), ("b1", ctypes.c_void_p), ("W2", ctypes.c_void_p), ("b2", ctypes.c_void_p),
                 ("width", ctypes.c_int32), ("beta", ctypes.c_float)]

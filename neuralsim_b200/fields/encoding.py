@@ -2,10 +2,12 @@
 (reference: nr3d_lib/nr3d_lib/models/grid_encodings/lotd/lotd.py:40-458, lotd_encoding.py, lotd_cfg.py:48-57).
 
 Three autograd functions carry first and second order gradients exactly like the reference's
-LoTDFunction / LoTDFunctionFwdDydx / LoTDFunctionBwdDydx; the kernels behind them are csrc/lotd.cu.
+LoTDFunction / LoTDFunctionFwdDydx / LoTDFunctionBwdDydx, batched tables included (a per-point batch index `bidx`,
+per-batch `batch_offsets`, or `input_batched` equal-size batches); the kernels behind them are csrc/lotd.cu.
 """
 from __future__ import annotations
 
+from math import prod
 from typing import Optional
 
 import numpy as np
@@ -53,49 +55,57 @@ def generate_meta(n_input_dim, lod_res, lod_n_feats, lod_types, hashmap_size=Non
     return _backend.LoDMeta(n_input_dim, lod_res, lod_n_feats, lod_types, hashmap_size, use_smooth_step)
 
 
+def _flat_bidx(bidx):
+    return None if bidx is None else bidx.contiguous().long().flatten()
+
+
 class LoTDFunction(torch.autograd.Function):
-    """y = encode(clamp(x)); backward gives dL_dgrid (and dL_dx when x needs it).  First order only."""
+    """y = encode(clamp(x)); backward gives dL_dgrid (and dL_dx when x needs it).  First order only.
+    bidx / batch_offsets / batch_data_size select each point's table when `grid` holds several (lotd.py:48-119)."""
 
     @staticmethod
-    def forward(ctx, meta, x, grid, loss_scale=1.0, max_level=None):
+    def forward(ctx, meta, x, grid, bidx=None, batch_offsets=None, batch_data_size=None, loss_scale=1.0, max_level=None):
         ctx.set_materialize_grads(False)
         prefix = x.shape[:-1]
         x = x.clamp(1.0e-6, 1 - 1.0e-6)
+        bidx = _flat_bidx(bidx)
         need_x = ctx.needs_input_grad[1]
-        y, dy_dx = _backend.lod_fwd(meta, x.flatten(0, -2).contiguous(), grid, None, None, None, max_level, need_x)
+        y, dy_dx = _backend.lod_fwd(meta, x.flatten(0, -2).contiguous(), grid, bidx, batch_offsets, batch_data_size, max_level, need_x)
         if need_x or ctx.needs_input_grad[2]:
-            ctx.save_for_backward(x, grid, dy_dx)
-            ctx.meta, ctx.prefix, ctx.loss_scale, ctx.max_level = meta, prefix, loss_scale, max_level
+            ctx.save_for_backward(x, grid, dy_dx, bidx, batch_offsets)
+            ctx.meta, ctx.prefix, ctx.loss_scale, ctx.max_level, ctx.batch_data_size = meta, prefix, loss_scale, max_level, batch_data_size
         return y.unflatten(0, prefix)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dL_dy):
         if dL_dy is None:
-            return None, None, None, None, None
-        x, grid, dy_dx = ctx.saved_tensors
+            return (None,) * 8
+        x, grid, dy_dx, bidx, batch_offsets = ctx.saved_tensors
         s = ctx.loss_scale
-        dL_dx, dL_dgrid = _backend.lod_bwd(ctx.meta, (dL_dy.flatten(0, -2) * s).contiguous(), x.flatten(0, -2), grid, dy_dx, None, None,
-                                           None, ctx.max_level, ctx.needs_input_grad[1], ctx.needs_input_grad[2])
+        dL_dx, dL_dgrid = _backend.lod_bwd(ctx.meta, (dL_dy.flatten(0, -2) * s).contiguous(), x.flatten(0, -2), grid, dy_dx, bidx, batch_offsets,
+                                           ctx.batch_data_size, ctx.max_level, ctx.needs_input_grad[1], ctx.needs_input_grad[2])
         dL_dx = None if dL_dx is None else dL_dx.unflatten(0, ctx.prefix) / s
         dL_dgrid = None if dL_dgrid is None else dL_dgrid / s
-        return None, dL_dx, dL_dgrid, None, None
+        return None, dL_dx, dL_dgrid, None, None, None, None, None
 
 
 class LoTDFunctionFwdDydx(torch.autograd.Function):
     """(y, dy_dx) = encode_with_jacobian(clamp(x)).  Use LoTDFunctionBwdDydx for nablas; this backward only
-    routes dL_dy to the table (and to x when `need_dL_dinput`)."""
+    routes dL_dy to the table (and to x when `need_dL_dinput`).  (lotd.py:121-191)"""
 
     @staticmethod
-    def forward(ctx, meta, x, grid, loss_scale=1.0, max_level=None, need_dL_dinput=None):
+    def forward(ctx, meta, x, grid, bidx=None, batch_offsets=None, batch_data_size=None, loss_scale=1.0, max_level=None, need_dL_dinput=None):
         if need_dL_dinput is None:
             need_dL_dinput = torch.is_grad_enabled() and x.requires_grad
         ctx.set_materialize_grads(False)
         prefix = x.shape[:-1]
         x = x.clamp(1.0e-6, 1 - 1.0e-6)
-        y, dy_dx = _backend.lod_fwd(meta, x.flatten(0, -2).contiguous(), grid, None, None, None, max_level, True)
-        ctx.save_for_backward(x, grid, dy_dx)
+        bidx = _flat_bidx(bidx)
+        y, dy_dx = _backend.lod_fwd(meta, x.flatten(0, -2).contiguous(), grid, bidx, batch_offsets, batch_data_size, max_level, True)
+        ctx.save_for_backward(x, grid, dy_dx, bidx, batch_offsets)
         ctx.meta, ctx.prefix, ctx.loss_scale, ctx.max_level, ctx.need_dL_dinput = meta, prefix, loss_scale, max_level, need_dL_dinput
+        ctx.batch_data_size = batch_data_size
         ctx.mark_non_differentiable(dy_dx)
         return y.unflatten(0, prefix), dy_dx
 
@@ -103,46 +113,90 @@ class LoTDFunctionFwdDydx(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, dL_dy, _):
         if dL_dy is None:
-            return None, None, None, None, None, None
-        x, grid, dy_dx = ctx.saved_tensors
+            return (None,) * 9
+        x, grid, dy_dx, bidx, batch_offsets = ctx.saved_tensors
         s = ctx.loss_scale
-        dL_dx, dL_dgrid = _backend.lod_bwd(ctx.meta, (dL_dy.flatten(0, -2) * s).contiguous(), x.flatten(0, -2), grid, dy_dx, None, None,
-                                           None, ctx.max_level, ctx.need_dL_dinput, ctx.needs_input_grad[2])
+        dL_dx, dL_dgrid = _backend.lod_bwd(ctx.meta, (dL_dy.flatten(0, -2) * s).contiguous(), x.flatten(0, -2), grid, dy_dx, bidx, batch_offsets,
+                                           ctx.batch_data_size, ctx.max_level, ctx.need_dL_dinput, ctx.needs_input_grad[2])
         dL_dx = None if dL_dx is None else dL_dx.unflatten(0, ctx.prefix) / s
         dL_dgrid = None if dL_dgrid is None else dL_dgrid / s
-        return None, dL_dx, dL_dgrid, None, None, None
+        return None, dL_dx, dL_dgrid, None, None, None, None, None, None
 
 
 class LoTDFunctionBwdDydx(torch.autograd.Function):
-    """dL_dx = J(x)^T dL_dy as a differentiable op: its backward is the second-order pass towards dL_dy and the table."""
+    """dL_dx = J(x)^T dL_dy as a differentiable op: its backward is the second-order pass towards dL_dy and the table.
+    (lotd.py:193-268)"""
 
     @staticmethod
-    def forward(ctx, meta, dL_dy, x, grid, dy_dx, loss_scale, max_level, grad_guard=None):
+    def forward(ctx, meta, dL_dy, x, grid, dy_dx, bidx=None, batch_offsets=None, batch_data_size=None, loss_scale=1.0, max_level=None,
+                grad_guard=None):
         ctx.set_materialize_grads(False)
         prefix = x.shape[:-1]
         x = x.clamp(1.0e-6, 1 - 1.0e-6)
+        bidx = _flat_bidx(bidx)
         dL_dx, _ = _backend.lod_bwd(meta, (dL_dy.flatten(0, -2) * loss_scale).contiguous(), x.flatten(0, -2).contiguous(), grid, dy_dx,
-                                    None, None, None, max_level, True, False)
+                                    bidx, batch_offsets, batch_data_size, max_level, True, False)
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[3]:
-            ctx.save_for_backward(dL_dy, x, grid, dy_dx.contiguous())
+            ctx.save_for_backward(dL_dy, x, grid, dy_dx.contiguous(), bidx, batch_offsets)
             ctx.meta, ctx.loss_scale, ctx.max_level, ctx.grad_guard = meta, loss_scale, max_level, grad_guard
+            ctx.batch_data_size = batch_data_size
         return dL_dx.unflatten(0, prefix) / loss_scale
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dL_ddLdx):
         if dL_ddLdx is None:
-            return (None,) * 8
-        dL_dy, x, grid, dy_dx = ctx.saved_tensors
+            return (None,) * 11
+        dL_dy, x, grid, dy_dx, bidx, batch_offsets = ctx.saved_tensors
         prefix, s = x.shape[:-1], ctx.loss_scale
         ddLdy, dgrid, _ = _backend.lod_bwd_bwd_input(
             ctx.meta, dL_ddLdx.flatten(0, -2).contiguous(), (dL_dy.flatten(0, -2) * s).contiguous(), x.flatten(0, -2), grid, dy_dx,
-            None, None, None, ctx.max_level, ctx.needs_input_grad[1], ctx.needs_input_grad[3], False)
+            bidx, batch_offsets, ctx.batch_data_size, ctx.max_level, ctx.needs_input_grad[1], ctx.needs_input_grad[3], False)
         ddLdy = None if ddLdy is None else ddLdy.unflatten(0, prefix)
         dgrid = None if dgrid is None else dgrid / s
         if ctx.grad_guard is not None and (dgrid is not None or ddLdy is not None):
             ctx.grad_guard.custom_grad_clip_step(dL_ddLdx, dy_dx, dgrid, ddLdy)
-        return None, ddLdy, None, dgrid, None, None, None, None
+        return None, ddLdy, None, dgrid, None, None, None, None, None, None, None
+
+
+def _batch_data_size(input, input_batched):
+    """input_batched: `input` is [B, ..., D] and its points of batch b read table b (lotd.py:275-279)"""
+    return prod(input.shape[1:-1]) if input_batched else 0
+
+
+def lotd_encoding(input, params, bidx=None, batch_offsets=None, input_batched=False, max_level=None,
+                  meta=None, n_input_dim=None, lod_res=None, lod_n_feats=None, lod_types=None):
+    """lotd.py:270-282"""
+    if meta is None:
+        meta = generate_meta(n_input_dim, lod_res, lod_n_feats, lod_types)
+    if input_batched:
+        bidx = None
+    loss_scale = 128.0 if params.dtype == torch.float16 else 1.0
+    return LoTDFunction.apply(meta, input, params, bidx, batch_offsets, _batch_data_size(input, input_batched), loss_scale, max_level)
+
+
+def lotd_encoding_fwd_dydx(input, params, bidx=None, batch_offsets=None, input_batched=False, max_level=None, need_dL_dinput: Optional[bool] = None,
+                           meta=None, n_input_dim=None, lod_res=None, lod_n_feats=None, lod_types=None):
+    """lotd.py:284-298 -> (y, dy_dx, meta)"""
+    if need_dL_dinput is None:
+        need_dL_dinput = torch.is_grad_enabled() and input.requires_grad
+    if meta is None:
+        meta = generate_meta(n_input_dim, lod_res, lod_n_feats, lod_types)
+    if input_batched:
+        bidx = None
+    loss_scale = 128.0 if params.dtype == torch.float16 else 1.0
+    y, dy_dx = LoTDFunctionFwdDydx.apply(meta, input, params, bidx, batch_offsets, _batch_data_size(input, input_batched), loss_scale, max_level,
+                                         need_dL_dinput)
+    return y, dy_dx, meta
+
+
+def lotd_encoding_bwd_dydx(meta, dL_dy, dy_dx, input, params, bidx=None, batch_offsets=None, input_batched=False, max_level=None):
+    """lotd.py:300-309"""
+    if input_batched:
+        bidx = None
+    loss_scale = 128.0 if params.dtype == torch.float16 else 1.0
+    return LoTDFunctionBwdDydx.apply(meta, dL_dy, input, params, dy_dx, bidx, batch_offsets, _batch_data_size(input, input_batched), loss_scale,
+                                     max_level)
 
 
 class LoTD(nn.Module):
@@ -169,14 +223,28 @@ class LoTD(nn.Module):
     level_sizes = property(lambda self: self.meta.level_sizes)
     level_n_params = property(lambda self: self.meta.level_n_params)
 
-    def forward(self, input, params, max_level: int = None):
-        return LoTDFunction.apply(self.meta, input, params.to(self.dtype), self.loss_scale, max_level)
+    # bidx / batch_offsets / input_batched: `params` holds several tables (lotd.py:425-458); keyword-only here, after max_level
+    def forward(self, input, params, max_level: int = None, *, bidx=None, batch_offsets=None, input_batched=False):
+        bds = self._batch_data_size(input, bidx, input_batched)
+        return LoTDFunction.apply(self.meta, input, params.to(self.dtype), bidx, batch_offsets, bds, self.loss_scale, max_level)
 
-    def forward_dydx(self, input, params, max_level: int = None, need_dL_dinput: Optional[bool] = None):
-        return LoTDFunctionFwdDydx.apply(self.meta, input, params.to(self.dtype), self.loss_scale, max_level, need_dL_dinput)
+    def forward_dydx(self, input, params, max_level: int = None, need_dL_dinput: Optional[bool] = None, *, bidx=None, batch_offsets=None,
+                     input_batched=False):
+        bds = self._batch_data_size(input, bidx, input_batched)
+        return LoTDFunctionFwdDydx.apply(self.meta, input, params.to(self.dtype), bidx, batch_offsets, bds, self.loss_scale, max_level,
+                                         need_dL_dinput)
 
-    def backward_dydx(self, dL_dy, dy_dx, input, params, max_level: int = None, grad_guard=None):
-        return LoTDFunctionBwdDydx.apply(self.meta, dL_dy, input, params.to(self.dtype), dy_dx, self.loss_scale, max_level, grad_guard)
+    def backward_dydx(self, dL_dy, dy_dx, input, params, max_level: int = None, grad_guard=None, *, bidx=None, batch_offsets=None,
+                      input_batched=False):
+        bds = self._batch_data_size(input, bidx, input_batched)
+        return LoTDFunctionBwdDydx.apply(self.meta, dL_dy, input, params.to(self.dtype), dy_dx, bidx, batch_offsets, bds, self.loss_scale,
+                                         max_level, grad_guard)
+
+    @staticmethod
+    def _batch_data_size(input, bidx, input_batched):
+        if input_batched:
+            assert bidx is None, 'bidx is only taken care of when input is not batched.'
+        return _batch_data_size(input, input_batched)
 
 
 class LoTDEncoding(nn.Module):
