@@ -206,8 +206,8 @@ int nsb_sh_encode_backward(const float *grad, const float *dy_dx, int64_t n, int
  * They replace chains of the calls above + the autocast MLPs of nr3d_lib/models/blocks/mlp.py with one
  * kernel each; numerics follow the same fp16 rounding points (see DESIGN.md "Numerics contract").
  * ---------------------------------------------------------------------------------------------- */
-typedef struct nsb_sdf_decoder {       /* LoTDSDF decoder 32->W->1, Softplus(beta)  (lotd_sdf.py:176-200) */
-    const void *W1;                    /* fp16 [W, F]   (fp32 master rounded by the caller) */
+typedef struct nsb_sdf_decoder {       /* LoTDSDF decoder F->W->1, Softplus(beta)  (lotd_sdf.py:176-200), F = n_encoded_dims */
+    const void *W1;                    /* fp16 [W, F]   (fp32 master rounded by the caller; row stride F) */
     const void *b1;                    /* fp16 [W] */
     const void *W2;                    /* fp16 [W] */
     const void *b2;                    /* fp16 [1] */
@@ -225,6 +225,9 @@ typedef struct nsb_occ_collect {
     float inv_s;
 } nsb_occ_collect;
 
+/* The tensor-core SDF, colour and up-sampling entry points below take 3-D LoTD tables of L = 1..16 pseudo levels with
+ * n_feat_per_pseudo_lvl == 2 and n_encoded_dims == 2L; the decoder's W1 is then [W x 2L].  Tables of more than 16 levels are refused
+ * (the error names the limit) and run on the unfused LoTD entry points.  h_out of nsb_fused_sdf needs 16 levels. */
 /* forward_sdf on N points: x in network space [-1,1]^3 (not yet /2+0.5).  sdf fp32 (fp16-valued). */
 int nsb_fused_sdf(const nsb_lotd_meta *meta_host, const void *params_half, const nsb_sdf_decoder *dec_host,
                   const float *x, int64_t n, int32_t max_level, float *sdf, void *h_out_half, void *stream);
@@ -410,9 +413,9 @@ int nsb_occ_ema_update(const float *pts, const float *val, int64_t n, int32_t va
  * its backward including the second-order pass through nablas (LoTDFunctionBwdDydx.backward, lotd.py:193-268) as two.
  * All weight pointers are fp16 device images of the fp32 masters (what autocast feeds the GEMMs). */
 typedef struct nsb_color_net {
-    const void *W1, *b1, *W2, *b2;            /* sdf decoder: [width x 32], [width], [1 x width], [1]              */
+    const void *W1, *b1, *W2, *b2;            /* sdf decoder: [width x 2L], [width], [1 x width], [1] (L levels, 1..16) */
     const void *R1, *rb1, *R2, *rb2, *R3, *rb3; /* radiance net: [rw x rad_in], [rw], [rw x rw], [rw], [3 x rw], [3] */
-    int32_t width, rad_width, rad_in, n_appear; /* rad_in = 3 + 16 + 3 + 32 + n_appear ([x, SH4(v), n, h, h_appear]) */
+    int32_t width, rad_width, rad_in, n_appear; /* rad_in = 3 + 16 + 3 + 2L + n_appear ([x, SH4(v), n, h, h_appear]) */
     float beta;                               /* Softplus beta of the decoder                                      */
     float nablas_scale[3];                    /* sdf_scale / radius3d_original                                     */
 } nsb_color_net;

@@ -25,7 +25,7 @@
 namespace nsb {
 
 struct ColorNetDev {
-    DecoderDevTC dec;                                   // sdf decoder: [width x 32], [width], [width], [1]
+    DecoderDevTC dec;                                   // sdf decoder: [width x 2L], [width], [width], [1]
     const __half *R1, *rb1, *R2, *rb2, *R3, *rb3;       // radiance net: [rw x rin], [rw], [rw x rw], [rw], [3 x rw], [3]
     int rw, rin, n_appear;
     float fac[3];                                       // sdf_scale / radius3d_original per axis
@@ -35,13 +35,14 @@ constexpr int XW = 64;                                  // padded radiance input
 constexpr int kTileBytes = kTile * XW * 2;              // one saved activation tile: 16 KB
 constexpr int kChunk = kTile * 16;                      // bytes of one 8-column chunk of a 128-row tile
 
-// internal radiance-input column -> reference column (or -1 for padding)
-__host__ __device__ inline int ref_col(int k, int n_appear) {
-    if (k < 32) return 22 + k;
+// internal radiance-input column -> reference column (or -1 for padding); the reference input is [x(3), SH(16), n(3), h(nh), h_appear]
+// with nh = 2L h columns, so rad_in = 22 + nh + n_appear, and the internal h columns nh..31 are padding
+__host__ __device__ inline int ref_col(int k, int n_appear, int nh) {
+    if (k < 32) return k < nh ? 22 + k : -1;
     if (k < 35) return k - 32;
     if (k < 51) return 3 + (k - 35);
     if (k < 54) return 19 + (k - 51);
-    if (k < 54 + n_appear) return k;
+    if (k < 54 + n_appear) return 22 + nh + (k - 54);
     return -1;
 }
 
@@ -99,11 +100,18 @@ constexpr int kColorGatherU = 4;
 // chunk-major X tile, zero above max_level, as gather_row_to_tile writes it) and its Jacobian J0[p], J1[p], which stay in registers until
 // g = U.W1 is known.  Fully unrolled, unlike the rolled gathers of the 16-24-warp kernels, so that J (96 floats) is statically indexed:
 // k_color_fwd runs 8 warps per SM and has no min-blocks bound, so it may use the registers.  The corner loads of kColorGatherU levels are
-// issued before any of them is consumed.
+// issued before any of them is consumed.  Levels p >= L = m.n_pseudo load nothing and write zero columns; a trip that starts at or above L
+// computes nothing, and in the trip that L cuts the levels >= L see zero corners (their J is zero and never read: nablas stops at L).
 __device__ __forceinline__ void gather_row_and_jacobian(const PLMeta &m, const __half *__restrict__ grid, const float (&xs)[3], int max_level,
                                                         uint8_t *tile, int r, float (&J0)[16][3], float (&J1)[16][3]) {
+    const uint32_t L = m.n_pseudo;
 #pragma unroll
     for (uint32_t p0 = 0; p0 < 16; p0 += kColorGatherU) {
+        if (p0 >= L) {                                         // uniform
+#pragma unroll
+            for (int u = 0; u < kColorGatherU; ++u) put_level_to_tile<kTile>(tile, r, p0 + u, 0u);
+            continue;
+        }
         uint32_t cell[kColorGatherU][8], raw[kColorGatherU][8];
         float w[kColorGatherU][8], fr[kColorGatherU][3], sc[kColorGatherU][3];
 #pragma unroll
@@ -112,13 +120,13 @@ __device__ __forceinline__ void gather_row_and_jacobian(const PLMeta &m, const _
         for (int u = 0; u < kColorGatherU; ++u) {
             const uint32_t *lp = level_cells_ptr(m, p0 + u, grid);
 #pragma unroll
-            for (int c = 0; c < 8; ++c) raw[u][c] = ld_nc_u32(lp + cell[u][c]);
+            for (int c = 0; c < 8; ++c) raw[u][c] = p0 + u < L ? ld_nc_u32(lp + cell[u][c]) : 0u;
         }
 #pragma unroll
         for (int u = 0; u < kColorGatherU; ++u) {
             const uint32_t p = p0 + u;
             const uint32_t packed = feat2_from_raw(raw[u], w[u]);
-            *reinterpret_cast<uint32_t *>(tile + (p >> 2) * (kTile * 16) + r * 16 + (p & 3) * 4) = ((int)m.level[p] <= max_level) ? packed : 0u;
+            put_level_to_tile<kTile>(tile, r, p, (p < L && (int)m.level[p] <= max_level) ? packed : 0u);
             jacobian_from_raw(raw[u], fr[u], sc[u], J0[p], J1[p]);
         }
     }
@@ -166,7 +174,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
     if constexpr (kRad) {
         for (int e = tid; e < XW * XW; e += kTile) {
             const int j = e % XW, k = e / XW;                  // (out j, in k)
-            const int rc = ref_col(k, net.n_appear);
+            const int rc = ref_col(k, net.n_appear, net.dec.nh);
             const __half v1 = (j < net.rw && rc >= 0) ? net.R1[j * net.rin + rc] : __float2half_rn(0.f);
             const __half v2 = (j < net.rw && k < net.rw) ? net.R2[j * net.rw + k] : __float2half_rn(0.f);
             *reinterpret_cast<__half *>(sR1 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v1;
@@ -238,7 +246,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 #pragma unroll
             for (uint32_t q = 0; q < 4; ++q) {
                 const uint32_t p = g4 * 4 + q;
-                if ((int)m.level[p] <= max_level) {
+                if (p < m.n_pseudo && (int)m.level[p] <= max_level) {
                     const float g0 = r16(gg[2 * q]), g1 = r16(gg[2 * q + 1]);
 #pragma unroll
                     for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g0, J0[p][d], nacc[d]);
@@ -362,7 +370,7 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     uint8_t *sY1 = sT + 3 * kTileBytes;                        // 20 KB [Y1 | 1 | 0]
     uint8_t *sXe = sY1 + kTile * NE * 2;                       // 20 KB [X | 1 gy3 | 0]
     uint8_t *sR2T = sXe + kTile * NE * 2;                      //  8 KB (N = in i, K = out j) = R2[j][i]
-    uint8_t *sR1h = sR2T + XW * XW * 2;                        //  4 KB (N = h column k, K = out j) = R1[j][22 + k]
+    uint8_t *sR1h = sR2T + XW * XW * 2;                        //  4 KB (N = h column k, K = out j) = R1[j][22 + k], zero for k >= 2L
     __shared__ float sR3[3][XW];
     __shared__ float sdb3[3];
     __shared__ __align__(8) uint64_t mbar_ld;
@@ -375,7 +383,7 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     }
     for (int e = tid; e < NF * XW; e += kTile) {
         const int k = e % NF, j = e / NF;
-        const __half v = j < net.rw ? net.R1[j * net.rin + 22 + k] : __float2half_rn(0.f);
+        const __half v = (j < net.rw && k < net.dec.nh) ? net.R1[j * net.rin + 22 + k] : __float2half_rn(0.f);
         *reinterpret_cast<__half *>(sR1h + (j / 8) * (NF * 16) + k * 16 + (j % 8) * 2) = v;
     }
     if (tid < XW) {
@@ -503,7 +511,7 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
                     const float a = xa[4 * c + 2 * r + j], b = xb[4 * c + 2 * r + j];
                     if (col < XW) {
                         if (col < net.rw) atomicAdd(dR2 + row * net.rw + col, a);
-                        const int rc = ref_col(col, net.n_appear);
+                        const int rc = ref_col(col, net.n_appear, net.dec.nh);
                         if (rc >= 0) atomicAdd(dR1 + row * net.rin + rc, b);
                     } else if (col == XW) {
                         atomicAdd(drb2 + row, a);
@@ -619,11 +627,11 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
             }
             *reinterpret_cast<uint4 *>(sT + kTileBytes + c * kChunk + tid * 16) = tc::pack8_f16(uu);
         }
-        // dg = J gin (fp16), level by level, into my row of Ge
+        // dg = J gin (fp16), level by level, into my row of Ge; zero for the levels >= L (columns 2L..31)
 #pragma unroll 4
         for (uint32_t p = 0; p < 16; ++p) {               // four levels per trip: 32 independent corner loads in flight (2 CTAs / SM: registers are free)
             uint32_t packed = 0;
-            if ((int)m.level[p] <= max_level) {
+            if (p < m.n_pseudo && (int)m.level[p] <= max_level) {
                 float J0[3], J1[3];
                 level_jacobian(m, p, xs, grid, J0, J1);
                 float a0 = 0.f, a1 = 0.f;
@@ -691,7 +699,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         __syncthreads();
         // ---- merged scatter
 #pragma unroll 1
-        for (uint32_t g4 = 0; g4 < 4; ++g4) {
+        for (uint32_t g4 = 0; g4 * 4 < m.n_pseudo; ++g4) {
             float gg[8], hz[8];
             tc::acc_ld8(stage, kS, tid, g4 * 8, gg);
             tc::acc_ld8(stage, kS, tid, NF + g4 * 8, hz);
@@ -702,7 +710,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
 #pragma unroll
             for (uint32_t q = 0; q < 4; ++q) {
                 const uint32_t p = g4 * 4 + q;
-                if ((int)m.level[p] > max_level) continue;               // uniform
+                if (p >= m.n_pseudo || (int)m.level[p] > max_level) continue;               // uniform
                 uint32_t cell[8];
                 float w[8], fr[3], sc[3], ua[8], ub[8];
                 level_cells3(m, p, xs, cell, w, fr, sc);
@@ -743,7 +751,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
 #pragma unroll
                 for (int j = 0; j < 2; ++j) {
                     const int col = tc::frag_col(c) + j;
-                    if (col < NF) atomicAdd(d_W1 + row * NF + col, wacc[4 * c + 2 * r + j]);
+                    if (col < net.dec.nh) atomicAdd(d_W1 + row * net.dec.nh + col, wacc[4 * c + 2 * r + j]);
                     else if (col == NF) atomicAdd(d_b1 + row, wacc[4 * c + 2 * r + j]);
                 }
             if (tc::frag_col(0) == 0) atomicAdd(d_W2 + row, vacc[2 * r]);
@@ -764,8 +772,8 @@ int make_net(const nsb_color_net *c, const nsb_lotd_meta *meta, PLMeta *m, Color
     if (int rc = make_decoder(meta, &dec, m, &d->dec, who)) return rc;
     if (radiance || c->rad_width != 0) {
         NSB_REQUIRE(c->rad_width >= 1 && c->rad_width <= 64, "%s: radiance width must be <= 64", who);
-        NSB_REQUIRE(c->n_appear >= 0 && c->n_appear <= 8 && c->rad_in == 54 + c->n_appear,
-                    "%s: radiance input must be [x(3), SH deg 4 (16), n(3), h(32), h_appear(<=8)]", who);
+        NSB_REQUIRE(c->n_appear >= 0 && c->n_appear <= 8 && c->rad_in == 22 + d->dec.nh + c->n_appear,
+                    "%s: radiance input must be [x(3), SH deg 4 (16), n(3), h(2L = %d), h_appear(<=8)]", who, d->dec.nh);
     } else {
         NSB_REQUIRE(!c->R1 && !c->rb1 && !c->R2 && !c->rb2 && !c->R3 && !c->rb3, "%s: rad_width 0 (no radiance net) needs NULL radiance pointers", who);
     }

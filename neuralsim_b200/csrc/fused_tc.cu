@@ -1,8 +1,8 @@
 // Fused forward_sdf and its backward with the decoder GEMMs on the Hopper tensor cores (wgmma), sm_90a.
 //
 // One CTA = 128 threads = one warpgroup = one tile of 128 points; thread r owns point r for the gather and the scatter:
-//   gather   thread r walks the 16 LoTD levels of its point (8 corner loads each); every level's two fp16 features go
-//            straight into its row of the A tile in shared memory (core-matrix layout of tc_util.cuh)
+//   gather   thread r walks the L (1..16) LoTD levels of its point (8 corner loads each); every level's two fp16 features go
+//            straight into its row of the A tile in shared memory (core-matrix layout of tc_util.cuh), columns 2L..31 are zero
 //   MMA      the warpgroup issues wgmma (M=64, N=64, K=16) x2 per 64-row half: Z[128 x 64] (fp32, registers) = H[128 x 32] . W1^T
 //   epilogue bias + Softplus(beta) with the autocast rounding points on the accumulator fragments, the 64 -> 1 layer as a
 //            dot product per row (16 hidden units per lane, summed over the lane quad) -> sdf[r]
@@ -107,8 +107,8 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
 //   MMA3: X[64 x 40]   += dZ^T . [H | 1 | 0..]    both operands are the tiles above read MN-major, K = the 128 points: [ dW1 | db1 ]
 //   MMA4: V[64 x 8]    += (d*a)^T . [1 0..]       column 0 = dW2
 //              X and V are register fragments carried over all tiles of the persistent CTA
-//   dH staged as fp32 rows in G (free once the MMAs have completed) -> scatter into the fp32 table gradient (8 corners x 16 levels,
-//   red.global.add.v2.f32);  db2 via a warp sum.
+//   dH staged as fp32 rows in G (free once the MMAs have completed) -> scatter into the fp32 table gradient (8 corners x L levels,
+//   red.global.add.v2.f32);  db2 via a warp sum.  Columns 2L..31 of H and dH are zero and neither scattered nor flushed.
 // =====================================================================================================================
 // Resident CTAs per SM of the persistent grid of k_sdf_bwd_tc: 51 KB of shared memory and 120 registers fit four.  On an H100
 // (NVIDIA H100 80GB HBM3, 400 W power limit) the kernel took 2.43 / 2.43 ms per bench step at 2 CTAs / SM, 2.24 / 2.19 ms at 3 and
@@ -208,14 +208,14 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         const bool active = valid && dd != 0.f;
         const bool warp_active = __any_sync(0xffffffffu, active);
 #pragma unroll 1
-        for (uint32_t g4 = 0; g4 < 4; ++g4) {
+        for (uint32_t g4 = 0; g4 * 4 < m.n_pseudo; ++g4) {
             float dh[8];
             tc::acc_ld8(stage, kS, tid, g4 * 8, dh);                // 4 levels x 2 features
             if (!warp_active) continue;
 #pragma unroll
             for (uint32_t q = 0; q < 4; ++q) {
                 const uint32_t p = g4 * 4 + q;
-                if ((int)m.level[p] > max_level) continue;               // uniform
+                if (p >= m.n_pseudo || (int)m.level[p] > max_level) continue;               // uniform
                 uint32_t cell[8];
                 float w[8], a[8], b[8];
                 level_cells3(m, p, xs, cell, w);
@@ -242,7 +242,7 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
 #pragma unroll
                 for (int j = 0; j < 2; ++j) {
                     const int col = tc::frag_col(c) + j;
-                    if (col < NF) atomicAdd(d_W1 + row * NF + col, xacc[4 * c + 2 * r + j]);
+                    if (col < dec.nh) atomicAdd(d_W1 + row * dec.nh + col, xacc[4 * c + 2 * r + j]);
                     else if (col == NF) atomicAdd(d_b1 + row, xacc[4 * c + 2 * r + j]);
                 }
             if (tc::frag_col(0) == 0) atomicAdd(d_W2 + row, vacc[2 * r]);

@@ -9,6 +9,7 @@ namespace nsb {
 struct DecoderDevTC {
     const __half *W1, *b1, *W2, *b2;
     int width;
+    int nh;                                // 2L: the decoder's input width = the row stride of W1 (L = PLMeta::n_pseudo, 1..16)
     float beta;
 };
 
@@ -38,15 +39,23 @@ __device__ __forceinline__ void occ_collect_point(const OccCollect &oc, const fl
 constexpr int kTile = 128;
 constexpr int NF = 32, HW = 64;           // features, hidden width (zero padded to 64)
 
-// the 16 levels of one point -> row `r` of a chunk-major [R x >=32] fp16 tile (4 bytes per level)
+// the L = m.n_pseudo (1..16) levels of one point -> row `r` of a chunk-major [R x >=32] fp16 tile (4 bytes per level); the feature
+// columns 2L..31 are written as zeros, so that nothing a previous tile left in shared memory reaches a wgmma (a stale fp16 Inf times a
+// zero weight is NaN), and levels >= L are neither read nor masked.
 // U levels per loop trip: the 8 U corner loads of a trip are independent, so U = 2 doubles the loads in flight per thread (the
 // latency-bound backward kernels run at 8-16 warps / SM; one level per trip thrashes L1 in the ray-major order of k_fused_sdf_tc);
-// full unrolling is avoided on purpose (instruction cache, see fused_tc.cu).
+// full unrolling is avoided on purpose (instruction cache, see fused_tc.cu).  An odd L ends with one level alone.
+template <int R>
+__device__ __forceinline__ void put_level_to_tile(uint8_t *tile, int r, uint32_t p, uint32_t v) {
+    *reinterpret_cast<uint32_t *>(tile + (p >> 2) * (R * 16) + r * 16 + (p & 3) * 4) = v;
+}
 template <int R, int U = 2>
 __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half *__restrict__ grid, const float (&xs)[3],
                                                    int max_level, uint8_t *tile, int r) {
+    const uint32_t L = m.n_pseudo;
+    uint32_t p0 = 0;
 #pragma unroll 1
-    for (uint32_t p0 = 0; p0 < 16; p0 += U) {
+    for (; p0 + U <= L; p0 += U) {
         uint32_t cell[U][8];
         float w[U][8];
         uint32_t packed[U];
@@ -57,9 +66,19 @@ __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             const uint32_t p = p0 + u;
-            *reinterpret_cast<uint32_t *>(tile + (p >> 2) * (R * 16) + r * 16 + (p & 3) * 4) = ((int)m.level[p] <= max_level) ? packed[u] : 0u;
+            put_level_to_tile<R>(tile, r, p, ((int)m.level[p] <= max_level) ? packed[u] : 0u);
         }
     }
+#pragma unroll 1
+    for (; p0 < L; ++p0) {
+        uint32_t cell[8];
+        float w[8];
+        level_cells3(m, p0, xs, cell, w);
+        const uint32_t packed = level_feat2_cells(level_cells_ptr(m, p0, grid), cell, w);
+        put_level_to_tile<R>(tile, r, p0, ((int)m.level[p0] <= max_level) ? packed : 0u);
+    }
+#pragma unroll 1
+    for (; p0 < 16; ++p0) put_level_to_tile<R>(tile, r, p0, 0u);
 }
 
 // Where the points of a kernel come from: x[i] (network space), or rays_o/rays_d[ray] + t[i] rays_d[ray] with ray = ridx[i] (or i).
@@ -123,21 +142,22 @@ __device__ __forceinline__ void softplus_as(float zz, const SoftplusK &K, float 
     s = lin ? 1.f : e * rcp_approx(d);
 }
 
-// W1 [width x 32] (fp16, row-major) -> chunk-major [64 x 32] B tile, rows >= width zero
+// W1 [width x 2L] (fp16, row-major) -> chunk-major [64 x 32] B tile, rows >= width and columns >= 2L zero
 __device__ __forceinline__ void stage_W1(const DecoderDevTC &dec, uint8_t *sB, int tid) {
     for (int e = tid; e < HW * (NF / 8); e += kTile) {
         const int j = e % HW, c = e / HW;
-        uint4 q = make_uint4(0, 0, 0, 0);
-        if (j < dec.width) q = *reinterpret_cast<const uint4 *>(dec.W1 + j * NF + c * 8);
-        *reinterpret_cast<uint4 *>(sB + c * (HW * 16) + j * 16) = q;
+        __align__(16) __half q[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) q[k] = (j < dec.width && c * 8 + k < dec.nh) ? dec.W1[j * dec.nh + c * 8 + k] : __float2half_rn(0.f);
+        *reinterpret_cast<uint4 *>(sB + c * (HW * 16) + j * 16) = *reinterpret_cast<const uint4 *>(q);
     }
 }
 
-// W1^T [32 x 64] -> chunk-major B tile (row = feature k, column = hidden j), columns >= width zero
+// W1^T [32 x 64] -> chunk-major B tile (row = feature k, column = hidden j), columns >= width and rows >= 2L zero
 __device__ __forceinline__ void stage_W1T(const DecoderDevTC &dec, uint8_t *sBT, int tid) {
     for (int e = tid; e < NF * HW; e += kTile) {
         const int k = e % NF, j = e / NF;
-        const __half v = j < dec.width ? dec.W1[j * NF + k] : __float2half_rn(0.f);
+        const __half v = (j < dec.width && k < dec.nh) ? dec.W1[j * dec.nh + k] : __float2half_rn(0.f);
         *reinterpret_cast<__half *>(sBT + (j / 8) * (NF * 16) + k * 16 + (j % 8) * 2) = v;
     }
 }
@@ -157,12 +177,15 @@ __device__ __forceinline__ void stage_decoder_vectors(const DecoderDevTC &dec, B
 }
 
 // Host: the LoTD layout and decoder the wgmma kernels are built for -> their kernel arguments (0, or 2 with the error set).
+// L = 1..16 levels of 2 features each in 3-D; the decoder's W1 is [width x 2L].
 inline int make_decoder(const nsb_lotd_meta *meta, const nsb_sdf_decoder *dec, PLMeta *m, DecoderDevTC *d, const char *who) {
     if (make_plmeta(meta, m)) return 2;
-    NSB_REQUIRE(m->n_pseudo == 16 && m->F == 2 && m->D == 3 && plmeta_two_feature_cells(*m), "%s: built for 16 x 2 LoTD features in 3-D", who);
+    NSB_REQUIRE(m->n_pseudo >= 1 && m->n_pseudo <= 16, "%s: built for 1 to 16 LoTD levels (got %u)", who, m->n_pseudo);
+    NSB_REQUIRE(m->F == 2 && m->D == 3 && m->n_out == 2 * m->n_pseudo && plmeta_two_feature_cells(*m), "%s: built for L x 2 LoTD features in 3-D", who);
     NSB_REQUIRE(plmeta_cell_key_fits(*m), "%s: a level resolution exceeds %u cells per axis (the backward's merge key)", who, 1u << kCellKeyBits);
     NSB_REQUIRE(dec->width >= 1 && dec->width <= 64, "%s: decoder width must be <= 64", who);
-    *d = DecoderDevTC{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2, dec->width, dec->beta};
+    *d = DecoderDevTC{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2, dec->width,
+                      2 * (int)m->n_pseudo, dec->beta};
     return 0;
 }
 

@@ -21,7 +21,8 @@ def color_net_c(t16, dec, rad, fac):
     """nsb_color_net over the fp16 images t16 = (W1, b1, W2, b2[, R1, rb1, R2, rb2, R3, rb3]) of the decoder layers `dec` and the radiance
     layers `rad` (None: the geometry-only net, rad_width = 0); fac: sdf_scale / radius3d_original per axis"""
     ptrs = [x.data_ptr() for x in t16] + [None] * (10 - len(t16))
-    rw, ri, na = (rad[0].out_features, rad[0].in_features, rad[0].in_features - 54) if rad is not None else (0, 0, 0)
+    # the radiance input is [x(3), SH4(v) (16), n(3), h(2L), h_appear(n_appear)]; the decoder's input is h
+    rw, ri, na = (rad[0].out_features, rad[0].in_features, rad[0].in_features - 22 - dec[0].in_features) if rad is not None else (0, 0, 0)
     return L.ColorNetC(*ptrs, dec[0].out_features, rw, ri, na, float(dec[0].activation.beta), (ctypes.c_float * 3)(*fac))
 
 

@@ -299,12 +299,14 @@ class LoTDSDF(nn.Module):
 
     # ---- fused no-grad query (csrc/fused.cu)
     def _fusable(self):
-        """the preconditions of the fused kernels (csrc/fused_tc.cu: `n_pseudo == 16 && F == 2 && plmeta_two_feature_cells`, width <= 64, both
-        biases, CUDA parameters); any other valid LoTD / decoder configuration takes the generic encoding -> decoder path of forward()"""
+        """the preconditions of the fused kernels (csrc/fused_tc_common.cuh make_decoder: 1 to 16 levels of 2 features, `plmeta_two_feature_cells`),
+        width <= 64, both biases, CUDA parameters); any other valid LoTD / decoder configuration, such as a table of 17 or more levels, takes
+        the generic encoding -> decoder path of forward()"""
         e, d = self.encoding, self.decoder
         m = e.meta
-        return (self.dtype == torch.half and e.window is None and d.D == 1 and e.out_features == 32 and e.in_features == 3
-                and m.n_pseudo_levels == 16 and m.n_feat_per_pseudo_lvl == 2 and all(f == 2 for f in m.level_n_feats)
+        return (self.dtype == torch.half and e.window is None and d.D == 1 and e.in_features == 3
+                and 1 <= m.n_pseudo_levels <= 16 and e.out_features == 2 * m.n_pseudo_levels
+                and m.n_feat_per_pseudo_lvl == 2 and all(f == 2 for f in m.level_n_feats)
                 and d.layers[0].out_features <= 64 and isinstance(d.layers[0].activation, nn.Softplus)
                 and d.layers[0].bias is not None and d.layers[1].bias is not None and e.flattened_params.is_cuda)
 

@@ -101,7 +101,8 @@ class LoTDNeuS(nn.Module):
                 and isinstance(r.embed_fn_view, SHEncoder) and r.embed_fn_view.degree == 4 and b.D == 2 and not b.skips and b.dtype == torch.half
                 and all(isinstance(l.activation, nn.ReLU) for l in b.layers[:2]) and isinstance(b.layers[2].activation, nn.Sigmoid)
                 and b.layers[0].out_features <= 64 and b.layers[1].out_features <= 64 and b.layers[1].in_features == b.layers[0].out_features
-                and 54 <= b.layers[0].in_features <= 62 and all(l.bias is not None for l in b.layers))
+                and 0 <= b.layers[0].in_features - self.implicit_surface.encoding.out_features - 22 <= 8
+                and all(l.bias is not None for l in b.layers))
 
     def _fused_color_state(self):
         """(fp16 table, nsb_color_net, the fp16 tensors it points at) -- rebuilt when a master changed."""

@@ -222,7 +222,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         # only the radiance head reads appearance codes: rays that render no rgb gather none
         ha = rays_h_appear.detach().contiguous().float() if (with_rgb and rays_h_appear is not None and model.use_h_appear) else None
         if ha is None and with_rgb and model.use_h_appear:
-            ha = torch.zeros(R, model.radiance_net.blocks.layers[0].in_features - 54, device=dev)
+            ha = torch.zeros(R, model.radiance_net.blocks.layers[0].in_features - 22 - model.implicit_surface.encoding.out_features, device=dev)
         n_ha = ha.shape[1] if ha is not None else 0
         rbuf = torch.zeros(R * (8 + n_ha), device=dev)     # the compacted rays in ONE zero-filled allocation (rows beyond the live count stay 0)
         o_c, d_c = rbuf[:3 * R].view(R, 3), rbuf[3 * R:6 * R].view(R, 3)
@@ -374,7 +374,9 @@ class StaticFrame:
         self.device = dev
         self.rays_o = torch.zeros(self.n_rays, 3, device=dev)
         self.rays_d = torch.zeros(self.n_rays, 3, device=dev)
-        na = h_appear_dim if h_appear_dim is not None else (model.radiance_net.blocks.layers[0].in_features - 54 if model.use_h_appear else 0)
+        # the radiance input is [x(3), SH4(v) (16), n(3), h(2L), h_appear]
+        na = h_appear_dim if h_appear_dim is not None else (
+            model.radiance_net.blocks.layers[0].in_features - 22 - model.implicit_surface.encoding.out_features if model.use_h_appear else 0)
         self.h_appear = torch.zeros(self.n_rays, na, device=dev) if na > 0 else None
         self.cnt = torch.zeros(32, dtype=torch.int64, device=dev)
         self.graph, self.loss, self.rendered, self.buffers, self._occ_captured = None, None, None, None, None
