@@ -447,8 +447,8 @@ int nsb_fused_color_bwd(const nsb_lotd_meta *meta_host, const void *params_half,
 /* ---------------------------------------------------------------- the persistent per-ray kernel (csrc/ray_upsample.cu)
  * The no-grad up-sampling half of neus_ray_query_march_occ_multi_upsample_compressed (neus_ray_query.py:861-905) for every hit ray as ONE
  * persistent kernel: sdf of the marched samples, then per stage cdf -> n_fine[i] inverse-cdf samples -> sdf -> merge, with the ray's samples in
- * shared memory (replaces 11 launches of the stage kernels above, with bit-identical results: the alpha, replay and scan device functions
- * are shared with them, the cdf / inverse-cdf / merge bodies are restated and tests/test_ray_upsample_edges_gpu.py pins them to the stage kernels).
+ * shared memory (replaces 11 launches of the stage kernels above, with bit-identical results: the alpha, replay, scan, cdf, inverse-cdf and
+ * merge device functions are the ones the stage kernels call, and tests/test_ray_upsample_edges_gpu.py pins the kernel to them).
  * fine_all[n_hit, sum(n_fine)] = cat of the stages' samples; the row of an empty pack or of an overflowing ray is not written.
  * n_fine / inv_s_stage / u_stage are HOST arrays of n_stage entries; u_stage[i] points to DEVICE memory with the n_fine[i] quantiles of stage i (linspace(0,1,n+2)[1:-1]: `perturb=False`).
  * A ray with more marched samples than the shared-memory capacity works in its slice of `scratch` (nsb_upsample_rays_scratch_floats(n_hit

@@ -23,27 +23,8 @@ k_upsample_cdf(const float *__restrict__ sdf, const float *__restrict__ dep, con
     const int lane = threadIdx.x & 31;
     n_packs = eff_n(n_packs, n_dev);
     for (int64_t p = gwarp(); p < n_packs; p += nwarps()) {
-        const int64_t b = pi[2 * p], n = pi[2 * p + 1];
-        float T = 1.f, carry = 0.f, last_excl = 0.f;
-        bool stopped = false;
-        int cnt = 0;
-        for (int64_t k0 = 0; k0 < n; k0 += 32) {
-            const int64_t k = k0 + lane;
-            float a = 0.f;
-            if (k < n) a = use_estimate ? upsample_alpha_at(sdf, dep, b, n, k, inv_s) : neus_alpha_at(sdf, b, n, k, inv_s);
-            float w;
-            bool sel;
-            replay_chunk(a, (int)min((int64_t)32, n - k0), lane, eps, thre, T, stopped, cnt, w, sel);
-            const float inc = warp_scan_incl(w, lane) + carry;
-            const float excl = inc - w;
-            if (k < n) cdf[b + k] = excl;
-            if (k == n - 1) last_excl = excl;
-            carry = __shfl_sync(0xffffffffu, inc, 31);
-        }
-        last_excl = __shfl_sync(0xffffffffu, last_excl, (int)((n - 1) & 31));
-        const float norm = fmaxf(last_excl, 1e-5f);
-        __syncwarp();
-        for (int64_t k = lane; k < n; k += 32) cdf[b + k] = __fdiv_rn(cdf[b + k], norm);
+        const int64_t b = pi[2 * p];
+        warp_upsample_cdf(sdf + b, dep + b, (int)pi[2 * p + 1], inv_s, use_estimate, eps, thre, cdf + b, lane);
     }
 }
 
@@ -58,21 +39,7 @@ k_invert_cdf_shared_u(const float *__restrict__ bins, const float *__restrict__ 
         const int64_t b = pi[2 * p];
         const uint32_t n = (uint32_t)pi[2 * p + 1];
         if (n == 0) { samples[t] = __int_as_float(0x7fc00000); continue; }       // an empty pack has no bin to place u in: NaN, nothing read
-        const float *bb = bins + b, *cc = cdfs + b;
-        const float uu = u[t - p * n_s];
-        uint32_t first = 0, count = n;                       // lower bound, clamped to n-1
-        while (count > 0) {
-            const uint32_t step = count >> 1, it = first + step;
-            if (cc[it] < uu) { first = it + 1; count -= step + 1; } else count = step;
-        }
-        const uint32_t pos = min(first, n - 1);
-        float r;
-        if (pos == 0) r = bb[0];
-        else {
-            const float c0 = cc[pos - 1], pmf = __fsub_rn(cc[pos], c0);
-            r = pmf < 1.0e-5f ? bb[pos - 1] : __fmaf_rn(__fdiv_rn(__fsub_rn(uu, c0), pmf), __fsub_rn(bb[pos], bb[pos - 1]), bb[pos - 1]);
-        }
-        samples[t] = r;
+        samples[t] = invert_cdf_one(bins + b, cdfs + b, n, u[t - p * n_s]);
     }
 }
 

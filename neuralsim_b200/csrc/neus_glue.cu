@@ -13,7 +13,7 @@
 // All outputs are the reference's values (same fp32 roundings).  Equal depths keep a fixed order: in the merge a b goes before an equal
 // a, in the boundary assembly the order is (coarse, run 0, run 1, ...).  The step's ties carry equal payloads, so only the sign bit
 // of a +0.0 / -0.0 tie shows it (tests/test_glue_edges_gpu.py pins it).
-#include "nsb_common.cuh"
+#include "neus_device.cuh"
 
 namespace nsb {
 
@@ -148,8 +148,7 @@ k_scan_counts(const int32_t *__restrict__ counts, int64_t n, int64_t seg, ScanWs
 }
 
 // ------------------------------------------------------------------------------------------------ merge with payloads
-// pack p of a: (dep_a, sdf_a)[pi_a[p]] sorted by depth; pack p of b: row p of (dep_b, sdf_b)[P, nb], sorted.
-// merged position of a_i = i + #{b <= a_i}, of b_j = j + #{a < b_j}  (kernel_merge_two_packs_sorted_aligned's rule).
+// pack p of a: (dep_a, sdf_a)[pi_a[p]] sorted by depth; pack p of b: row p of (dep_b, sdf_b)[P, nb], sorted; merged by warp_merge.
 // pi_m[p] = (pi_a[p].first + p * nb, n_a + nb).  One warp per pack; b lives in shared memory.
 constexpr int kMergeWarps = 8;
 __global__ void __launch_bounds__(kMergeWarps * 32)
@@ -167,26 +166,7 @@ k_merge_vals(const float *__restrict__ dep_a, const float *__restrict__ sdf_a, c
         for (int j = lane; j < nb; j += 32) bb[j] = dep_b[p * nb + j];
         __syncwarp();
         if (lane == 0) { pi_m[2 * p] = m0; pi_m[2 * p + 1] = na + nb; }
-        for (int64_t i = lane; i < na; i += 32) {
-            const float v = dep_a[a0 + i];
-            int lo = 0, cnt = nb;                         // upper bound of v in b
-            while (cnt > 0) {
-                const int step = cnt >> 1;
-                if (bb[lo + step] <= v) { lo += step + 1; cnt -= step + 1; } else cnt = step;
-            }
-            dep_m[m0 + i + lo] = v;
-            if (sdf_m) sdf_m[m0 + i + lo] = sdf_a[a0 + i];
-        }
-        for (int j = lane; j < nb; j += 32) {
-            const float v = bb[j];
-            int64_t lo = 0, cnt = na;                     // lower bound of v in a
-            while (cnt > 0) {
-                const int64_t step = cnt >> 1;
-                if (dep_a[a0 + lo + step] < v) { lo += step + 1; cnt -= step + 1; } else cnt = step;
-            }
-            dep_m[m0 + j + lo] = v;
-            if (sdf_m) sdf_m[m0 + j + lo] = sdf_b[p * nb + j];
-        }
+        warp_merge(dep_a + a0, sdf_a + a0, (int)na, bb, sdf_b + p * nb, nb, dep_m + m0, sdf_m ? sdf_m + m0 : nullptr, lane);
     }
 }
 
@@ -201,16 +181,6 @@ struct AsmRuns { int n, len[kAsmMaxRuns]; };              // the fine row is a c
 __device__ __forceinline__ float interval_mid(float v, float next, bool last) {
     const float diff = last ? 0.f : __fsub_rn(next, v);
     return __fadd_rn(v, __fmul_rn(diff, 0.5f));
-}
-
-__device__ __forceinline__ int count_less(const float *a, int n, float v, bool or_equal) {   // #{a_i < v} or #{a_i <= v}, a sorted
-    int lo = 0, cnt = n;
-    while (cnt > 0) {
-        const int step = cnt >> 1;
-        const float u = a[lo + step];
-        if (or_equal ? (u <= v) : (u < v)) { lo += step + 1; cnt -= step + 1; } else cnt = step;
-    }
-    return lo;
 }
 
 // kAsmChunk consecutive rays per warp trip: ONE search of the first ray in ridx_hit (18 dependent L2 loads on a frame -- half of the
@@ -229,11 +199,7 @@ k_assemble_boundary(const float *__restrict__ coarse, int64_t n_rays, int nc, co
     const int64_t n_chunks = (n_rays + kAsmChunk - 1) / kAsmChunk;
     for (int64_t c = gwarp_(); c < n_chunks; c += nwarps_()) {
         const int64_t r0 = c * kAsmChunk;
-        int64_t lo0 = 0, cnt = n_hit;                     // lower bound of r0 in ridx_hit
-        while (cnt > 0) {
-            const int64_t step = cnt >> 1;
-            if (ridx_hit[lo0 + step] < r0) { lo0 += step + 1; cnt -= step + 1; } else cnt = step;
-        }
+        const int64_t lo0 = partition_point(ridx_hit, n_hit, [&](int64_t x) { return x < r0; });     // lower bound of r0 in ridx_hit
         long long cand = -1;                              // lane k: the k-th listed ray at or after r0
         if (lane < kAsmChunk && lo0 + lane < n_hit) cand = ridx_hit[lo0 + lane];
         int used = 0;                                     // listed rays among r0 .. r - 1
@@ -266,7 +232,7 @@ k_assemble_boundary(const float *__restrict__ coarse, int64_t n_rays, int nc, co
                 for (int q = -1; q < runs.n; ++q) {
                     const int len = q < 0 ? nc : runs.len[q];
                     if (e >= start && e < start + len) rank += e - start;
-                    else rank += count_less(raw + start, len, v, /*or_equal=*/start < e);
+                    else rank += partition_point(raw + start, len, [&](float u) { return start < e ? u <= v : u < v; });
                     start += len;
                 }
                 srt[rank] = v;

@@ -4,10 +4,9 @@
 // (graphics/neus.py:_query_fused, reference neus_ray_query.py:861-905) and keeps the ray's samples in shared memory in between.
 // A CTA of 128 threads owns a group of 4 consecutive hit rays: warp w <-> ray w for the per-ray stages; for the SDF evaluations the four rays'
 // pending samples are concatenated into 128-point tiles of the usual gather -> wgmma -> SFU pipeline (sdf_of_tile, fused_tc_common.cuh).
-// Shared with the stand-alone kernels (neus_device.cuh): upsample_alpha_at, neus_alpha_at, replay_chunk and warp_scan_incl.  Restated here on
-// plain pointers: warp_upsample_cdf, invert_cdf_one and warp_merge are the statements of k_upsample_cdf, k_invert_cdf_shared_u and
-// k_merge_vals, so their bit-equality is not by construction; tests/test_ray_upsample_edges_gpu.py pins them (and the group-to-group state
-// below) to the stage kernels bit for bit and to float64 at their edges.
+// The per-ray stage bodies warp_upsample_cdf, invert_cdf_one and warp_merge are the ones k_upsample_cdf, k_invert_cdf_shared_u and
+// k_merge_vals call (neus_device.cuh), on the ray's samples in shared memory here; tests/test_ray_upsample_edges_gpu.py pins the kernel
+// (and its group-to-group state below) to the stage kernels bit for bit and to float64 at its edges.
 // Output: fine[n_hit, sum(n_fine)] -- what `torch.cat(fine_stages, -1)` is on the multi-kernel path.  A ray whose samples do not fit the
 // per-ray shared-memory capacity (kCap) works on a slice of a global scratch buffer instead (same code: the stage bodies take plain
 // pointers).  Overflow: overflow[j] is set to 1 (and nothing else is written to it) for a ray with more than long_cap - merged marched
@@ -35,69 +34,6 @@ struct UpsampleArgs {
     const float *u[kMaxStage];   // the n_fine[i] quantiles of stage i (linspace(0, 1, n + 2)[1:-1], made by torch)
     float eps, thre;
 };
-
-// ---- warp-per-ray stage bodies on plain pointers (shared memory here); same statements as k_upsample_cdf / k_invert_cdf_shared_u / k_merge_vals
-__device__ __forceinline__ void warp_upsample_cdf(const float *sdf, const float *dep, int n, float inv_s, int use_estimate, float eps, float thre,
-                                                  float *cdf, int lane) {
-    float T = 1.f, carry = 0.f, last_excl = 0.f;
-    bool stopped = false;
-    int cnt = 0;
-    for (int k0 = 0; k0 < n; k0 += 32) {
-        const int k = k0 + lane;
-        float a = 0.f;
-        if (k < n) a = use_estimate ? upsample_alpha_at(sdf, dep, 0, n, k, inv_s) : neus_alpha_at(sdf, 0, n, k, inv_s);
-        float w;
-        bool sel;
-        replay_chunk(a, min(32, n - k0), lane, eps, thre, T, stopped, cnt, w, sel);
-        const float inc = warp_scan_incl(w, lane) + carry;
-        const float excl = inc - w;
-        if (k < n) cdf[k] = excl;
-        if (k == n - 1) last_excl = excl;
-        carry = __shfl_sync(0xffffffffu, inc, 31);
-    }
-    last_excl = __shfl_sync(0xffffffffu, last_excl, (n - 1) & 31);
-    const float norm = fmaxf(last_excl, 1e-5f);
-    __syncwarp();
-    for (int k = lane; k < n; k += 32) cdf[k] = __fdiv_rn(cdf[k], norm);
-    __syncwarp();
-}
-
-__device__ __forceinline__ float invert_cdf_one(const float *bb, const float *cc, uint32_t n, float uu) {
-    uint32_t first = 0, count = n;                       // lower bound, clamped to n-1
-    while (count > 0) {
-        const uint32_t step = count >> 1, it = first + step;
-        if (cc[it] < uu) { first = it + 1; count -= step + 1; } else count = step;
-    }
-    const uint32_t pos = n ? min(first, n - 1) : 0;
-    if (pos == 0) return bb[0];
-    const float c0 = cc[pos - 1], pmf = __fsub_rn(cc[pos], c0);
-    return pmf < 1.0e-5f ? bb[pos - 1] : __fmaf_rn(__fdiv_rn(__fsub_rn(uu, c0), pmf), __fsub_rn(bb[pos], bb[pos - 1]), bb[pos - 1]);
-}
-
-__device__ __forceinline__ void warp_merge(const float *dep_a, const float *sdf_a, int na, const float *dep_b, const float *sdf_b, int nb,
-                                           float *dep_m, float *sdf_m, int lane) {
-    for (int i = lane; i < na; i += 32) {
-        const float v = dep_a[i];
-        int lo = 0, cnt = nb;                            // upper bound of v in b
-        while (cnt > 0) {
-            const int step = cnt >> 1;
-            if (dep_b[lo + step] <= v) { lo += step + 1; cnt -= step + 1; } else cnt = step;
-        }
-        dep_m[i + lo] = v;
-        sdf_m[i + lo] = sdf_a[i];
-    }
-    for (int j = lane; j < nb; j += 32) {
-        const float v = dep_b[j];
-        int lo = 0, cnt = na;                            // lower bound of v in a
-        while (cnt > 0) {
-            const int step = cnt >> 1;
-            if (dep_a[lo + step] < v) { lo += step + 1; cnt -= step + 1; } else cnt = step;
-        }
-        dep_m[j + lo] = v;
-        sdf_m[j + lo] = sdf_b[j];
-    }
-    __syncwarp();
-}
 
 __global__ void __launch_bounds__(kTile)
 k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ rays_o,

@@ -1,8 +1,8 @@
 """The persistent up-sampling kernel (csrc/ray_upsample.cu: k_upsample_persistent) at its capacity, group and tie edges.
 
-Its per-ray bodies warp_upsample_cdf, invert_cdf_one and warp_merge restate k_upsample_cdf, k_invert_cdf_shared_u and k_merge_vals on plain
-pointers, and its own logic carries state from one 4-ray group to the next (cur, the p_t / p_sdf / p_cdf pointers, s_n, the ray's scratch
-slice).  Every case here is checked two ways:
+Its per-ray bodies warp_upsample_cdf, invert_cdf_one and warp_merge (csrc/neus_device.cuh) are the ones k_upsample_cdf, k_invert_cdf_shared_u
+and k_merge_vals call, here on a ray's samples in shared memory or scratch, and its own logic carries state from one 4-ray group to the next
+(cur, the p_t / p_sdf / p_cdf pointers, s_n, the ray's scratch slice).  Every case here is checked two ways:
   A  bit for bit against the stage-kernel chain fused_sdf_rays -> upsample_cdf -> sample_cdf_uniform -> merge_sorted_vals (and, with
      sample collection on, the occupancy evidence against the chain's and against OccGridEma.collect_samples on the evaluated points);
   B  per stage against float64 (oracle/neus64.py), teacher-forced on the chain's merged t, sdf and fp32 cdf: the cdf within C_CDF / EST_CDF

@@ -1,6 +1,6 @@
 """The persistent per-ray kernel (csrc/ray_upsample.cu): the no-grad up-sampling half of the NeuS query in ONE launch must give, bit for bit,
 the samples the stage kernels give, including rays whose samples do not fit shared memory.  tests/test_ray_upsample_edges_gpu.py pins
-its restated cdf / inverse-cdf / merge bodies and its group-to-group state at their edges."""
+it, with its group-to-group state, at its capacity, group and tie edges."""
 import pytest
 import torch
 
