@@ -189,8 +189,9 @@ int nsb_interleave_linstep(const float *start, const int64_t *num_steps, const i
                            void *stream);
 int nsb_interleave_arange(const int64_t *num_steps, const int64_t *cumsum_steps, int64_t n_packs, int64_t *out,
                           int64_t *nidx, void *stream);
-/* packed_sort_qsort: ascending, in place on vals; idx (may be NULL) receives global gather indices. */
-int nsb_packed_sort(float *vals, const int64_t *pack_infos, int64_t n_packs, int64_t *idx, void *stream);
+/* packed_sort_qsort: ascending per pack (stable, NaN last), in place on vals [n_vals]; the last pack must end at n_vals.
+ * idx (may be NULL) receives the global gather indices of the packed elements; elements between packs are not touched. */
+int nsb_packed_sort(float *vals, int64_t n_vals, const int64_t *pack_infos, int64_t n_packs, int64_t *idx, void *stream);
 int nsb_mark_pack_boundaries(const int64_t *ids, int64_t n, int32_t *out, void *stream);
 
 /* ------------------------------------------------------------------------------------------------

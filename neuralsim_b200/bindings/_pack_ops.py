@@ -199,13 +199,14 @@ def interleave_linstep(start, num_steps, step_size, return_idx=True):
 
 
 def packed_sort_qsort(vals, pack_infos, return_idx=True):
-    """In place on `vals` (ascending per pack); returns the global gather indices."""
-    if not vals.is_contiguous() or vals.dtype != torch.float32:
-        raise RuntimeError("packed_sort_qsort: vals must be a contiguous float32 tensor (sorted in place)")
+    """In place on `vals` (ascending per pack, stable, NaN last); returns the global gather indices, the identity on elements
+    between packs (the reference's arange)."""
+    if not vals.is_contiguous() or vals.dtype != torch.float32 or vals.dim() != 1:
+        raise RuntimeError("packed_sort_qsort: vals must be a 1-D contiguous float32 tensor (sorted in place)")
     pack_infos = _pi(pack_infos)
-    idx = torch.empty(vals.shape[0], dtype=torch.int64, device=vals.device) if return_idx else None
-    L.check(L.lib().nsb_packed_sort(L.ptr(vals), L.ptr(pack_infos), L.c_i64(pack_infos.shape[0]), L.ptr(idx, allow_none=True),
-                                    L.stream_ptr()), "packed_sort_qsort")
+    idx = torch.arange(vals.shape[0], dtype=torch.int64, device=vals.device) if return_idx else None
+    L.check(L.lib().nsb_packed_sort(L.ptr(vals), L.c_i64(vals.shape[0]), L.ptr(pack_infos), L.c_i64(pack_infos.shape[0]),
+                                    L.ptr(idx, allow_none=True), L.stream_ptr()), "packed_sort_qsort")
     return idx
 
 

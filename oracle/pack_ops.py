@@ -44,8 +44,9 @@ def interleave_linstep(start, num_steps, step_size, return_idx=True):
     step = step.astype(s.dtype)
     nidx = np.repeat(np.arange(n.size, dtype=np.int64), n)
     j = np.concatenate([np.arange(k, dtype=np.int64) for k in n]) if n.size else np.zeros(0, np.int64)
-    if s.dtype == np.float32:   # start + j*step is one fused multiply-add in the compiled reference kernel (fp64 product is exact)
-        out = (s[nidx].astype(np.float64) + j.astype(np.float64) * step[nidx].astype(np.float64)).astype(np.float32)
+    if s.dtype == np.float32:   # start + (float)j*step is one fused multiply-add in the compiled reference kernel (fp64 product is exact)
+        jf = j.astype(np.float32).astype(np.float64)               # (scalar_t)j: rounds once j is past 2^24
+        out = (s[nidx].astype(np.float64) + jf * step[nidx].astype(np.float64)).astype(np.float32)
     else:
         out = (s[nidx] + (j.astype(s.dtype) * step[nidx]).astype(s.dtype)).astype(s.dtype)
     return torch.from_numpy(out), (torch.from_numpy(nidx) if return_idx else None)
@@ -213,7 +214,7 @@ def packed_invert_cdf(bins, cdfs, u_vals, pack_infos):
             pos = _binary_search(cc, u)
             bidx[p, i] = pos + b
             if pos == 0:
-                samples[p, i] = bb[0]
+                samples[p, i] = b_[b]          # bins[begin]: an empty pack reads the element after it
             else:
                 pmf = dt(cc[pos] - cc[pos - 1])
                 if pmf < eps:
@@ -336,7 +337,8 @@ def packed_alpha_to_vw_backward(weights, grad_weights, alphas, pack_infos, early
             al = a[b + j]
             if al < thre:
                 continue
-            ga[b + j] = dt(dt(dt(gw[b + j] * T) - accum) / max(dt(one - al), dt(1e-10)))
+            # fmaxf(1 - alpha, 1e-10f): the number when the other operand is NaN (Python's max would return the NaN)
+            ga[b + j] = dt(dt(dt(gw[b + j] * T) - accum) / np.fmax(dt(one - al), dt(1e-10)))
             accum = dt(accum - dt(gw[b + j] * w[b + j]))
             T = dt(T * dt(one - al))
     return torch.from_numpy(ga)
