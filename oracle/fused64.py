@@ -19,9 +19,9 @@ Rounding points (r16 = round to fp16; names as in the kernels' header comments):
            table, per corner: r16(g) wsum(gin) + (dz W1 + dh_r) w
   sdf backward (k_sdf_bwd_tc)   dz = r16(d w2 s);  da = r16(d a16);  dW1 = dz^T H;  db1 = sum dz;  dW2 = sum da;  table: (dz W1) w
 
-With rounding=False every r16 is the identity and h / J are the exact trilinear interpolation of the (fp16-valued) table and its
-derivative, so the hand-written backward passes below are the exact gradients of the unrounded model (tests/test_fused64_oracle.py
-checks them against torch double-backward).
+With rounding=False every r16 is the identity, cotangents are taken in float64 instead of fp32, and h / J are the exact trilinear
+interpolation of the (fp16-valued) table and its derivative, so the hand-written backward passes below are the exact gradients of
+the unrounded model (tests/test_fused64_oracle.py checks them against torch double-backward).
 """
 from __future__ import annotations
 
@@ -69,6 +69,11 @@ class Fused64:
         return cls(s.encoding.flattened_params, s.encoding.lotd_cfg, d[0].weight, d[0].bias, d[1].weight, d[1].bias,
                    r[0].weight, r[0].bias, r[1].weight, r[1].bias, r[2].weight, r[2].bias,
                    beta=float(d[0].activation.beta), fac=fac, max_level=max_level, rounding=rounding)
+
+    @property
+    def f32(self):
+        """the type the kernels receive cotangents in: fp32, or float64 without rounding"""
+        return np.float32 if self.rounding else np.float64
 
     def r16(self, v):
         return v.astype(np.float16).astype(np.float64) if self.rounding else v
@@ -185,7 +190,7 @@ class Fused64:
         xs = self.xs_of(x)
         h, _ = self.features(xs)
         z, lin, s, a16, sdf = self._decoder(h)
-        d = np.asarray(d_sdf, dtype=np.float32).astype(np.float64)[:, None]
+        d = np.asarray(d_sdf, dtype=self.f32).astype(np.float64)[:, None]
         dz = self.r16(d * self.W2[0] * s)
         da = self.r16(d * a16)
         dH = dz @ self.W1
@@ -195,7 +200,7 @@ class Fused64:
         """k_color_rad_bwd + k_color_sdf_bwd: gradients of sum(g_sdf sdf + g_nablas nablas + g_rgb rgb) through the forward
         `fwd` (color_forward) -> dict(grid [P], W1, b1, W2, b2, R1, rb1, R2, rb2, R3, rb3), float64"""
         N = fwd["sdf"].shape[0]
-        f32 = lambda v, shape: np.zeros(shape) if v is None else np.asarray(v, dtype=np.float32).astype(np.float64)
+        f32 = lambda v, shape: np.zeros(shape) if v is None else np.asarray(v, dtype=self.f32).astype(np.float64)
         g_sdf, g_nab, g_rgb = f32(g_sdf, (N,)), f32(g_nablas, (N, 3)), f32(g_rgb, (N, 3))
         rgb, X, Y1, Y2 = fwd["rgb"], fwd["X"], fwd["Y1"], fwd["Y2"]
         out = {}
