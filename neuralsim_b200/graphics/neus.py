@@ -11,9 +11,12 @@ Two implementations of the same function live here: the op-by-op chain in the re
 `nr3d_lib`-named wrapper of this package), and `_query_fused`, one launch per stage (csrc/neus_glue.cu, neus_fused.cu, fused_tc.cu,
 color_tc.cu), taken when the model offers `forward_sdf_on_rays` and the occupancy grid is a single 3-D grid.  FUSED_STAGES = False
 forces the chain; tests/test_neus_fused_gpu.py renders with both and compares samples, images and gradients.
+Both read their settings from `query_config`; `_query_fused` and the one-launch step (graphics/neus_static.py, on capacities and
+device counts) run the up-sampling and the boundary samples as `upsample_boundary`.
 """
 from __future__ import annotations
 
+from collections import namedtuple
 from operator import itemgetter
 
 import torch
@@ -40,7 +43,79 @@ def use_persistent_upsample(n_rays: int) -> bool:
 
 __all__ = ["neus_cdf", "neus_ray_cdf_to_alpha", "neus_ray_sdf_to_alpha", "neus_ray_sdf_to_vw", "neus_packed_cdf_to_alpha",
            "neus_packed_sdf_to_alpha", "neus_packed_sdf_to_upsample_alpha", "neus_ray_sdf_to_upsample_alpha",
-           "neus_ray_query_march_occ_multi_upsample_compressed"]
+           "neus_ray_query_march_occ_multi_upsample_compressed", "QueryConfig", "query_config", "upsample_boundary"]
+
+
+# the settings of one query as the query uses them (query_config)
+QueryConfig = namedtuple("QueryConfig", "num_coarse factors num_fine upsample_inv_s use_estimate_alpha nablas_has_grad step_size dt_gamma max_steps "
+                                        "max_step_size march_fusable")
+
+
+def query_config(num_coarse=0, coarse_step_cfg=dict(step_mode="linear"), chunksize_query=2 ** 24, march_cfg=dict(), num_fine=8, upsample_inv_s=64.,
+                 upsample_s_divisor=1.0, upsample_inv_s_factors=(1, 4, 16), upsample_use_estimate_alpha=False, nablas_has_grad=False) -> QueryConfig:
+    """`ray_query_cfg.query_param` (the keywords and defaults of the query below; chunksize_query is unused) and the model's
+    upsample_s_divisor -> QueryConfig: num_fine odd-ised, one per stage of `factors`; upsample_inv_s over the divisor; step_size and
+    dt_gamma times step_size_factor; march_fusable: march_cfg holds no other key (neus_fused.march_lean runs it).  The host-sized query,
+    the one-launch step and its arena sizes (graphics/neus_static.py) read it, so they draw the same samples."""
+    factors = tuple(upsample_inv_s_factors)
+    n_stage = len(factors)
+    if isinstance(num_fine, int):
+        num_fine = [num_fine] * n_stage
+    assert len(num_fine) == n_stage, f"num_fine should be of the same length={n_stage} with upsample"
+    step_mode = coarse_step_cfg.get("step_mode", "linear")
+    if num_coarse > 0 and step_mode != "linear":
+        raise RuntimeError(f"coarse step_mode={step_mode!r} is not built (CFG uses 'linear')")
+    fac = march_cfg.get("step_size_factor", 1.0)
+    return QueryConfig(num_coarse=int(num_coarse), factors=factors, num_fine=tuple(n // 2 * 2 + 1 for n in num_fine),
+                       upsample_inv_s=upsample_inv_s / upsample_s_divisor, use_estimate_alpha=bool(upsample_use_estimate_alpha),
+                       nablas_has_grad=nablas_has_grad, step_size=march_cfg.get("step_size", 1e-3) * fac, dt_gamma=march_cfg.get("dt_gamma", 0.0) * fac,
+                       max_steps=int(march_cfg.get("max_steps", 512)), max_step_size=march_cfg.get("max_step_size", 1e10),
+                       march_fusable=set(march_cfg) <= {"step_size", "max_steps", "max_step_size", "dt_gamma", "step_size_factor"})
+
+
+@torch.no_grad()
+def upsample_boundary(marched, rays_o, rays_d, coarse, cfg: QueryConfig, sdf_on_rays, block_order=None, *, table=None, perturb=False, counts=None,
+                      n_out=None, want_mid=True, want_ridx=True):
+    """sdf of the marched samples (ridx_hit, pack_infos, depth, ridx), the up-sampling stages (cdf -> inverse-cdf samples -> sdf -> merge)
+    and the boundary samples of the coarse [R, num_coarse + 1] and fine depths -> neus_fused.assemble_boundary's (d1, mid, ridx_all, pack_infos).
+    sdf_on_rays(ridx, t, packs, count) -> contiguous f32 sdf [t.numel()]: the caller's query (forward_sdf_on_rays' packs).  block_order(via):
+    the pixel-block order of the packs on rays `via`; None: the rays are not image-ordered.  table = (meta, grid16, dec, max_level, collect)
+    lets the persistent kernel run.  perturb: stratified samples (packed_sample_cdf).  counts = (cnt, CNT_SLOTS of graphics/neus_static.py):
+    sizes on the device, capacity-sized buffers (n_out merged samples); None: host sizes."""
+    ridx_hit, pack_infos, depth, ridx = marched
+    n_stage = len(cfg.factors)
+
+    def count(name, i=0):
+        return None if counts is None else (counts[0], counts[1][name] + i)
+
+    hit = count("hit")
+    if use_persistent_upsample(rays_o.shape[0]) and not perturb and table is not None:
+        # the whole no-grad half in ONE persistent per-ray kernel (csrc/ray_upsample.cu); same values as the stage kernels below
+        meta, grid16, dec, max_level, collect = table
+        fine_all, _overflow = neus_fused.upsample_rays(meta, grid16, dec, ridx_hit, pack_infos, depth, rays_o, rays_d, [cfg.upsample_inv_s * f for f in cfg.factors],
+                                                       cfg.num_fine, max_level=max_level, max_steps=cfg.max_steps, use_estimate_alpha=cfg.use_estimate_alpha,
+                                                       collect=collect, count=hit)
+    else:
+        # marched packs are ragged (20-100 samples per ray): tiles of 32 rays would be padded to the longest and the samples of one ray
+        # are already close together, so they are queried in ray-major order (measured faster than ray-tiled); the fine queries have
+        # uniform packs and are ray-tiled whenever the rays are image-ordered
+        sdf = sdf_on_rays(ridx, depth, None, count("marched"))
+        order_f = block_order(ridx_hit) if block_order is not None and n_stage > 1 else None
+        fine_stages = []
+        for i, (factor, nf) in enumerate(zip(cfg.factors, cfg.num_fine)):
+            cdf = neus_fused.upsample_cdf(sdf, depth, pack_infos, cfg.upsample_inv_s * factor, cfg.use_estimate_alpha, count=hit)
+            if perturb:                  # one stratified u per pack and sample (raysample.py:38-61)
+                fine = packed_sample_cdf(depth, cdf, pack_infos, nf, perturb=True)[0]
+            else:
+                fine = neus_fused.sample_cdf_uniform(depth, cdf, pack_infos, nf, count=hit)
+            fine_stages.append(fine)
+            if i < n_stage - 1:         # (the reference also merges after the last stage; nothing reads that result)
+                packs = (get_pack_infos_from_batch(ridx_hit.shape[0], nf, device=fine.device), ridx_hit, order_f) if block_order is not None else None
+                sdf_fine = sdf_on_rays(ridx_hit, fine, packs, hit if packs is not None else count("fine0", i))
+                depth, sdf, pack_infos = neus_fused.merge_sorted_vals(depth, sdf, pack_infos, fine, sdf_fine, n_out=n_out, count=hit)
+        fine_all = (torch.cat(fine_stages, dim=-1) if n_stage > 1 else fine_stages[0]).contiguous()
+    return neus_fused.assemble_boundary(coarse, ridx_hit, fine_all, cfg.num_fine, want_mid=want_mid, want_ridx=want_ridx,
+                                        count=None if counts is None else (counts[0], counts[1]["n_rays"], counts[1]["hit"]))
 
 
 def neus_cdf(x, inv_s):
@@ -105,68 +180,38 @@ def neus_ray_sdf_to_upsample_alpha(sdf, depth_samples, inv_s):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-def _query_fused(model, ray_tested, view_dirs, rays_h_appear, *, perturb=False, with_rgb, with_normal, nablas_has_grad, forward_inv_s, num_coarse, march_cfg, num_fine,
-                 upsample_inv_s, factors, use_estimate_alpha):
+def _query_fused(model, ray_tested, view_dirs, rays_h_appear, cfg: QueryConfig, *, perturb=False, with_rgb, with_normal, forward_inv_s):
     """The query below with every stage between the big kernels as ONE launch (csrc/neus_glue.cu, csrc/neus_fused.cu) and three host
     reads in total (march size, compression size, + the ray test's): same samples, same values as the chain it replaces (with `perturb`,
     the same random stream too) -- the chain
     stays in this file as the specification (tests/test_neus_fused_gpu.py runs both).  None -> no ray marched into an occupied voxel
     (the caller falls back to the general path for that rare case)."""
     rays_o, rays_d, near, far, rays_inds = itemgetter("rays_o", "rays_d", "near", "far", "rays_inds")(ray_tested)
-    dtype, n_stage = rays_o.dtype, len(factors)
-    mc = dict(march_cfg)
-    fac = mc.pop("step_size_factor", 1.0)
-    mc["step_size"] = mc.get("step_size", 1e-3) * fac
-    mc["dt_gamma"] = mc.get("dt_gamma", 0.0) * fac
-    mc.setdefault("max_steps", 512)
+    dtype = rays_o.dtype
     rays_o, rays_d = rays_o.contiguous(), rays_d.contiguous()
-    depths_coarse_1 = batch_sample_step_linear(near, far, num_coarse + 1, prefix_shape=[rays_o.shape[0]], perturb=perturb)
-    marched = neus_fused.march_lean(model.accel.occ.occ_grid, rays_o, rays_d, near.contiguous(), far.contiguous(), **mc)
+    depths_coarse_1 = batch_sample_step_linear(near, far, cfg.num_coarse + 1, prefix_shape=[rays_o.shape[0]], perturb=perturb).contiguous()
+    marched = neus_fused.march_lean(model.accel.occ.occ_grid, rays_o, rays_d, near.contiguous(), far.contiguous(), step_size=cfg.step_size,
+                                    max_steps=cfg.max_steps, max_step_size=cfg.max_step_size, dt_gamma=cfg.dt_gamma)
     if marched is None:
         return None
-    ridx_hit, pinfo_march, depth_samples, ridx = marched
     if perturb:
         # the single-grid marcher jitters only `deltas` (occgrid_raymarch.py:96-110), which this query never reads; the draw is made
         # anyway so that the random stream -- and therefore every later sample -- is the one the op-by-op chain consumes
-        torch.rand(depth_samples.shape, dtype=depth_samples.dtype, device=depth_samples.device)
-    pack_infos = pinfo_march
+        torch.rand_like(marched[2])
     coherent = bool(ray_tested.get("rays_coherent", False))      # image-ordered rays: ray-tiled traversal inside the SDF kernel
     rays_row = ray_tested.get("rays_row") if coherent else None   # ... in 8 x 4 pixel blocks
     surf = getattr(model, "implicit_surface", None)
-    if use_persistent_upsample(rays_o.shape[0]) and not perturb and surf is not None and getattr(surf, "_fusable", lambda: False)():
-        # the whole no-grad half in ONE persistent per-ray kernel (csrc/ray_upsample.cu); same values as the stage kernels below
-        grid16, dec = surf._fused_state()
-        accel = getattr(model, "accel", None)
-        collect = accel.occ.collect_struct() if (model.training and accel is not None) else None
-        fine_all, _overflow = neus_fused.upsample_rays(surf.encoding.meta, grid16, dec, ridx_hit, pack_infos, depth_samples, rays_o, rays_d,
-                                                       [upsample_inv_s * f for f in factors], num_fine, max_level=surf._ml(getattr(model, "max_level", None)),
-                                                       max_steps=mc["max_steps"], use_estimate_alpha=use_estimate_alpha, collect=collect)
-        with torch.no_grad():
-            d1, mid, ridx_all, pinfo = neus_fused.assemble_boundary(depths_coarse_1.contiguous(), ridx_hit, fine_all, run_len=list(num_fine))
-        return _query_fused_tail(model, ray_tested, view_dirs, rays_h_appear, rays_o, rays_d, rays_inds, d1, mid, ridx_all, pinfo, pinfo_march, coherent, dtype,
-                                 with_rgb=with_rgb, with_normal=with_normal, nablas_has_grad=nablas_has_grad, forward_inv_s=forward_inv_s)
-    with torch.no_grad():
-        # marched packs are ragged (20-100 samples per ray): tiles of 32 rays would be padded to the longest and the samples of one ray
-        # are already close together, so they are queried in ray-major order (measured faster than ray-tiled); the boundary and fine
-        # queries have uniform packs and are ray-tiled whenever the rays are image-ordered
-        sdf = model.forward_sdf_on_rays(ridx, depth_samples, rays_o, rays_d)["sdf"].to(dtype)
-        fine_stages = []
-        order_f = neus_fused.block_order(rays_inds, ridx_hit, rays_row) if rays_row is not None and n_stage > 1 else None
-        for i, factor in enumerate(factors):
-            cdf = neus_fused.upsample_cdf(sdf, depth_samples, pack_infos, upsample_inv_s * factor, use_estimate_alpha)
-            if perturb:                  # one stratified u per pack and sample (raysample.py:38-61)
-                fine = packed_sample_cdf(depth_samples, cdf, pack_infos, num_fine[i], perturb=True)[0]
-            else:
-                fine = neus_fused.sample_cdf_uniform(depth_samples, cdf, pack_infos, num_fine[i])
-            fine_stages.append(fine)
-            if i < n_stage - 1:         # (the reference also merges after the last stage; nothing reads that result)
-                packs = (get_pack_infos_from_batch(ridx_hit.shape[0], fine.shape[1], device=fine.device), ridx_hit, order_f) if coherent else None
-                sdf_fine = model.forward_sdf_on_rays(ridx_hit, fine, rays_o, rays_d, packs=packs)["sdf"].to(dtype).contiguous()
-                depth_samples, sdf, pack_infos = neus_fused.merge_sorted_vals(depth_samples, sdf, pack_infos, fine, sdf_fine)
-        fine_all = torch.cat(fine_stages, dim=-1) if n_stage > 1 else fine_stages[0]
-        d1, mid, ridx_all, pinfo = neus_fused.assemble_boundary(depths_coarse_1.contiguous(), ridx_hit, fine_all.contiguous(), run_len=[f.shape[1] for f in fine_stages])
-    return _query_fused_tail(model, ray_tested, view_dirs, rays_h_appear, rays_o, rays_d, rays_inds, d1, mid, ridx_all, pinfo, pinfo_march, coherent, dtype,
-                             with_rgb=with_rgb, with_normal=with_normal, nablas_has_grad=nablas_has_grad, forward_inv_s=forward_inv_s)
+    table = None
+    if surf is not None and getattr(surf, "_fusable", lambda: False)():
+        table = (surf.encoding.meta, *surf._fused_state(), surf._ml(getattr(model, "max_level", None)),
+                 model.accel.occ.collect_struct() if model.training else None)
+    # the model's query: the module path for tables the fused kernels do not cover, and the accel's sample collection
+    d1, mid, ridx_all, pinfo = upsample_boundary(
+        marched, rays_o, rays_d, depths_coarse_1, cfg,
+        lambda ridx, t, packs, _count: model.forward_sdf_on_rays(ridx, t, rays_o, rays_d, packs=packs)["sdf"].to(dtype).contiguous(),
+        (lambda via: neus_fused.block_order(rays_inds, via, rays_row)) if rays_row is not None else None, table=table, perturb=perturb)
+    return _query_fused_tail(model, ray_tested, view_dirs, rays_h_appear, rays_o, rays_d, rays_inds, d1, mid, ridx_all, pinfo, marched[1], coherent, dtype,
+                             with_rgb=with_rgb, with_normal=with_normal, nablas_has_grad=cfg.nablas_has_grad, forward_inv_s=forward_inv_s)
 
 
 def _query_fused_tail(model, ray_tested, view_dirs, rays_h_appear, rays_o, rays_d, rays_inds, d1, mid, ridx_all, pinfo, pinfo_march, coherent, dtype, *,
@@ -233,16 +278,11 @@ def neus_ray_query_march_occ_multi_upsample_compressed(
         return empty, {}
     use_h_appear = getattr(model, "use_h_appear", False) and with_rgb
     use_view_dirs = getattr(model, "use_view_dirs", False) and with_rgb
-    n_stage = len(upsample_inv_s_factors)
-    if isinstance(num_fine, int):
-        num_fine = [num_fine] * n_stage
-    assert len(num_fine) == n_stage, f"num_fine should be of the same length={n_stage} with upsample"
-    num_fine = [n // 2 * 2 + 1 for n in num_fine]
-    upsample_inv_s = upsample_inv_s / upsample_s_divisor
+    cfg = query_config(num_coarse=num_coarse, coarse_step_cfg=coarse_step_cfg, chunksize_query=chunksize_query, march_cfg=march_cfg, num_fine=num_fine,
+                       upsample_inv_s=upsample_inv_s, upsample_s_divisor=upsample_s_divisor, upsample_inv_s_factors=upsample_inv_s_factors,
+                       upsample_use_estimate_alpha=upsample_use_estimate_alpha, nablas_has_grad=nablas_has_grad)
+    n_stage = len(cfg.factors)
     forward_inv_s = model.forward_inv_s() if forward_inv_s is None else forward_inv_s
-    step_mode = coarse_step_cfg.get("step_mode", "linear")
-    if num_coarse > 0 and step_mode != "linear":
-        raise RuntimeError(f"coarse step_mode={step_mode!r} is not built (CFG uses 'linear')")
 
     rays_o, rays_d, near, far, rays_inds = itemgetter("rays_o", "rays_d", "near", "far", "rays_inds")(ray_tested)
     rays_h_appear = ray_tested["rays_h_appear"] if use_h_appear else None
@@ -263,20 +303,18 @@ def neus_ray_query_march_occ_multi_upsample_compressed(
         x_ = torch.addcmul(rays_o[r2], rays_d[r2], t_.unsqueeze(-1))
         return model.forward_sdf(x_.flatten(0, -2), **cond_kw(r2.reshape(-1)))["sdf"].view(t_.shape)
 
-    if (FUSED_STAGES and not cond and num_coarse > 0 and rays_o.is_cuda and dtype == torch.float32 and hasattr(model, "forward_sdf_on_rays")
+    if (FUSED_STAGES and not cond and cfg.num_coarse > 0 and rays_o.is_cuda and dtype == torch.float32 and hasattr(model, "forward_sdf_on_rays")
             and getattr(getattr(model.accel, "occ", None), "occ_grid", None) is not None and model.accel.occ.occ_grid.dim() == 3
-            and not (rays_o.requires_grad or rays_d.requires_grad or near.requires_grad or far.requires_grad)
-            and set(march_cfg) <= {"step_size", "max_steps", "max_step_size", "dt_gamma", "step_size_factor"}):
-        ret = _query_fused(model, ray_tested, view_dirs, rays_h_appear, perturb=perturb, with_rgb=with_rgb, with_normal=with_normal, nablas_has_grad=nablas_has_grad,
-                           forward_inv_s=forward_inv_s, num_coarse=num_coarse, march_cfg=march_cfg, num_fine=num_fine, upsample_inv_s=upsample_inv_s,
-                           factors=upsample_inv_s_factors, use_estimate_alpha=upsample_use_estimate_alpha)
+            and not (rays_o.requires_grad or rays_d.requires_grad or near.requires_grad or far.requires_grad) and cfg.march_fusable):
+        ret = _query_fused(model, ray_tested, view_dirs, rays_h_appear, cfg, perturb=perturb, with_rgb=with_rgb, with_normal=with_normal,
+                           forward_inv_s=forward_inv_s)
         if ret is not None:
             return ret
 
-    if num_coarse > 0:
-        depths_coarse_1, deltas_coarse_1 = batch_sample_step_linear(near, far, num_coarse + 1, perturb=perturb, return_dt=True)
+    if cfg.num_coarse > 0:
+        depths_coarse_1, deltas_coarse_1 = batch_sample_step_linear(near, far, cfg.num_coarse + 1, perturb=perturb, return_dt=True)
     marched = model.accel.ray_march(rays_o, rays_d, near=near, far=far, perturb=perturb, **march_cfg)
-    net_kw = dict(nablas_has_grad=nablas_has_grad, with_rgb=with_rgb, with_normal=with_normal, dtype=dtype, cond_kw=cond_kw if cond else None)
+    net_kw = dict(nablas_has_grad=cfg.nablas_has_grad, with_rgb=with_rgb, with_normal=with_normal, dtype=dtype, cond_kw=cond_kw if cond else None)
 
     if marched.ridx_hit is not None:
         # ---------------- up-sample on the marched samples (no grad)
@@ -287,25 +325,25 @@ def neus_ray_query_march_occ_multi_upsample_compressed(
         with torch.no_grad():
             sdf = model.forward_sdf(marched.samples, **cond_kw(marched.ridx))["sdf"].to(dtype)
             fine_stages = []
-            for i, factor in enumerate(upsample_inv_s_factors):
+            for i, factor in enumerate(cfg.factors):
                 if FUSED_STAGES:
-                    cdf = neus_fused.upsample_cdf(sdf, depth_samples, pack_infos, upsample_inv_s * factor, upsample_use_estimate_alpha)
+                    cdf = neus_fused.upsample_cdf(sdf, depth_samples, pack_infos, cfg.upsample_inv_s * factor, cfg.use_estimate_alpha)
                 else:
-                    if upsample_use_estimate_alpha:
-                        alpha = neus_packed_sdf_to_upsample_alpha(sdf, depth_samples, upsample_inv_s * factor, pack_infos)
+                    if cfg.use_estimate_alpha:
+                        alpha = neus_packed_sdf_to_upsample_alpha(sdf, depth_samples, cfg.upsample_inv_s * factor, pack_infos)
                     else:
-                        alpha = neus_packed_sdf_to_alpha(sdf, upsample_inv_s * factor, pack_infos)
+                        alpha = neus_packed_sdf_to_alpha(sdf, cfg.upsample_inv_s * factor, pack_infos)
                     vw = packed_alpha_to_vw(alpha, pack_infos)
                     cdf = packed_cumsum(vw, pack_infos, exclusive=True)
                     norm = cdf[pack_infos[:, 0] + pack_infos[:, 1] - 1].clamp_min(1e-5)
                     cdf = packed_div(cdf, norm, pack_infos)
                 if FUSED_STAGES and not perturb:
-                    fine = neus_fused.sample_cdf_uniform(depth_samples, cdf, pack_infos, num_fine[i])
+                    fine = neus_fused.sample_cdf_uniform(depth_samples, cdf, pack_infos, cfg.num_fine[i])
                 else:
-                    fine = packed_sample_cdf(depth_samples, cdf, pack_infos, num_fine[i], perturb=perturb)[0]
+                    fine = packed_sample_cdf(depth_samples, cdf, pack_infos, cfg.num_fine[i], perturb=perturb)[0]
                 fine_stages.append(fine)
                 if n_stage > 1:
-                    pinfo_fine = get_pack_infos_from_batch(n_hit, num_fine[i], device=device)
+                    pinfo_fine = get_pack_infos_from_batch(n_hit, cfg.num_fine[i], device=device)
                     pidx0, pidx1, pack_infos = merge_two_packs_sorted_aligned(depth_samples, pack_infos, fine.flatten(), pinfo_fine, b_sorted=True)
                     n_old = depth_samples.numel()
                     merged = depth_samples.new_empty([n_old + fine.numel()])
@@ -319,7 +357,7 @@ def neus_ray_query_march_occ_multi_upsample_compressed(
             depths_1 = torch.cat(fine_stages, dim=-1).sort(dim=-1).values if n_stage > 1 else fine_stages[0]
 
         # ---------------- boundary points with grad, alpha, compression
-        if num_coarse == 0:
+        if cfg.num_coarse == 0:
             x = torch.addcmul(rays_o[marched.ridx_hit].unsqueeze(-2), rays_d[marched.ridx_hit].unsqueeze(-2), depths_1.unsqueeze(-1))
             alpha = neus_ray_sdf_to_alpha(sdf_on_rays(marched.ridx_hit, depths_1).to(dtype) if cond else
                                           model.forward_sdf(x.flatten(0, -2))["sdf"].to(dtype).view(depths_1.shape), forward_inv_s)
@@ -364,13 +402,13 @@ def neus_ray_query_march_occ_multi_upsample_compressed(
         return volume_buffer, details
 
     # ---------------- no ray hit the occupancy grid
-    if num_coarse == 0:
+    if cfg.num_coarse == 0:
         return empty, {}
     x = torch.addcmul(rays_o.unsqueeze(-2), rays_d.unsqueeze(-2), depths_coarse_1.unsqueeze(-1))
     sdf_c = (sdf_on_rays(torch.arange(R, device=device), depths_coarse_1) if cond else model.forward_sdf(x.flatten(0, -2))["sdf"].view(depths_coarse_1.shape)).to(dtype)
     alpha_coarse = neus_ray_sdf_to_alpha(sdf_c, forward_inv_s)
-    depths_coarse = depths_coarse_1[..., :num_coarse] + deltas_coarse_1[..., :num_coarse] / 2.
-    pack_infos_coarse = get_pack_infos_from_batch(R, num_coarse, device=device)
+    depths_coarse = depths_coarse_1[..., :cfg.num_coarse] + deltas_coarse_1[..., :cfg.num_coarse] / 2.
+    pack_infos_coarse = get_pack_infos_from_batch(R, cfg.num_coarse, device=device)
     nidx_useful, pack_infos_useful, pidx_useful = packed_volume_render_compression(alpha_coarse.flatten(), pack_infos_coarse)
     if nidx_useful.numel() == 0:
         return empty, {}

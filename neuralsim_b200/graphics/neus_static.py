@@ -3,8 +3,9 @@ fwd+bwd step can be captured in ONE CUDA graph and replayed with a single launch
 
 Same kernels, same values as `graphics.neus._query_fused` + `fields.neus.volume_integration` (reference:
 nr3d_lib/graphics/neus/neus_ray_query.py:732-1104, app/renderers/single_volume_renderer.py:73-102,136-460): the only difference
-is where the sizes live.  The reference reads ~25 sizes back per `ray_query` (SURVEY.md §8a a9); `_query_fused` reads three (+ one
-in the backward); here the three scans leave their totals in a device block `cnt` (layout: include/neuralsim_b200.h, nsb_query_counts),
+is where the sizes live; the settings (`graphics.neus.query_config`) and the up-sampling (`graphics.neus.upsample_boundary`) are
+shared code.  The reference reads ~25 sizes back per `ray_query` (SURVEY.md §8a a9); `_query_fused` reads three (+ one in the
+backward); here the three scans leave their totals in a device block `cnt` (layout: include/neuralsim_b200.h, nsb_query_counts),
 every buffer is allocated at a fixed CAPACITY and every kernel processes `min(capacity, *count)` items (nsb_bind_device_counts).
 Capacities: rays -> R (the chunk), boundary samples -> R (n_coarse + 1 + sum n_fine), marched / merged samples -> `march_cap`,
 samples kept by the compression -> `kept_cap`.  If a frame needs more than a capacity the step renders nothing and raises bit 0 / 1 of
@@ -22,8 +23,8 @@ import torch.nn.functional as F
 from .. import _lib as L
 from ..fields.fused_color import ColorQuery, SharedTableGrad, _FusedColor, color_net_c
 from ..fields.networks import sdf_bwd, sdf_decoder_c, sdf_fwd
+from .neus import query_config, upsample_boundary
 from .raysample import batch_sample_step_linear
-from .pack_ops import get_pack_infos_from_batch
 from . import neus_fused as NF
 
 __all__ = ["render_static", "StaticFrame", "CNT_SLOTS"]
@@ -157,18 +158,6 @@ def _fp16_images(model, radiance=True):
     return t, sdf_decoder_c(t[1:5], d), color_net_c(t[1:], d, b, model._nablas_fac()), ps
 
 
-def static_supported(model, cfg):
-    qp = dict(model.ray_query_cfg.get("query_param", {}) or {})
-    occ = getattr(getattr(model, "accel", None), "occ", None)
-    if cfg.get("with_rgb", True):
-        net_ok = getattr(model, "_color_fusable", lambda: False)() and model.use_view_dirs
-    else:                                                    # sdf / nablas only (or alpha only): the geometry-only colour query, if any
-        net_ok = getattr(model, "_geometry_fusable", lambda: False)()
-    return (net_ok and occ is not None and occ.occ_grid.dim() == 3
-            and occ.occ_grid.numel() * 4 // 32 <= 96 * 1024 and qp.get("num_coarse", 0) > 0 and len(qp.get("upsample_inv_s_factors", (1, 4, 16))) <= 4
-            and qp.get("coarse_step_cfg", {}).get("step_mode", "linear") == "linear")
-
-
 def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=None, march_cap, kept_cap, coherent=False, with_rgb=True, with_normal=True,
                   perturb=False, training=None, depth_use_normalized_vw=True, cnt=None):
     """One chunk of rays, ray test -> query -> integration, without a host read.  -> (rendered dict of whole-chunk images, cnt int64[32]).
@@ -182,20 +171,10 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
                            "use the host-sized path (SingleVolumeRenderer.render)")
     training = model.training if training is None else training
     R, dev = rays_o.shape[0], rays_o.device
-    qp = dict(model.ray_query_cfg.get("query_param", {}) or {})
-    nc1 = int(qp["num_coarse"]) + 1
-    factors = list(qp.get("upsample_inv_s_factors", (1, 4, 16)))
-    n_stage = len(factors)
-    num_fine = qp.get("num_fine", 8)
-    num_fine = [num_fine] * n_stage if isinstance(num_fine, int) else list(num_fine)
-    num_fine = [n // 2 * 2 + 1 for n in num_fine]
-    upsample_inv_s = qp.get("upsample_inv_s", 64.) / model.upsample_s_divisor
-    use_est = bool(qp.get("upsample_use_estimate_alpha", False))
-    nablas_has_grad = bool(qp.get("nablas_has_grad", False))
-    mc = dict(qp.get("march_cfg", {}))
-    fac = mc.pop("step_size_factor", 1.0)
-    step_size, dt_gamma = mc.get("step_size", 1e-3) * fac, mc.get("dt_gamma", 0.0) * fac
-    max_steps, max_step_size = int(mc.get("max_steps", 512)), mc.get("max_step_size", 1e10)
+    cfg = query_config(**(model.ray_query_cfg.get("query_param", {}) or {}), upsample_s_divisor=model.upsample_s_divisor)
+    if cfg.num_coarse <= 0:
+        raise RuntimeError("render_static: num_coarse=0 is not built (the boundary samples are the coarse and the fine ones)")
+    nc1, max_steps = cfg.num_coarse + 1, cfg.max_steps
     march_cap, kept_cap = int(march_cap), int(kept_cap)
     if cnt is None:
         cnt = torch.zeros(32, dtype=torch.int64, device=dev)
@@ -239,22 +218,22 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         bits = NF.pack_occ_bits(occ_grid)
         roi = torch.tensor([-1, -1, -1, 1, 1, 1], dtype=torch.float32, device=dev) if getattr(model, "_static_roi", None) is None else model._static_roi
         model._static_roi = roi
-        margs = NF.march_args(o_c, d_c, n_c, f_c, roi, occ_grid, step_size, max_step_size, dt_gamma, max_steps)
+        margs = NF.march_args(o_c, d_c, n_c, f_c, roi, occ_grid, cfg.step_size, cfg.max_step_size, cfg.dt_gamma, max_steps)
         num_steps = torch.empty(R, dtype=torch.int32, device=dev)
         # small batches: a march costs the latency of its longest ray -> march ONCE, recording the samples per ray, and copy (csrc/march.cu)
         rec_t = torch.empty(R * max_steps, dtype=torch.float32, device=dev) if march_onepass(R, max_steps) else None
         with L.KERNEL_TIMER.time("march", R):
             if rec_t is not None:
                 _call(lib.nsb_ray_marching_record, "ray_marching_record", cnt, CNT_SLOTS["n_rays"], None, L.c_i64(R), P(o_c, "f32"), P(d_c, "f32"), P(n_c, "f32"),
-                      P(f_c, "f32"), P(roi, "f32"), L.c_i32(res[0]), L.c_i32(res[1]), L.c_i32(res[2]), P(g8, "u8"), L.c_f32(step_size), L.c_f32(max_step_size),
-                      L.c_f32(dt_gamma), ctypes.c_uint32(max_steps), P(num_steps), P(rec_t), P(bits), L.stream_ptr())
+                      P(f_c, "f32"), P(roi, "f32"), L.c_i32(res[0]), L.c_i32(res[1]), L.c_i32(res[2]), P(g8, "u8"), L.c_f32(cfg.step_size), L.c_f32(cfg.max_step_size),
+                      L.c_f32(cfg.dt_gamma), ctypes.c_uint32(max_steps), P(num_steps), P(rec_t), P(bits), L.stream_ptr())
             else:
                 NF.march_listed(margs, bits, num_steps=num_steps, count=(cnt, CNT_SLOTS["n_rays"]))
         info2 = torch.empty(R, 2, dtype=torch.int32, device=dev)
         ridx_hit = torch.empty(R, dtype=torch.int64, device=dev)
         pack_infos = torch.empty(R, 2, dtype=torch.int64, device=dev)
         _scan(num_steps, cnt, CNT_SLOTS["marched_raw"], info2=info2, index=ridx_hit, pack=pack_infos, ws=st.ws[1])
-        _query_counts(cnt, 0, nc1, num_fine, march_cap, kept_cap)
+        _query_counts(cnt, 0, nc1, cfg.num_fine, march_cap, kept_cap)
         depth = torch.empty(march_cap, dtype=torch.float32, device=dev)
         ridx32 = torch.empty(march_cap, dtype=torch.int32, device=dev)
         with L.KERNEL_TIMER.time("march", R):
@@ -265,36 +244,19 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
                 NF.march_listed(margs, bits, info2=info2, t_starts=depth, ridx=ridx32, ray_list=ridx_hit, n_list=R, count=(cnt, CNT_SLOTS["hit"]))
         ridx = ridx32.long()
         # ---------------- up-sampling (no grad)
-        from . import neus as GN
-        hit = (cnt, CNT_SLOTS["hit"])
-        if GN.use_persistent_upsample(R):                    # ONE persistent per-ray kernel (csrc/ray_upsample.cu): small batches (graphics/neus.py)
-            fine_all, _ovf = NF.upsample_rays(st.meta, st.grid16, st.dec, ridx_hit, pack_infos, depth, o_c, d_c, [upsample_inv_s * f for f in factors], num_fine,
-                                              max_level=st.ml, max_steps=max_steps, use_estimate_alpha=use_est, collect=st.collect, count=hit)
-        else:
-            fine_stages = []
-            order_f = _block_order(rays_inds, ridx_hit, R, cnt, CNT_SLOTS["hit"]) if coherent and n_stage > 1 else None
-            sdf = torch.empty(march_cap, dtype=torch.float32, device=dev)
-            with L.KERNEL_TIMER.time("lotd_gather", march_cap):
-                sdf_fwd(st.meta, st.grid16, st.dec, sdf, st.ml, rays_o=o_c, rays_d=d_c, t=depth, ridx=ridx, collect=st.collect, count=(cnt, CNT_SLOTS["marched"]))
-            for i, factor in enumerate(factors):
-                cdf = NF.upsample_cdf(sdf, depth, pack_infos, upsample_inv_s * factor, use_est, count=hit)
-                nf = num_fine[i]
-                fine = NF.sample_cdf_uniform(depth, cdf, pack_infos, nf, count=hit)
-                fine_stages.append(fine)
-                if i < n_stage - 1:
-                    sdf_fine = torch.empty(R * nf, dtype=torch.float32, device=dev)
-                    with L.KERNEL_TIMER.time("lotd_gather", R * nf):
-                        if coherent:
-                            sdf_fwd(st.meta, st.grid16, st.dec, sdf_fine, st.ml, rays_o=o_c, rays_d=d_c, t=fine.view(-1),
-                                    packs=(get_pack_infos_from_batch(R, nf, device=dev), ridx_hit, order_f), collect=st.collect, count=hit)
-                        else:
-                            sdf_fwd(st.meta, st.grid16, st.dec, sdf_fine, st.ml, rays_o=o_c, rays_d=d_c, t=fine.view(-1),
-                                    ridx=ridx_hit.unsqueeze(-1).expand(R, nf).reshape(-1).contiguous(), collect=st.collect, count=(cnt, CNT_SLOTS["fine0"] + i))
-                    depth, sdf, pack_infos = NF.merge_sorted_vals(depth, sdf, pack_infos, fine, sdf_fine, n_out=march_cap, count=hit)
-            fine_all = (torch.cat(fine_stages, dim=-1) if n_stage > 1 else fine_stages[0]).contiguous()
+        def sdf_on_rays(ridx_, t, packs, count):
+            """the fused SDF query of the capacity-sized samples t (the counted ones are queried)"""
+            sdf = torch.empty(t.numel(), dtype=torch.float32, device=dev)
+            with L.KERNEL_TIMER.time("lotd_gather", t.numel()):
+                if packs is None and t.dim() == 2:
+                    ridx_ = ridx_.unsqueeze(-1).expand(t.shape).reshape(-1)
+                sdf_fwd(st.meta, st.grid16, st.dec, sdf, st.ml, rays_o=o_c, rays_d=d_c, t=t.view(-1), ridx=ridx_, packs=packs, collect=st.collect, count=count)
+            return sdf
         # the ray of every boundary sample: only the incoherent boundary query (one sample per row) reads it; everything else derives it
-        d1, _mid, ridx_all, pinfo = NF.assemble_boundary(coarse, ridx_hit, fine_all, num_fine, want_mid=False, want_ridx=not coherent,
-                                                         count=(cnt, CNT_SLOTS["n_rays"], CNT_SLOTS["hit"]))
+        d1, _mid, ridx_all, pinfo = upsample_boundary((ridx_hit, pack_infos, depth, ridx), o_c, d_c, coarse, cfg, sdf_on_rays,
+                                                      (lambda via: _block_order(rays_inds, via, R, cnt, CNT_SLOTS["hit"])) if coherent else None,
+                                                      table=(st.meta, st.grid16, st.dec, st.ml, st.collect), counts=(cnt, CNT_SLOTS), n_out=march_cap,
+                                                      want_mid=False, want_ridx=not coherent)
     # ---------------- boundary SDF (grad) -> alpha -> compression
     s = model.implicit_surface
     dl = s.decoder.layers
@@ -304,7 +266,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         inv_s = torch.tensor(float(inv_s), device=dev)
     alpha_k, t_k, ridx_k, pinfo_kept, rays_inds_hit = _StaticBoundary.apply(
         st, d1, pinfo, ridx_all, order_b, rays_inds, kept_cap,
-        (nc1, num_fine, march_cap, kept_cap), inv_s, table, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
+        (nc1, cfg.num_fine, march_cap, kept_cap), inv_s, table, dl[0].weight, dl[0].bias, dl[1].weight, dl[1].bias)
     # ---------------- colour / normal query on the kept samples (none when neither is rendered: depth and mask need alpha alone)
     rgb = nab = x = None
     if with_rgb or with_normal:
@@ -317,7 +279,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         out = _FusedColor.apply(q, ridx_k, t_k, view_dirs, ha_c, keep_acts, *params)
         nab, x = out[1], out[-1]
         rgb = out[2] if with_rgb else None
-        if not nablas_has_grad:
+        if not cfg.nablas_has_grad:
             nab = nab.detach()
     nab_i = nab if with_normal else None
     if nab_i is not None and not training:
@@ -391,10 +353,7 @@ class StaticFrame:
         r.train(self.model.training)
         out = r.ray_query(self.model, self.rays_o, self.rays_d, self.h_appear, return_buffer=True, return_details=True)
         det, vb = out.get("details", {}), out["volume_buffer"]
-        qp = dict(self.model.ray_query_cfg.get("query_param", {}) or {})
-        nf = qp.get("num_fine", 8)
-        nf = [nf] * len(qp.get("upsample_inv_s_factors", (1, 4, 16))) if isinstance(nf, int) else list(nf)
-        nf = [n // 2 * 2 + 1 for n in nf]
+        nf = query_config(**(self.model.ray_query_cfg.get("query_param", {}) or {}), upsample_s_divisor=self.model.upsample_s_divisor).num_fine
         M = int(det["march.num_per_ray"].sum()) if "march.num_per_ray" in det else 0
         n_hit = int(det["march.num_per_ray"].shape[0]) if "march.num_per_ray" in det else 0
         K = int(vb["t"].shape[0]) if vb.get("type") == "packed" else 0
