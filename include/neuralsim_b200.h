@@ -444,6 +444,19 @@ int nsb_fused_color_bwd(const nsb_lotd_meta *meta_host, const void *params_half,
                         const float *g_sdf, const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid, float *d_W1,
                         float *d_b1, float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2, float *d_R3,
                         float *d_rb3, void *stream);
+/* nsb_fused_color_bwd plus the gradient to the appearance codes h_appear[R, n_appear] of the forward (the reference's RadianceNet input
+ * columns after h, looked up per ray in single_volume_renderer.py:170-175, so autograd carries it back to the per-image codes):
+ * d_h_appear[ray_map[ridx[i]]] += sum over the points i of a ray of dL/dh_appear_i (ray_map NULL: row ridx[i]; ridx NULL: row i).
+ * g_rgb is required and the net must have n_appear >= 1.  ha_scratch[n, 8] fp32 workspace (the per-point rows).  The points of a ray
+ * must be consecutive (packed samples) for the sum to be deterministic: each ray's points are then summed by one warp in a fixed order
+ * and added once onto the caller's zeros.  Rays without a point are not written; with device counts, neither are points or rays past
+ * the count.  Everything else as nsb_fused_color_bwd, which computes the same bits in dh_scratch and the other outputs. */
+int nsb_fused_color_bwd_appear(const nsb_lotd_meta *meta_host, const void *params_half, const nsb_color_net *net_host, const float *x,
+                               const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, int64_t n, int32_t max_level,
+                               const void *act_z, const void *act_x, const void *act_y1, const void *act_y2, const float *rgb,
+                               const float *g_sdf, const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid, float *d_W1,
+                               float *d_b1, float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2, float *d_R3,
+                               float *d_rb3, float *ha_scratch, const int64_t *ray_map, float *d_h_appear, void *stream);
 
 /* ---------------------------------------------------------------- the persistent per-ray kernel (csrc/ray_upsample.cu)
  * The no-grad up-sampling half of neus_ray_query_march_occ_multi_upsample_compressed (neus_ray_query.py:861-905) for every hit ray as ONE

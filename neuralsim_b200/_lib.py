@@ -68,6 +68,8 @@ def lib():
         _lib.nsb_mc_count.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, f64, vp, vp, vp, vp, vp]
         _lib.nsb_mc_vertices.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, f64, vp, vp, vp, vp, vp, vp, vp]
         _lib.nsb_mc_triangles.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp, vp, i64, vp, vp]
+        # the colour backward with the appearance-code gradient: 8 pointers, n, max_level, 23 pointers (activations, cotangents, outputs), stream
+        _lib.nsb_fused_color_bwd_appear.argtypes = [vp] * 8 + [i64, i32] + [vp] * 23 + [vp]
     return _lib
 
 

@@ -354,14 +354,18 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 //   X3 += y2^T  . [1 gy3 0..]                (M64 N8  K128, MN-major): cols 1..3 = dR3^T
 // XA, XB and X3 are register fragments carried over all tiles of the persistent CTA; the dY1 ReLU mask runs on the dY1 fragments, and
 // dh goes from its fragments straight to global memory, so the kernel stages no fp32 rows (~104 KB of shared memory: 2 CTAs / SM).
+// kAppear adds the appearance-code gradient of every point (the codes are the radiance input's columns 54..54 + n_appear):
+//   da  = dZ1 . R1[:, h_appear]    (M128 N8 K64)     A = T block 1,                     B = R1a^T tile (1 KB more shared memory)
+// written from its fragments like dh, as rows of 8 floats (zero beyond n_appear); k_appear_ray_sum adds them up per ray.
 // The three saved activation tiles of a point tile (X, Y1, Y2: 3 x 16 KB, each contiguous in global memory and in shared memory) are
 // fetched by the bulk async copy engine (cp.async.bulk -> mbarrier), issued by one thread; the fetch of the NEXT tile starts as soon
 // as the last MMA that reads the current tiles has completed, so it overlaps the dh store and the next prologue.
+template <bool kAppear>
 __global__ void __launch_bounds__(kTile, kColorBwdCtasPerSM)
 k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uint8_t *__restrict__ Y1t, const uint8_t *__restrict__ Y2t,
                 const float *__restrict__ rgb, const float *__restrict__ g_rgb, int64_t n, float *__restrict__ dh_out,
                 float *__restrict__ dR1, float *__restrict__ drb1, float *__restrict__ dR2, float *__restrict__ drb2,
-                float *__restrict__ dR3, float *__restrict__ drb3, const int64_t *__restrict__ n_dev) {
+                float *__restrict__ dR3, float *__restrict__ drb3, const int64_t *__restrict__ n_dev, float *__restrict__ da_out) {
     n = eff_n(n, n_dev);
     constexpr int NE = 80;                                     // 64 columns + the [1, gy3, 0..] chunk + a zero chunk (N % 16 == 0)
     extern __shared__ uint8_t dyn_smem[];
@@ -371,6 +375,7 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     uint8_t *sXe = sY1 + kTile * NE * 2;                       // 20 KB [X | 1 gy3 | 0]
     uint8_t *sR2T = sXe + kTile * NE * 2;                      //  8 KB (N = in i, K = out j) = R2[j][i]
     uint8_t *sR1h = sR2T + XW * XW * 2;                        //  4 KB (N = h column k, K = out j) = R1[j][22 + k], zero for k >= 2L
+    uint8_t *sR1a = sR1h + NF * XW * 2;                        //  1 KB (kAppear; N = code column k, K = out j) = R1[j][22 + 2L + k], zero for k >= n_appear
     __shared__ float sR3[3][XW];
     __shared__ float sdb3[3];
     __shared__ __align__(8) uint64_t mbar_ld;
@@ -385,6 +390,13 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         const int k = e % NF, j = e / NF;
         const __half v = (j < net.rw && k < net.dec.nh) ? net.R1[j * net.rin + 22 + k] : __float2half_rn(0.f);
         *reinterpret_cast<__half *>(sR1h + (j / 8) * (NF * 16) + k * 16 + (j % 8) * 2) = v;
+    }
+    if constexpr (kAppear) {
+        for (int e = tid; e < 8 * XW; e += kTile) {
+            const int k = e % 8, j = e / 8;
+            const __half v = (j < net.rw && k < net.n_appear) ? net.R1[j * net.rin + 22 + net.dec.nh + k] : __float2half_rn(0.f);
+            *reinterpret_cast<__half *>(sR1a + (j / 8) * (8 * 16) + k * 16 + (j % 8) * 2) = v;
+        }
     }
     if (tid < XW) {
 #pragma unroll
@@ -472,6 +484,9 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         __syncthreads();
         float dh[2][NF / 2];
         tc::mma_m128<32, 0, 0, XW / 16>(dh, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(r1h_addr, NF), false);   // dh = dZ1 . R1[:, h]
+        float da[2][4];
+        if constexpr (kAppear)
+            tc::mma_m128<8, 0, 0, XW / 16>(da, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(tc::smem_u32(sR1a), 8), false);   // da = dZ1 . R1[:, h_appear]
         // weight gradients: contract over the 128 points
         tc::mma_m64<NE, 1, 1, kTile / 16>(xa, tc::mnmajor(t_addr, kTile), tc::mnmajor(y1_addr, kTile), true);
         tc::mma_m64<NE, 1, 1, kTile / 16>(xb, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(xe_addr, kTile), true);
@@ -495,6 +510,7 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
 #pragma unroll
                     for (int c = 0; c < NF / 8; ++c)
                         *reinterpret_cast<float2 *>(dh_out + row * NF + tc::frag_col(c)) = make_float2(dh[h][4 * c + 2 * r], dh[h][4 * c + 2 * r + 1]);
+                    if constexpr (kAppear) *reinterpret_cast<float2 *>(da_out + row * 8 + tc::frag_col(0)) = make_float2(da[h][2 * r], da[h][2 * r + 1]);
                 }
             }
     }
@@ -525,6 +541,52 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
             }
         }
         if (tid < 3) atomicAdd(drb3 + tid, sdb3[tid]);
+    }
+}
+
+// Per-ray sum of the appearance-code gradients k_color_rad_bwd<true> wrote per point (rows of 8 floats).  The points of a ray are
+// consecutive (packed samples), so a ray is a run of equal ridx.  A warp looks at 32 points; for each run that starts among them, in
+// order, the whole warp walks the run 32 points at a time (lane l adds points start + l, start + l + 32, ...; the run ends at the first
+// point of another ray), reduces the lanes' sums by a fixed butterfly and adds the result once to row ray_map[ray] (ray_map NULL: row
+// ray) of d_h_appear [., n_appear].  One add per ray onto the caller's zeros in an order fixed by the run's position: the same bits on
+// every run.  (A ray whose points form several runs -- unsorted ridx -- gets one atomic add per run.)
+__global__ void __launch_bounds__(256)
+k_appear_ray_sum(const float *__restrict__ rows, const int64_t *__restrict__ ridx, int64_t n, int n_appear, const int64_t *__restrict__ ray_map,
+                 float *__restrict__ d_h_appear, const int64_t *__restrict__ n_dev) {
+    n = eff_n(n, n_dev);
+    const int lane = threadIdx.x & 31;
+    const int64_t n_warps = (int64_t)gridDim.x * (blockDim.x / 32);
+    for (int64_t w = blockIdx.x * (int64_t)(blockDim.x / 32) + threadIdx.x / 32; w * 32 < n; w += n_warps) {   // warp-uniform
+        const int64_t i = w * 32 + lane;
+        const int64_t ray = i < n ? (ridx ? ridx[i] : i) : -1;
+        uint32_t heads = __ballot_sync(~0u, i < n && (!ridx || i == 0 || ridx[i - 1] != ray));
+        while (heads) {
+            const int src = __ffs(heads) - 1;
+            heads &= heads - 1;
+            const int64_t r = __shfl_sync(~0u, ray, src);
+            float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            for (int64_t base = w * 32 + src;; base += 32) {
+                const int64_t j = base + lane;
+                const bool same = j < n && (ridx ? ridx[j] == r : j == base);
+                const uint32_t stop = ~__ballot_sync(~0u, same);
+                const int end = stop ? __ffs(stop) - 1 : 32;        // the run continues in lanes [0, end) of this block
+                if (lane < end) {
+                    const float4 a = *reinterpret_cast<const float4 *>(rows + j * 8), b = *reinterpret_cast<const float4 *>(rows + j * 8 + 4);
+                    acc[0] += a.x; acc[1] += a.y; acc[2] += a.z; acc[3] += a.w; acc[4] += b.x; acc[5] += b.y; acc[6] += b.z; acc[7] += b.w;
+                }
+                if (end < 32) break;
+            }
+#pragma unroll
+            for (int k = 0; k < 8; ++k)
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1) acc[k] += __shfl_xor_sync(~0u, acc[k], off);
+            if (lane < n_appear) {
+                float v = acc[0];
+#pragma unroll
+                for (int k = 1; k < 8; ++k) v = lane == k ? acc[k] : v;
+                atomicAdd(d_h_appear + (ray_map ? ray_map[r] : r) * n_appear + lane, v);
+            }
+        }
     }
 }
 
@@ -832,35 +894,43 @@ extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params
     return check_launch("nsb_fused_color_fwd");
 }
 
-extern "C" int nsb_fused_color_bwd(const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x, const float *rays_o,
-                                   const float *rays_d, const int64_t *ridx, const float *t, int64_t n, int32_t max_level, const void *act_z,
-                                   const void *act_x, const void *act_y1, const void *act_y2, const float *rgb, const float *g_sdf,
-                                   const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid, float *d_W1, float *d_b1,
-                                   float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2, float *d_R3, float *d_rb3,
-                                   void *stream) {
+// the two backward kernels (k_color_rad_bwd<kAppear> only with g_rgb), then with kAppear the per-ray sum of the code gradients
+template <bool kAppear>
+static int color_bwd(const char *who, const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x, const float *rays_o,
+                     const float *rays_d, const int64_t *ridx, const float *t, int64_t n, int32_t max_level, const void *act_z, const void *act_x,
+                     const void *act_y1, const void *act_y2, const float *rgb, const float *g_sdf, const float *g_nablas, const float *g_rgb,
+                     float *dh_scratch, float *d_grid, float *d_W1, float *d_b1, float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2,
+                     float *d_rb2, float *d_R3, float *d_rb3, float *ha_scratch, const int64_t *ray_map, float *d_h_appear, void *stream) {
     const DevCounts dn = take_counts();
     if (n == 0) return 0;
-    NSB_REQUIRE(meta && params_half && net && act_z && act_x, "nsb_fused_color_bwd: NULL argument");
-    NSB_REQUIRE(d_grid && d_W1 && d_b1 && d_W2 && d_b2, "nsb_fused_color_bwd: NULL gradient buffer");
+    NSB_REQUIRE(meta && params_half && net && act_z && act_x, "%s: NULL argument", who);
+    NSB_REQUIRE(d_grid && d_W1 && d_b1 && d_W2 && d_b2, "%s: NULL gradient buffer", who);
     if (g_rgb) {                                               // the radiance backward's inputs and outputs
-        NSB_REQUIRE(act_y1 && act_y2 && rgb && dh_scratch, "nsb_fused_color_bwd: NULL argument (g_rgb given)");
-        NSB_REQUIRE(d_R1 && d_rb1 && d_R2 && d_rb2 && d_R3 && d_rb3, "nsb_fused_color_bwd: NULL radiance gradient buffer (g_rgb given)");
+        NSB_REQUIRE(act_y1 && act_y2 && rgb && dh_scratch, "%s: NULL argument (g_rgb given)", who);
+        NSB_REQUIRE(d_R1 && d_rb1 && d_R2 && d_rb2 && d_R3 && d_rb3, "%s: NULL radiance gradient buffer (g_rgb given)", who);
     }
-    NSB_REQUIRE(x || (rays_o && rays_d && t), "nsb_fused_color_bwd: need x or (rays_o, rays_d, t)");
+    if (kAppear) NSB_REQUIRE(g_rgb && ha_scratch && d_h_appear, "%s: needs g_rgb, ha_scratch and d_h_appear", who);
+    NSB_REQUIRE(x || (rays_o && rays_d && t), "%s: need x or (rays_o, rays_d, t)", who);
     PLMeta m;
     ColorNetDev d;
-    if (int rc = make_net(net, meta, &m, &d, "nsb_fused_color_bwd", g_rgb != nullptr)) return rc;
+    if (int rc = make_net(net, meta, &m, &d, who, g_rgb != nullptr)) return rc;
+    if (kAppear) NSB_REQUIRE(d.n_appear >= 1, "%s: the net has no appearance channels", who);
     cudaStream_t s = (cudaStream_t)stream;
     const float *dh = nullptr;
     if (g_rgb) {
-        constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + 1024;   // 101 KB
-        opt_in_smem(k_color_rad_bwd, kSmemR);
-        if (int rc = require_ctas_per_sm(k_color_rad_bwd, kTile, kSmemR, kColorBwdCtasPerSM, "nsb_fused_color_bwd(radiance)")) return rc;
-        k_color_rad_bwd<<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemR, s>>>(d, (const uint8_t *)act_x, (const uint8_t *)act_y1,
-                                                                                               (const uint8_t *)act_y2, rgb, g_rgb, n, dh_scratch, d_R1,
-                                                                                               d_rb1, d_R2, d_rb2, d_R3, d_rb3, dn.a);
+        constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + (kAppear ? 8 * XW * 2 : 0) + 1024;   // 101 (102) KB
+        opt_in_smem(k_color_rad_bwd<kAppear>, kSmemR);
+        if (int rc = require_ctas_per_sm(k_color_rad_bwd<kAppear>, kTile, kSmemR, kColorBwdCtasPerSM, "nsb_fused_color_bwd(radiance)")) return rc;
+        k_color_rad_bwd<kAppear><<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemR, s>>>(
+            d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n, dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3,
+            dn.a, ha_scratch);
         if (int rc = check_launch("nsb_fused_color_bwd(radiance)")) return rc;
         dh = dh_scratch;
+        if (kAppear) {
+            const int64_t blocks = (n + 255) / 256;                    // 8 warps of 32 points per block
+            k_appear_ray_sum<<<(unsigned)(blocks < (1 << 20) ? blocks : (1 << 20)), 256, 0, s>>>(ha_scratch, ridx, n, d.n_appear, ray_map, d_h_appear, dn.a);
+            if (int rc = check_launch("nsb_fused_color_bwd_appear(ray sum)")) return rc;
+        }
     }
     constexpr int kSmemS = 3 * kTileBytes + 2 * kTile * 48 * 2 + 2 * HW * NF * 2 + kTileBytes + 1024;   // 97 KB
     opt_in_smem(k_color_sdf_bwd, kSmemS);
@@ -869,4 +939,26 @@ extern "C" int nsb_fused_color_bwd(const nsb_lotd_meta *meta, const void *params
     k_color_sdf_bwd<<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
                                                                           g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level, d_grid, d_W1, d_b1, d_W2, d_b2, dn.a);
     return check_launch("nsb_fused_color_bwd(sdf)");
+}
+
+extern "C" int nsb_fused_color_bwd(const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x, const float *rays_o,
+                                   const float *rays_d, const int64_t *ridx, const float *t, int64_t n, int32_t max_level, const void *act_z,
+                                   const void *act_x, const void *act_y1, const void *act_y2, const float *rgb, const float *g_sdf,
+                                   const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid, float *d_W1, float *d_b1,
+                                   float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2, float *d_R3, float *d_rb3,
+                                   void *stream) {
+    return color_bwd<false>("nsb_fused_color_bwd", meta, params_half, net, x, rays_o, rays_d, ridx, t, n, max_level, act_z, act_x, act_y1, act_y2, rgb,
+                            g_sdf, g_nablas, g_rgb, dh_scratch, d_grid, d_W1, d_b1, d_W2, d_b2, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, nullptr, nullptr,
+                            nullptr, stream);
+}
+
+extern "C" int nsb_fused_color_bwd_appear(const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x,
+                                          const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, int64_t n, int32_t max_level,
+                                          const void *act_z, const void *act_x, const void *act_y1, const void *act_y2, const float *rgb,
+                                          const float *g_sdf, const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid,
+                                          float *d_W1, float *d_b1, float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2,
+                                          float *d_R3, float *d_rb3, float *ha_scratch, const int64_t *ray_map, float *d_h_appear, void *stream) {
+    return color_bwd<true>("nsb_fused_color_bwd_appear", meta, params_half, net, x, rays_o, rays_d, ridx, t, n, max_level, act_z, act_x, act_y1, act_y2,
+                           rgb, g_sdf, g_nablas, g_rgb, dh_scratch, d_grid, d_W1, d_b1, d_W2, d_b2, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, ha_scratch,
+                           ray_map, d_h_appear, stream);
 }

@@ -3,7 +3,7 @@
 `fused_color(model, ridx, t, rays_o, rays_d, view_dirs, h_appear)` computes, for the packed samples x = o[ridx] + d[ridx] t,
 what `LoTDNeuS.forward(x, v=, h_appear=, nablas_has_grad=True)` computes in the reference
 (nr3d_lib/models/fields/neus/lotd_neus.py:141-167): sdf, nablas (analytic, differentiable -> second-order table / decoder
-gradients) and rgb.  The unfused module path (`LoTDNeuS.forward`) stays the specification the tests compare against.
+gradients) and rgb; appearance codes that require grad get their gradient (summed over each ray's samples).  The unfused module path (`LoTDNeuS.forward`) stays the specification the tests compare against.
 With `with_rgb=False` it is `forward_sdf_nablas` alone (k_color_fwd<false>: no radiance head runs, two activation tiles are kept instead of
 four, and only the table and the decoder are inputs of the op), for models without a radiance net and for rays that render no rgb.
 """
@@ -68,14 +68,16 @@ class _TableGradSink(autograd.Function):
 
 class ColorQuery:
     """what the forward and backward launches of one colour query share: the table's meta and fp16 image, the net struct and the fp16
-    tensors it points at, the rays, max level, the occupancy collection, the device count (_lib.call's count=, None: host-sized) and
-    the step's shared table gradient (a SharedTableGrad, None: the backward fills its own)"""
-    __slots__ = ("meta", "grid16", "net", "held", "rays_o", "rays_d", "ml", "collect", "count", "table_grad")
+    tensors it points at, the rays, max level, the occupancy collection, the device count (_lib.call's count=, None: host-sized),
+    the step's shared table gradient (a SharedTableGrad, None: the backward fills its own) and the step's appearance-code gradient
+    (None, or (d_h_appear, ray_map): the backward adds the code gradient of ray r into d_h_appear[ray_map[r]], which the caller
+    zero-fills -- for codes that are not an autograd input of the op, as in the one-launch step)"""
+    __slots__ = ("meta", "grid16", "net", "held", "rays_o", "rays_d", "ml", "collect", "count", "table_grad", "appear_grad")
 
-    def __init__(self, meta, grid16, net, held, rays_o, rays_d, ml, collect, count, table_grad=None):
+    def __init__(self, meta, grid16, net, held, rays_o, rays_d, ml, collect, count, table_grad=None, appear_grad=None):
         self.meta, self.grid16, self.net, self.held = meta, grid16, net, held
         self.rays_o, self.rays_d, self.ml, self.collect, self.count = rays_o, rays_d, ml, collect, count
-        self.table_grad = table_grad
+        self.table_grad, self.appear_grad = table_grad, appear_grad
 
 
 class _FusedColor(autograd.Function):
@@ -101,6 +103,7 @@ class _FusedColor(autograd.Function):
                    L.c_i64(n), L.c_i32(q.ml), P(sdf), P(nab), P(rgb, allow_none=not rad), P(x), *ap,
                    ctypes.byref(q.collect) if q.collect is not None else None, L.stream_ptr(), count=q.count)
         ctx.q, ctx.ridx, ctx.t, ctx.n, ctx.rad = q, ridx, t, n, rad
+        ctx.ha_shape = h_appear.shape if h_appear is not None else None
         ctx.held = (acts, rgb)
         ctx.shapes = [p.shape for p in params]
         ctx.set_materialize_grads(False)
@@ -126,7 +129,10 @@ class _FusedColor(autograd.Function):
         for sh, k in zip(ctx.shapes[1:], sizes):
             grads.append(small[o:o + k].view(sh))
             o += k
-        ret = (None,) * 6 + ((d_grid if q.table_grad is None else None),) + tuple(grads[1:])
+        # the code gradient: of the op's h_appear input, or into the step's buffer (ColorQuery.appear_grad)
+        d_ha = torch.zeros(ctx.ha_shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[4] else None
+        appear = (d_ha, None) if d_ha is not None else q.appear_grad
+        ret = (None,) * 4 + (d_ha, None, (d_grid if q.table_grad is None else None)) + tuple(grads[1:])
         if g_sdf is None and g_nab is None and g_rgb is None:
             return ret
         c = lambda g: None if g is None else g.contiguous().float()
@@ -134,17 +140,23 @@ class _FusedColor(autograd.Function):
         dh = torch.empty(n, 32, dtype=torch.float32, device=dev) if g_rgb is not None else None
         P = L.ptr
         ag = [P(g) for g in grads] + [None] * (11 - len(grads))          # d_R* / d_rb*: NULL without the radiance net's parameters
+        args = (q.meta.c_ref, P(q.grid16, "f16"), ctypes.byref(q.net), None, P(q.rays_o, "f32"), P(q.rays_d, "f32"), P(ctx.ridx, "i64"), P(ctx.t, "f32"),
+                L.c_i64(n), L.c_i32(q.ml), P(acts[0]), P(acts[1]), *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]), P(rgb, allow_none=True),
+                P(g_sdf, allow_none=True), P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh, allow_none=True), *ag)
         with L.KERNEL_TIMER.time("fused_color_bwd", n):
-            L.call(L.lib().nsb_fused_color_bwd, "fused_color_bwd", q.meta.c_ref, P(q.grid16, "f16"), ctypes.byref(q.net), None, P(q.rays_o, "f32"),
-                   P(q.rays_d, "f32"), P(ctx.ridx, "i64"), P(ctx.t, "f32"), L.c_i64(n), L.c_i32(q.ml), P(acts[0]), P(acts[1]),
-                   *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]), P(rgb, allow_none=True), P(g_sdf, allow_none=True),
-                   P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh, allow_none=True), *ag, L.stream_ptr(), count=q.count)
+            if appear is not None and g_rgb is not None:
+                ha_rows = torch.empty(n, 8, dtype=torch.float32, device=dev)        # per-sample code gradients, summed per ray in the call
+                L.call(L.lib().nsb_fused_color_bwd_appear, "fused_color_bwd_appear", *args, P(ha_rows), P(appear[1], "i64", allow_none=True),
+                       P(appear[0], "f32"), L.stream_ptr(), count=q.count)
+            else:
+                L.call(L.lib().nsb_fused_color_bwd, "fused_color_bwd", *args, L.stream_ptr(), count=q.count)
         return ret
 
 
 def fused_color(model, ridx, t, rays_o, rays_d, view_dirs=None, h_appear=None, *, nablas_has_grad=True, collect=None, with_rgb=True):
     """-> dict(sdf [n], nablas [n,3], rgb [n,3] (with_rgb only), x [n,3]).  Gradients flow to the table and the decoder, and with rgb to the
-    radiance net."""
+    radiance net and to h_appear [R, n_appear] if it requires grad (the samples of a ray must then be consecutive, as packed samples are,
+    for the per-ray sum to be deterministic)."""
     s = model.implicit_surface
     d = s.decoder.layers
     params = (s.encoding.flattened_params, d[0].weight, d[0].bias, d[1].weight, d[1].bias)
@@ -154,8 +166,8 @@ def fused_color(model, ridx, t, rays_o, rays_d, view_dirs=None, h_appear=None, *
     grid16, net, held = model._fused_color_state() if with_rgb else model._fused_geometry_state()
     q = ColorQuery(s.encoding.meta, grid16, net, held, rays_o.detach().contiguous().float(), rays_d.detach().contiguous().float(), s._ml(model.max_level),
                    collect, None)
-    keep = torch.is_grad_enabled() and any(p.requires_grad for p in params)
-    ha = None if (h_appear is None or not with_rgb) else h_appear.detach().contiguous().float()
+    ha = None if (h_appear is None or not with_rgb) else h_appear.contiguous().float()
+    keep = torch.is_grad_enabled() and (any(p.requires_grad for p in params) or (ha is not None and ha.requires_grad))
     vd = view_dirs.detach().contiguous().float() if with_rgb else None
     out = _FusedColor.apply(q, ridx.reshape(-1).contiguous().long(), t.detach().reshape(-1).contiguous().float(), vd, ha, keep, *params)
     sdf, nab, x = out[0], out[1], out[-1]

@@ -50,7 +50,10 @@ class AABBSpace(nn.Module):
         """Slab test against the unit cube -> dict(num_rays, rays_inds, near, far, rays_o, rays_d, **extras) of the hit rays."""
         if (FUSED_RAY_TEST and rays_o.is_cuda and rays_o.dim() == 2 and rays_o.dtype == torch.float32 and rays_d.dtype == torch.float32 and return_rays
                 and not rays_o.requires_grad and not rays_d.requires_grad and not isinstance(near, torch.Tensor) and not isinstance(far, torch.Tensor)):
-            return self._ray_test_fused(rays_o, rays_d, near, far, normalized, extra_ray_data)
+            ret = self._ray_test_fused(rays_o, rays_d, near, far, normalized, extra_ray_data)
+            # per-ray data that requires grad (learnable appearance codes) is indexed here, outside the test's no_grad, so autograd reaches it
+            ret.update({k: v[ret["rays_inds"]] for k, v in extra_ray_data.items() if isinstance(v, torch.Tensor) and v.requires_grad})
+            return ret
         if not normalized:
             rays_o, rays_d = self.normalize_rays(rays_o, rays_d)
         with torch.no_grad():
@@ -98,7 +101,8 @@ class AABBSpace(nn.Module):
         ex_c = torch.empty(n, ex.shape[1], device=dev) if ex is not None else None
         NF.gather_rays(ridx, n, tested[:4], (o_c, d_c, n_c, f_c), ex, ex_c)
         ret = dict(num_rays=n, rays_inds=ridx, near=n_c, far=f_c)
-        ret.update({k: (ex_c if k == fused_key else (v[ridx] if isinstance(v, torch.Tensor) else v)) for k, v in extra_ray_data.items()})
+        ret.update({k: (ex_c if k == fused_key else (v[ridx] if isinstance(v, torch.Tensor) else v)) for k, v in extra_ray_data.items()
+                    if not (isinstance(v, torch.Tensor) and v.requires_grad)})                # those: ray_test, with grad
         ret.update(rays_o=o_c, rays_d=d_c)
         # image-ordered rays (>= 3/4 of the rays neighbour their predecessor): the queries traverse samples ray-tiled (csrc/fused_tc.cu)
         ret["rays_coherent"] = R > 64 and sc["extra"][0] >= 0.75 * (R - 1)

@@ -244,8 +244,8 @@ def _net_forward_into(volume_buffer, model, rays_o, rays_d, view_dirs, rays_h_ap
         volume_buffer["net_x"] = out["x"]
         volume_buffer["nablas"] = out["nablas"].to(dtype)
         return
-    if (fused and with_rgb and view_dirs is not None and getattr(model, "_color_fusable", lambda: False)()
-            and not (rays_h_appear is not None and rays_h_appear.requires_grad) and not view_dirs.requires_grad):
+    # appearance codes that require grad (per-image codes in training) get their gradient from the fused op; view directions do not
+    if (fused and with_rgb and view_dirs is not None and getattr(model, "_color_fusable", lambda: False)() and not view_dirs.requires_grad):
         out = model.forward_on_rays(ridx_all, depths, rays_o, rays_d, view_dirs, rays_h_appear, nablas_has_grad=nablas_has_grad)
         volume_buffer["net_x"] = out["x"]
         volume_buffer["nablas"] = out["nablas"].to(dtype)

@@ -159,10 +159,11 @@ def _fp16_images(model, radiance=True):
 
 
 def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=None, march_cap, kept_cap, coherent=False, with_rgb=True, with_normal=True,
-                  perturb=False, training=None, depth_use_normalized_vw=True, cnt=None):
+                  perturb=False, training=None, depth_use_normalized_vw=True, cnt=None, d_h_appear=None):
     """One chunk of rays, ray test -> query -> integration, without a host read.  -> (rendered dict of whole-chunk images, cnt int64[32]).
     `coherent`: image-ordered rays (the boundary / fine queries then walk the samples ray-tiled) -- a host decision here (the host-sized
-    path measures it in the ray-test kernel)."""
+    path measures it in the ray-test kernel).  `d_h_appear` [R, n_appear] (optional): zero-filled here, and the backward pass writes the
+    gradient of the codes rays_h_appear into it, in the caller's ray order (the codes themselves are read detached)."""
     P, lib = L.ptr, L.lib()
     if with_rgb and getattr(model, "radiance_net", None) is None:
         raise RuntimeError("render_static(with_rgb=True): the model has no radiance net (radiance_cfg=False); render it with with_rgb=False")
@@ -207,6 +208,10 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         o_c, d_c = rbuf[:3 * R].view(R, 3), rbuf[3 * R:6 * R].view(R, 3)
         n_c, f_c = rbuf[6 * R:7 * R], rbuf[7 * R:8 * R]
         ha_c = rbuf[8 * R:].view(R, n_ha) if ha is not None else None
+        if d_h_appear is not None:
+            if ha is None:
+                raise RuntimeError("render_static(d_h_appear=...): the colour query reads no appearance codes (with_rgb=False or a model without them)")
+            d_h_appear.zero_()                              # the backward adds each kept ray's sum once into its row
         NF.gather_rays(rays_inds, R, tested[:4], (o_c, d_c, n_c, f_c), ha, ha_c, count=(cnt, CNT_SLOTS["n_rays"]))
         st.rays_o, st.rays_d = o_c, d_c
         view_dirs = (d_c / d_c.norm(dim=-1).clamp_min(1.0e-10).unsqueeze(-1)).contiguous() if with_rgb else None
@@ -274,8 +279,10 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         if with_rgb:
             b = model.radiance_net.blocks.layers
             params += (b[0].weight, b[0].bias, b[1].weight, b[1].bias, b[2].weight, b[2].bias)
-        keep_acts = torch.is_grad_enabled() and any(p.requires_grad for p in params)
-        q = ColorQuery(st.meta, st.grid16, st.net, st.held, st.rays_o, st.rays_d, st.ml, st.collect, (cnt, CNT_SLOTS["kept"]), st.table_grad)
+        keep_acts = torch.is_grad_enabled() and (any(p.requires_grad for p in params) or d_h_appear is not None)
+        # the code gradient of the compacted ray r goes to row rays_inds[r] of d_h_appear (the kernels stop at the device counts)
+        q = ColorQuery(st.meta, st.grid16, st.net, st.held, st.rays_o, st.rays_d, st.ml, st.collect, (cnt, CNT_SLOTS["kept"]), st.table_grad,
+                       (d_h_appear, rays_inds) if d_h_appear is not None else None)
         out = _FusedColor.apply(q, ridx_k, t_k, view_dirs, ha_c, keep_acts, *params)
         nab, x = out[1], out[-1]
         rgb = out[2] if with_rgb else None
@@ -321,13 +328,18 @@ class StaticFrame:
         frame.rendered["rgb_volume"], p.grad                    # static outputs / accumulated gradients
         frame.check()                                           # optional: one D2H of the counts; re-captures with larger arenas on overflow
 
+    `h_appear_grad=True` (off by default: the graph is fixed at capture, and the step does a little more work): every step also writes
+    `frame.d_h_appear` [n_rays, n_appear], the gradient of the loss with respect to the rays' appearance codes in the order they were
+    passed (rows of rays that keep no sample are 0; each step overwrites it).  The codes are inputs the caller copies in, so the caller
+    applies it to its own codes, e.g. `codes.backward(frame.d_h_appear)`.
+
     The first call probes the sizes with the host-sized path (SingleVolumeRenderer.ray_query, no grad), sizes the arenas with `slack`,
     warms up and captures.  Gradients are accumulated into `p.grad` (kept in place; `zero_grads=True` or a `pre_hook` zeroes them inside the graph).
     Capture precondition (PyTorch): no autograd graph of an EARLIER backward on the default stream may still be referenced (a kept loss / rendered
     tensor): it pins the parameters' AccumulateGrad nodes to the default stream, which cannot take part in a capture."""
 
     def __init__(self, model, n_rays, loss_fn=None, *, near=None, far=None, with_rgb=True, with_normal=True, slack=1.5, march_cap=None, kept_cap=None,
-                 coherent=None, use_graph=True, zero_grads=False, h_appear_dim=None, pre_hook=None):
+                 coherent=None, use_graph=True, zero_grads=False, h_appear_dim=None, pre_hook=None, h_appear_grad=False):
         self.model, self.n_rays, self.loss_fn = model, int(n_rays), loss_fn
         self.near, self.far, self.with_rgb, self.with_normal, self.slack = near, far, with_rgb, with_normal, float(slack)
         self.march_cap, self.kept_cap, self.coherent = march_cap, kept_cap, coherent
@@ -340,6 +352,9 @@ class StaticFrame:
         na = h_appear_dim if h_appear_dim is not None else (
             model.radiance_net.blocks.layers[0].in_features - 22 - model.implicit_surface.encoding.out_features if model.use_h_appear else 0)
         self.h_appear = torch.zeros(self.n_rays, na, device=dev) if na > 0 else None
+        if h_appear_grad and (self.h_appear is None or not with_rgb or not model.use_h_appear):
+            raise RuntimeError("StaticFrame(h_appear_grad=True): the step renders no rgb from appearance codes")
+        self.d_h_appear = torch.zeros(self.n_rays, na, device=dev) if h_appear_grad else None
         self.cnt = torch.zeros(32, dtype=torch.int64, device=dev)
         self.graph, self.loss, self.rendered, self.buffers, self._occ_captured = None, None, None, None, None
         self.captures = 0
@@ -384,7 +399,8 @@ class StaticFrame:
             cv._use_w_dev = True                             # inv_s annealing weight from a device scalar (refreshed in step())
         try:
             rendered, _, buffers = render_static(self.model, self.rays_o, self.rays_d, self.h_appear, near=self.near, far=self.far, march_cap=self.march_cap,
-                                                 kept_cap=self.kept_cap, coherent=bool(self.coherent), with_rgb=self.with_rgb, with_normal=self.with_normal, cnt=self.cnt)
+                                                 kept_cap=self.kept_cap, coherent=bool(self.coherent), with_rgb=self.with_rgb, with_normal=self.with_normal, cnt=self.cnt,
+                                                 d_h_appear=self.d_h_appear)
         finally:
             if cv is not None:
                 cv._use_w_dev = False
