@@ -268,6 +268,19 @@ int nsb_fused_sdf_bwd_indexed(const nsb_lotd_meta *meta_host, const void *params
                               const float *d_sdf, const int64_t *keep, int64_t n, int32_t max_level, float *d_grid, float *d_W1,
                               float *d_b1, float *d_W2, float *d_b2, void *stream);
 
+/* nsb_fused_sdf_bwd_indexed on samples of rays, plus the gradient to the rays.  The depths t are constants (the reference computes them
+ * without grad) and the encoding's input gradient is first order (its input Hessian is not formed on the reference's hot path), so
+ * sample x = o + d t gets g_x = (1/2) sum over levels of J^T dL/dh (at the point the table clamps x / 2 + 1/2 to, unmasked), and
+ *   d_rays_o[ray_map[r]] += sum over the samples s of ray r of g_x(s),   d_rays_d[ray_map[r]] += sum of t_s g_x(s)
+ * (ray_map NULL: row r; a NULL output is not written).  gx_scratch[n, 8] fp32 workspace (one row per launch row).  The samples of a ray must
+ * be consecutive (packed samples) for the sums to be deterministic: each ray's samples are summed by one warp in a fixed order and added
+ * once onto the caller's zeros.  Rays without a sample are not written; with device counts, neither are rows or rays past the count.
+ * Table and decoder gradients: the same bits as nsb_fused_sdf_bwd_indexed. */
+int nsb_fused_sdf_bwd_rays(const nsb_lotd_meta *meta_host, const void *params_half, const nsb_sdf_decoder *dec_host, const float *rays_o,
+                           const float *rays_d, const int64_t *ridx, const float *t, const float *d_sdf, const int64_t *keep, int64_t n,
+                           int32_t max_level, float *d_grid, float *d_W1, float *d_b1, float *d_W2, float *d_b2, float *gx_scratch,
+                           const int64_t *ray_map, float *d_rays_o, float *d_rays_d, void *stream);
+
 /* ---------------------------------------------------------------- device-resident sizes (a step without host reads)
  * The reference reads every data-dependent size back to the host (`.item()`, `nonzero()`: ~25 syncs per ray_query, SURVEY.md §8a a9).
  * Here a size may stay in device memory: nsb_bind_device_counts(c0, c1) binds one or two device int64 to the calling thread; the NEXT
@@ -457,6 +470,25 @@ int nsb_fused_color_bwd_appear(const nsb_lotd_meta *meta_host, const void *param
                                const float *g_sdf, const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid, float *d_W1,
                                float *d_b1, float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2, float *d_R3,
                                float *d_rb3, float *ha_scratch, const int64_t *ray_map, float *d_h_appear, void *stream);
+/* nsb_fused_color_bwd with any of the appearance-code and ray gradients (the shipped configurations train both).  Every output is
+ * optional; NULL means not wanted, and with none this is nsb_fused_color_bwd.
+ *   d_h_appear: as nsb_fused_color_bwd_appear (needs g_rgb and ha_scratch[n, 8]).
+ *   d_rays_o, d_rays_d, d_view_dirs [R, 3]: the gradient to the rays of the points x = rays_o[ridx] + rays_d[ridx] t (x must be NULL) and
+ *   to the per-ray view directions view_dirs[R, 3] the forward read (needed with g_rgb).  The depths t are constants.  A point gets
+ *     g_x = (1/2) sum over levels of J^T (dh_z + dh_r) + dL/dx of the radiance input      g_v = (dSH4/dv)^T dL/dSH of the radiance input
+ *   with dh_z the decoder's and dh_r the radiance net's cotangent of the features (first order: the table-Hessian term of the nablas
+ *   backward does not reach x, as the reference's encoding does not form its input Hessian on the hot path); then per ray
+ *     d_rays_o[ray_map[r]] += sum of g_x,   d_rays_d[ray_map[r]] += sum of t g_x,   d_view_dirs[ray_map[r]] += sum of g_v
+ *   (ray_map NULL: row r).  ray_scratch[n, 36] fp32 workspace.  The caller zero-fills the outputs; the sums are deterministic for packed
+ *   samples, as for the codes.  The caller maps d_view_dirs onto its rays (view_dirs = rays_d / |rays_d| with a constant norm).
+ * Everything else as nsb_fused_color_bwd, which computes the same bits in the other outputs. */
+int nsb_fused_color_bwd_grads(const nsb_lotd_meta *meta_host, const void *params_half, const nsb_color_net *net_host, const float *x,
+                              const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, int64_t n, int32_t max_level,
+                              const void *act_z, const void *act_x, const void *act_y1, const void *act_y2, const float *rgb,
+                              const float *g_sdf, const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid, float *d_W1,
+                              float *d_b1, float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2, float *d_R3,
+                              float *d_rb3, const float *view_dirs, float *ha_scratch, const int64_t *ray_map, float *d_h_appear,
+                              float *ray_scratch, float *d_rays_o, float *d_rays_d, float *d_view_dirs, void *stream);
 
 /* ---------------------------------------------------------------- the persistent per-ray kernel (csrc/ray_upsample.cu)
  * The no-grad up-sampling half of neus_ray_query_march_occ_multi_upsample_compressed (neus_ray_query.py:861-905) for every hit ray as ONE

@@ -70,6 +70,9 @@ def lib():
         _lib.nsb_mc_triangles.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp, vp, i64, vp, vp]
         # the colour backward with the appearance-code gradient: 8 pointers, n, max_level, 23 pointers (activations, cotangents, outputs), stream
         _lib.nsb_fused_color_bwd_appear.argtypes = [vp] * 8 + [i64, i32] + [vp] * 23 + [vp]
+        # the backward passes with ray gradients (colour: + view_dirs, codes and rays; SDF: rays)
+        _lib.nsb_fused_color_bwd_grads.argtypes = [vp] * 8 + [i64, i32] + [vp] * 28 + [vp]
+        _lib.nsb_fused_sdf_bwd_rays.argtypes = [vp] * 9 + [i64, i32] + [vp] * 9 + [vp]
     return _lib
 
 

@@ -47,34 +47,6 @@ __host__ __device__ inline int ref_col(int k, int n_appear, int nh) {
 }
 
 
-// d(y_f)/d(x_d) of one level (both features) from its 8 corner cells as loaded, exactly as k_lotd_fwd<3,2,true,true> computes dy_dx
-__device__ __forceinline__ void jacobian_from_raw(const uint32_t (&raw)[8], const float (&fr)[3], const float (&scale)[3], float (&J0)[3],
-                                                  float (&J1)[3]) {
-    float2 v[8];
-#pragma unroll
-    for (int c = 0; c < 8; ++c) v[c] = __half22float2(*reinterpret_cast<const __half2 *>(&raw[c]));
-#pragma unroll
-    for (int gd = 0; gd < 3; ++gd) {
-        float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            float ww = scale[gd];
-            int left = 0;
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-                const int d = k >= gd ? k + 1 : k;
-                if (c & (1 << k)) { ww = __fmul_rn(ww, fr[d]); left += 1 << d; }
-                else ww = __fmul_rn(ww, __fsub_rn(1.f, fr[d]));
-            }
-            const int right = left + (1 << gd);
-            a0 = __fmaf_rn(ww, __fsub_rn(v[right].x, v[left].x), a0);
-            a1 = __fmaf_rn(ww, __fsub_rn(v[right].y, v[left].y), a1);
-        }
-        J0[gd] = a0;
-        J1[gd] = a1;
-    }
-}
-
 __device__ __forceinline__ void level_jacobian(const PLMeta &m, uint32_t p, const float (&xs)[3], const __half *__restrict__ grid,
                                                float (&J0)[3], float (&J1)[3]) {
     uint32_t cell[8], raw[8];
@@ -356,16 +328,21 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 // dh goes from its fragments straight to global memory, so the kernel stages no fp32 rows (~104 KB of shared memory: 2 CTAs / SM).
 // kAppear adds the appearance-code gradient of every point (the codes are the radiance input's columns 54..54 + n_appear):
 //   da  = dZ1 . R1[:, h_appear]    (M128 N8 K64)     A = T block 1,                     B = R1a^T tile (1 KB more shared memory)
-// written from its fragments like dh, as rows of 8 floats (zero beyond n_appear); k_appear_ray_sum adds them up per ray.
+// written from its fragments like dh, as rows of 8 floats (zero beyond n_appear); k_ray_row_sum adds them up per ray.
+// kRays adds the gradient of every point's position and SH view embedding (the reference's radiance input columns 0..18):
+//   dxv = dZ1 . R1[:, 0:19]       (M128 N32 K64)     A = T block 1,                     B = R1x^T tile (4 KB more shared memory)
+// written as rows of 24 floats [dL/dx (3) | dL/dSH (16) | 0]; k_color_sdf_bwd<true> adds dL/dx to the table's input gradient and maps
+// dL/dSH to the view direction.
 // The three saved activation tiles of a point tile (X, Y1, Y2: 3 x 16 KB, each contiguous in global memory and in shared memory) are
 // fetched by the bulk async copy engine (cp.async.bulk -> mbarrier), issued by one thread; the fetch of the NEXT tile starts as soon
 // as the last MMA that reads the current tiles has completed, so it overlaps the dh store and the next prologue.
-template <bool kAppear>
+template <bool kAppear, bool kRays>
 __global__ void __launch_bounds__(kTile, kColorBwdCtasPerSM)
 k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uint8_t *__restrict__ Y1t, const uint8_t *__restrict__ Y2t,
                 const float *__restrict__ rgb, const float *__restrict__ g_rgb, int64_t n, float *__restrict__ dh_out,
                 float *__restrict__ dR1, float *__restrict__ drb1, float *__restrict__ dR2, float *__restrict__ drb2,
-                float *__restrict__ dR3, float *__restrict__ drb3, const int64_t *__restrict__ n_dev, float *__restrict__ da_out) {
+                float *__restrict__ dR3, float *__restrict__ drb3, const int64_t *__restrict__ n_dev, float *__restrict__ da_out,
+                float *__restrict__ xv_out) {
     n = eff_n(n, n_dev);
     constexpr int NE = 80;                                     // 64 columns + the [1, gy3, 0..] chunk + a zero chunk (N % 16 == 0)
     extern __shared__ uint8_t dyn_smem[];
@@ -376,6 +353,7 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     uint8_t *sR2T = sXe + kTile * NE * 2;                      //  8 KB (N = in i, K = out j) = R2[j][i]
     uint8_t *sR1h = sR2T + XW * XW * 2;                        //  4 KB (N = h column k, K = out j) = R1[j][22 + k], zero for k >= 2L
     uint8_t *sR1a = sR1h + NF * XW * 2;                        //  1 KB (kAppear; N = code column k, K = out j) = R1[j][22 + 2L + k], zero for k >= n_appear
+    uint8_t *sR1x = sR1a + 8 * XW * 2;                         //  4 KB (kRays; N = input column k, K = out j) = R1[j][k], zero for k >= 19
     __shared__ float sR3[3][XW];
     __shared__ float sdb3[3];
     __shared__ __align__(8) uint64_t mbar_ld;
@@ -396,6 +374,13 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
             const int k = e % 8, j = e / 8;
             const __half v = (j < net.rw && k < net.n_appear) ? net.R1[j * net.rin + 22 + net.dec.nh + k] : __float2half_rn(0.f);
             *reinterpret_cast<__half *>(sR1a + (j / 8) * (8 * 16) + k * 16 + (j % 8) * 2) = v;
+        }
+    }
+    if constexpr (kRays) {
+        for (int e = tid; e < NF * XW; e += kTile) {
+            const int k = e % NF, j = e / NF;
+            const __half v = (j < net.rw && k < 19) ? net.R1[j * net.rin + k] : __float2half_rn(0.f);
+            *reinterpret_cast<__half *>(sR1x + (j / 8) * (NF * 16) + k * 16 + (j % 8) * 2) = v;
         }
     }
     if (tid < XW) {
@@ -487,6 +472,9 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         float da[2][4];
         if constexpr (kAppear)
             tc::mma_m128<8, 0, 0, XW / 16>(da, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(tc::smem_u32(sR1a), 8), false);   // da = dZ1 . R1[:, h_appear]
+        float dxv[2][NF / 2];
+        if constexpr (kRays)
+            tc::mma_m128<32, 0, 0, XW / 16>(dxv, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(tc::smem_u32(sR1x), NF), false);   // dxv = dZ1 . R1[:, 0:19]
         // weight gradients: contract over the 128 points
         tc::mma_m64<NE, 1, 1, kTile / 16>(xa, tc::mnmajor(t_addr, kTile), tc::mnmajor(y1_addr, kTile), true);
         tc::mma_m64<NE, 1, 1, kTile / 16>(xb, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(xe_addr, kTile), true);
@@ -511,6 +499,11 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
                     for (int c = 0; c < NF / 8; ++c)
                         *reinterpret_cast<float2 *>(dh_out + row * NF + tc::frag_col(c)) = make_float2(dh[h][4 * c + 2 * r], dh[h][4 * c + 2 * r + 1]);
                     if constexpr (kAppear) *reinterpret_cast<float2 *>(da_out + row * 8 + tc::frag_col(0)) = make_float2(da[h][2 * r], da[h][2 * r + 1]);
+                    if constexpr (kRays) {
+#pragma unroll
+                        for (int c = 0; c < 3; ++c)
+                            *reinterpret_cast<float2 *>(xv_out + row * 24 + tc::frag_col(c)) = make_float2(dxv[h][4 * c + 2 * r], dxv[h][4 * c + 2 * r + 1]);
+                    }
                 }
             }
     }
@@ -544,52 +537,6 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     }
 }
 
-// Per-ray sum of the appearance-code gradients k_color_rad_bwd<true> wrote per point (rows of 8 floats).  The points of a ray are
-// consecutive (packed samples), so a ray is a run of equal ridx.  A warp looks at 32 points; for each run that starts among them, in
-// order, the whole warp walks the run 32 points at a time (lane l adds points start + l, start + l + 32, ...; the run ends at the first
-// point of another ray), reduces the lanes' sums by a fixed butterfly and adds the result once to row ray_map[ray] (ray_map NULL: row
-// ray) of d_h_appear [., n_appear].  One add per ray onto the caller's zeros in an order fixed by the run's position: the same bits on
-// every run.  (A ray whose points form several runs -- unsorted ridx -- gets one atomic add per run.)
-__global__ void __launch_bounds__(256)
-k_appear_ray_sum(const float *__restrict__ rows, const int64_t *__restrict__ ridx, int64_t n, int n_appear, const int64_t *__restrict__ ray_map,
-                 float *__restrict__ d_h_appear, const int64_t *__restrict__ n_dev) {
-    n = eff_n(n, n_dev);
-    const int lane = threadIdx.x & 31;
-    const int64_t n_warps = (int64_t)gridDim.x * (blockDim.x / 32);
-    for (int64_t w = blockIdx.x * (int64_t)(blockDim.x / 32) + threadIdx.x / 32; w * 32 < n; w += n_warps) {   // warp-uniform
-        const int64_t i = w * 32 + lane;
-        const int64_t ray = i < n ? (ridx ? ridx[i] : i) : -1;
-        uint32_t heads = __ballot_sync(~0u, i < n && (!ridx || i == 0 || ridx[i - 1] != ray));
-        while (heads) {
-            const int src = __ffs(heads) - 1;
-            heads &= heads - 1;
-            const int64_t r = __shfl_sync(~0u, ray, src);
-            float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-            for (int64_t base = w * 32 + src;; base += 32) {
-                const int64_t j = base + lane;
-                const bool same = j < n && (ridx ? ridx[j] == r : j == base);
-                const uint32_t stop = ~__ballot_sync(~0u, same);
-                const int end = stop ? __ffs(stop) - 1 : 32;        // the run continues in lanes [0, end) of this block
-                if (lane < end) {
-                    const float4 a = *reinterpret_cast<const float4 *>(rows + j * 8), b = *reinterpret_cast<const float4 *>(rows + j * 8 + 4);
-                    acc[0] += a.x; acc[1] += a.y; acc[2] += a.z; acc[3] += a.w; acc[4] += b.x; acc[5] += b.y; acc[6] += b.z; acc[7] += b.w;
-                }
-                if (end < 32) break;
-            }
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-#pragma unroll
-                for (int off = 16; off > 0; off >>= 1) acc[k] += __shfl_xor_sync(~0u, acc[k], off);
-            if (lane < n_appear) {
-                float v = acc[0];
-#pragma unroll
-                for (int k = 1; k < 8; ++k) v = lane == k ? acc[k] : v;
-                atomicAdd(d_h_appear + (ray_map ? ray_map[r] : r) * n_appear + lane, v);
-            }
-        }
-    }
-}
-
 // ===================================================================================================================== sdf / nablas backward
 // T = [dz | u | v] (128 x 192).  gin = dL/dnablas * fac * 0.5 (cotangent of nablas01), dsdf optional, dh_r = dL/dh from the radiance net.
 //   dg_f = sum_d gin_d J[f][d]  (k_lotd_ddLdy)                                   -> fp16 tile Ge = [dG | 1 0..]
@@ -606,11 +553,18 @@ k_appear_ray_sum(const float *__restrict__ rows, const int64_t *__restrict__ rid
 // The saved Z tile (16 KB) and the H half of the saved X tile (8 KB) are fetched by the bulk async copy engine into shared memory, and
 // the NEXT tile's fetch is issued right after the last MMA of the current tile -- it runs behind the whole scatter phase.  (Reading Z
 // straight from global memory in the two epilogue loops costs 16 dependent round trips per tile at 8 warps per SM.)
+// kXGrad adds the gradient of every point's ray (the depths t are constants): the scatter loop loads the corners of each level it scatters
+// to once more and adds J^T (dhz + dh_r) to the point's table-space input gradient (first order: the table-Hessian term of the scatter does
+// not reach x), which is mapped to network space and added to dL/dx of the radiance input (xv rows of k_color_rad_bwd<., true>, NULL
+// without rgb); dL/dSH of those rows is mapped to the view direction through the SH Jacobian.  Each point writes a row of 12 floats
+// [g_x | t g_x | g_v | 0 0 0], which k_ray_row_sum adds up per ray.
+template <bool kXGrad>
 __global__ void __launch_bounds__(kTile, kColorBwdCtasPerSM)
 k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev net, const PointSrc ps, const uint8_t *__restrict__ Zt,
                 const uint8_t *__restrict__ Xt, const float *__restrict__ g_nab, const float *__restrict__ g_sdf, const float *__restrict__ dh_r,
                 int64_t n, int max_level, float *__restrict__ d_grid, float *__restrict__ d_W1, float *__restrict__ d_b1, float *__restrict__ d_W2,
-                float *__restrict__ d_b2, const int64_t *__restrict__ n_dev) {
+                float *__restrict__ d_b2, const int64_t *__restrict__ n_dev, const float *__restrict__ xv_rows,
+                const float *__restrict__ view_dirs, float *__restrict__ gx_out) {
     n = eff_n(n, n_dev);
     constexpr int NX = 48;                                     // 32 + the [1 0..] chunk + a zero chunk (N % 16 == 0)
     extern __shared__ uint8_t dyn_smem[];
@@ -760,6 +714,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         tc::frag_store<NF>(dhz, stage, kS, NF);
         __syncthreads();
         // ---- merged scatter
+        float gx[3] = {0.f, 0.f, 0.f};
 #pragma unroll 1
         for (uint32_t g4 = 0; g4 * 4 < m.n_pseudo; ++g4) {
             float gg[8], hz[8];
@@ -778,6 +733,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
                 level_cells3(m, p, xs, cell, w, fr, sc);
                 const float g0 = valid ? r16(gg[2 * q]) : 0.f, g1 = valid ? r16(gg[2 * q + 1]) : 0.f;
                 const float h0 = valid ? hz[2 * q] : 0.f, h1 = valid ? hz[2 * q + 1] : 0.f;
+                if constexpr (kXGrad) level_input_grad(m, p, grid, cell, fr, sc, h0, h1, gx);
 #pragma unroll
                 for (int c = 0; c < 8; ++c) {
                     float wsum = 0.f;
@@ -799,6 +755,30 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
 #pragma unroll
                     for (int c = 0; c < 8; ++c) red_add2(gp + cell[c], ua[c], ub[c]);
                 }
+            }
+        }
+        if constexpr (kXGrad) {
+            if (valid) {
+                float g[3], gv[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+                for (int d = 0; d < 3; ++d) g[d] = input_grad_to_net(gx[d]);
+                if (xv_rows) {
+                    const float *xr = xv_rows + i * 24;
+#pragma unroll
+                    for (int d = 0; d < 3; ++d) g[d] = __fadd_rn(g[d], xr[d]);
+                    float jx[16], jy[16], jz[16];
+                    sh_jacobian(view_dirs[ray * 3], view_dirs[ray * 3 + 1], view_dirs[ray * 3 + 2], 4, jx, jy, jz);
+#pragma unroll
+                    for (int c = 0; c < 16; ++c) {
+                        const float dsh = xr[3 + c];
+                        gv[0] = fmaf(dsh, jx[c], gv[0]); gv[1] = fmaf(dsh, jy[c], gv[1]); gv[2] = fmaf(dsh, jz[c], gv[2]);
+                    }
+                }
+                const float tt = ps.t[i];
+                float4 *o = reinterpret_cast<float4 *>(gx_out + i * 12);
+                o[0] = make_float4(g[0], g[1], g[2], __fmul_rn(tt, g[0]));
+                o[1] = make_float4(__fmul_rn(tt, g[1]), __fmul_rn(tt, g[2]), gv[0], gv[1]);
+                o[2] = make_float4(gv[2], 0.f, 0.f, 0.f);
             }
         }
         __syncthreads();
@@ -894,13 +874,15 @@ extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params
     return check_launch("nsb_fused_color_fwd");
 }
 
-// the two backward kernels (k_color_rad_bwd<kAppear> only with g_rgb), then with kAppear the per-ray sum of the code gradients
-template <bool kAppear>
+// the two backward kernels (k_color_rad_bwd only with g_rgb), then with kAppear the per-ray sum of the code gradients and with kRays the
+// per-ray sum of the ray gradients
+template <bool kAppear, bool kRays>
 static int color_bwd(const char *who, const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x, const float *rays_o,
                      const float *rays_d, const int64_t *ridx, const float *t, int64_t n, int32_t max_level, const void *act_z, const void *act_x,
                      const void *act_y1, const void *act_y2, const float *rgb, const float *g_sdf, const float *g_nablas, const float *g_rgb,
                      float *dh_scratch, float *d_grid, float *d_W1, float *d_b1, float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2,
-                     float *d_rb2, float *d_R3, float *d_rb3, float *ha_scratch, const int64_t *ray_map, float *d_h_appear, void *stream) {
+                     float *d_rb2, float *d_R3, float *d_rb3, const float *view_dirs, float *ha_scratch, const int64_t *ray_map, float *d_h_appear,
+                     float *ray_scratch, float *d_rays_o, float *d_rays_d, float *d_view_dirs, void *stream) {
     const DevCounts dn = take_counts();
     if (n == 0) return 0;
     NSB_REQUIRE(meta && params_half && net && act_z && act_x, "%s: NULL argument", who);
@@ -910,6 +892,10 @@ static int color_bwd(const char *who, const nsb_lotd_meta *meta, const void *par
         NSB_REQUIRE(d_R1 && d_rb1 && d_R2 && d_rb2 && d_R3 && d_rb3, "%s: NULL radiance gradient buffer (g_rgb given)", who);
     }
     if (kAppear) NSB_REQUIRE(g_rgb && ha_scratch && d_h_appear, "%s: needs g_rgb, ha_scratch and d_h_appear", who);
+    if (kRays) {
+        NSB_REQUIRE(!x && rays_o && rays_d && t && ray_scratch, "%s: ray gradients need the points as rays (x NULL, rays_o, rays_d, t) and ray_scratch", who);
+        NSB_REQUIRE(!g_rgb || view_dirs, "%s: ray gradients with g_rgb need view_dirs", who);
+    }
     NSB_REQUIRE(x || (rays_o && rays_d && t), "%s: need x or (rays_o, rays_d, t)", who);
     PLMeta m;
     ColorNetDev d;
@@ -917,28 +903,37 @@ static int color_bwd(const char *who, const nsb_lotd_meta *meta, const void *par
     if (kAppear) NSB_REQUIRE(d.n_appear >= 1, "%s: the net has no appearance channels", who);
     cudaStream_t s = (cudaStream_t)stream;
     const float *dh = nullptr;
+    float *xv_rows = (kRays && g_rgb) ? ray_scratch + n * 12 : nullptr;   // [n, 24] after the [n, 12] ray rows
     if (g_rgb) {
-        constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + (kAppear ? 8 * XW * 2 : 0) + 1024;   // 101 (102) KB
-        opt_in_smem(k_color_rad_bwd<kAppear>, kSmemR);
-        if (int rc = require_ctas_per_sm(k_color_rad_bwd<kAppear>, kTile, kSmemR, kColorBwdCtasPerSM, "nsb_fused_color_bwd(radiance)")) return rc;
-        k_color_rad_bwd<kAppear><<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemR, s>>>(
+        constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + (kAppear || kRays ? 8 * XW * 2 : 0) +
+                               (kRays ? NF * XW * 2 : 0) + 1024;   // 101 (102 with codes, 106 with rays) KB
+        opt_in_smem(k_color_rad_bwd<kAppear, kRays>, kSmemR);
+        if (int rc = require_ctas_per_sm(k_color_rad_bwd<kAppear, kRays>, kTile, kSmemR, kColorBwdCtasPerSM, "nsb_fused_color_bwd(radiance)")) return rc;
+        k_color_rad_bwd<kAppear, kRays><<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemR, s>>>(
             d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n, dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3,
-            dn.a, ha_scratch);
+            dn.a, ha_scratch, xv_rows);
         if (int rc = check_launch("nsb_fused_color_bwd(radiance)")) return rc;
         dh = dh_scratch;
         if (kAppear) {
-            const int64_t blocks = (n + 255) / 256;                    // 8 warps of 32 points per block
-            k_appear_ray_sum<<<(unsigned)(blocks < (1 << 20) ? blocks : (1 << 20)), 256, 0, s>>>(ha_scratch, ridx, n, d.n_appear, ray_map, d_h_appear, dn.a);
-            if (int rc = check_launch("nsb_fused_color_bwd_appear(ray sum)")) return rc;
+            k_ray_row_sum<8><<<row_sum_blocks(n), 256, 0, s>>>(ha_scratch, ridx, nullptr, n, d.n_appear, ray_map,
+                                                                RowSumOut{{d_h_appear, nullptr, nullptr}, d.n_appear}, dn.a);
+            if (int rc = check_launch("nsb_fused_color_bwd(code sum)")) return rc;
         }
     }
     constexpr int kSmemS = 3 * kTileBytes + 2 * kTile * 48 * 2 + 2 * HW * NF * 2 + kTileBytes + 1024;   // 97 KB
-    opt_in_smem(k_color_sdf_bwd, kSmemS);
-    if (int rc = require_ctas_per_sm(k_color_sdf_bwd, kTile, kSmemS, kColorBwdCtasPerSM, "nsb_fused_color_bwd(sdf)")) return rc;
+    opt_in_smem(k_color_sdf_bwd<kRays>, kSmemS);
+    if (int rc = require_ctas_per_sm(k_color_sdf_bwd<kRays>, kTile, kSmemS, kColorBwdCtasPerSM, "nsb_fused_color_bwd(sdf)")) return rc;
     const PointSrc ps{x, rays_o, rays_d, t, ridx};
-    k_color_sdf_bwd<<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemS, s>>>(m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x,
-                                                                          g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level, d_grid, d_W1, d_b1, d_W2, d_b2, dn.a);
-    return check_launch("nsb_fused_color_bwd(sdf)");
+    k_color_sdf_bwd<kRays><<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemS, s>>>(
+        m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x, g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level,
+        d_grid, d_W1, d_b1, d_W2, d_b2, dn.a, xv_rows, view_dirs, ray_scratch);
+    if (int rc = check_launch("nsb_fused_color_bwd(sdf)")) return rc;
+    if (kRays) {
+        k_ray_row_sum<12><<<row_sum_blocks(n), 256, 0, s>>>(ray_scratch, ridx, nullptr, n, 9, ray_map, RowSumOut{{d_rays_o, d_rays_d, d_view_dirs}, 3},
+                                                             dn.a);
+        return check_launch("nsb_fused_color_bwd(ray sum)");
+    }
+    return 0;
 }
 
 extern "C" int nsb_fused_color_bwd(const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x, const float *rays_o,
@@ -947,9 +942,9 @@ extern "C" int nsb_fused_color_bwd(const nsb_lotd_meta *meta, const void *params
                                    const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid, float *d_W1, float *d_b1,
                                    float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2, float *d_R3, float *d_rb3,
                                    void *stream) {
-    return color_bwd<false>("nsb_fused_color_bwd", meta, params_half, net, x, rays_o, rays_d, ridx, t, n, max_level, act_z, act_x, act_y1, act_y2, rgb,
-                            g_sdf, g_nablas, g_rgb, dh_scratch, d_grid, d_W1, d_b1, d_W2, d_b2, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, nullptr, nullptr,
-                            nullptr, stream);
+    return color_bwd<false, false>("nsb_fused_color_bwd", meta, params_half, net, x, rays_o, rays_d, ridx, t, n, max_level, act_z, act_x, act_y1, act_y2,
+                                   rgb, g_sdf, g_nablas, g_rgb, dh_scratch, d_grid, d_W1, d_b1, d_W2, d_b2, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, nullptr,
+                                   nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 extern "C" int nsb_fused_color_bwd_appear(const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x,
@@ -958,7 +953,26 @@ extern "C" int nsb_fused_color_bwd_appear(const nsb_lotd_meta *meta, const void 
                                           const float *g_sdf, const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid,
                                           float *d_W1, float *d_b1, float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2,
                                           float *d_R3, float *d_rb3, float *ha_scratch, const int64_t *ray_map, float *d_h_appear, void *stream) {
-    return color_bwd<true>("nsb_fused_color_bwd_appear", meta, params_half, net, x, rays_o, rays_d, ridx, t, n, max_level, act_z, act_x, act_y1, act_y2,
-                           rgb, g_sdf, g_nablas, g_rgb, dh_scratch, d_grid, d_W1, d_b1, d_W2, d_b2, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, ha_scratch,
-                           ray_map, d_h_appear, stream);
+    return color_bwd<true, false>("nsb_fused_color_bwd_appear", meta, params_half, net, x, rays_o, rays_d, ridx, t, n, max_level, act_z, act_x, act_y1,
+                                  act_y2, rgb, g_sdf, g_nablas, g_rgb, dh_scratch, d_grid, d_W1, d_b1, d_W2, d_b2, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3,
+                                  nullptr, ha_scratch, ray_map, d_h_appear, nullptr, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int nsb_fused_color_bwd_grads(const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x,
+                                         const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, int64_t n, int32_t max_level,
+                                         const void *act_z, const void *act_x, const void *act_y1, const void *act_y2, const float *rgb,
+                                         const float *g_sdf, const float *g_nablas, const float *g_rgb, float *dh_scratch, float *d_grid,
+                                         float *d_W1, float *d_b1, float *d_W2, float *d_b2, float *d_R1, float *d_rb1, float *d_R2, float *d_rb2,
+                                         float *d_R3, float *d_rb3, const float *view_dirs, float *ha_scratch, const int64_t *ray_map,
+                                         float *d_h_appear, float *ray_scratch, float *d_rays_o, float *d_rays_d, float *d_view_dirs, void *stream) {
+    const char *who = "nsb_fused_color_bwd_grads";
+    const bool appear = d_h_appear != nullptr, rays = d_rays_o || d_rays_d || d_view_dirs;
+#define NSB_COLOR_BWD(A, R)                                                                                                                       \
+    color_bwd<A, R>(who, meta, params_half, net, x, rays_o, rays_d, ridx, t, n, max_level, act_z, act_x, act_y1, act_y2, rgb, g_sdf, g_nablas, g_rgb, \
+                    dh_scratch, d_grid, d_W1, d_b1, d_W2, d_b2, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3, view_dirs, ha_scratch, ray_map, d_h_appear,    \
+                    ray_scratch, d_rays_o, d_rays_d, d_view_dirs, stream)
+    const int rc = appear ? (rays ? NSB_COLOR_BWD(true, true) : NSB_COLOR_BWD(true, false))
+                          : (rays ? NSB_COLOR_BWD(false, true) : NSB_COLOR_BWD(false, false));
+#undef NSB_COLOR_BWD
+    return rc;
 }

@@ -115,13 +115,16 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
 // 2.16 / 2.13 ms at 4 (profiles/bwd_kernels.py, the three builds alternated in one run; 2.48 ms before its sums moved to registers).
 constexpr int kSdfBwdCtasPerSM = 4;
 
-template <bool FROM_RAYS>
+// kXGrad (points from rays only) adds the gradient of every point's ray, the depths t being constants: the scatter loads the corners of
+// each level it scatters to once more and adds J^T dH to the point's table-space input gradient g, which is mapped to network space and
+// written as row i_ (the kernel's row, not keep[i_]) of gx_out [n, 8] = [g | t g | 0 0]; k_ray_row_sum adds the rows up per ray.
+template <bool FROM_RAYS, bool kXGrad>
 __global__ void __launch_bounds__(kTile, kSdfBwdCtasPerSM)
 k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ x,
              const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
              const float *__restrict__ t, const float *__restrict__ d_sdf, int64_t n, int max_level, float *__restrict__ d_grid,
              float *__restrict__ d_W1, float *__restrict__ d_b1, float *__restrict__ d_W2, float *__restrict__ d_b2,
-             const int64_t *__restrict__ keep, const int64_t *__restrict__ n_dev) {
+             const int64_t *__restrict__ keep, const int64_t *__restrict__ n_dev, float *__restrict__ gx_out) {
     n = eff_n(n, n_dev);
     constexpr int NX = 40, GW = 128;                          // NX: features + [1,0,..] chunk; GW: dz | d*a
     constexpr int kS = tc::acc_stride(NF);                    // staged dH rows for the scatter: 18 KB, aliasing G
@@ -207,6 +210,7 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         // ---- my dH row -> scatter into the table gradient; only the reductions are predicated on "this point carries gradient".
         const bool active = valid && dd != 0.f;
         const bool warp_active = __any_sync(0xffffffffu, active);
+        float gx[3] = {0.f, 0.f, 0.f};
 #pragma unroll 1
         for (uint32_t g4 = 0; g4 * 4 < m.n_pseudo; ++g4) {
             float dh[8];
@@ -217,9 +221,11 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
                 const uint32_t p = g4 * 4 + q;
                 if (p >= m.n_pseudo || (int)m.level[p] > max_level) continue;               // uniform
                 uint32_t cell[8];
-                float w[8], a[8], b[8];
-                level_cells3(m, p, xs, cell, w);
+                float w[8], a[8], b[8], fr[3], sc[3];
+                if constexpr (kXGrad) level_cells3(m, p, xs, cell, w, fr, sc);
+                else level_cells3(m, p, xs, cell, w);
                 const float g0 = active ? dh[2 * q] : 0.f, g1 = active ? dh[2 * q + 1] : 0.f;
+                if constexpr (kXGrad) level_input_grad(m, p, grid, cell, fr, sc, g0, g1, gx);
 #pragma unroll
                 for (int c = 0; c < 8; ++c) { a[c] = g0 * w[c]; b[c] = g1 * w[c]; }
                 if (warp_merge_updates(cell_key3(m, p, xs), active, a, b, lane)) {   // neighbouring samples, same cell
@@ -227,6 +233,17 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
 #pragma unroll
                     for (int c = 0; c < 8; ++c) red_add2(gp + cell[c], a[c], b[c]);
                 }
+            }
+        }
+        if constexpr (kXGrad) {
+            if (valid) {
+                float g[3];
+#pragma unroll
+                for (int d = 0; d < 3; ++d) g[d] = input_grad_to_net(gx[d]);
+                const float tt = t[i];
+                float4 *o = reinterpret_cast<float4 *>(gx_out + i_ * 8);
+                o[0] = make_float4(g[0], g[1], g[2], __fmul_rn(tt, g[0]));
+                o[1] = make_float4(__fmul_rn(tt, g[1]), __fmul_rn(tt, g[2]), 0.f, 0.f);
             }
         }
         __syncthreads();                                         // tiles + staged rows free for the next iteration
@@ -289,28 +306,50 @@ extern "C" int nsb_fused_sdf_bwd(const nsb_lotd_meta *meta, const void *params_h
                                      stream);
 }
 
+// the backward of the fused SDF query, with kXGrad the per-point ray rows and their per-ray sums (k_ray_row_sum, color_tc.cu)
+template <bool kXGrad>
+static int sdf_bwd(const char *who, const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *x, const float *rays_o,
+                   const float *rays_d, const int64_t *ridx, const float *t, const float *d_sdf, const int64_t *keep, int64_t n, int32_t max_level,
+                   float *d_grid, float *d_W1, float *d_b1, float *d_W2, float *d_b2, float *gx_scratch, const int64_t *ray_map, float *d_rays_o,
+                   float *d_rays_d, void *stream) {
+    const DevCounts dn = take_counts();
+    if (n == 0) return 0;
+    NSB_REQUIRE(meta && params_half && dec && d_sdf && d_grid && d_W1 && d_b1 && d_W2 && d_b2, "%s: NULL argument", who);
+    NSB_REQUIRE(x || (rays_o && rays_d && t), "%s: need x or (rays_o, rays_d, t)", who);
+    if (kXGrad) NSB_REQUIRE(!x && gx_scratch, "%s: ray gradients need the points as rays (x NULL) and gx_scratch", who);
+    PLMeta m;
+    DecoderDevTC d;
+    if (int rc = make_decoder(meta, dec, &m, &d, who)) return rc;
+    constexpr int kBwdSmem = (128 * 40 + 128 * 128 + 64 * 32 + 32 * 64) * 2 + 128;       // 50 KB
+    auto kern = x == nullptr ? k_sdf_bwd_tc<true, kXGrad> : k_sdf_bwd_tc<false, false>;
+    opt_in_smem(kern, kBwdSmem);
+    if (int rc = require_ctas_per_sm(kern, kTile, kBwdSmem, kSdfBwdCtasPerSM, who)) return rc;
+    const unsigned grid = persistent_grid((n + kTile - 1) / kTile, kSdfBwdCtasPerSM);
+    cudaStream_t s = (cudaStream_t)stream;
+    const int ml = max_level < 0 ? -1 : max_level;
+    kern<<<grid, kTile, kBwdSmem, s>>>(m, (const __half *)params_half, d, x, x ? nullptr : rays_o, x ? nullptr : rays_d, x ? nullptr : ridx,
+                                       x ? nullptr : t, d_sdf, n, ml, d_grid, d_W1, d_b1, d_W2, d_b2, keep, dn.a, gx_scratch);
+    if (int rc = check_launch(who)) return rc;
+    if (kXGrad) {
+        if (!d_rays_o && !d_rays_d) return 0;
+        k_ray_row_sum<8><<<row_sum_blocks(n), 256, 0, s>>>(gx_scratch, ridx, keep, n, 6, ray_map, RowSumOut{{d_rays_o, d_rays_d, nullptr}, 3}, dn.a);
+        return check_launch("nsb_fused_sdf_bwd_rays(ray sum)");
+    }
+    return 0;
+}
+
 extern "C" int nsb_fused_sdf_bwd_indexed(const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *x,
                                          const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, const float *d_sdf,
                                          const int64_t *keep, int64_t n, int32_t max_level, float *d_grid, float *d_W1, float *d_b1, float *d_W2,
                                          float *d_b2, void *stream) {
-    const DevCounts dn = take_counts();
-    if (n == 0) return 0;
-    NSB_REQUIRE(meta && params_half && dec && d_sdf && d_grid && d_W1 && d_b1 && d_W2 && d_b2, "nsb_fused_sdf_bwd: NULL argument");
-    NSB_REQUIRE(x || (rays_o && rays_d && t), "nsb_fused_sdf_bwd: need x or (rays_o, rays_d, t)");
-    PLMeta m;
-    DecoderDevTC d;
-    if (int rc = make_decoder(meta, dec, &m, &d, "nsb_fused_sdf_bwd")) return rc;
-    constexpr int kBwdSmem = (128 * 40 + 128 * 128 + 64 * 32 + 32 * 64) * 2 + 128;       // 50 KB
-    opt_in_smem(k_sdf_bwd_tc<true>, kBwdSmem);
-    opt_in_smem(k_sdf_bwd_tc<false>, kBwdSmem);
-    if (int rc = require_ctas_per_sm(x == nullptr ? k_sdf_bwd_tc<true> : k_sdf_bwd_tc<false>, kTile, kBwdSmem, kSdfBwdCtasPerSM, "nsb_fused_sdf_bwd"))
-        return rc;
-    const unsigned grid = persistent_grid((n + kTile - 1) / kTile, kSdfBwdCtasPerSM);
-    cudaStream_t s = (cudaStream_t)stream;
-    const int ml = max_level < 0 ? -1 : max_level;
-    if (x == nullptr) k_sdf_bwd_tc<true><<<grid, kTile, kBwdSmem, s>>>(m, (const __half *)params_half, d, nullptr, rays_o, rays_d, ridx, t, d_sdf, n, ml,
-                                                                d_grid, d_W1, d_b1, d_W2, d_b2, keep, dn.a);
-    else k_sdf_bwd_tc<false><<<grid, kTile, kBwdSmem, s>>>(m, (const __half *)params_half, d, x, nullptr, nullptr, nullptr, nullptr, d_sdf, n, ml,
-                                                    d_grid, d_W1, d_b1, d_W2, d_b2, keep, dn.a);
-    return check_launch("nsb_fused_sdf_bwd");
+    return sdf_bwd<false>("nsb_fused_sdf_bwd", meta, params_half, dec, x, rays_o, rays_d, ridx, t, d_sdf, keep, n, max_level, d_grid, d_W1, d_b1, d_W2,
+                          d_b2, nullptr, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int nsb_fused_sdf_bwd_rays(const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *rays_o,
+                                      const float *rays_d, const int64_t *ridx, const float *t, const float *d_sdf, const int64_t *keep, int64_t n,
+                                      int32_t max_level, float *d_grid, float *d_W1, float *d_b1, float *d_W2, float *d_b2, float *gx_scratch,
+                                      const int64_t *ray_map, float *d_rays_o, float *d_rays_d, void *stream) {
+    return sdf_bwd<true>("nsb_fused_sdf_bwd_rays", meta, params_half, dec, nullptr, rays_o, rays_d, ridx, t, d_sdf, keep, n, max_level, d_grid, d_W1,
+                         d_b1, d_W2, d_b2, gx_scratch, ray_map, d_rays_o, d_rays_d, stream);
 }

@@ -81,6 +81,52 @@ __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half
     for (; p0 < 16; ++p0) put_level_to_tile<R>(tile, r, p0, 0u);
 }
 
+// d(y_f)/d(x_d) of one level (both features) from its 8 corner cells as loaded, exactly as k_lotd_fwd<3,2,true,true> computes dy_dx
+__device__ __forceinline__ void jacobian_from_raw(const uint32_t (&raw)[8], const float (&fr)[3], const float (&scale)[3], float (&J0)[3],
+                                                  float (&J1)[3]) {
+    float2 v[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) v[c] = __half22float2(*reinterpret_cast<const __half2 *>(&raw[c]));
+#pragma unroll
+    for (int gd = 0; gd < 3; ++gd) {
+        float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            float ww = scale[gd];
+            int left = 0;
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+                const int d = k >= gd ? k + 1 : k;
+                if (c & (1 << k)) { ww = __fmul_rn(ww, fr[d]); left += 1 << d; }
+                else ww = __fmul_rn(ww, __fsub_rn(1.f, fr[d]));
+            }
+            const int right = left + (1 << gd);
+            a0 = __fmaf_rn(ww, __fsub_rn(v[right].x, v[left].x), a0);
+            a1 = __fmaf_rn(ww, __fsub_rn(v[right].y, v[left].y), a1);
+        }
+        J0[gd] = a0;
+        J1[gd] = a1;
+    }
+}
+
+// The input gradient of one level, first order (the encoding's input Hessian is not formed, as on the reference's hot path):
+// gx += J0 h0 + J1 h1, with J from the level's 8 corners (loaded here) and (h0, h1) the cotangent of the level's two features.
+__device__ __forceinline__ void level_input_grad(const PLMeta &m, uint32_t p, const __half *__restrict__ grid, const uint32_t (&cell)[8],
+                                                 const float (&fr)[3], const float (&sc)[3], float h0, float h1, float (&gx)[3]) {
+    uint32_t raw[8];
+    const uint32_t *lp = level_cells_ptr(m, p, grid);
+#pragma unroll
+    for (int c = 0; c < 8; ++c) raw[c] = ld_nc_u32(lp + cell[c]);
+    float J0[3], J1[3];
+    jacobian_from_raw(raw, fr, sc, J0, J1);
+#pragma unroll
+    for (int d = 0; d < 3; ++d) gx[d] = __fmaf_rn(h1, J1[d], __fmaf_rn(h0, J0[d], gx[d]));
+}
+
+// table-space input gradient -> network space: the table sees x / 2 + 1/2.  The encoding clamps that to [1e-6, 1 - 1e-6] inside its op
+// and returns the input gradient at the clamped point without masking it (LoTDFunction*, lotd.py), so neither is it masked here.
+__device__ __forceinline__ float input_grad_to_net(float g) { return __fmul_rn(g, 0.5f); }
+
 // Where the points of a kernel come from: x[i] (network space), or rays_o/rays_d[ray] + t[i] rays_d[ray] with ray = ridx[i] (or i).
 struct PointSrc {
     const float *x, *rays_o, *rays_d, *t;
@@ -174,6 +220,73 @@ __device__ __forceinline__ void stage_decoder_vectors(const DecoderDevTC &dec, B
     if constexpr (kB2) {
         if (tid == 0) *sb2 = __half2float(dec.b2[0]);
     }
+}
+
+// Per-ray sum of per-point gradient rows (W floats each): the appearance-code rows of k_color_rad_bwd<true, .>, and the ray rows
+// [dL/do | dL/dd | dL/dv | 0] of k_color_sdf_bwd<true> and k_sdf_bwd_tc<true, true>.  Row j belongs to ray ridx[keep[j]] (keep NULL:
+// ridx[j]; ridx NULL: ray j).  The points of a ray are consecutive (packed samples), so a ray is a run of equal rays.  A warp looks at 32
+// rows; for each run that starts among them, in order, the whole warp walks the run 32 rows at a time (lane l adds rows start + l,
+// start + l + 32, ...; the run ends at the first row of another ray), reduces the lanes' sums by a fixed butterfly and adds column c < n_out
+// once to out.p[c / out.k][ray_map[ray] * out.k + c % out.k] (ray_map NULL: row ray; a NULL output is not written).  One add per ray
+// onto the caller's zeros in an order fixed by the run's position: the same bits on every run.  (A ray whose points form several runs --
+// unsorted rays -- gets one atomic add per run.)
+struct RowSumOut {
+    float *p[3];
+    int k;                                                     // columns per output
+};
+template <int W>
+__global__ void __launch_bounds__(256)
+k_ray_row_sum(const float *__restrict__ rows, const int64_t *__restrict__ ridx, const int64_t *__restrict__ keep, int64_t n, int n_out,
+              const int64_t *__restrict__ ray_map, const RowSumOut out, const int64_t *__restrict__ n_dev) {
+    n = eff_n(n, n_dev);
+    const int lane = threadIdx.x & 31;
+    const int64_t n_warps = (int64_t)gridDim.x * (blockDim.x / 32);
+    auto ray_of = [&](int64_t j) { return ridx[keep ? keep[j] : j]; };
+    for (int64_t w = blockIdx.x * (int64_t)(blockDim.x / 32) + threadIdx.x / 32; w * 32 < n; w += n_warps) {   // warp-uniform
+        const int64_t i = w * 32 + lane;
+        const int64_t ray = i < n ? (ridx ? ray_of(i) : i) : -1;
+        uint32_t heads = __ballot_sync(~0u, i < n && (!ridx || i == 0 || ray_of(i - 1) != ray));
+        while (heads) {
+            const int src = __ffs(heads) - 1;
+            heads &= heads - 1;
+            const int64_t r = __shfl_sync(~0u, ray, src);
+            float acc[W];
+#pragma unroll
+            for (int k = 0; k < W; ++k) acc[k] = 0.f;
+            for (int64_t base = w * 32 + src;; base += 32) {
+                const int64_t j = base + lane;
+                const bool same = j < n && (ridx ? ray_of(j) == r : j == base);
+                const uint32_t stop = ~__ballot_sync(~0u, same);
+                const int end = stop ? __ffs(stop) - 1 : 32;        // the run continues in lanes [0, end) of this block
+                if (lane < end) {
+#pragma unroll
+                    for (int q = 0; q < W / 4; ++q) {
+                        const float4 a = *reinterpret_cast<const float4 *>(rows + j * W + 4 * q);
+                        acc[4 * q] += a.x; acc[4 * q + 1] += a.y; acc[4 * q + 2] += a.z; acc[4 * q + 3] += a.w;
+                    }
+                }
+                if (end < 32) break;
+            }
+#pragma unroll
+            for (int k = 0; k < W; ++k)
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1) acc[k] += __shfl_xor_sync(~0u, acc[k], off);
+            if (lane < n_out) {
+                float v = acc[0];
+#pragma unroll
+                for (int k = 1; k < W; ++k) v = lane == k ? acc[k] : v;
+                const int which = lane / out.k;
+                float *o = which == 0 ? out.p[0] : (which == 1 ? out.p[1] : out.p[2]);
+                if (o) atomicAdd(o + (ray_map ? ray_map[r] : r) * out.k + (lane - which * out.k), v);
+            }
+        }
+    }
+}
+
+// blocks of k_ray_row_sum over n rows: 8 warps of 32 rows per block, at most 2^20 blocks (the warps loop beyond)
+inline unsigned row_sum_blocks(int64_t n) {
+    const int64_t blocks = (n + 255) / 256;
+    return (unsigned)(blocks < (1 << 20) ? blocks : (1 << 20));
 }
 
 // Host: the LoTD layout and decoder the wgmma kernels are built for -> their kernel arguments (0, or 2 with the error set).

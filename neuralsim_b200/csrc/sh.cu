@@ -6,30 +6,6 @@
 
 namespace nsb {
 
-// analytic d(basis)/d(x,y,z); rows dx, dy, dz of length C^2
-__device__ __forceinline__ void sh_jacobian(float x, float y, float z, int C, float *dx, float *dy, float *dz) {
-    dx[0] = dy[0] = dz[0] = 0.f;
-    if (C <= 1) return;
-    dx[1] = 0.f; dy[1] = -0.48860251190291987f; dz[1] = 0.f;
-    dx[2] = 0.f; dy[2] = 0.f; dz[2] = 0.48860251190291987f;
-    dx[3] = -0.48860251190291987f; dy[3] = 0.f; dz[3] = 0.f;
-    if (C <= 2) return;
-    const float x2 = x * x, y2 = y * y, z2 = z * z;
-    dx[4] = 1.0925484305920792f * y;  dy[4] = 1.0925484305920792f * x;  dz[4] = 0.f;
-    dx[5] = 0.f;                      dy[5] = -1.0925484305920792f * z; dz[5] = -1.0925484305920792f * y;
-    dx[6] = 0.f;                      dy[6] = 0.f;                      dz[6] = 1.8923493915151199f * z;
-    dx[7] = -1.0925484305920792f * z; dy[7] = 0.f;                      dz[7] = -1.0925484305920792f * x;
-    dx[8] = 1.0925484305920792f * x;  dy[8] = -1.0925484305920792f * y; dz[8] = 0.f;
-    if (C <= 3) return;
-    dx[9] = -3.5402615395598609f * x * y;            dy[9] = 1.7701307697799304f * (y2 - x2);          dz[9] = 0.f;
-    dx[10] = 2.8906114426405538f * y * z;            dy[10] = 2.8906114426405538f * x * z;             dz[10] = 2.8906114426405538f * x * y;
-    dx[11] = 0.f;                                    dy[11] = 0.45704579946446572f * (1.0f - 5.0f * z2); dz[11] = -4.5704579946446572f * y * z;
-    dx[12] = 0.f;                                    dy[12] = 0.f;                                     dz[12] = 1.1195289977703462f * (5.0f * z2 - 1.0f);
-    dx[13] = 0.45704579946446572f * (1.0f - 5.0f * z2); dy[13] = 0.f;                                  dz[13] = -4.5704579946446572f * x * z;
-    dx[14] = 2.8906114426405538f * x * z;            dy[14] = -2.8906114426405538f * y * z;            dz[14] = 1.4453057213202769f * (x2 - y2);
-    dx[15] = 1.7701307697799304f * (y2 - x2);        dy[15] = 3.5402615395598609f * x * y;             dz[15] = 0.f;
-}
-
 __global__ void __launch_bounds__(256)
 k_sh_fwd(const float *__restrict__ in, float *__restrict__ out, int64_t n, int C, float *__restrict__ dy_dx) {
     const int C2 = C * C;

@@ -3,7 +3,7 @@
 `fused_color(model, ridx, t, rays_o, rays_d, view_dirs, h_appear)` computes, for the packed samples x = o[ridx] + d[ridx] t,
 what `LoTDNeuS.forward(x, v=, h_appear=, nablas_has_grad=True)` computes in the reference
 (nr3d_lib/models/fields/neus/lotd_neus.py:141-167): sdf, nablas (analytic, differentiable -> second-order table / decoder
-gradients) and rgb; appearance codes that require grad get their gradient (summed over each ray's samples).  The unfused module path (`LoTDNeuS.forward`) stays the specification the tests compare against.
+gradients) and rgb; appearance codes, rays and view directions that require grad get their gradient (summed over each ray's samples).  The unfused module path (`LoTDNeuS.forward`) stays the specification the tests compare against.
 With `with_rgb=False` it is `forward_sdf_nablas` alone (k_color_fwd<false>: no radiance head runs, two activation tiles are kept instead of
 four, and only the table and the decoder are inputs of the op), for models without a radiance net and for rays that render no rgb.
 """
@@ -81,10 +81,11 @@ class ColorQuery:
 
 
 class _FusedColor(autograd.Function):
-    """q: ColorQuery; params: the five SDF parameters (table, W1, b1, W2, b2), then the six radiance parameters when rgb is computed"""
+    """q: ColorQuery; params: the five SDF parameters (table, W1, b1, W2, b2), then the six radiance parameters when rgb is computed.
+    rays_o / rays_d (or None): the rays q holds detached copies of, as inputs of the op, so that learnable rays get their gradient."""
 
     @staticmethod
-    def forward(ctx, q, ridx, t, view_dirs, h_appear, keep, *params):
+    def forward(ctx, q, ridx, t, view_dirs, h_appear, rays_o, rays_d, keep, *params):
         rad = len(params) > 5
         n, dev = t.numel(), t.device
         sdf = torch.empty(n, dtype=torch.float32, device=dev)
@@ -104,6 +105,7 @@ class _FusedColor(autograd.Function):
                    ctypes.byref(q.collect) if q.collect is not None else None, L.stream_ptr(), count=q.count)
         ctx.q, ctx.ridx, ctx.t, ctx.n, ctx.rad = q, ridx, t, n, rad
         ctx.ha_shape = h_appear.shape if h_appear is not None else None
+        ctx.vd = view_dirs
         ctx.held = (acts, rgb)
         ctx.shapes = [p.shape for p in params]
         ctx.set_materialize_grads(False)
@@ -130,9 +132,13 @@ class _FusedColor(autograd.Function):
             grads.append(small[o:o + k].view(sh))
             o += k
         # the code gradient: of the op's h_appear input, or into the step's buffer (ColorQuery.appear_grad)
-        d_ha = torch.zeros(ctx.ha_shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[4] else None
+        ng = ctx.needs_input_grad
+        d_ha = torch.zeros(ctx.ha_shape, dtype=torch.float32, device=dev) if ng[4] else None
         appear = (d_ha, None) if d_ha is not None else q.appear_grad
-        ret = (None,) * 4 + (d_ha, None, (d_grid if q.table_grad is None else None)) + tuple(grads[1:])
+        # the gradients of learnable rays and view directions (summed per ray in the call)
+        zeros3 = lambda want, like: torch.zeros(like.shape, dtype=torch.float32, device=dev) if want else None
+        d_vd, d_ro, d_rd = zeros3(ng[3] and ctx.rad, ctx.vd), zeros3(ng[5], q.rays_o), zeros3(ng[6], q.rays_d)
+        ret = (None,) * 3 + (d_vd, d_ha, d_ro, d_rd, None, (d_grid if q.table_grad is None else None)) + tuple(grads[1:])
         if g_sdf is None and g_nab is None and g_rgb is None:
             return ret
         c = lambda g: None if g is None else g.contiguous().float()
@@ -143,8 +149,17 @@ class _FusedColor(autograd.Function):
         args = (q.meta.c_ref, P(q.grid16, "f16"), ctypes.byref(q.net), None, P(q.rays_o, "f32"), P(q.rays_d, "f32"), P(ctx.ridx, "i64"), P(ctx.t, "f32"),
                 L.c_i64(n), L.c_i32(q.ml), P(acts[0]), P(acts[1]), *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]), P(rgb, allow_none=True),
                 P(g_sdf, allow_none=True), P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh, allow_none=True), *ag)
+        rays = d_ro is not None or d_rd is not None or (d_vd is not None and g_rgb is not None)
         with L.KERNEL_TIMER.time("fused_color_bwd", n):
-            if appear is not None and g_rgb is not None:
+            if rays:
+                ha = appear if (appear is not None and g_rgb is not None) else (None, None)
+                ha_rows = torch.empty(n, 8, dtype=torch.float32, device=dev) if ha[0] is not None else None
+                ray_rows = torch.empty(n, 36, dtype=torch.float32, device=dev)      # per-sample ray rows and radiance input gradients
+                L.call(L.lib().nsb_fused_color_bwd_grads, "fused_color_bwd_grads", *args, P(ctx.vd, "f32", allow_none=True),
+                       P(ha_rows, allow_none=True), P(ha[1], "i64", allow_none=True), P(ha[0], "f32", allow_none=True), P(ray_rows),
+                       P(d_ro, allow_none=True), P(d_rd, allow_none=True), P(d_vd if g_rgb is not None else None, allow_none=True), L.stream_ptr(),
+                       count=q.count)
+            elif appear is not None and g_rgb is not None:
                 ha_rows = torch.empty(n, 8, dtype=torch.float32, device=dev)        # per-sample code gradients, summed per ray in the call
                 L.call(L.lib().nsb_fused_color_bwd_appear, "fused_color_bwd_appear", *args, P(ha_rows), P(appear[1], "i64", allow_none=True),
                        P(appear[0], "f32"), L.stream_ptr(), count=q.count)
@@ -155,8 +170,8 @@ class _FusedColor(autograd.Function):
 
 def fused_color(model, ridx, t, rays_o, rays_d, view_dirs=None, h_appear=None, *, nablas_has_grad=True, collect=None, with_rgb=True):
     """-> dict(sdf [n], nablas [n,3], rgb [n,3] (with_rgb only), x [n,3]).  Gradients flow to the table and the decoder, and with rgb to the
-    radiance net and to h_appear [R, n_appear] if it requires grad (the samples of a ray must then be consecutive, as packed samples are,
-    for the per-ray sum to be deterministic)."""
+    radiance net, and to h_appear [R, n_appear], rays_o, rays_d [R, 3] and view_dirs [R, 3] if they require grad (the samples of a ray must
+    then be consecutive, as packed samples are, for the per-ray sums to be deterministic; the depths t are constants)."""
     s = model.implicit_surface
     d = s.decoder.layers
     params = (s.encoding.flattened_params, d[0].weight, d[0].bias, d[1].weight, d[1].bias)
@@ -167,9 +182,10 @@ def fused_color(model, ridx, t, rays_o, rays_d, view_dirs=None, h_appear=None, *
     q = ColorQuery(s.encoding.meta, grid16, net, held, rays_o.detach().contiguous().float(), rays_d.detach().contiguous().float(), s._ml(model.max_level),
                    collect, None)
     ha = None if (h_appear is None or not with_rgb) else h_appear.contiguous().float()
-    keep = torch.is_grad_enabled() and (any(p.requires_grad for p in params) or (ha is not None and ha.requires_grad))
-    vd = view_dirs.detach().contiguous().float() if with_rgb else None
-    out = _FusedColor.apply(q, ridx.reshape(-1).contiguous().long(), t.detach().reshape(-1).contiguous().float(), vd, ha, keep, *params)
+    vd = view_dirs.contiguous().float() if with_rgb else None
+    ro, rd = (rays_o, rays_d) if (rays_o.requires_grad or rays_d.requires_grad) else (None, None)
+    keep = torch.is_grad_enabled() and (any(p.requires_grad for p in params) or any(v is not None and v.requires_grad for v in (ha, vd, ro, rd)))
+    out = _FusedColor.apply(q, ridx.reshape(-1).contiguous().long(), t.detach().reshape(-1).contiguous().float(), vd, ha, ro, rd, keep, *params)
     sdf, nab, x = out[0], out[1], out[-1]
     if not nablas_has_grad:
         nab = nab.detach()

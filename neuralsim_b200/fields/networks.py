@@ -157,12 +157,20 @@ def sdf_fwd(meta, grid16, dec, sdf, max_level, *, x=None, rays_o=None, rays_d=No
     return sdf
 
 
-def sdf_bwd(meta, grid16, dec, d_sdf, n, max_level, grads, *, x=None, rays=None, keep=None, count=None):
+def sdf_bwd(meta, grid16, dec, d_sdf, n, max_level, grads, *, x=None, rays=None, keep=None, count=None, ray_grads=None):
     """one launch of the fused SDF backward (nsb_fused_sdf_bwd_indexed), accumulated into grads = (d_grid, d_W1, d_b1, d_W2, d_b2): row i of
-    the n rows is sample keep[i] (keep None: i) of the points x or of rays = (rays_o, rays_d, ridx, t)"""
+    the n rows is sample keep[i] (keep None: i) of the points x or of rays = (rays_o, rays_d, ridx, t).  ray_grads = (d_rays_o | None,
+    d_rays_d | None) (rays only): nsb_fused_sdf_bwd_rays also adds each ray's gradient into them"""
     P = L.ptr
-    pts = (P(x, "f32"), None, None, None, None) if x is not None else (None, P(rays[0], "f32"), P(rays[1], "f32"), P(rays[2], "i64"), P(rays[3], "f32"))
     d_grid, d_W1, d_b1, d_W2, d_b2 = grads
+    if ray_grads is not None:
+        gx = torch.empty(n, 8, dtype=torch.float32, device=d_sdf.device)              # per-row ray gradients, summed per ray in the call
+        L.call(L.lib().nsb_fused_sdf_bwd_rays, "fused_sdf_bwd_rays", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), P(rays[0], "f32"),
+               P(rays[1], "f32"), P(rays[2], "i64"), P(rays[3], "f32"), P(d_sdf, "f32"), P(keep, "i64", allow_none=True), L.c_i64(n),
+               L.c_i32(max_level), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2), P(gx), None, P(ray_grads[0], "f32", allow_none=True),
+               P(ray_grads[1], "f32", allow_none=True), L.stream_ptr(), count=count)
+        return
+    pts = (P(x, "f32"), None, None, None, None) if x is not None else (None, P(rays[0], "f32"), P(rays[1], "f32"), P(rays[2], "i64"), P(rays[3], "f32"))
     L.call(L.lib().nsb_fused_sdf_bwd_indexed, "fused_sdf_bwd", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), *pts, P(d_sdf, "f32"),
            P(keep, "i64", allow_none=True), L.c_i64(n), L.c_i32(max_level), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2), L.stream_ptr(), count=count)
 
@@ -170,10 +178,12 @@ def sdf_bwd(meta, grid16, dec, d_sdf, n, max_level, grads, *, x=None, rays=None,
 class _FusedSDF(autograd.Function):
     """sdf = decoder(LoTD(x)) as ONE op with a hand-written backward (csrc/fused_tc.cu): forward keeps nothing but its
     inputs, backward recomputes features / pre-activations and accumulates straight into fp32 gradients of the table and
-    the four decoder tensors.  `x` is either points [N,3] or a (ridx, t, rays_o, rays_d, packs | None) tuple (x = o[ridx] + d[ridx] t)."""
+    the four decoder tensors.  `x` is either points [N,3] or a (ridx, t, rays_o, rays_d, packs | None) tuple (x = o[ridx] + d[ridx] t).
+    With the tuple, the optional inputs rays_o / rays_d are the rays the tuple holds detached copies of: when they require grad, the
+    backward returns their gradient (the depths t are constants, as in the reference)."""
 
     @staticmethod
-    def forward(ctx, owner, pts, max_level, collect, grid, W1, b1, W2, b2):
+    def forward(ctx, owner, pts, max_level, collect, grid, W1, b1, W2, b2, rays_o=None, rays_d=None):
         grid16, dec = owner._fused_state()
         meta = owner.encoding.meta
         if isinstance(pts, tuple):
@@ -189,6 +199,7 @@ class _FusedSDF(autograd.Function):
         ctx.owner, ctx.pts, ctx.max_level, ctx.n = owner, pts, max_level, n
         ctx.held = (grid16, dec, owner._fused_cache[1])          # the fp16 images the forward used (the tensors `dec` points into stay alive)
         ctx.shapes = (grid.shape, W1.shape, b1.shape, W2.shape, b2.shape)
+        ctx.ray_shapes = (rays_o.shape if rays_o is not None else None, rays_d.shape if rays_d is not None else None)
         return sdf
 
     @staticmethod
@@ -203,13 +214,17 @@ class _FusedSDF(autograd.Function):
         d_W1, d_b1 = small[:ks[0]].view(w1s), small[ks[0]:ks[0] + ks[1]].view(b1s)
         d_W2, d_b2 = small[ks[0] + ks[1]:ks[0] + ks[1] + ks[2]].view(w2s), small[ks[0] + ks[1] + ks[2]:].view(b2s)
         d_sdf = d_sdf.contiguous().float()
+        ng = ctx.needs_input_grad
+        d_ro = torch.zeros(ctx.ray_shapes[0], dtype=torch.float32, device=dev) if len(ng) > 9 and ng[9] else None
+        d_rd = torch.zeros(ctx.ray_shapes[1], dtype=torch.float32, device=dev) if len(ng) > 10 and ng[10] else None
+        ray_grads = (d_ro, d_rd) if (d_ro is not None or d_rd is not None) else None
         # Most boundary points of a NeuS ray carry an exactly-zero cotangent (saturated sigmoid far from the surface, samples
         # behind the early-stop): only the others are recomputed (the reference's scatter kernel skips them one by one).
         from ..graphics.neus_fused import scan_counts      # compaction without a driver-level sync (the size is polled from pinned memory)
         keep = scan_counts(d_sdf.ne(0).to(torch.int32), want_index=True)["index"]
         n = keep.numel()
         if n == 0:
-            return None, None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2
+            return None, None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2, d_ro, d_rd
         sparse = n < 0.9 * ctx.n
         if sparse:
             d_sdf = d_sdf[keep]
@@ -222,8 +237,8 @@ class _FusedSDF(autograd.Function):
             x, rays = (ctx.pts[keep] if sparse else ctx.pts), None
         n = n if sparse else ctx.n
         with L.KERNEL_TIMER.time("fused_sdf_bwd", n):
-            sdf_bwd(meta, grid16, dec, d_sdf, n, ctx.max_level, (d_grid, d_W1, d_b1, d_W2, d_b2), x=x, rays=rays)
-        return None, None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2
+            sdf_bwd(meta, grid16, dec, d_sdf, n, ctx.max_level, (d_grid, d_W1, d_b1, d_W2, d_b2), x=x, rays=rays, ray_grads=ray_grads)
+        return None, None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2, d_ro, d_rd
 
 
 class LoTDSDF(nn.Module):
@@ -277,7 +292,10 @@ class LoTDSDF(nn.Module):
             ridx = ridx.unsqueeze(-1).expand(shape)
         pts = (ridx.reshape(-1).contiguous().long(), t.detach().reshape(-1).contiguous().float(), rays_o.detach().contiguous(),
                rays_d.detach().contiguous(), packs)
-        sdf = _FusedSDF.apply(self, pts, self._ml(max_level), collect, self.encoding.flattened_params, d[0].weight, d[0].bias, d[1].weight, d[1].bias)
+        # learnable rays (pose refinement) are inputs of the op, so that it returns their gradient
+        rays = (rays_o, rays_d) if (rays_o.requires_grad or rays_d.requires_grad) else ()
+        sdf = _FusedSDF.apply(self, pts, self._ml(max_level), collect, self.encoding.flattened_params, d[0].weight, d[0].bias, d[1].weight, d[1].bias,
+                              *rays)
         return sdf.view(shape)
 
     def forward_sdf_nablas(self, x, *, has_grad: bool = None, nablas_has_grad: bool = None, max_level: int = None, grad_guard=None):

@@ -79,7 +79,7 @@ class LoTDNeuS(nn.Module):
         if self.implicit_surface._fusable():
             if not torch.is_grad_enabled():
                 return dict(sdf=self.implicit_surface.fused_sdf_rays(ridx, t, rays_o, rays_d, max_level=self.max_level, packs=packs, collect=collect))
-            if not (t.requires_grad or rays_o.requires_grad or rays_d.requires_grad):
+            if not t.requires_grad:                              # learnable rays get their gradient from the fused op
                 return dict(sdf=self.implicit_surface.fused_sdf_rays_autograd(ridx, t, rays_o, rays_d, max_level=self.max_level, packs=packs,
                                                                               collect=collect))
         if t.dim() == 2:

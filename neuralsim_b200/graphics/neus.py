@@ -234,9 +234,9 @@ def _query_fused_tail(model, ray_tested, view_dirs, rays_h_appear, rays_o, rays_
 
 def _net_forward_into(volume_buffer, model, rays_o, rays_d, view_dirs, rays_h_appear, ridx_all, depths, *, nablas_has_grad,
                       with_rgb, with_normal, dtype, cond_kw=None):
-    fused = (FUSED_STAGES and cond_kw is None and not depths.requires_grad
-             # learnable rays (pose refinement): the reference's model.forward(x = o + d t) carries d(loss)/d(rays); the fused op detaches them
-             and not (rays_o.requires_grad or rays_d.requires_grad))
+    # learnable rays (pose refinement) and their view directions get their gradient from the fused ops, as from the reference's
+    # model.forward(x = o + d t, v): the depths are constants
+    fused = FUSED_STAGES and cond_kw is None and not depths.requires_grad
     if fused and not with_rgb and with_normal and getattr(model, "_geometry_fusable", lambda: False)():
         # LiDAR-style rays (with_rgb=False, with_normal=True: code_single/tools/train.py:900) and models without a radiance net: sdf +
         # second-order nablas from the geometry-only fused op; no radiance head runs and nothing reaches a radiance net
@@ -244,8 +244,8 @@ def _net_forward_into(volume_buffer, model, rays_o, rays_d, view_dirs, rays_h_ap
         volume_buffer["net_x"] = out["x"]
         volume_buffer["nablas"] = out["nablas"].to(dtype)
         return
-    # appearance codes that require grad (per-image codes in training) get their gradient from the fused op; view directions do not
-    if (fused and with_rgb and view_dirs is not None and getattr(model, "_color_fusable", lambda: False)() and not view_dirs.requires_grad):
+    # appearance codes that require grad (per-image codes in training) get their gradient from the fused op, as do rays and view directions
+    if fused and with_rgb and view_dirs is not None and getattr(model, "_color_fusable", lambda: False)():
         out = model.forward_on_rays(ridx_all, depths, rays_o, rays_d, view_dirs, rays_h_appear, nablas_has_grad=nablas_has_grad)
         volume_buffer["net_x"] = out["x"]
         volume_buffer["nablas"] = out["nablas"].to(dtype)
@@ -305,7 +305,7 @@ def neus_ray_query_march_occ_multi_upsample_compressed(
 
     if (FUSED_STAGES and not cond and cfg.num_coarse > 0 and rays_o.is_cuda and dtype == torch.float32 and hasattr(model, "forward_sdf_on_rays")
             and getattr(getattr(model.accel, "occ", None), "occ_grid", None) is not None and model.accel.occ.occ_grid.dim() == 3
-            and not (rays_o.requires_grad or rays_d.requires_grad or near.requires_grad or far.requires_grad) and cfg.march_fusable):
+            and not (near.requires_grad or far.requires_grad) and cfg.march_fusable):
         ret = _query_fused(model, ray_tested, view_dirs, rays_h_appear, cfg, perturb=perturb, with_rgb=with_rgb, with_normal=with_normal,
                            forward_inv_s=forward_inv_s)
         if ret is not None:

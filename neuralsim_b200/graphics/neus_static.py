@@ -283,7 +283,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         # the code gradient of the compacted ray r goes to row rays_inds[r] of d_h_appear (the kernels stop at the device counts)
         q = ColorQuery(st.meta, st.grid16, st.net, st.held, st.rays_o, st.rays_d, st.ml, st.collect, (cnt, CNT_SLOTS["kept"]), st.table_grad,
                        (d_h_appear, rays_inds) if d_h_appear is not None else None)
-        out = _FusedColor.apply(q, ridx_k, t_k, view_dirs, ha_c, keep_acts, *params)
+        out = _FusedColor.apply(q, ridx_k, t_k, view_dirs, ha_c, None, None, keep_acts, *params)
         nab, x = out[1], out[-1]
         rgb = out[2] if with_rgb else None
         if not cfg.nablas_has_grad:

@@ -7,7 +7,7 @@ process, each timed with CUDA events around whole steps (forward + backward, end
   graph-off     StaticFrame with h_appear_grad=False (codes read, no code gradient)
   graph-on      StaticFrame with h_appear_grad=True
   graph-on+apply  the same, and the trainer's codes[image].backward(frame.d_h_appear) after each replay
-Then k_color_rad_bwd<false> / <true> and k_appear_ray_sum under torch.profiler (a separate run of host-sized steps with detached and
+Then k_color_rad_bwd<false> / <true> and k_ray_row_sum under torch.profiler (a separate run of host-sized steps with detached and
 with learnable codes).  Prints one JSON line per round and a summary line with the GPU name, power limit and SM clocks read in the same run.
 
     python profiles/appear_grad_step.py --steps 20 --warmup 5 --rounds 3
@@ -116,7 +116,7 @@ def main():
                 C.loss_cam(renderer.render(model, o, d, rays_h_appear=ha)["rendered"]).backward()
             torch.cuda.synchronize()
         for e in prof.key_averages():
-            if "k_color_rad_bwd" in e.key or "k_appear_ray_sum" in e.key:
+            if "k_color_rad_bwd" in e.key or "k_ray_row_sum" in e.key:
                 kern[f"{label}: {e.key.split('(')[0]}"] = dict(calls=e.count, us_per_call=round(e.device_time_total / max(e.count, 1), 1))
     print(json.dumps(dict(summary={k: dict(median_ms=round(statistics.median(v), 3), min_ms=round(min(v), 3)) for k, v in times.items()},
                           kernels=kern, steps=args.steps, rounds=args.rounds, rays=C.N_CAM, gpu=gpu_info(),
