@@ -286,7 +286,7 @@ int nsb_fused_sdf_bwd_rays(const nsb_lotd_meta *meta_host, const void *params_ha
  * Here a size may stay in device memory: nsb_bind_device_counts(c0, c1) binds one or two device int64 to the calling thread; the NEXT
  * count-aware entry point of that thread consumes (and clears) the binding and its kernel processes min(n_arg, *c0) items -- n_arg
  * (the `n` / `n_packs` / `n_rays` / `n_list` argument) then is the CAPACITY the buffers and the grid were sized for.  c1 is the second
- * count of nsb_assemble_boundary (n_hit).  Count-aware: nsb_gather_rays, nsb_ray_marching_listed (first round: num_steps of the rays
+ * count of nsb_assemble_boundary (n_hit).  Count-aware: nsb_gather_rays / _backward, nsb_ray_marching_listed (first round: num_steps of the rays
  * in [*c0, n_rays) is written as 0; second round: the listed rays), nsb_ray_marching_record / nsb_march_compact (the same), nsb_fused_sdf_collect / _rays / _packs, nsb_ray_block_order, nsb_fused_sdf_bwd(_indexed),
  * nsb_neus_upsample_cdf, nsb_packed_invert_cdf_shared_u, nsb_merge_sorted_vals, nsb_assemble_boundary, nsb_neus_alpha_forward
  * (num_steps of the packs in [*c0, n_packs) is written as 0) / _backward / _backward_kept / _backward_kept_list, nsb_compact_samples, nsb_scatter_f32, nsb_flag_nonzero,
@@ -409,6 +409,15 @@ int nsb_ray_block_order(const int64_t *pix, const int64_t *via, int64_t n_packs,
  * the compacted outputs. */
 int nsb_gather_rays(const int64_t *idx, int64_t n, const float *o_n, const float *d_n, const float *near, const float *far, float *o_c,
                     float *d_c, float *near_c, float *far_c, const float *extra, float *extra_c, int32_t extra_cols, void *stream);
+/* The adjoint of nsb_ray_test_aabb's normalisation (o' = (o - c) / r, d' = d / r), of nsb_gather_rays, and of the view directions
+ * view_dirs = d_c / clamp(|d_c|, 1e-10) with the norm held constant (aabb.py normalize_rays; neus_ray_query.py:793-794): the gradient to
+ * the caller's rays for learnable rays.  g_o, g_d, g_vd [R, 3]: the gradient to the compacted ray j's o_c, d_c and view_dirs, held at row
+ * idx[j] (the ray map the SDF and colour backward passes add through); vnorm[n]: the clamped norms the forward divided by, in compacted
+ * order (needed with g_vd; g_vd NULL: no view-direction term, as for rays that render no rgb).  radius3: HOST pointer to 3 floats.
+ * For j < n, i = idx[j]:  d_rays_o[i] = (0 + g_o[i]) / r,  d_rays_d[i] = (0 + (g_d[i] + g_vd[i] / vnorm[j])) / r  (IEEE division, the
+ * order torch autograd adds and divides in).  Other rows are not written: the caller zero-fills them. */
+int nsb_gather_rays_backward(const int64_t *idx, int64_t n, const float *radius3, const float *g_o, const float *g_d, const float *g_vd,
+                             const float *vnorm, float *d_rays_o, float *d_rays_d, void *stream);
 
 /* ---------------------------------------------------------------- occupancy-grid maintenance (csrc/occ_ema.cu)
  * OccGridEma._step_update_occ (nr3d_lib/models/accelerations/occgrid/ema_single.py:176-190; occgrid/utils.py:63-101) in three small launches:

@@ -73,6 +73,8 @@ def lib():
         # the backward passes with ray gradients (colour: + view_dirs, codes and rays; SDF: rays)
         _lib.nsb_fused_color_bwd_grads.argtypes = [vp] * 8 + [i64, i32] + [vp] * 28 + [vp]
         _lib.nsb_fused_sdf_bwd_rays.argtypes = [vp] * 9 + [i64, i32] + [vp] * 9 + [vp]
+        # the adjoint of the ray test's normalisation and gather (count-aware): idx, n, radius3 (host float[3]), 6 pointers, stream
+        _lib.nsb_gather_rays_backward.argtypes = [vp, i64] + [vp] * 7 + [vp]
     return _lib
 
 

@@ -450,6 +450,37 @@ k_gather_rays(const int64_t *__restrict__ idx, int64_t n, const float *__restric
     }
 }
 
+// Adjoint of the ray test's normalisation and gather, and of the view directions, for learnable rays:
+//   o' = (o - c) / r, d' = d / r              (nr3d_lib/models/spatial/aabb.py:71-80, normalize_rays)
+//   o_c = o'[idx], d_c = d'[idx]              (k_gather_rays; aabb.py:97-99 indexes the rays that pass)
+//   view_dirs = d_c / clamp(|d_c|, 1e-10)     with the norm detached (nr3d_lib/graphics/neus/neus_ray_query.py:793-794)
+// g_o, g_d, g_vd hold the loss's gradient to o_c, d_c and view_dirs of compacted ray j at row idx[j] (the caller's order: the SDF and
+// colour backward passes add their per-ray sums there through the ray map idx); vnorm[j] is the clamped norm the forward divided by.
+// For j below the count, with i = idx[j]:
+//   d_o[i] = (0 + g_o[i]) / r          d_d[i] = (0 + (g_d[i] + g_vd[i] / vnorm[j])) / r          (per axis; g_vd NULL: no view term)
+// which is what torch autograd computes for the same chain: the three contributions to d_c arrive as colour + boundary (both inside
+// g_d) and then the view term (DivBackward of view_dirs, created before both ops, runs after them), the index backward adds onto zeros,
+// and the division's backward divides by r (IEEE division, not a reciprocal).  Rows of rays that fail the test are not written.
+__global__ void __launch_bounds__(256)
+k_gather_rays_backward(const int64_t *__restrict__ idx, int64_t n, const float r0, const float r1, const float r2,
+                       const float *__restrict__ g_o, const float *__restrict__ g_d, const float *__restrict__ g_vd, const float *__restrict__ vnorm,
+                       float *__restrict__ d_o, float *__restrict__ d_d, const int64_t *__restrict__ n_dev) {
+    n = eff_n(n, n_dev);
+    const float r[3] = {r0, r1, r2};
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
+        const int64_t i = idx[j];
+        const float vn = g_vd ? vnorm[j] : 1.f;
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            float gd = g_d[i * 3 + d];
+            if (g_vd) gd = __fadd_rn(gd, __fdiv_rn(g_vd[i * 3 + d], vn));
+            d_o[i * 3 + d] = __fdiv_rn(__fadd_rn(0.f, g_o[i * 3 + d]), r[d]);
+            d_d[i * 3 + d] = __fdiv_rn(__fadd_rn(0.f, gd), r[d]);
+        }
+    }
+}
+
 // flag[i] = (v[i] != 0) for i < n_eff, 0 up to the capacity n: the input of the scan that compacts the samples with a non-zero cotangent
 __global__ void __launch_bounds__(256)
 k_flag_nonzero(const float *__restrict__ v, int64_t n, int32_t *__restrict__ flag, const int64_t *__restrict__ n_dev) {
@@ -613,4 +644,15 @@ extern "C" int nsb_gather_rays(const int64_t *idx, int64_t n, const float *o_n, 
     NSB_REQUIRE(extra_cols == 0 || (extra && extra_c), "nsb_gather_rays: extra payload needs both pointers");
     k_gather_rays<<<wave_grid(n, 256, 8), 256, 0, STREAM>>>(idx, n, o_n, d_n, near, far, o_c, d_c, near_c, far_c, extra, extra_c, extra_cols, dn.a);
     return check_launch("nsb_gather_rays");
+}
+
+extern "C" int nsb_gather_rays_backward(const int64_t *idx, int64_t n, const float *radius3, const float *g_o, const float *g_d, const float *g_vd,
+                                        const float *vnorm, float *d_rays_o, float *d_rays_d, void *stream) {
+    const DevCounts dn = take_counts();
+    if (n == 0) return 0;
+    NSB_REQUIRE(idx && radius3 && g_o && g_d && d_rays_o && d_rays_d, "nsb_gather_rays_backward: NULL argument");
+    NSB_REQUIRE(!g_vd || vnorm, "nsb_gather_rays_backward: the view-direction term needs vnorm");
+    k_gather_rays_backward<<<wave_grid(n, 256, 8), 256, 0, STREAM>>>(idx, n, radius3[0], radius3[1], radius3[2], g_o, g_d, g_vd, vnorm, d_rays_o,
+                                                                     d_rays_d, dn.a);
+    return check_launch("nsb_gather_rays_backward");
 }

@@ -37,9 +37,11 @@ class SharedTableGrad:
     def __init__(self):
         self.buf = None
 
-    def route(self, table):
-        """-> the table as the input of the nodes that scatter into this holder"""
-        return _TableGradSink.apply(self, table)
+    def route(self, table, anchor=None):
+        """-> the table as the input of the nodes that scatter into this holder.  anchor (optional): a tensor that requires grad, an input
+        of the identity node too, so that the nodes' outputs require grad -- and their backward passes run -- even when the table does not
+        (a step that returns only gradients to its inputs); its node's backward runs after this one's, so after all the nodes'"""
+        return _TableGradSink.apply(self, table, anchor)
 
     def take(self, shape, device):
         """(inside a backward) -> the buffer, zero-filled by the first caller of this backward pass"""
@@ -52,7 +54,7 @@ class _TableGradSink(autograd.Function):
     """identity on the table; its backward passes the holder's buffer on (see SharedTableGrad)"""
 
     @staticmethod
-    def forward(ctx, holder, table):
+    def forward(ctx, holder, table, anchor=None):
         ctx.holder = holder
         ctx.set_materialize_grads(False)
         return table.view_as(table)
@@ -63,7 +65,7 @@ class _TableGradSink(autograd.Function):
         buf, ctx.holder.buf = ctx.holder.buf, None
         if g is not None:                          # a consumer that returned its own table gradient
             buf = g if buf is None else buf.add_(g)
-        return None, buf
+        return None, buf, None
 
 
 class ColorQuery:
@@ -71,13 +73,17 @@ class ColorQuery:
     tensors it points at, the rays, max level, the occupancy collection, the device count (_lib.call's count=, None: host-sized),
     the step's shared table gradient (a SharedTableGrad, None: the backward fills its own) and the step's appearance-code gradient
     (None, or (d_h_appear, ray_map): the backward adds the code gradient of ray r into d_h_appear[ray_map[r]], which the caller
-    zero-fills -- for codes that are not an autograd input of the op, as in the one-launch step)"""
-    __slots__ = ("meta", "grid16", "net", "held", "rays_o", "rays_d", "ml", "collect", "count", "table_grad", "appear_grad")
+    zero-fills -- for codes that are not an autograd input of the op, as in the one-launch step) and the step's ray gradient (None, or
+    (d_rays_o, d_rays_d, d_view_dirs | None, ray_map): the backward adds ray r's gradient to its rays and view direction at row
+    ray_map[r] of the caller's zero-filled buffers; the entry point takes one ray map, so with both it must be the codes' one)"""
+    __slots__ = ("meta", "grid16", "net", "held", "rays_o", "rays_d", "ml", "collect", "count", "table_grad", "appear_grad", "ray_grad")
 
-    def __init__(self, meta, grid16, net, held, rays_o, rays_d, ml, collect, count, table_grad=None, appear_grad=None):
+    def __init__(self, meta, grid16, net, held, rays_o, rays_d, ml, collect, count, table_grad=None, appear_grad=None, ray_grad=None):
         self.meta, self.grid16, self.net, self.held = meta, grid16, net, held
         self.rays_o, self.rays_d, self.ml, self.collect, self.count = rays_o, rays_d, ml, collect, count
-        self.table_grad, self.appear_grad = table_grad, appear_grad
+        self.table_grad, self.appear_grad, self.ray_grad = table_grad, appear_grad, ray_grad
+        if appear_grad is not None and ray_grad is not None and appear_grad[1] is not ray_grad[3]:
+            raise RuntimeError("ColorQuery: the code and ray gradients must share one ray map")
 
 
 class _FusedColor(autograd.Function):
@@ -149,15 +155,18 @@ class _FusedColor(autograd.Function):
         args = (q.meta.c_ref, P(q.grid16, "f16"), ctypes.byref(q.net), None, P(q.rays_o, "f32"), P(q.rays_d, "f32"), P(ctx.ridx, "i64"), P(ctx.t, "f32"),
                 L.c_i64(n), L.c_i32(q.ml), P(acts[0]), P(acts[1]), *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]), P(rgb, allow_none=True),
                 P(g_sdf, allow_none=True), P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh, allow_none=True), *ag)
-        rays = d_ro is not None or d_rd is not None or (d_vd is not None and g_rgb is not None)
+        # the ray targets: the op's ray inputs (rows in ray order), or the step's buffers (ColorQuery.ray_grad, through its ray map)
+        ro_t, rd_t, vd_t, ray_map = (d_ro, d_rd, d_vd, None) if q.ray_grad is None else q.ray_grad
+        rays = ro_t is not None or rd_t is not None or (vd_t is not None and g_rgb is not None)
         with L.KERNEL_TIMER.time("fused_color_bwd", n):
             if rays:
                 ha = appear if (appear is not None and g_rgb is not None) else (None, None)
                 ha_rows = torch.empty(n, 8, dtype=torch.float32, device=dev) if ha[0] is not None else None
                 ray_rows = torch.empty(n, 36, dtype=torch.float32, device=dev)      # per-sample ray rows and radiance input gradients
+                ray_map = ha[1] if ray_map is None else ray_map
                 L.call(L.lib().nsb_fused_color_bwd_grads, "fused_color_bwd_grads", *args, P(ctx.vd, "f32", allow_none=True),
-                       P(ha_rows, allow_none=True), P(ha[1], "i64", allow_none=True), P(ha[0], "f32", allow_none=True), P(ray_rows),
-                       P(d_ro, allow_none=True), P(d_rd, allow_none=True), P(d_vd if g_rgb is not None else None, allow_none=True), L.stream_ptr(),
+                       P(ha_rows, allow_none=True), P(ray_map, "i64", allow_none=True), P(ha[0], "f32", allow_none=True), P(ray_rows),
+                       P(ro_t, allow_none=True), P(rd_t, allow_none=True), P(vd_t if g_rgb is not None else None, allow_none=True), L.stream_ptr(),
                        count=q.count)
             elif appear is not None and g_rgb is not None:
                 ha_rows = torch.empty(n, 8, dtype=torch.float32, device=dev)        # per-sample code gradients, summed per ray in the call

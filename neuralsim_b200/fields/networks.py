@@ -160,15 +160,16 @@ def sdf_fwd(meta, grid16, dec, sdf, max_level, *, x=None, rays_o=None, rays_d=No
 def sdf_bwd(meta, grid16, dec, d_sdf, n, max_level, grads, *, x=None, rays=None, keep=None, count=None, ray_grads=None):
     """one launch of the fused SDF backward (nsb_fused_sdf_bwd_indexed), accumulated into grads = (d_grid, d_W1, d_b1, d_W2, d_b2): row i of
     the n rows is sample keep[i] (keep None: i) of the points x or of rays = (rays_o, rays_d, ridx, t).  ray_grads = (d_rays_o | None,
-    d_rays_d | None) (rays only): nsb_fused_sdf_bwd_rays also adds each ray's gradient into them"""
+    d_rays_d | None[, ray_map]) (rays only): nsb_fused_sdf_bwd_rays also adds each ray's gradient into them (at row ray_map[ray])"""
     P = L.ptr
     d_grid, d_W1, d_b1, d_W2, d_b2 = grads
     if ray_grads is not None:
         gx = torch.empty(n, 8, dtype=torch.float32, device=d_sdf.device)              # per-row ray gradients, summed per ray in the call
+        ray_map = ray_grads[2] if len(ray_grads) > 2 else None
         L.call(L.lib().nsb_fused_sdf_bwd_rays, "fused_sdf_bwd_rays", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), P(rays[0], "f32"),
                P(rays[1], "f32"), P(rays[2], "i64"), P(rays[3], "f32"), P(d_sdf, "f32"), P(keep, "i64", allow_none=True), L.c_i64(n),
-               L.c_i32(max_level), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2), P(gx), None, P(ray_grads[0], "f32", allow_none=True),
-               P(ray_grads[1], "f32", allow_none=True), L.stream_ptr(), count=count)
+               L.c_i32(max_level), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2), P(gx), P(ray_map, "i64", allow_none=True),
+               P(ray_grads[0], "f32", allow_none=True), P(ray_grads[1], "f32", allow_none=True), L.stream_ptr(), count=count)
         return
     pts = (P(x, "f32"), None, None, None, None) if x is not None else (None, P(rays[0], "f32"), P(rays[1], "f32"), P(rays[2], "i64"), P(rays[3], "f32"))
     L.call(L.lib().nsb_fused_sdf_bwd_indexed, "fused_sdf_bwd", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), *pts, P(d_sdf, "f32"),

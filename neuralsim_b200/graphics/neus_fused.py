@@ -17,7 +17,7 @@ import torch
 from .. import _lib as L
 
 __all__ = ["upsample_cdf", "sample_cdf_uniform", "neus_alpha_compress", "neus_alpha_compact", "composite", "scan_counts", "merge_sorted_vals",
-           "assemble_boundary", "march_lean", "upsample_rays", "block_order", "ray_block_order", "ray_test_aabb", "gather_rays", "scan_launch", "march_listed",
+           "assemble_boundary", "march_lean", "upsample_rays", "block_order", "ray_block_order", "ray_test_aabb", "gather_rays", "gather_rays_backward", "scan_launch", "march_listed",
            "pack_occ_bits", "alpha_forward", "compact_samples"]
 
 # `count=` of the launch functions below: None, or (cnt, k0[, k1]) -- the sizes live in the device count block cnt and the size arguments
@@ -224,6 +224,16 @@ def gather_rays(idx, n, tested, out, extra=None, extra_c=None, *, count=None):
     (o_n, d_n, nr, fr), (o_c, d_c, n_c, f_c), P = tested, out, L.ptr
     L.call(L.lib().nsb_gather_rays, "gather_rays", P(idx, "i64"), L.c_i64(n), P(o_n), P(d_n), P(nr), P(fr), P(o_c), P(d_c), P(n_c), P(f_c),
            P(extra, allow_none=True), P(extra_c, allow_none=True), L.c_i32(0 if extra is None else extra.shape[1]), L.stream_ptr(), count=count)
+
+
+def gather_rays_backward(idx, n, radius3, grads, vnorm, out, *, count=None):
+    """nsb_gather_rays_backward: the adjoint of ray_test_aabb's normalisation, gather_rays and the view directions.  grads = (g_o, g_d,
+    g_vd | None) [R, 3] in the caller's row order (row idx[j] of compacted ray j), vnorm [n] the compacted rays' clamped direction norms
+    (None without g_vd), radius3 the box's host float[3] half-size -> out = (d_rays_o, d_rays_d) [R, 3], rows idx[:n] written (the caller
+    zero-fills the others)"""
+    (g_o, g_d, g_vd), (d_o, d_d), P = grads, out, L.ptr
+    L.call(L.lib().nsb_gather_rays_backward, "gather_rays_backward", P(idx, "i64"), L.c_i64(n), radius3, P(g_o, "f32"), P(g_d, "f32"),
+           P(g_vd, "f32", allow_none=True), P(vnorm, "f32", allow_none=True), P(d_o, "f32"), P(d_d, "f32"), L.stream_ptr(), count=count)
 
 
 @torch.no_grad()

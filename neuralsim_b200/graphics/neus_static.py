@@ -130,15 +130,35 @@ class _StaticBoundary(torch.autograd.Function):
             keep = torch.empty(n_list, dtype=torch.int64, device=dev)
             _call(lib.nsb_neus_alpha_backward_kept_list, "neus_alpha_backward_kept_list", cnt, CNT_SLOTS["kept_rays"], None, *a, P(g, "f32"),
                   P(d_sdf, "f32"), P(offs, "i32"), L.c_i64(R), P(keep), P(ray), L.stream_ptr())
+            # with the ray gradient, the listed samples' rows (one per list slot: the scratch is sized n_list) are summed per ray -- a ray's
+            # listed samples are consecutive, so the sums are deterministic -- into the step's accumulators (st.ray_grads)
             with L.KERNEL_TIMER.time("fused_sdf_bwd", n_list):
                 sdf_bwd(st.meta, st.grid16, st.dec, d_sdf, n_list, st.ml, (d_grid, d_W1, d_b1, d_W2, d_b2), rays=(st.rays_o, st.rays_d, ray, d1), keep=keep,
-                        count=(cnt, CNT_SLOTS["nonzero"]))
+                        count=(cnt, CNT_SLOTS["nonzero"]), ray_grads=st.ray_grads)
         return (None,) * 8 + (d_inv.reshape(inv_shape), None, d_W1, d_b1, d_W2, d_b2)
+
+
+class _RayGradAdjoint(torch.autograd.Function):
+    """identity on a scalar leaf that requires grad (the anchor of the table's route node, SharedTableGrad.route).  Autograd runs this
+    backward after the route node's, which runs after every node that reads the routed table -- the boundary and the colour query -- so
+    here both have added their ray rows into the step's accumulators, and `run` maps them onto the caller's rays
+    (nsb_gather_rays_backward)."""
+
+    @staticmethod
+    def forward(ctx, run, anchor):
+        ctx.run = run
+        return anchor.view_as(anchor)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, _g):
+        ctx.run()
+        return None, None
 
 
 class _State:
     """what the kernels of one static step share"""
-    __slots__ = ("meta", "grid16", "dec", "net", "held", "rays_o", "rays_d", "ml", "collect", "cnt", "ws", "table_grad")
+    __slots__ = ("meta", "grid16", "dec", "net", "held", "rays_o", "rays_d", "ml", "collect", "cnt", "ws", "table_grad", "ray_grads")
 
 
 def _fp16_images(model, radiance=True):
@@ -159,11 +179,14 @@ def _fp16_images(model, radiance=True):
 
 
 def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=None, march_cap, kept_cap, coherent=False, with_rgb=True, with_normal=True,
-                  perturb=False, training=None, depth_use_normalized_vw=True, cnt=None, d_h_appear=None):
+                  perturb=False, training=None, depth_use_normalized_vw=True, cnt=None, d_h_appear=None, d_rays=None):
     """One chunk of rays, ray test -> query -> integration, without a host read.  -> (rendered dict of whole-chunk images, cnt int64[32]).
     `coherent`: image-ordered rays (the boundary / fine queries then walk the samples ray-tiled) -- a host decision here (the host-sized
     path measures it in the ray-test kernel).  `d_h_appear` [R, n_appear] (optional): zero-filled here, and the backward pass writes the
-    gradient of the codes rays_h_appear into it, in the caller's ray order (the codes themselves are read detached)."""
+    gradient of the codes rays_h_appear into it, in the caller's ray order (the codes themselves are read detached).  `d_rays` =
+    (d_rays_o, d_rays_d) [R, 3] (optional): the same for the rays -- zero-filled here, and the backward pass writes the gradient of the
+    loss to rays_o and rays_d (the caller's frame and order; 0 for rays that miss the box or keep no sample), the depths held constant
+    as on the host-sized path."""
     P, lib = L.ptr, L.lib()
     if with_rgb and getattr(model, "radiance_net", None) is None:
         raise RuntimeError("render_static(with_rgb=True): the model has no radiance net (radiance_cfg=False); render it with with_rgb=False")
@@ -214,7 +237,17 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
             d_h_appear.zero_()                              # the backward adds each kept ray's sum once into its row
         NF.gather_rays(rays_inds, R, tested[:4], (o_c, d_c, n_c, f_c), ha, ha_c, count=(cnt, CNT_SLOTS["n_rays"]))
         st.rays_o, st.rays_d = o_c, d_c
-        view_dirs = (d_c / d_c.norm(dim=-1).clamp_min(1.0e-10).unsqueeze(-1)).contiguous() if with_rgb else None
+        vnorm = d_c.norm(dim=-1).clamp_min(1.0e-10) if with_rgb else None         # held constant, as the host-sized path holds it
+        view_dirs = (d_c / vnorm.unsqueeze(-1)).contiguous() if with_rgb else None
+        st.ray_grads, ray_g = None, None
+        if d_rays is not None:
+            # the backward passes add each compacted ray's gradient to its o_c, d_c (and view direction) at the ray's row in the caller's
+            # order -- the ray map of the codes, which the colour entry point shares -- and the adjoint of the ray test then divides by r
+            for t in d_rays:
+                t.zero_()
+            ray_g = torch.zeros(3 if with_rgb else 2, R, 3, device=dev)
+            ray_g = (ray_g[0], ray_g[1], ray_g[2] if with_rgb else None)           # g_o, g_d, g_vd (no view term without rgb)
+            st.ray_grads = (ray_g[0], ray_g[1], rays_inds)
         # ---------------- coarse samples + march
         coarse = batch_sample_step_linear(n_c, f_c, nc1, prefix_shape=[R], perturb=perturb).contiguous()
         occ_grid = model.accel.occ.occ_grid
@@ -266,7 +299,14 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     s = model.implicit_surface
     dl = s.decoder.layers
     inv_s = model.forward_inv_s()
-    table = st.table_grad.route(s.encoding.flattened_params)            # the table as both backward nodes' input
+    anchor = None
+    if d_rays is not None:
+        # after both backward nodes: the adjoint of the ray test, from the accumulators to the caller's rays (the anchor also makes the
+        # nodes run when no parameter requires grad: a pose refined against a fixed model)
+        def ray_adjoint():
+            NF.gather_rays_backward(rays_inds, R, r3, ray_g, vnorm, d_rays, count=(cnt, CNT_SLOTS["n_rays"]))
+        anchor = _RayGradAdjoint.apply(ray_adjoint, torch.zeros((), device=dev, requires_grad=True))
+    table = st.table_grad.route(s.encoding.flattened_params, anchor)    # the table as both backward nodes' input
     if not isinstance(inv_s, torch.Tensor):
         inv_s = torch.tensor(float(inv_s), device=dev)
     alpha_k, t_k, ridx_k, pinfo_kept, rays_inds_hit = _StaticBoundary.apply(
@@ -279,10 +319,12 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         if with_rgb:
             b = model.radiance_net.blocks.layers
             params += (b[0].weight, b[0].bias, b[1].weight, b[1].bias, b[2].weight, b[2].bias)
-        keep_acts = torch.is_grad_enabled() and (any(p.requires_grad for p in params) or d_h_appear is not None)
-        # the code gradient of the compacted ray r goes to row rays_inds[r] of d_h_appear (the kernels stop at the device counts)
+        keep_acts = torch.is_grad_enabled() and (any(p.requires_grad for p in params) or d_h_appear is not None or d_rays is not None)
+        # the code (and ray) gradient of the compacted ray r goes to row rays_inds[r] of d_h_appear (and of the ray accumulators; the
+        # kernels stop at the device counts)
         q = ColorQuery(st.meta, st.grid16, st.net, st.held, st.rays_o, st.rays_d, st.ml, st.collect, (cnt, CNT_SLOTS["kept"]), st.table_grad,
-                       (d_h_appear, rays_inds) if d_h_appear is not None else None)
+                       (d_h_appear, rays_inds) if d_h_appear is not None else None,
+                       ray_g + (rays_inds,) if d_rays is not None else None)
         out = _FusedColor.apply(q, ridx_k, t_k, view_dirs, ha_c, None, None, keep_acts, *params)
         nab, x = out[1], out[-1]
         rgb = out[2] if with_rgb else None
@@ -333,13 +375,22 @@ class StaticFrame:
     passed (rows of rays that keep no sample are 0; each step overwrites it).  The codes are inputs the caller copies in, so the caller
     applies it to its own codes, e.g. `codes.backward(frame.d_h_appear)`.
 
+    `ray_grad=True` (off by default, for the same reasons): every step also writes `frame.d_rays_o` and `frame.d_rays_d` [n_rays, 3], the
+    gradient of the loss with respect to the rays passed, in their order and frame (world; the depths are held constant, as on the
+    host-sized path; rows of rays that miss the box or keep no sample are 0; each step overwrites them).  The rays are copied in, so a
+    trainer that refines its pose applies the gradient to the pose itself, outside the graph:
+
+        o, d = pose_transform(pose, rays_o_cam, rays_d_cam)       # learnable rays
+        loss = frame.step(o.detach(), d.detach(), codes)
+        torch.autograd.backward([o, d], [frame.d_rays_o, frame.d_rays_d])      # -> pose.grad
+
     The first call probes the sizes with the host-sized path (SingleVolumeRenderer.ray_query, no grad), sizes the arenas with `slack`,
     warms up and captures.  Gradients are accumulated into `p.grad` (kept in place; `zero_grads=True` or a `pre_hook` zeroes them inside the graph).
     Capture precondition (PyTorch): no autograd graph of an EARLIER backward on the default stream may still be referenced (a kept loss / rendered
     tensor): it pins the parameters' AccumulateGrad nodes to the default stream, which cannot take part in a capture."""
 
     def __init__(self, model, n_rays, loss_fn=None, *, near=None, far=None, with_rgb=True, with_normal=True, slack=1.5, march_cap=None, kept_cap=None,
-                 coherent=None, use_graph=True, zero_grads=False, h_appear_dim=None, pre_hook=None, h_appear_grad=False):
+                 coherent=None, use_graph=True, zero_grads=False, h_appear_dim=None, pre_hook=None, h_appear_grad=False, ray_grad=False):
         self.model, self.n_rays, self.loss_fn = model, int(n_rays), loss_fn
         self.near, self.far, self.with_rgb, self.with_normal, self.slack = near, far, with_rgb, with_normal, float(slack)
         self.march_cap, self.kept_cap, self.coherent = march_cap, kept_cap, coherent
@@ -355,6 +406,9 @@ class StaticFrame:
         if h_appear_grad and (self.h_appear is None or not with_rgb or not model.use_h_appear):
             raise RuntimeError("StaticFrame(h_appear_grad=True): the step renders no rgb from appearance codes")
         self.d_h_appear = torch.zeros(self.n_rays, na, device=dev) if h_appear_grad else None
+        self.d_rays_o = self.d_rays_d = None
+        if ray_grad:
+            self.d_rays_o, self.d_rays_d = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)
         self.cnt = torch.zeros(32, dtype=torch.int64, device=dev)
         self.graph, self.loss, self.rendered, self.buffers, self._occ_captured = None, None, None, None, None
         self.captures = 0
@@ -400,7 +454,7 @@ class StaticFrame:
         try:
             rendered, _, buffers = render_static(self.model, self.rays_o, self.rays_d, self.h_appear, near=self.near, far=self.far, march_cap=self.march_cap,
                                                  kept_cap=self.kept_cap, coherent=bool(self.coherent), with_rgb=self.with_rgb, with_normal=self.with_normal, cnt=self.cnt,
-                                                 d_h_appear=self.d_h_appear)
+                                                 d_h_appear=self.d_h_appear, d_rays=(self.d_rays_o, self.d_rays_d) if self.d_rays_o is not None else None)
         finally:
             if cv is not None:
                 cv._use_w_dev = False

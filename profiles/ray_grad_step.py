@@ -6,8 +6,11 @@ each timed with CUDA events around whole steps (forward + backward, ending in a 
                 the boundary SDF and the colour / normal query on the module path (no-grad march and up-sampling stay fused)
   host-fused    the same step on the fused query with the ray gradient (nsb_fused_sdf_bwd_rays, nsb_fused_color_bwd_grads)
   host-fixed    the fused step with a pose that needs no grad (the same rays, detached): the cost of the ray gradient itself
-The one-launch graph step does not return a ray gradient, so it has no arm.  Prints one JSON line per round and a summary line with the
-GPU name, power limit and SM clocks read in the same run.
+  graph         the one-launch graph step: one StaticFrame for the camera rays (h_appear_grad=True, ray_grad=True) and one for the LiDAR
+                rays (with_rgb=False, ray_grad=True), replayed on the posed rays; the trainer's backward of the codes and of the pose
+                (torch.autograd.backward of the rays with frame.d_rays_o / d_rays_d) runs outside the graphs
+  graph-fixed   the same frames without ray_grad, the pose held fixed (the codes still get their gradient)
+Prints one JSON line per round and a summary line with the GPU name, power limit and SM clocks read in the same run.
 
     python profiles/ray_grad_step.py --steps 20 --warmup 5 --rounds 3
 """
@@ -90,8 +93,37 @@ def main():
         loss = C.loss_cam(r_cam.render(model, o1, d1, rays_h_appear=codes[img])["rendered"]) + C.loss_lidar(r_lidar.render(model, o2, d2)["rendered"])
         loss.backward()
 
+    # the graph step: per arm a camera frame (zeroes the gradients in its graph) and a LiDAR frame (adds to them), sized on every batch
+    from neuralsim_b200.graphics.neus_static import StaticFrame
+    frames = {}
+    for learn in (True, False):
+        fc = StaticFrame(model, C.N_CAM, loss_fn=C.loss_cam, near=C.NEAR, far=C.FAR, slack=2.0, zero_grads=True, h_appear_grad=True, ray_grad=learn)
+        fl = StaticFrame(model, C.N_LIDAR, loss_fn=C.loss_lidar, near=C.NEAR, far=C.FAR, with_rgb=False, slack=2.0, ray_grad=learn)
+        with torch.no_grad():
+            for co, cd, lo, ld, _ in batches:
+                for f, (o, d) in ((fc, pose(params, co, cd)), (fl, pose(params, lo, ld))):
+                    f.rays_o.copy_(o); f.rays_d.copy_(d); f._size()
+        frames[learn] = (fc, fl)
+
+    def graph_step(b, learnable):
+        co, cd, lo, ld, img = b
+        select(False)
+        codes.grad = params.grad = None
+        fc, fl = frames[learnable]
+        p = params if learnable else params.detach()
+        o1, d1 = pose(p, co, cd)
+        o2, d2 = pose(p, lo, ld)
+        ha = codes[img]
+        fc.step(o1.detach(), d1.detach(), ha.detach())
+        fl.step(o2.detach(), d2.detach())
+        if learnable:
+            torch.autograd.backward([ha, o1, d1, o2, d2], [fc.d_h_appear, fc.d_rays_o, fc.d_rays_d, fl.d_rays_o, fl.d_rays_d])
+        else:
+            ha.backward(fc.d_h_appear)
+
     arms = {"host-parent": lambda b: host_step(b, True), "host-fused": lambda b: host_step(b, False),
-            "host-fixed": lambda b: host_step(b, False, learnable=False)}
+            "host-fixed": lambda b: host_step(b, False, learnable=False), "graph": lambda b: graph_step(b, True),
+            "graph-fixed": lambda b: graph_step(b, False)}
     for name, fn in arms.items():
         for s in range(args.warmup):
             fn(batches[s % n_img])
