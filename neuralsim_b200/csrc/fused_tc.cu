@@ -1,6 +1,7 @@
 // Fused forward_sdf and its backward with the decoder GEMMs on the Hopper tensor cores (wgmma), sm_90a.
 //
-// One CTA = 128 threads = one warpgroup = one tile of 128 points; thread r owns point r for the gather and the scatter:
+// One CTA = 128 threads = one warpgroup = one tile of 128 points; thread r owns point r for the gather and the scatter (the ray-tiled
+// query, MODE 2 below, gives the gather and the MMA + epilogue to different warps of a larger CTA, with the same per-row arithmetic):
 //   gather   thread r walks the L (1..16) LoTD levels of its point (8 corner loads each); every level's two fp16 features go
 //            straight into its row of the A tile in shared memory (core-matrix layout of tc_util.cuh), columns 2L..31 are zero
 //   MMA      the warpgroup issues wgmma (M=64, N=64, K=16) x2 per 64-row half: Z[128 x 64] (fp32, registers) = H[128 x 32] . W1^T
@@ -16,55 +17,69 @@ namespace nsb {
 // MODE 2: the same packed samples traversed RAY-TILED: a tile = 32 packs (rays) x 4 consecutive samples, lane = ray, warp = sample
 //         ordinal.  The 32 packs of group g are order[32 g .. 32 g + 32) -- nsb_ray_block_order puts an 8 x 4 pixel block of an image
 //         there -- or, with order == NULL, packs 32 g .. 32 g + 32 (a 32 x 1 strip of one image row).  For coherent rays the 32 lanes
-//         of a gather instruction then sit in neighbouring cells -> few 128 B lines per request; the L1 tag stage is what bounds this
-//         kernel, and a block touches fewer lines than a strip (DESIGN.md §5).  sdf is written to the packed slot, so nothing
-//         downstream changes.  Incoherent rays (random training pixels) keep MODE 1: locality along the ray.
-// CTAs of k_fused_sdf_tc per SM in the persistent grid, points / rays (modes 0, 1) and ray-tiled packs (mode 2).  5 would fit modes 0 and 1
-// (90 registers, ~13 KB of shared memory), but their gather is L1-bound and more warps gathering at once evict each other's lines: on an
-// H100 (NVIDIA H100 80GB HBM3, 700 W) the boundary query of an 800x600 frame, then walked in 32 x 1 strips, took 5.8 ms per launch at
-// 4 CTAs / SM, 7.3-7.4 ms at 5 and 6.5 ms at 6 (bench.py, alternated).  In 8 x 4 pixel blocks a warp touches fewer lines (DESIGN.md §5) and
-// 5 CTAs / SM are faster than 4; measured on an H100 80GB HBM3 at a 400 W power limit in DESIGN.md §6.
-constexpr int kSdfCtasPerSM = 4, kSdfPackCtasPerSM = 5;       // mode 2's register budget is set by __launch_bounds__ (0 = none for modes 0, 1)
+//         of a gather instruction then sit in neighbouring cells -> few 128 B lines per request, and a block touches fewer lines than
+//         a strip (DESIGN.md §5).  sdf is written to the packed slot, so nothing downstream changes.  Incoherent rays (random training
+//         pixels) keep MODE 1: locality along the ray.
+// CTAs of k_fused_sdf_tc per SM in the persistent grid of modes 0 and 1 (points / rays).  5 would fit (90 registers, ~13 KB of shared
+// memory), but their gather is L1-bound and more warps gathering at once evict each other's lines: on an H100 (NVIDIA H100 80GB HBM3,
+// 700 W) the boundary query of an 800x600 frame, then walked in 32 x 1 strips, took 5.8 ms per launch at 4 CTAs / SM, 7.3-7.4 ms at 5
+// and 6.5 ms at 6 (bench.py, alternated).
+constexpr int kSdfCtasPerSM = 4;
 
-template <int MODE>
-__global__ void __launch_bounds__(kTile, MODE == 2 ? kSdfPackCtasPerSM : 0)
-k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ x,
-               const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
-               const float *__restrict__ t, int64_t n, int max_level, float *__restrict__ sdf, const int64_t *__restrict__ pack_infos,
-               const int64_t *__restrict__ pack_ray, const int64_t *__restrict__ order, int64_t n_packs, const OccCollect oc,
-               const int64_t *__restrict__ n_dev) {
-    if (MODE == 2) n_packs = eff_n(n_packs, n_dev); else n = eff_n(n, n_dev);       // device-resident count (nsb_bind_device_counts)
-    __shared__ __align__(128) uint8_t sA[kTile * NF * 2];    // 8 KB : features, chunk-major core-matrix layout
-    __shared__ __align__(128) uint8_t sB[HW * NF * 2];       // 4 KB : W1 [64 x 32], same layout
-    __shared__ float sb1[HW], sW2[HW], srow[kTile];
-    __shared__ float sb2;
+// MODE 2 is warp-specialised: a CTA = one consumer warpgroup (warps 0..3: MMA + epilogue + store) and kPackSets sets of 4 producer warps
+// (the gather), which hand 128-row A tiles over a ring of kPackSlots shared-memory slots guarded by "full" / "empty" mbarriers.  Tile j of
+// a CTA (its groups in grid-stride order, each group's sample ordinals 4 at a time) is gathered by set j % kPackSets into slot
+// j % kPackSlots; the consumer takes the tiles in order.  The gather warps thus never wait on a CTA barrier, the MMA or the SFU epilogue,
+// and the consumer's epilogue of one tile overlaps the gather of the next ones.  One CTA of 5 sets (20 gather warps) per SM, launched at
+// 80 registers and split by setmaxnreg, 72 for the gather and 120 for the 64 accumulators of the epilogue; 7 slots (~71 KB).  On an H100
+// (NVIDIA H100 80GB HBM3, 700 W) the boundary query of an 800x600 frame took 4.31-4.36 ms per step at this size, 4.62-4.65 ms with 4 sets
+// (16 gather warps, 96 registers, no split) and 5.14-5.19 ms before the split into roles (5 CTAs of 128 threads per SM) (bench.py,
+// alternated, DESIGN.md §6).  2 CTAs of 2 sets per SM would cap every thread at 80 registers: the epilogue spills.
+constexpr int kPackSets = 5, kPackSlots = 7, kPackCtasPerSM = 1;
+// registers per thread after the split (setmaxnreg): 20 producer warps x 72 + 4 consumer warps x 120 = the 768 x 80 the CTA is launched with
+constexpr int kPackProducerRegs = 72, kPackConsumerRegs = 120;
+static_assert(kPackSets * kTile * kPackProducerRegs + kTile * kPackConsumerRegs <= kTile * (1 + kPackSets) * 80, "register split");
+constexpr int kPackThreads = kTile * (1 + kPackSets);
+constexpr int kPackSmem = kPackSlots * (kTile * NF * 2 + kTile * 12) + HW * NF * 2 + 2 * HW * 4 + kPackSlots * 20 + 16 + 128;
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    stage_W1(dec, sB, tid);
-    stage_decoder_vectors(dec, sb1, sW2, &sb2, tid);
-    tc::fence_async_smem();
-    __syncthreads();
-    const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
+// one slot of the ring: the A tile (8 KB) and, per row, the output index (-1: no sample) and the occupancy voxel of the sample
+struct PackSlots {
+    uint8_t *a;                            // [kPackSlots][kTile * NF * 2]
+    int64_t *out;                          // [kPackSlots][kTile]
+    int *voxel;                            // [kPackSlots][kTile]
+    uint64_t *full, *empty;                // [kPackSlots]: 128 producer arrivals / 128 consumer arrivals per phase
+    int *end;                              // [kPackSlots]: 1 = no tile, the CTA's work is done
+};
 
-    if (MODE == 2) {
-        const int64_t n_groups = (n_packs + 31) / 32;
-        for (int64_t g = blockIdx.x; g < n_groups; g += gridDim.x) {
-            const int64_t slot = g * 32 + lane;
-            int64_t first = 0, cnt = 0, ray = 0;
-            if (slot < n_packs) {
-                const int64_t p = order ? order[slot] : slot;
-                first = pack_infos[2 * p]; cnt = pack_infos[2 * p + 1]; ray = pack_ray ? pack_ray[p] : p;
-            }
+// the producer side of MODE 2: set `set` walks every group of this CTA, gathers its tiles j (j % kPackSets == set) into the ring and,
+// when it owns the index past the last tile, posts the end marker there.  Lane = pack (ray), warp w of the set = sample ordinal k0 + w.
+__device__ __forceinline__ void sdf_packs_produce(const PLMeta &m, const __half *__restrict__ grid, int max_level, const float *__restrict__ rays_o,
+                                                  const float *__restrict__ rays_d, const float *__restrict__ t, const int64_t *__restrict__ pack_infos,
+                                                  const int64_t *__restrict__ pack_ray, const int64_t *__restrict__ order, int64_t n_packs,
+                                                  const OccCollect &oc, const PackSlots &ring, int set, int w, int lane) {
+    const int row = w * 32 + lane;
+    const int64_t n_groups = (n_packs + 31) / 32;
+    uint32_t j = 0;                                            // the CTA's tile counter
+    for (int64_t g = blockIdx.x; g < n_groups; g += gridDim.x) {
+        const int64_t slot = g * 32 + lane;
+        int64_t first = 0, cnt = 0, ray = 0;
+        if (slot < n_packs) {
+            const int64_t p = order ? order[slot] : slot;
+            first = pack_infos[2 * p]; cnt = pack_infos[2 * p + 1]; ray = pack_ray ? pack_ray[p] : p;
+        }
+        int max_n = (int)cnt;
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) max_n = max(max_n, __shfl_xor_sync(0xffffffffu, max_n, s));
+        const uint32_t tiles = (uint32_t)(max_n + 3) / 4;
+        uint32_t mine = j + (uint32_t)((set - (int)(j % kPackSets) + kPackSets) % kPackSets);   // my first tile index >= j
+        if (mine < j + tiles) {
             float o[3] = {0.f, 0.f, 0.f}, d[3] = {0.f, 0.f, 0.f};
             if (cnt > 0) {
 #pragma unroll
                 for (int q = 0; q < 3; ++q) { o[q] = rays_o[ray * 3 + q]; d[q] = rays_d[ray * 3 + q]; }
             }
-            int max_n = (int)cnt;
-#pragma unroll
-            for (int s = 16; s > 0; s >>= 1) max_n = max(max_n, __shfl_xor_sync(0xffffffffu, max_n, s));
-            for (int k0 = 0; k0 < max_n; k0 += kTile / 32) {
-                const int k = k0 + warp;
+            for (; mine < j + tiles; mine += kPackSets) {
+                const int k = (int)(mine - j) * 4 + w;
                 const bool valid = k < cnt;
                 float xs[3] = {0.f, 0.f, 0.f};
                 if (valid) {
@@ -74,14 +89,112 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
                 }
 #pragma unroll
                 for (int q = 0; q < 3; ++q) xs[q] = to_table_space(xs[q]);
-                const float v = sdf_of_tile(ctx, xs, tid);
-                if (valid) {
-                    sdf[first + k] = v;
-                    if (oc.pcl) occ_collect_point(oc, xs, v);
+                const uint32_t s = mine % kPackSlots;
+                tc::mbar_wait(&ring.empty[s], ((mine / kPackSlots) & 1u) ^ 1u);
+                gather_row_to_tile<kTile>(m, grid, xs, max_level, ring.a + s * (kTile * NF * 2), row);
+                ring.out[s * kTile + row] = valid ? first + k : -1;
+                ring.voxel[s * kTile + row] = (valid && oc.pcl) ? occ_voxel(oc, xs) : 0;
+                tc::fence_async_smem();                        // the tile's generic-proxy writes -> visible to the wgmma (async proxy)
+                tc::mbar_arrive(&ring.full[s]);
+            }
+        }
+        j += tiles;
+    }
+    if ((int)(j % kPackSets) == set) {                         // the end marker, in tile j's place
+        const uint32_t s = j % kPackSlots;
+        tc::mbar_wait(&ring.empty[s], ((j / kPackSlots) & 1u) ^ 1u);
+        if (row == 0) ring.end[s] = 1;
+        tc::mbar_arrive(&ring.full[s]);
+    }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(MODE == 2 ? kPackThreads : kTile, MODE == 2 ? kPackCtasPerSM : 0)
+k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ x,
+               const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
+               const float *__restrict__ t, int64_t n, int max_level, float *__restrict__ sdf, const int64_t *__restrict__ pack_infos,
+               const int64_t *__restrict__ pack_ray, const int64_t *__restrict__ order, int64_t n_packs, const OccCollect oc,
+               const int64_t *__restrict__ n_dev) {
+    const int tid = threadIdx.x;
+    if constexpr (MODE == 2) {
+        const int warp = tid >> 5, lane = tid & 31;
+        n_packs = eff_n(n_packs, n_dev);                       // device-resident count (nsb_bind_device_counts)
+        extern __shared__ uint8_t dyn_smem[];
+        uint8_t *base = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 127) & ~uintptr_t(127));
+        PackSlots ring;
+        ring.a = base;                                                            // kPackSlots x 8 KB : the A tiles
+        uint8_t *sB = ring.a + kPackSlots * (kTile * NF * 2);                     //  4 KB : W1 [64 x 32]
+        ring.out = reinterpret_cast<int64_t *>(sB + HW * NF * 2);
+        ring.voxel = reinterpret_cast<int *>(ring.out + kPackSlots * kTile);
+        float *sb1 = reinterpret_cast<float *>(ring.voxel + kPackSlots * kTile), *sW2 = sb1 + HW;
+        ring.full = reinterpret_cast<uint64_t *>(sW2 + HW);
+        ring.empty = ring.full + kPackSlots;
+        ring.end = reinterpret_cast<int *>(ring.empty + kPackSlots);
+        float *sb2 = reinterpret_cast<float *>(ring.end + kPackSlots);
+        if (tid < kTile) {
+            stage_W1(dec, sB, tid);
+            stage_decoder_vectors(dec, sb1, sW2, sb2, tid);
+        }
+        if (tid < kPackSlots) {
+            tc::mbar_init(&ring.full[tid], kTile);
+            tc::mbar_init(&ring.empty[tid], kTile);
+            ring.end[tid] = 0;
+        }
+        tc::fence_mbar_init();
+        tc::fence_async_smem();
+        __syncthreads();
+        if (warp >= 4) {                                       // producers
+            tc::setmaxnreg_dec<kPackProducerRegs>();
+            sdf_packs_produce(m, grid, max_level, rays_o, rays_d, t, pack_infos, pack_ray, order, n_packs, oc, ring, (warp - 4) >> 2, warp & 3, lane);
+            return;
+        }
+        tc::setmaxnreg_inc<kPackConsumerRegs>();
+        // consumer warpgroup: tile j from slot j % kPackSlots -> MMA -> slot free -> epilogue -> sdf of each row from its quad's lane 0
+        const uint32_t b_addr = tc::smem_u32(sB);
+        const SoftplusK spk(dec.beta);
+        const float b2 = *sb2;
+        for (uint32_t j = 0;; ++j) {
+            const uint32_t s = j % kPackSlots;
+            tc::mbar_wait(&ring.full[s], (j / kPackSlots) & 1u);
+            if (ring.end[s]) break;
+            float z[2][HW / 2];
+            tc::mma_m128<HW, 0, 0, NF / 16>(z, tc::kmajor(tc::smem_u32(ring.a + s * (kTile * NF * 2)), kTile), tc::kmajor(b_addr, HW), false);
+            int64_t out_i[2][2];
+            int vox[2][2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int row = h * 64 + tc::frag_row(i);
+                    out_i[h][i] = ring.out[s * kTile + row];
+                    vox[h][i] = ring.voxel[s * kTile + row];
                 }
+            tc::mbar_arrive(&ring.empty[s]);                   // the MMA has read the tile, the row data are in registers
+            float v[2][2];
+            sdf_rows_of_frags(z, sb1, sW2, spk, v);
+            if ((lane & 3) == 0) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        if (out_i[h][i] < 0) continue;
+                        const float r = r16(v[h][i] + b2);
+                        sdf[out_i[h][i]] = r;
+                        if (oc.pcl) occ_collect_voxel(oc, vox[h][i], r);
+                    }
             }
         }
     } else {
+        n = eff_n(n, n_dev);                                   // device-resident count (nsb_bind_device_counts)
+        __shared__ __align__(128) uint8_t sA[kTile * NF * 2];    // 8 KB : features, chunk-major core-matrix layout
+        __shared__ __align__(128) uint8_t sB[HW * NF * 2];       // 4 KB : W1 [64 x 32], same layout
+        __shared__ float sb1[HW], sW2[HW], srow[kTile];
+        __shared__ float sb2;
+        stage_W1(dec, sB, tid);
+        stage_decoder_vectors(dec, sb1, sW2, &sb2, tid);
+        tc::fence_async_smem();
+        __syncthreads();
+        const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
         const int64_t n_tiles = (n + kTile - 1) / kTile;
         for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             const int64_t i = tile * kTile + tid;
@@ -287,11 +400,12 @@ extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *pa
     const __half *g = (const __half *)params_half;
     const OccCollect oc = occ_collect_of(collect);
     const unsigned tiles = persistent_grid((n + kTile - 1) / kTile, kSdfCtasPerSM);
-    if (mode == 2 && require_ctas_per_sm(k_fused_sdf_tc<2>, kTile, 0, kSdfPackCtasPerSM, "nsb_fused_sdf (packs)")) return 2;
-    if (mode == 2)            // a work unit of mode 2 is a group of 32 packs
-        k_fused_sdf_tc<2><<<persistent_grid((n_packs + 31) / 32, kSdfPackCtasPerSM), kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf,
-                                                                                                 pack_infos, pack_ray, pack_order, n_packs, oc, dn.a);
-    else if (mode == 1)
+    if (mode == 2) {          // a work unit of mode 2 is a group of 32 packs
+        opt_in_smem(k_fused_sdf_tc<2>, kPackSmem);
+        if (int rc = require_ctas_per_sm(k_fused_sdf_tc<2>, kPackThreads, kPackSmem, kPackCtasPerSM, "nsb_fused_sdf (packs)")) return rc;
+        k_fused_sdf_tc<2><<<persistent_grid((n_packs + 31) / 32, kPackCtasPerSM), kPackThreads, kPackSmem, s>>>(
+            m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf, pack_infos, pack_ray, pack_order, n_packs, oc, dn.a);
+    } else if (mode == 1)
         k_fused_sdf_tc<1><<<tiles, kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, ridx, t, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a);
     else
         k_fused_sdf_tc<0><<<tiles, kTile, 0, s>>>(m, g, d, x, nullptr, nullptr, nullptr, nullptr, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a);

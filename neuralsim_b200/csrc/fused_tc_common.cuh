@@ -25,15 +25,21 @@ inline OccCollect occ_collect_of(const nsb_occ_collect *c) {       // NULL or no
     return OccCollect{nullptr, 1, 1, 1, 0.f};
 }
 __device__ __forceinline__ float r16(float v) { return __half2float(__float2half_rn(v)); }
-__device__ __forceinline__ void occ_collect_point(const OccCollect &oc, const float (&xs)[3], float sdf) {
+__device__ __forceinline__ int occ_voxel(const OccCollect &oc, const float (&xs)[3]) {
     const int ix = min(max((int)__fmul_rn(xs[0], (float)oc.rx), 0), oc.rx - 1);
     const int iy = min(max((int)__fmul_rn(xs[1], (float)oc.ry), 0), oc.ry - 1);
     const int iz = min(max((int)__fmul_rn(xs[2], (float)oc.rz), 0), oc.rz - 1);
+    return (ix * oc.ry + iy) * oc.rz + iz;
+}
+__device__ __forceinline__ void occ_collect_voxel(const OccCollect &oc, int voxel, float sdf) {
     // (1. / cosh((inv_s * x / 2.).clamp(-20, 20))) ** 2 on a half tensor: every op rounds to fp16 (maths/common.py:122-133)
     const float a = fminf(fmaxf(r16(r16(__fmul_rn(sdf, oc.inv_s)) * 0.5f), -20.f), 20.f);
     const float r = r16(__fdiv_rn(1.f, r16(coshf(a))));
     const float v = r16(__fmul_rn(r, r));
-    if (v > 0.f) atomicMax(reinterpret_cast<int *>(oc.pcl) + ((ix * oc.ry + iy) * oc.rz + iz), __float_as_int(v));   // v >= 0: int order == float order
+    if (v > 0.f) atomicMax(reinterpret_cast<int *>(oc.pcl) + voxel, __float_as_int(v));   // v >= 0: int order == float order
+}
+__device__ __forceinline__ void occ_collect_point(const OccCollect &oc, const float (&xs)[3], float sdf) {
+    occ_collect_voxel(oc, occ_voxel(oc, xs), sdf);
 }
 
 constexpr int kTile = 128;
@@ -315,33 +321,46 @@ struct SdfTile {
     SoftplusK spk;
 };
 
+// The decoder's epilogue on the accumulator fragments Z = H . W1^T of a 128-row tile (warpgroup-collective): out[h][i] = the 64 -> 1
+// layer of row 64h + tc::frag_row(i) without b2, in every lane of the row's quad.  Each lane folds its 16 of the row's 64 hidden units,
+// the quad sums the four parts in a fixed order (the same for every row, so a point's sdf does not depend on where it sits in the tile).
+__device__ __forceinline__ void sdf_rows_of_frags(const float (&z)[2][HW / 2], const float *sb1, const float *sW2, const SoftplusK &spk,
+                                                  float (&out)[2][2]) {
+    const int q = threadIdx.x & 3;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            float o = 0.f;
+#pragma unroll
+            for (int ch = 0; ch < HW / 8; ++ch)
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const int col = ch * 8 + 2 * q + j;
+                    const float zz = r16(z[h][4 * ch + 2 * i + j] + sb1[col]);
+                    o = fmaf(r16(softplus_a(zz, spk)), sW2[col], o);
+                }
+            o += __shfl_xor_sync(0xffffffffu, o, 1);
+            o += __shfl_xor_sync(0xffffffffu, o, 2);
+            out[h][i] = o;
+        }
+}
+
 // all 128 threads: my point's table coordinates -> my sdf (fp16-rounded, as fp32).  Ends with the CTA barrier that frees the tile.
-// The epilogue runs on the accumulator fragments: each lane folds its 16 of a row's 64 hidden units, the quad sums the four parts
-// in a fixed order (the same for every row, so a point's sdf does not depend on where it sits in the tile).
 __device__ __forceinline__ float sdf_of_tile(const SdfTile &c, const float (&xs)[3], int tid) {
     gather_row_to_tile<kTile>(c.m, c.grid, xs, c.max_level, c.sA, tid);
     tc::fence_async_smem();                // generic-proxy smem writes -> visible to the tensor core (async proxy)
     __syncthreads();
     float z[2][HW / 2];
     tc::mma_m128<HW, 0, 0, NF / 16>(z, tc::kmajor(c.a_addr, kTile), tc::kmajor(c.b_addr, HW), false);
-    const int lane = tid & 31, q = lane & 3;
+    float out[2][2];
+    sdf_rows_of_frags(z, c.sb1, c.sW2, c.spk, out);
+    if ((tid & 3) == 0) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            float out = 0.f;
-#pragma unroll
-            for (int ch = 0; ch < HW / 8; ++ch)
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    const int col = ch * 8 + 2 * q + j;
-                    const float zz = r16(z[h][4 * ch + 2 * i + j] + c.sb1[col]);
-                    out = fmaf(r16(softplus_a(zz, c.spk)), c.sW2[col], out);
-                }
-            out += __shfl_xor_sync(0xffffffffu, out, 1);
-            out += __shfl_xor_sync(0xffffffffu, out, 2);
-            if (q == 0) c.srow[h * 64 + (tid >> 5) * 16 + (lane >> 2) + 8 * i] = out;
-        }
+            for (int i = 0; i < 2; ++i) c.srow[h * 64 + tc::frag_row(i)] = out[h][i];
+    }
     __syncthreads();
     return r16(c.srow[tid] + c.sb2);
 }

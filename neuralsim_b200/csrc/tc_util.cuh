@@ -1,6 +1,6 @@
 // Hopper tensor-core plumbing used by the fused MLP kernels: warpgroup MMAs (wgmma) with both operands in shared memory
-// and fp32 accumulators in registers.  Inline PTX only (no CUTLASS dependency).  Every kernel that uses it runs one
-// warpgroup (128 threads) per CTA; the MMA helpers are collective over it and must be reached by all 128 threads.
+// and fp32 accumulators in registers.  Inline PTX only (no CUTLASS dependency).  The MMA helpers are collective over one
+// warpgroup (128 threads, warps 0..3 of the CTA: frag_row / frag_col read threadIdx.x) and must be reached by all 128 threads.
 //
 // Shared-memory operand layout ("canonical K-major, no swizzle", what cute calls Layout_K_INTER_Atom):
 //   the tile is cut into core matrices of 8 rows x 16 bytes (8 fp16 along K); a core matrix is 128 contiguous
@@ -228,6 +228,11 @@ __device__ __forceinline__ void acc_ld8(const float *acc, int stride, int row, i
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
+// one arrival of the calling thread (release: its earlier shared-memory writes are visible to whoever waits on the phase)
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// returns once the phase of parity `parity` has completed (the barrier starts in phase 0: parity 1 passes at once)
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tWAIT_%=:\n\t"
@@ -251,6 +256,12 @@ __device__ __forceinline__ void tma_load_bulk(void *smem_dst, const void *gmem_s
                  ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
                  : "memory");
 }
+
+// warp-specialised kernels: hand registers from the warpgroups that need few to those that need many (sm_90a; N % 8 == 0, warpgroup-collective)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
