@@ -290,7 +290,7 @@ int nsb_fused_sdf_bwd_rays(const nsb_lotd_meta *meta_host, const void *params_ha
  * in [*c0, n_rays) is written as 0; second round: the listed rays), nsb_ray_marching_record / nsb_march_compact (the same), nsb_fused_sdf_collect / _rays / _packs, nsb_ray_block_order, nsb_fused_sdf_bwd(_indexed),
  * nsb_neus_upsample_cdf, nsb_packed_invert_cdf_shared_u, nsb_merge_sorted_vals, nsb_assemble_boundary, nsb_neus_alpha_forward
  * (num_steps of the packs in [*c0, n_packs) is written as 0) / _backward / _backward_kept / _backward_kept_list, nsb_compact_samples, nsb_scatter_f32, nsb_flag_nonzero,
- * nsb_fused_color_fwd / _bwd, nsb_composite_forward / _backward.  With every size on the device a whole fwd+bwd step has no host
+ * nsb_fused_color_fwd / _bwd, nsb_composite_forward / _backward, nsb_lidar_los_rows / _loss_reduce / _los_backward.  With every size on the device a whole fwd+bwd step has no host
  * read and can be captured in a CUDA graph (neuralsim_b200/graphics/neus_static.py). */
 int nsb_bind_device_counts(const int64_t *count0, const int64_t *count1);
 /* flag[i] = (v[i] != 0) for i < live count, 0 up to n (count-aware). */
@@ -418,6 +418,44 @@ int nsb_gather_rays(const int64_t *idx, int64_t n, const float *o_n, const float
  * order torch autograd adds and divides in).  Other rows are not written: the caller zero-fills them. */
 int nsb_gather_rays_backward(const int64_t *idx, int64_t n, const float *radius3, const float *g_o, const float *g_d, const float *g_vd,
                              const float *vnorm, float *d_rays_o, float *d_rays_d, void *stream);
+
+/* ---------------------------------------------------------------- the StreetSurf LiDAR loss (csrc/lidar_loss.cu)
+ * LidarLoss.forward with the depth term and the `neus_unisim` line-of-sight term (app/loss/lidar.py:174-210, 254-294) on the renderer's
+ * own buffers, and its adjoint: the cotangents of the composite's depth_volume and vw (nsb_composite_backward's g_depth, g_vw).  R rays
+ * (the whole-image index; R is the batch, never a device count); blk = {w_depth, w_los, epsilon}: device fp32[3], refreshed by the host
+ * before each step.  fn_type: 0 = l1 (recon.py:40-53), 1 = l2_relative (x - y)^2 / (x^2 + 1e-2) (recon.py:119-129).  All sums are
+ * deterministic; every fp32 operation rounds as torch's does (no contraction).
+ *
+ * nsb_lidar_mask_err: mask[r] = (mask_pred[r] > thresh) & (gt[r] > 0), REPLACED by gt[r] <= discard_toofar if has_toofar (lidar.py:264-266:
+ *   the reference assigns there); err[r] = |pred[r] - gt[r]| mask[r] (l1_loss(.., reduction='none'), lidar.py:280; loss/utils.py:31-32).
+ * nsb_kth_smallest: *out = torch.sort(v).values[k] bit for bit, on the device (lidar.py:281-283 with k = R // 2): an 8-bit-digit radix
+ *   select on keys that order like torch.sort (NaN last; a NaN result is returned without its sign).  n <= 65536: one CTA, one launch;
+ *   beyond that, four histogram passes over `scratch` (nsb_kth_smallest_scratch_bytes(); zero-filled here).  n < 2^31, 0 <= k < n.
+ * nsb_lidar_rows: mask[r] &= !(err[r] > *median * median_factor) (strict >, the product rounded in fp32; median NULL: no discard,
+ *   lidar.py:284); depth_row[r] = f(pred[r], gt[r]) mask[r] (may be NULL); los_row[r] = 0 (may be NULL).
+ * nsb_lidar_los_rows: one warp per kept ray p < n_packs (count-aware: the rays that keep samples): los_row[rays_inds_hit[p]] =
+ *   mask[r] sum_i [|t_i - gt[r]| > epsilon] vw_i^2 over the ray's samples (lidar.py:195-199: the per-ray packed_sum).
+ * nsb_lidar_loss_reduce: out[0] = w_depth sum_r depth_row[r] / R (the 'mean' reduction divides by R, loss/utils.py:21-22);
+ *   out[1] = w_los sum_r los_row[r] / n_kept, 0 when n_kept == 0 (lidar.py:208-210; count-aware: n_kept).  One CTA, fp64 sums over the
+ *   R whole-image rows in one fixed order: the result does not depend on the kept-sample arena or the kept rays' order.  Either row
+ *   array may be NULL (that term is 0).
+ * nsb_lidar_depth_backward: g_depth[r] = f'(pred, gt) mask[r] g_out[0] w_depth / R (l1: sign with sign(0) = 0; l2_relative: both the
+ *   numerator and the denominator differentiated, as autograd does).  The mask is a constant (the reference's `.data`).
+ * nsb_lidar_los_backward: g_vw[i] = g_out[1] w_los / n_kept mask[r] [|t_i - gt[r]| > epsilon] 2 vw_i for the samples of the kept rays
+ *   (count-aware: n_kept); other rows of g_vw are not written. */
+int64_t nsb_kth_smallest_scratch_bytes(void);
+int nsb_lidar_mask_err(const float *pred, const float *mask_pred, const float *gt, int64_t n, float mask_pred_thresh, int32_t has_toofar,
+                       float discard_toofar, float *mask, float *err, void *stream);
+int nsb_kth_smallest(const float *v, int64_t n, int64_t k, float *out, void *scratch, void *stream);
+int nsb_lidar_rows(const float *pred, const float *gt, const float *err, const float *median, float median_factor, int32_t fn_type, int64_t n,
+                   float *mask, float *depth_row, float *los_row, void *stream);
+int nsb_lidar_los_rows(const float *t, const float *vw, const int64_t *pack_infos, const int64_t *rays_inds_hit, int64_t n_packs,
+                       const float *gt, const float *mask, const float *blk, float *los_row, void *stream);
+int nsb_lidar_loss_reduce(const float *depth_row, const float *los_row, int64_t n, int64_t n_kept, const float *blk, float *out, void *stream);
+int nsb_lidar_depth_backward(const float *pred, const float *gt, const float *mask, int64_t n, int32_t fn_type, const float *blk,
+                             const float *g_out, float *g_depth, void *stream);
+int nsb_lidar_los_backward(const float *t, const float *vw, const int64_t *pack_infos, const int64_t *rays_inds_hit, int64_t n_packs,
+                           const float *gt, const float *mask, const float *blk, const float *g_out, float *g_vw, void *stream);
 
 /* ---------------------------------------------------------------- occupancy-grid maintenance (csrc/occ_ema.cu)
  * OccGridEma._step_update_occ (nr3d_lib/models/accelerations/occgrid/ema_single.py:176-190; occgrid/utils.py:63-101) in three small launches:

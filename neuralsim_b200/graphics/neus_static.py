@@ -27,7 +27,7 @@ from .neus import query_config, upsample_boundary
 from .raysample import batch_sample_step_linear
 from . import neus_fused as NF
 
-__all__ = ["render_static", "StaticFrame", "CNT_SLOTS"]
+__all__ = ["render_static", "StaticFrame", "CNT_SLOTS", "static_volume_buffer"]
 
 CNT_SLOTS = dict(n_rays=0, pairs=2, marched_raw=3, hit_raw=4, kept_raw=6, kept_rays_raw=7, nonzero=9, marched=12, hit=13, fine0=14,
                  boundary=18, kept=19, overflow=20, kept_rays=21, merged0=22, rays_if_kept_fits=26, row_len=27)
@@ -361,6 +361,15 @@ def sliced_volume_buffer(buffers, cnt):
     return vb
 
 
+def static_volume_buffer(buffers, cnt):
+    """The volume buffer a loss inside the captured step reads (StaticFrame(loss_on_ret=True)): the step's capacity-sized kept-sample
+    buffers t, vw [kept_cap], rays_inds_hit, pack_infos_hit [R], ridx, with their sizes in the device count block `cnt` (CNT_SLOTS:
+    "kept" samples, "kept_rays" rays).  No host read.  Its type "packed_static" is one the reference's losses refuse, so nothing reads
+    the capacity-sized tensors as if they were exact-size."""
+    return dict(type="packed_static", t=buffers["t"], vw=buffers["vw"], rays_inds_hit=buffers["rays_inds_hit"], pack_infos_hit=buffers["pack_infos_hit"],
+                ridx=buffers["ridx"], cnt=cnt, CNT_SLOTS=CNT_SLOTS)
+
+
 # ---------------------------------------------------------------------------------------------------------------- one-launch step
 class StaticFrame:
     """fwd (+ loss + bwd) of one fixed-size ray batch as ONE CUDA graph launch.
@@ -384,14 +393,20 @@ class StaticFrame:
         loss = frame.step(o.detach(), d.detach(), codes)
         torch.autograd.backward([o, d], [frame.d_rays_o, frame.d_rays_d])      # -> pose.grad
 
+    `loss_on_ret=True` (off by default: then `loss_fn(rendered)`): `loss_fn` receives the reference-shaped `ret = {"rendered": ...,
+    "volume_buffer": vb}`, vb = static_volume_buffer(...) (the capacity-sized kept-sample buffers and their device counts), so a loss on
+    the per-sample buffers -- neuralsim_b200.loss.LidarLoss -- runs inside the captured step.  Per-step inputs of such a loss are static
+    buffers the caller refreshes before `step()` (LidarLoss.set_step).
+
     The first call probes the sizes with the host-sized path (SingleVolumeRenderer.ray_query, no grad), sizes the arenas with `slack`,
     warms up and captures.  Gradients are accumulated into `p.grad` (kept in place; `zero_grads=True` or a `pre_hook` zeroes them inside the graph).
     Capture precondition (PyTorch): no autograd graph of an EARLIER backward on the default stream may still be referenced (a kept loss / rendered
     tensor): it pins the parameters' AccumulateGrad nodes to the default stream, which cannot take part in a capture."""
 
     def __init__(self, model, n_rays, loss_fn=None, *, near=None, far=None, with_rgb=True, with_normal=True, slack=1.5, march_cap=None, kept_cap=None,
-                 coherent=None, use_graph=True, zero_grads=False, h_appear_dim=None, pre_hook=None, h_appear_grad=False, ray_grad=False):
-        self.model, self.n_rays, self.loss_fn = model, int(n_rays), loss_fn
+                 coherent=None, use_graph=True, zero_grads=False, h_appear_dim=None, pre_hook=None, h_appear_grad=False, ray_grad=False,
+                 loss_on_ret=False):
+        self.model, self.n_rays, self.loss_fn, self.loss_on_ret = model, int(n_rays), loss_fn, bool(loss_on_ret)
         self.near, self.far, self.with_rgb, self.with_normal, self.slack = near, far, with_rgb, with_normal, float(slack)
         self.march_cap, self.kept_cap, self.coherent = march_cap, kept_cap, coherent
         self.use_graph, self.zero_grads, self.pre_hook = use_graph, zero_grads, pre_hook
@@ -460,7 +475,7 @@ class StaticFrame:
                 cv._use_w_dev = False
         loss = None
         if self.loss_fn is not None:
-            loss = self.loss_fn(rendered)
+            loss = self.loss_fn(dict(rendered=rendered, volume_buffer=static_volume_buffer(buffers, self.cnt)) if self.loss_on_ret else rendered)
             if loss.requires_grad:
                 loss.backward()
             loss = loss.detach()
