@@ -63,6 +63,9 @@ def batched_ray_marching(rays_o, rays_d, t_min, t_max, batch_inds, batch_data_si
     """-> [packed_info, t_starts, t_ends, ridx, bidx, gidx]   (batched_marching.cu:154-287)"""
     if grid_binary.dim() != 4:
         raise RuntimeError("batched_ray_marching: expected grid_binary [B,X,Y,Z]")
+    if batch_data_size and rays_o.shape[0] % int(batch_data_size) != 0:        # batched_marching.cu:206
+        raise RuntimeError(f"batched_ray_marching: Expect nonzero `batch_data_size`={int(batch_data_size)} to be a divisor of "
+                           f"`n_rays`={rays_o.shape[0]}")
     if batch_inds is None:
         if not batch_data_size:
             raise RuntimeError("batched_ray_marching: need batch_inds or batch_data_size")

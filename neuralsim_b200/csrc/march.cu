@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(256) k_ray_marching(const MarchArgs a) {
                     a.t_starts[base + j] = t0;
                     if (a.t_ends) a.t_ends[base + j] = t1;
                     a.ridx[base + j] = (int32_t)i;
-                    if (a.gidx) a.gidx[base + j] = gi;
+                    if (a.gidx) a.gidx[base + j] = (int32_t)(gi + b * cells);   // batched: flat over [B, X, Y, Z] (batched_marching.cu:62,115)
                     if (a.bidx) a.bidx[base + j] = b;
                 } else if (REC) {
                     a.rec_t[i * (int64_t)a.max_steps + j] = t0;

@@ -127,6 +127,8 @@ int nsb_oracle_ray_marching(int n_rays, const float *rays_o, const float *rays_d
             uint32_t n = march_one(rays_o + 3 * i, rays_d + 3 * i, t_min[i], t_max[i], r, res, g, step_size, max_step_size,
                                    dt_gamma, (uint32_t)cnt, i, t_starts + base, t_ends + base, ridx + base,
                                    gidx ? gidx + base : NULL);
+            /* the batched voxel index is flat over [B, X, Y, Z]: grid_idx + batch_ind * X*Y*Z (batched_marching.cu:62,115) */
+            if (gidx) for (uint32_t k = 0; k < n; ++k) gidx[base + k] += (int32_t)(gsz * b);
             if (bidx) for (uint32_t k = 0; k < n; ++k) bidx[base + k] = b;
         }
     }
