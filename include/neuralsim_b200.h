@@ -293,6 +293,13 @@ int nsb_fused_sdf_bwd_rays(const nsb_lotd_meta *meta_host, const void *params_ha
  * nsb_fused_color_fwd / _bwd, nsb_composite_forward / _backward, nsb_lidar_los_rows / _loss_reduce / _los_backward.  With every size on the device a whole fwd+bwd step has no host
  * read and can be captured in a CUDA graph (neuralsim_b200/graphics/neus_static.py). */
 int nsb_bind_device_counts(const int64_t *count0, const int64_t *count1);
+/* The LoTD level bound in device memory, for a step whose level changes between graph replays (the hard-mask level schedule of an
+ * annealed encoding): nsb_bind_device_max_level(level) binds one device int32 to the calling thread; the NEXT level-aware entry point of
+ * that thread consumes (and clears) the binding, and its kernels read *level (clamped to [-1, L-1]) instead of the max_level argument.
+ * Level-aware: the tensor-core SDF query (nsb_fused_sdf_collect in all modes, nsb_fused_sdf_packs, and nsb_fused_sdf / _rays unless they
+ * run the CUDA-core kernel: h_out or the "sdf_simt" option), nsb_fused_sdf_bwd / _bwd_indexed / _bwd_rays, nsb_fused_color_fwd,
+ * nsb_fused_color_bwd / _bwd_appear / _bwd_grads, nsb_upsample_rays / nsb_upsample_persistent.  NULL: the max_level argument (the default). */
+int nsb_bind_device_max_level(const int32_t *level);
 /* flag[i] = (v[i] != 0) for i < live count, 0 up to n (count-aware). */
 int nsb_flag_nonzero(const float *v, int64_t n, int32_t *flag, void *stream);
 /* Derived sizes of one NeuS query in a device block `counts` of >= 32 int64 (zero-filled once per query):

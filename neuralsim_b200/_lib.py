@@ -90,18 +90,25 @@ def slot(cnt, k):
     return ctypes.c_void_p(cnt.data_ptr() + 8 * k)
 
 
-def call(fn, what, *args, count=None):
+def call(fn, what, *args, count=None, level=None):
     """fn(*args) checked.  count = (cnt, k0[, k1]): the launch processes the device-resident counts cnt[k0] (and cnt[k1]) instead of
-    its size arguments, which then are the capacities (nsb_bind_device_counts: bound to this thread for the one call, then cleared)."""
-    if count is None:
+    its size arguments, which then are the capacities (nsb_bind_device_counts: bound to this thread for the one call, then cleared).
+    level: the max_level the call was given; when it is a device int32 scalar, the kernels read it there (nsb_bind_device_max_level, bound
+    for the one call) and the host argument c_level(level) is a placeholder."""
+    dev_level = isinstance(level, torch.Tensor)
+    if count is None and not dev_level:
         check(fn(*args), what)
         return
     l = lib()
-    l.nsb_bind_device_counts(slot(count[0], count[1]), slot(count[0], count[2]) if len(count) > 2 else _NULL)
+    if count is not None:
+        l.nsb_bind_device_counts(slot(count[0], count[1]), slot(count[0], count[2]) if len(count) > 2 else _NULL)
+    if dev_level:
+        l.nsb_bind_device_max_level(ptr(level, "i32", "max_level"))
     try:
         rc = fn(*args)
     finally:
         l.nsb_bind_device_counts(_NULL, _NULL)
+        l.nsb_bind_device_max_level(_NULL)
     check(rc, what)
 
 
@@ -150,6 +157,11 @@ def c_i64(v):
 
 def c_i32(v):
     return ctypes.c_int32(int(v))
+
+
+def c_level(max_level):
+    """the int32 max_level argument of a level-aware entry point; for a device level (see call) a placeholder the kernels do not read"""
+    return c_i32(-1 if isinstance(max_level, torch.Tensor) else max_level)
 
 
 def c_f32(v):

@@ -121,7 +121,10 @@ def accelerate(ref_model, *, patch=True) -> LoTDNeuSModel:
         def _sync(self):
             o = self._nsb
             o.train(self.training)
+            # the level the reference's queries use: `max_level or encoding.max_level` (lotd_neus.py:127, lotd_encoding.py:162); the
+            # model's own max_level stays None, the annealer sets the encoding's (lotd_encoding.py:146-148)
             o.max_level = getattr(self, "max_level", None)
+            o.implicit_surface.encoding.max_level = getattr(self.implicit_surface.encoding, "max_level", None)
             o.upsample_s_divisor = getattr(self, "upsample_s_divisor", 1.0)
             o.ctrl_var.set_iter(getattr(self.ctrl_var, "it", getattr(self, "it", 0)))
             occ_r, occ_o = self.accel.occ, o.accel.occ

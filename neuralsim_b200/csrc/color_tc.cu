@@ -69,17 +69,17 @@ __device__ __forceinline__ void unpack8(const uint4 &q, float (&v)[8]) {
 constexpr int kColorGatherU = 4;
 
 // The one table gather of the colour forward: each level's 8 corners are loaded once and give both its fp16 feature pair (-> row r of the
-// chunk-major X tile, zero above max_level, as gather_row_to_tile writes it) and its Jacobian J0[p], J1[p], which stay in registers until
+// chunk-major X tile, zero from level La on, as gather_row_to_tile writes it) and its Jacobian J0[p], J1[p], which stay in registers until
 // g = U.W1 is known.  Fully unrolled, unlike the rolled gathers of the 16-24-warp kernels, so that J (96 floats) is statically indexed:
 // k_color_fwd runs 8 warps per SM and has no min-blocks bound, so it may use the registers.  The corner loads of kColorGatherU levels are
-// issued before any of them is consumed.  Levels p >= L = m.n_pseudo load nothing and write zero columns; a trip that starts at or above L
-// computes nothing, and in the trip that L cuts the levels >= L see zero corners (their J is zero and never read: nablas stops at L).
-__device__ __forceinline__ void gather_row_and_jacobian(const PLMeta &m, const __half *__restrict__ grid, const float (&xs)[3], int max_level,
+// issued before any of them is consumed.  Only the La active levels (active_levels) are loaded: levels p >= La load nothing and write zero
+// columns; a trip that starts at or above La computes nothing, and in the trip that La cuts the levels >= La see zero corners (their J is
+// zero and never read: nablas stops at La).
+__device__ __forceinline__ void gather_row_and_jacobian(const PLMeta &m, const __half *__restrict__ grid, const float (&xs)[3], uint32_t La,
                                                         uint8_t *tile, int r, float (&J0)[16][3], float (&J1)[16][3]) {
-    const uint32_t L = m.n_pseudo;
 #pragma unroll
     for (uint32_t p0 = 0; p0 < 16; p0 += kColorGatherU) {
-        if (p0 >= L) {                                         // uniform
+        if (p0 >= La) {                                        // uniform
 #pragma unroll
             for (int u = 0; u < kColorGatherU; ++u) put_level_to_tile<kTile>(tile, r, p0 + u, 0u);
             continue;
@@ -92,13 +92,13 @@ __device__ __forceinline__ void gather_row_and_jacobian(const PLMeta &m, const _
         for (int u = 0; u < kColorGatherU; ++u) {
             const uint32_t *lp = level_cells_ptr(m, p0 + u, grid);
 #pragma unroll
-            for (int c = 0; c < 8; ++c) raw[u][c] = p0 + u < L ? ld_nc_u32(lp + cell[u][c]) : 0u;
+            for (int c = 0; c < 8; ++c) raw[u][c] = p0 + u < La ? ld_nc_u32(lp + cell[u][c]) : 0u;
         }
 #pragma unroll
         for (int u = 0; u < kColorGatherU; ++u) {
             const uint32_t p = p0 + u;
             const uint32_t packed = feat2_from_raw(raw[u], w[u]);
-            put_level_to_tile<kTile>(tile, r, p, (p < L && (int)m.level[p] <= max_level) ? packed : 0u);
+            put_level_to_tile<kTile>(tile, r, p, p < La ? packed : 0u);
             jacobian_from_raw(raw[u], fr[u], sc[u], J0[p], J1[p]);
         }
     }
@@ -125,8 +125,10 @@ __global__ void __launch_bounds__(kTile)
 k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev net, const PointSrc ps, const float *__restrict__ view_dirs,
             const float *__restrict__ h_appear, int64_t n, int max_level, float *__restrict__ sdf_out, float *__restrict__ nab_out,
             float *__restrict__ rgb_out, float *__restrict__ x_out, uint8_t *__restrict__ Zt, uint8_t *__restrict__ Xt,
-            uint8_t *__restrict__ Y1t, uint8_t *__restrict__ Y2t, const OccCollect oc, const int64_t *__restrict__ n_dev) {
+            uint8_t *__restrict__ Y1t, uint8_t *__restrict__ Y2t, const OccCollect oc, const int64_t *__restrict__ n_dev,
+            const int32_t *__restrict__ ml_dev) {
     n = eff_n(n, n_dev);
+    const uint32_t La = active_levels(max_level, ml_dev, m.n_pseudo);
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
     uint8_t *sX = tiles;                                       // 16 KB [h | x sh n ha 0] (geometry-only: 8 KB, the h half)
@@ -179,7 +181,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         int64_t ray;
         load_point(ps, ps.x == nullptr, i, valid, xn, xs, ray);
         float J0[16][3], J1[16][3];
-        gather_row_and_jacobian(m, grid, xs, max_level, sX, tid, J0, J1);                  // h -> chunks 0..3 of X, J -> registers
+        gather_row_and_jacobian(m, grid, xs, La, sX, tid, J0, J1);                  // h -> chunks 0..3 of X, J -> registers
         tc::fence_async_smem();
         __syncthreads();
         tc::mma_to_rows<64, 0, 0, NF / 16>(acc, kS, 0, tc::kmajor(x_addr, kTile), tc::kmajor(w1_addr, HW), false);   // Z = H . W1^T
@@ -218,7 +220,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 #pragma unroll
             for (uint32_t q = 0; q < 4; ++q) {
                 const uint32_t p = g4 * 4 + q;
-                if (p < m.n_pseudo && (int)m.level[p] <= max_level) {
+                if (p < La) {
                     const float g0 = r16(gg[2 * q]), g1 = r16(gg[2 * q + 1]);
 #pragma unroll
                     for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g0, J0[p][d], nacc[d]);
@@ -564,8 +566,9 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
                 const uint8_t *__restrict__ Xt, const float *__restrict__ g_nab, const float *__restrict__ g_sdf, const float *__restrict__ dh_r,
                 int64_t n, int max_level, float *__restrict__ d_grid, float *__restrict__ d_W1, float *__restrict__ d_b1, float *__restrict__ d_W2,
                 float *__restrict__ d_b2, const int64_t *__restrict__ n_dev, const float *__restrict__ xv_rows,
-                const float *__restrict__ view_dirs, float *__restrict__ gx_out) {
+                const float *__restrict__ view_dirs, float *__restrict__ gx_out, const int32_t *__restrict__ ml_dev) {
     n = eff_n(n, n_dev);
+    const uint32_t La = active_levels(max_level, ml_dev, m.n_pseudo);
     constexpr int NX = 48;                                     // 32 + the [1 0..] chunk + a zero chunk (N % 16 == 0)
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
@@ -643,11 +646,11 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
             }
             *reinterpret_cast<uint4 *>(sT + kTileBytes + c * kChunk + tid * 16) = tc::pack8_f16(uu);
         }
-        // dg = J gin (fp16), level by level, into my row of Ge; zero for the levels >= L (columns 2L..31)
+        // dg = J gin (fp16), level by level, into my row of Ge; zero for the levels >= La (columns 2La..31)
 #pragma unroll 4
         for (uint32_t p = 0; p < 16; ++p) {               // four levels per trip: 32 independent corner loads in flight (2 CTAs / SM: registers are free)
             uint32_t packed = 0;
-            if (p < m.n_pseudo && (int)m.level[p] <= max_level) {
+            if (p < La) {
                 float J0[3], J1[3];
                 level_jacobian(m, p, xs, grid, J0, J1);
                 float a0 = 0.f, a1 = 0.f;
@@ -716,7 +719,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         // ---- merged scatter
         float gx[3] = {0.f, 0.f, 0.f};
 #pragma unroll 1
-        for (uint32_t g4 = 0; g4 * 4 < m.n_pseudo; ++g4) {
+        for (uint32_t g4 = 0; g4 * 4 < La; ++g4) {
             float gg[8], hz[8];
             tc::acc_ld8(stage, kS, tid, g4 * 8, gg);
             tc::acc_ld8(stage, kS, tid, NF + g4 * 8, hz);
@@ -727,7 +730,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
 #pragma unroll
             for (uint32_t q = 0; q < 4; ++q) {
                 const uint32_t p = g4 * 4 + q;
-                if (p >= m.n_pseudo || (int)m.level[p] > max_level) continue;               // uniform
+                if (p >= La) continue;                                                       // uniform
                 uint32_t cell[8];
                 float w[8], fr[3], sc[3], ua[8], ub[8];
                 level_cells3(m, p, xs, cell, w, fr, sc);
@@ -836,6 +839,7 @@ extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params
                                    int64_t n, int32_t max_level, float *sdf, float *nablas, float *rgb, float *x_out, void *act_z, void *act_x,
                                    void *act_y1, void *act_y2, const nsb_occ_collect *collect, void *stream) {
     const DevCounts dn = take_counts();
+    const int32_t *ml_dev = take_max_level();
     if (n == 0) return 0;
     const bool rad = rgb != nullptr;
     NSB_REQUIRE(meta && params_half && net && sdf && nablas && (view_dirs || !rad), "nsb_fused_color_fwd: NULL argument");
@@ -861,7 +865,7 @@ extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params
         if (int rc = require_ctas_per_sm(k_color_fwd<false>, kTile, kSmemG, kColorGeoCtasPerSM, "nsb_fused_color_fwd(geometry)")) return rc;
         k_color_fwd<false><<<persistent_grid(n_tiles(n), kColorGeoCtasPerSM), kTile, kSmemG, (cudaStream_t)stream>>>(
             m, (const __half *)params_half, d, ps, nullptr, nullptr, n, ml, sdf, nablas, nullptr, x_out, (uint8_t *)act_z, (uint8_t *)act_x,
-            nullptr, nullptr, occ_collect_of(collect), dn.a);
+            nullptr, nullptr, occ_collect_of(collect), dn.a, ml_dev);
         return check_launch("nsb_fused_color_fwd");
     }
     NSB_REQUIRE(d.n_appear == 0 || h_appear, "nsb_fused_color_fwd: h_appear is NULL but the net has %d appearance channels", d.n_appear);
@@ -870,7 +874,7 @@ extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params
     k_color_fwd<true><<<persistent_grid(n_tiles(n), 2), kTile, kSmem, (cudaStream_t)stream>>>(m, (const __half *)params_half, d, ps, view_dirs, h_appear, n,
                                                                                              ml, sdf, nablas, rgb, x_out, (uint8_t *)act_z,
                                                                                              (uint8_t *)act_x, (uint8_t *)act_y1, (uint8_t *)act_y2,
-                                                                                             occ_collect_of(collect), dn.a);
+                                                                                             occ_collect_of(collect), dn.a, ml_dev);
     return check_launch("nsb_fused_color_fwd");
 }
 
@@ -884,6 +888,7 @@ static int color_bwd(const char *who, const nsb_lotd_meta *meta, const void *par
                      float *d_rb2, float *d_R3, float *d_rb3, const float *view_dirs, float *ha_scratch, const int64_t *ray_map, float *d_h_appear,
                      float *ray_scratch, float *d_rays_o, float *d_rays_d, float *d_view_dirs, void *stream) {
     const DevCounts dn = take_counts();
+    const int32_t *ml_dev = take_max_level();
     if (n == 0) return 0;
     NSB_REQUIRE(meta && params_half && net && act_z && act_x, "%s: NULL argument", who);
     NSB_REQUIRE(d_grid && d_W1 && d_b1 && d_W2 && d_b2, "%s: NULL gradient buffer", who);
@@ -926,7 +931,7 @@ static int color_bwd(const char *who, const nsb_lotd_meta *meta, const void *par
     const PointSrc ps{x, rays_o, rays_d, t, ridx};
     k_color_sdf_bwd<kRays><<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemS, s>>>(
         m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x, g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level,
-        d_grid, d_W1, d_b1, d_W2, d_b2, dn.a, xv_rows, view_dirs, ray_scratch);
+        d_grid, d_W1, d_b1, d_W2, d_b2, dn.a, xv_rows, view_dirs, ray_scratch, ml_dev);
     if (int rc = check_launch("nsb_fused_color_bwd(sdf)")) return rc;
     if (kRays) {
         k_ray_row_sum<12><<<row_sum_blocks(n), 256, 0, s>>>(ray_scratch, ridx, nullptr, n, 9, ray_map, RowSumOut{{d_rays_o, d_rays_d, d_view_dirs}, 3},

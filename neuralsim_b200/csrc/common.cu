@@ -29,6 +29,13 @@ DevCounts take_counts() {
     g_counts = DevCounts{nullptr, nullptr};
     return c;
 }
+
+static thread_local const int32_t *g_max_level = nullptr;
+const int32_t *take_max_level() {
+    const int32_t *l = g_max_level;
+    g_max_level = nullptr;
+    return l;
+}
 }  // namespace nsb
 
 namespace nsb {
@@ -65,6 +72,12 @@ int max_active_ctas(const void *kernel, int dev, int block, int smem_bytes) {
 // See include/neuralsim_b200.h: the binding is consumed (and cleared) by the next count-aware launch of this thread.
 extern "C" int nsb_bind_device_counts(const int64_t *count0, const int64_t *count1) {
     nsb::g_counts = nsb::DevCounts{count0, count1};
+    return 0;
+}
+
+// See include/neuralsim_b200.h: consumed (and cleared) by the next level-aware launch of this thread.
+extern "C" int nsb_bind_device_max_level(const int32_t *level) {
+    nsb::g_max_level = level;
     return 0;
 }
 

@@ -53,7 +53,7 @@ struct PackSlots {
 
 // the producer side of MODE 2: set `set` walks every group of this CTA, gathers its tiles j (j % kPackSets == set) into the ring and,
 // when it owns the index past the last tile, posts the end marker there.  Lane = pack (ray), warp w of the set = sample ordinal k0 + w.
-__device__ __forceinline__ void sdf_packs_produce(const PLMeta &m, const __half *__restrict__ grid, int max_level, const float *__restrict__ rays_o,
+__device__ __forceinline__ void sdf_packs_produce(const PLMeta &m, const __half *__restrict__ grid, uint32_t La, const float *__restrict__ rays_o,
                                                   const float *__restrict__ rays_d, const float *__restrict__ t, const int64_t *__restrict__ pack_infos,
                                                   const int64_t *__restrict__ pack_ray, const int64_t *__restrict__ order, int64_t n_packs,
                                                   const OccCollect &oc, const PackSlots &ring, int set, int w, int lane) {
@@ -91,7 +91,7 @@ __device__ __forceinline__ void sdf_packs_produce(const PLMeta &m, const __half 
                 for (int q = 0; q < 3; ++q) xs[q] = to_table_space(xs[q]);
                 const uint32_t s = mine % kPackSlots;
                 tc::mbar_wait(&ring.empty[s], ((mine / kPackSlots) & 1u) ^ 1u);
-                gather_row_to_tile<kTile>(m, grid, xs, max_level, ring.a + s * (kTile * NF * 2), row);
+                gather_row_to_tile<kTile>(m, grid, xs, La, ring.a + s * (kTile * NF * 2), row);
                 ring.out[s * kTile + row] = valid ? first + k : -1;
                 ring.voxel[s * kTile + row] = (valid && oc.pcl) ? occ_voxel(oc, xs) : 0;
                 tc::fence_async_smem();                        // the tile's generic-proxy writes -> visible to the wgmma (async proxy)
@@ -114,8 +114,9 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
                const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
                const float *__restrict__ t, int64_t n, int max_level, float *__restrict__ sdf, const int64_t *__restrict__ pack_infos,
                const int64_t *__restrict__ pack_ray, const int64_t *__restrict__ order, int64_t n_packs, const OccCollect oc,
-               const int64_t *__restrict__ n_dev) {
+               const int64_t *__restrict__ n_dev, const int32_t *__restrict__ ml_dev) {
     const int tid = threadIdx.x;
+    const uint32_t La = active_levels(max_level, ml_dev, m.n_pseudo);
     if constexpr (MODE == 2) {
         const int warp = tid >> 5, lane = tid & 31;
         n_packs = eff_n(n_packs, n_dev);                       // device-resident count (nsb_bind_device_counts)
@@ -145,7 +146,7 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
         __syncthreads();
         if (warp >= 4) {                                       // producers
             tc::setmaxnreg_dec<kPackProducerRegs>();
-            sdf_packs_produce(m, grid, max_level, rays_o, rays_d, t, pack_infos, pack_ray, order, n_packs, oc, ring, (warp - 4) >> 2, warp & 3, lane);
+            sdf_packs_produce(m, grid, La, rays_o, rays_d, t, pack_infos, pack_ray, order, n_packs, oc, ring, (warp - 4) >> 2, warp & 3, lane);
             return;
         }
         tc::setmaxnreg_inc<kPackConsumerRegs>();
@@ -194,7 +195,7 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
         stage_decoder_vectors(dec, sb1, sW2, &sb2, tid);
         tc::fence_async_smem();
         __syncthreads();
-        const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
+        const SdfTile ctx{m, grid, La, sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
         const int64_t n_tiles = (n + kTile - 1) / kTile;
         for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             const int64_t i = tile * kTile + tid;
@@ -237,8 +238,9 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
              const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
              const float *__restrict__ t, const float *__restrict__ d_sdf, int64_t n, int max_level, float *__restrict__ d_grid,
              float *__restrict__ d_W1, float *__restrict__ d_b1, float *__restrict__ d_W2, float *__restrict__ d_b2,
-             const int64_t *__restrict__ keep, const int64_t *__restrict__ n_dev, float *__restrict__ gx_out) {
+             const int64_t *__restrict__ keep, const int64_t *__restrict__ n_dev, float *__restrict__ gx_out, const int32_t *__restrict__ ml_dev) {
     n = eff_n(n, n_dev);
+    const uint32_t La = active_levels(max_level, ml_dev, m.n_pseudo);
     constexpr int NX = 40, GW = 128;                          // NX: features + [1,0,..] chunk; GW: dz | d*a
     constexpr int kS = tc::acc_stride(NF);                    // staged dH rows for the scatter: 18 KB, aliasing G
     extern __shared__ uint8_t dyn_smem[];                     // 50 KB of tiles (> the 48 KB static limit)
@@ -278,7 +280,7 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         load_point(PointSrc{x, rays_o, rays_d, t, ridx}, FROM_RAYS, i, valid, xs);
         const float dd = valid ? d_sdf[i] : 0.f;
         sdd[tid] = dd;                                           // read by the fragment owners of my row
-        gather_row_to_tile<kTile>(m, grid, xs, max_level, sA, tid);
+        gather_row_to_tile<kTile>(m, grid, xs, La, sA, tid);
         tc::fence_async_smem();
         __syncthreads();
         {
@@ -325,14 +327,14 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         const bool warp_active = __any_sync(0xffffffffu, active);
         float gx[3] = {0.f, 0.f, 0.f};
 #pragma unroll 1
-        for (uint32_t g4 = 0; g4 * 4 < m.n_pseudo; ++g4) {
+        for (uint32_t g4 = 0; g4 * 4 < La; ++g4) {
             float dh[8];
             tc::acc_ld8(stage, kS, tid, g4 * 8, dh);                // 4 levels x 2 features
             if (!warp_active) continue;
 #pragma unroll
             for (uint32_t q = 0; q < 4; ++q) {
                 const uint32_t p = g4 * 4 + q;
-                if (p >= m.n_pseudo || (int)m.level[p] > max_level) continue;               // uniform
+                if (p >= La) continue;                                                       // uniform
                 uint32_t cell[8];
                 float w[8], a[8], b[8], fr[3], sc[3];
                 if constexpr (kXGrad) level_cells3(m, p, xs, cell, w, fr, sc);
@@ -392,6 +394,7 @@ extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *pa
                                        int32_t max_level, float *sdf, void *stream, int mode, const int64_t *pack_infos,
                                        const int64_t *pack_ray, const int64_t *pack_order, int64_t n_packs, const nsb_occ_collect *collect) {
     const DevCounts dn = take_counts();
+    const int32_t *ml_dev = take_max_level();
     PLMeta m;
     DecoderDevTC d;
     if (int rc = make_decoder(meta, dec, &m, &d, "nsb_fused_sdf (tensor-core)")) return rc;
@@ -404,11 +407,11 @@ extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *pa
         opt_in_smem(k_fused_sdf_tc<2>, kPackSmem);
         if (int rc = require_ctas_per_sm(k_fused_sdf_tc<2>, kPackThreads, kPackSmem, kPackCtasPerSM, "nsb_fused_sdf (packs)")) return rc;
         k_fused_sdf_tc<2><<<persistent_grid((n_packs + 31) / 32, kPackCtasPerSM), kPackThreads, kPackSmem, s>>>(
-            m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf, pack_infos, pack_ray, pack_order, n_packs, oc, dn.a);
+            m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf, pack_infos, pack_ray, pack_order, n_packs, oc, dn.a, ml_dev);
     } else if (mode == 1)
-        k_fused_sdf_tc<1><<<tiles, kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, ridx, t, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a);
+        k_fused_sdf_tc<1><<<tiles, kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, ridx, t, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a, ml_dev);
     else
-        k_fused_sdf_tc<0><<<tiles, kTile, 0, s>>>(m, g, d, x, nullptr, nullptr, nullptr, nullptr, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a);
+        k_fused_sdf_tc<0><<<tiles, kTile, 0, s>>>(m, g, d, x, nullptr, nullptr, nullptr, nullptr, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a, ml_dev);
     return check_launch("nsb_fused_sdf(tc)");
 }
 
@@ -427,6 +430,7 @@ static int sdf_bwd(const char *who, const nsb_lotd_meta *meta, const void *param
                    float *d_grid, float *d_W1, float *d_b1, float *d_W2, float *d_b2, float *gx_scratch, const int64_t *ray_map, float *d_rays_o,
                    float *d_rays_d, void *stream) {
     const DevCounts dn = take_counts();
+    const int32_t *ml_dev = take_max_level();
     if (n == 0) return 0;
     NSB_REQUIRE(meta && params_half && dec && d_sdf && d_grid && d_W1 && d_b1 && d_W2 && d_b2, "%s: NULL argument", who);
     NSB_REQUIRE(x || (rays_o && rays_d && t), "%s: need x or (rays_o, rays_d, t)", who);
@@ -442,7 +446,7 @@ static int sdf_bwd(const char *who, const nsb_lotd_meta *meta, const void *param
     cudaStream_t s = (cudaStream_t)stream;
     const int ml = max_level < 0 ? -1 : max_level;
     kern<<<grid, kTile, kBwdSmem, s>>>(m, (const __half *)params_half, d, x, x ? nullptr : rays_o, x ? nullptr : rays_d, x ? nullptr : ridx,
-                                       x ? nullptr : t, d_sdf, n, ml, d_grid, d_W1, d_b1, d_W2, d_b2, keep, dn.a, gx_scratch);
+                                       x ? nullptr : t, d_sdf, n, ml, d_grid, d_W1, d_b1, d_W2, d_b2, keep, dn.a, gx_scratch, ml_dev);
     if (int rc = check_launch(who)) return rc;
     if (kXGrad) {
         if (!d_rays_o && !d_rays_d) return 0;

@@ -45,23 +45,31 @@ __device__ __forceinline__ void occ_collect_point(const OccCollect &oc, const fl
 constexpr int kTile = 128;
 constexpr int NF = 32, HW = 64;           // features, hidden width (zero padded to 64)
 
-// the L = m.n_pseudo (1..16) levels of one point -> row `r` of a chunk-major [R x >=32] fp16 tile (4 bytes per level); the feature
-// columns 2L..31 are written as zeros, so that nothing a previous tile left in shared memory reaches a wgmma (a stale fp16 Inf times a
-// zero weight is NaN), and levels >= L are neither read nor masked.
+// The levels a launch uses: 0..max_level of the L = m.n_pseudo levels (make_decoder: pseudo level p is level p), i.e. the prefix of
+// clamp(max_level + 1, 0, L) levels.  max_level is the host argument, or -- with a device level bound to the launch (ml_dev,
+// nsb_bind_device_max_level) -- the value in device memory, read once at the start of the kernel and clamped to [-1, L-1].  Uniform across
+// the CTA.
+__device__ __forceinline__ uint32_t active_levels(int max_level, const int32_t *__restrict__ ml_dev, uint32_t L) {
+    const int ml = ml_dev ? *ml_dev : max_level;
+    return ml < 0 ? 0u : (ml >= (int)L - 1 ? L : (uint32_t)ml + 1u);
+}
+
+// the La active levels of one point -> row `r` of a chunk-major [R x >=32] fp16 tile (4 bytes per level); the feature columns 2La..31
+// are written as zeros, so that nothing a previous tile left in shared memory reaches a wgmma (a stale fp16 Inf times a zero weight is
+// NaN), and levels >= La are not read: a masked level costs its zero columns, not its 8 corner loads.
 // U levels per loop trip: the 8 U corner loads of a trip are independent, so U = 2 doubles the loads in flight per thread (the
 // latency-bound backward kernels run at 8-16 warps / SM; one level per trip thrashes L1 in the ray-major order of k_fused_sdf_tc);
-// full unrolling is avoided on purpose (instruction cache, see fused_tc.cu).  An odd L ends with one level alone.
+// full unrolling is avoided on purpose (instruction cache, see fused_tc.cu).  An odd La ends with one level alone.
 template <int R>
 __device__ __forceinline__ void put_level_to_tile(uint8_t *tile, int r, uint32_t p, uint32_t v) {
     *reinterpret_cast<uint32_t *>(tile + (p >> 2) * (R * 16) + r * 16 + (p & 3) * 4) = v;
 }
 template <int R, int U = 2>
 __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half *__restrict__ grid, const float (&xs)[3],
-                                                   int max_level, uint8_t *tile, int r) {
-    const uint32_t L = m.n_pseudo;
+                                                   uint32_t La, uint8_t *tile, int r) {
     uint32_t p0 = 0;
 #pragma unroll 1
-    for (; p0 + U <= L; p0 += U) {
+    for (; p0 + U <= La; p0 += U) {
         uint32_t cell[U][8];
         float w[U][8];
         uint32_t packed[U];
@@ -70,18 +78,14 @@ __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half
 #pragma unroll
         for (int u = 0; u < U; ++u) packed[u] = level_feat2_cells(level_cells_ptr(m, p0 + u, grid), cell[u], w[u]);
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const uint32_t p = p0 + u;
-            put_level_to_tile<R>(tile, r, p, ((int)m.level[p] <= max_level) ? packed[u] : 0u);
-        }
+        for (int u = 0; u < U; ++u) put_level_to_tile<R>(tile, r, p0 + u, packed[u]);
     }
 #pragma unroll 1
-    for (; p0 < L; ++p0) {
+    for (; p0 < La; ++p0) {
         uint32_t cell[8];
         float w[8];
         level_cells3(m, p0, xs, cell, w);
-        const uint32_t packed = level_feat2_cells(level_cells_ptr(m, p0, grid), cell, w);
-        put_level_to_tile<R>(tile, r, p0, ((int)m.level[p0] <= max_level) ? packed : 0u);
+        put_level_to_tile<R>(tile, r, p0, level_feat2_cells(level_cells_ptr(m, p0, grid), cell, w));
     }
 #pragma unroll 1
     for (; p0 < 16; ++p0) put_level_to_tile<R>(tile, r, p0, 0u);
@@ -302,6 +306,8 @@ inline int make_decoder(const nsb_lotd_meta *meta, const nsb_sdf_decoder *dec, P
     NSB_REQUIRE(m->n_pseudo >= 1 && m->n_pseudo <= 16, "%s: built for 1 to 16 LoTD levels (got %u)", who, m->n_pseudo);
     NSB_REQUIRE(m->F == 2 && m->D == 3 && m->n_out == 2 * m->n_pseudo && plmeta_two_feature_cells(*m), "%s: built for L x 2 LoTD features in 3-D", who);
     NSB_REQUIRE(plmeta_cell_key_fits(*m), "%s: a level resolution exceeds %u cells per axis (the backward's merge key)", who, 1u << kCellKeyBits);
+    for (uint32_t p = 0; p < m->n_pseudo; ++p)        // 2-feature levels: the active levels are a prefix (active_levels)
+        NSB_REQUIRE(m->level[p] == p, "%s: pseudo level %u is level %u, not itself", who, p, m->level[p]);
     NSB_REQUIRE(dec->width >= 1 && dec->width <= 64, "%s: decoder width must be <= 64", who);
     *d = DecoderDevTC{(const __half *)dec->W1, (const __half *)dec->b1, (const __half *)dec->W2, (const __half *)dec->b2, dec->width,
                       2 * (int)m->n_pseudo, dec->beta};
@@ -312,7 +318,7 @@ inline int make_decoder(const nsb_lotd_meta *meta, const nsb_sdf_decoder *dec, P
 struct SdfTile {
     const PLMeta &m;
     const __half *grid;
-    int max_level;
+    uint32_t La;                           // active levels (active_levels)
     uint8_t *sA;
     uint32_t a_addr, b_addr;
     float *srow;                           // [kTile] shared: the sdf of each row, handed from the fragment owners to the row's thread
@@ -348,7 +354,7 @@ __device__ __forceinline__ void sdf_rows_of_frags(const float (&z)[2][HW / 2], c
 
 // all 128 threads: my point's table coordinates -> my sdf (fp16-rounded, as fp32).  Ends with the CTA barrier that frees the tile.
 __device__ __forceinline__ float sdf_of_tile(const SdfTile &c, const float (&xs)[3], int tid) {
-    gather_row_to_tile<kTile>(c.m, c.grid, xs, c.max_level, c.sA, tid);
+    gather_row_to_tile<kTile>(c.m, c.grid, xs, c.La, c.sA, tid);
     tc::fence_async_smem();                // generic-proxy smem writes -> visible to the tensor core (async proxy)
     __syncthreads();
     float z[2][HW / 2];

@@ -83,6 +83,10 @@ __device__ __forceinline__ int64_t eff_n(int64_t n, const int64_t *__restrict__ 
     return n;
 }
 
+// Device-resident LoTD level bound (nsb_bind_device_max_level): the level-aware entry points take the binding of the calling thread and
+// their kernels read *level instead of the host max_level argument.
+const int32_t *take_max_level();
+
 // Grid size for grid-stride kernels: a whole number of waves of `ctas_per_sm` resident CTAs on all SMs.
 inline unsigned wave_grid(int64_t work_items, int block, int ctas_per_sm) {
     int64_t need = (work_items + block - 1) / block;

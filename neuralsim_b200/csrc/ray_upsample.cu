@@ -40,7 +40,7 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
                       const float *__restrict__ rays_d, const float *__restrict__ t_starts, const int64_t *__restrict__ pack_infos,
                       const int64_t *__restrict__ ridx_hit, int64_t n_hit, int max_level, const UpsampleArgs ua, float *__restrict__ fine_all,
                       int nf_total, int32_t *__restrict__ overflow, float *__restrict__ scratch, int long_cap, const OccCollect oc,
-                      const int64_t *__restrict__ n_dev) {
+                      const int64_t *__restrict__ n_dev, const int32_t *__restrict__ ml_dev) {
     n_hit = eff_n(n_hit, n_dev);
     __shared__ __align__(128) uint8_t sA[kTile * NF * 2];
     __shared__ __align__(128) uint8_t sB[HW * NF * 2];
@@ -57,7 +57,7 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
     stage_decoder_vectors(dec, sb1, sW2, &sb2, tid);
     tc::fence_async_smem();
     __syncthreads();
-    const SdfTile ctx{m, grid, max_level, sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
+    const SdfTile ctx{m, grid, active_levels(max_level, ml_dev, m.n_pseudo), sA, tc::smem_u32(sA), tc::smem_u32(sB), srow, sb1, sW2, sb2, SoftplusK(dec.beta)};
     int room = kCap;                                     // a ray must hold its marched samples + every merged stage
     for (int i = 0; i + 1 < ua.n_stage; ++i) room -= ua.n_fine[i];
 
@@ -190,6 +190,7 @@ extern "C" int nsb_upsample_rays(const nsb_lotd_meta *meta, const void *params_h
                                  int32_t use_estimate_alpha, float early_stop_eps, float alpha_thre, float *fine_all, int32_t *overflow,
                                  float *scratch, int32_t long_cap, const nsb_occ_collect *collect, void *stream) {
     const DevCounts dn = take_counts();
+    const int32_t *ml_dev = take_max_level();
     if (n_hit == 0) return 0;
     NSB_REQUIRE(meta && params_half && dec && rays_o && rays_d && t_starts && pack_infos && ridx_hit && n_fine && inv_s_stage && u_stage && fine_all && overflow,
                 "nsb_upsample_persistent: NULL argument");
@@ -215,6 +216,6 @@ extern "C" int nsb_upsample_rays(const nsb_lotd_meta *meta, const void *params_h
     NSB_REQUIRE(scratch == nullptr || long_cap > kCap, "nsb_upsample_rays: long_cap must exceed the shared-memory capacity (%d)", kCap);
     k_upsample_persistent<<<upsample_grid(n_hit), kTile, 0, (cudaStream_t)stream>>>(
         m, (const __half *)params_half, d, rays_o, rays_d, t_starts, pack_infos, ridx_hit, n_hit, max_level < 0 ? -1 : max_level, ua, fine_all, nf_total,
-        overflow, scratch, long_cap, occ_collect_of(collect), dn.a);
+        overflow, scratch, long_cap, occ_collect_of(collect), dn.a, ml_dev);
     return check_launch("nsb_upsample_rays");
 }

@@ -247,12 +247,45 @@ class LoTD(nn.Module):
         return _batch_data_size(input, input_batched)
 
 
+class MultiresAnnealer(nn.Module):
+    """The level schedule of a multi-resolution encoding (multires_annealer.py:19-64), hard-mask form: `forward(it)` -> (max_level, None);
+    levels 0..max_level are used.  max_level starts at `start_level` (clamped to [-1, L-1]; -1 = no level) at `start_it` and gains one level
+    per 1/(L-1-start_level) of the stages up to `stop_it`; a stage is `update_every` iterations.  Before the first `set_iter` / `forward(it)`
+    the annealer is in its stop state (all levels).  It holds no tensors: the state dict of the encoding does not change."""
+
+    def __init__(self, level_n_feats, type: str, stop_it: int, start_it: int = 0, update_every: int = 1, start_level: int = 0):
+        super().__init__()
+        if type == "cosine":
+            raise RuntimeError("MultiresAnnealer: anneal type 'cosine' is not built (its per-feature window is not applied by the fused kernels); "
+                               "use 'hardmask'")
+        if type != "hardmask":
+            raise RuntimeError(f"Invalid anneal_type={type}")
+        self.num_levels = len(level_n_feats)
+        self.start_it, self.stop_it, self.update_every = int(start_it), int(stop_it), int(update_every)
+        self.total_stages = (self.stop_it - self.start_it) // self.update_every
+        if self.total_stages == 0:
+            raise RuntimeError(f"MultiresAnnealer: stop_it={self.stop_it}, start_it={self.start_it}, update_every={self.update_every} give no stage "
+                               "to anneal over ((stop_it - start_it) // update_every == 0)")
+        self.it = self.stop_it
+        self.start_level = max(min(int(start_level), self.num_levels - 1), -1)
+
+    def set_iter(self, it: int):
+        self.it = it
+
+    def forward(self, it: int = None):
+        it = self.it if it is None else it
+        alpha = min(1.0, max(0.0, ((it - self.start_it) // self.update_every) / self.total_stages))
+        length = (self.num_levels - 1) - self.start_level
+        return self.start_level + min(int(alpha * length), length), None
+
+
 class LoTDEncoding(nn.Module):
     """LoTD + its parameter table `flattened_params` (fp32 master) for inputs in [-1,1]^D
-    (lotd_encoding.py:37-213; state-dict key `...encoding.flattened_params`)."""
+    (lotd_encoding.py:37-213; state-dict key `...encoding.flattened_params`).  anneal_cfg (lotd_encoding.py:99-103): the keys of
+    MultiresAnnealer; `set_anneal_iter(it)` then sets `max_level` (every query without an explicit level uses it)."""
 
     def __init__(self, input_ch=3, *, lotd_cfg: dict = None, lotd_auto_compute_cfg: dict = None, param_init_cfg=dict(type="uniform_to_type", bound=1.0e-4),
-                 dtype=torch.half, device=None, generator=None, lotd_use_cuboid=False, aabb=None):
+                 dtype=torch.half, device=None, generator=None, lotd_use_cuboid=False, aabb=None, anneal_cfg: dict = None):
         super().__init__()
         if lotd_cfg is None:
             auto = dict(lotd_auto_compute_cfg or dict(type="gen_ngp"))
@@ -275,6 +308,7 @@ class LoTDEncoding(nn.Module):
         self.dtype = dtype
         self.in_features, self.out_features = input_ch, self.lotd.out_features
         self.max_level, self.window = None, None
+        self.annealer = MultiresAnnealer(self.lotd.level_n_feats, **anneal_cfg) if anneal_cfg is not None else None
         bound = float(param_init_cfg.get("bound", 1.0e-4))
         p = torch.empty(self.lotd.n_params, dtype=torch.float, device=device)
         p.uniform_(-bound, bound, generator=generator)
@@ -283,6 +317,10 @@ class LoTDEncoding(nn.Module):
     @property
     def meta(self):
         return self.lotd.meta
+
+    def set_anneal_iter(self, cur_it: int):
+        if self.annealer is not None:
+            self.max_level, self.window = self.annealer(cur_it)
 
     @property
     def inference_param(self):

@@ -70,7 +70,7 @@ class _TableGradSink(autograd.Function):
 
 class ColorQuery:
     """what the forward and backward launches of one colour query share: the table's meta and fp16 image, the net struct and the fp16
-    tensors it points at, the rays, max level, the occupancy collection, the device count (_lib.call's count=, None: host-sized),
+    tensors it points at, the rays, max level (a host int, or a device int32 scalar: _lib.call's level=), the occupancy collection, the device count (_lib.call's count=, None: host-sized),
     the step's shared table gradient (a SharedTableGrad, None: the backward fills its own) and the step's appearance-code gradient
     (None, or (d_h_appear, ray_map): the backward adds the code gradient of ray r into d_h_appear[ray_map[r]], which the caller
     zero-fills -- for codes that are not an autograd input of the op, as in the one-launch step) and the step's ray gradient (None, or
@@ -107,8 +107,8 @@ class _FusedColor(autograd.Function):
         with L.KERNEL_TIMER.time("fused_color_fwd", n):
             L.call(L.lib().nsb_fused_color_fwd, "fused_color_fwd", q.meta.c_ref, P(q.grid16, "f16"), ctypes.byref(q.net), None, P(q.rays_o, "f32"),
                    P(q.rays_d, "f32"), P(ridx, "i64"), P(t, "f32"), P(view_dirs, "f32", allow_none=not rad), P(h_appear, "f32", allow_none=True),
-                   L.c_i64(n), L.c_i32(q.ml), P(sdf), P(nab), P(rgb, allow_none=not rad), P(x), *ap,
-                   ctypes.byref(q.collect) if q.collect is not None else None, L.stream_ptr(), count=q.count)
+                   L.c_i64(n), L.c_level(q.ml), P(sdf), P(nab), P(rgb, allow_none=not rad), P(x), *ap,
+                   ctypes.byref(q.collect) if q.collect is not None else None, L.stream_ptr(), count=q.count, level=q.ml)
         ctx.q, ctx.ridx, ctx.t, ctx.n, ctx.rad = q, ridx, t, n, rad
         ctx.ha_shape = h_appear.shape if h_appear is not None else None
         ctx.vd = view_dirs
@@ -153,7 +153,7 @@ class _FusedColor(autograd.Function):
         P = L.ptr
         ag = [P(g) for g in grads] + [None] * (11 - len(grads))          # d_R* / d_rb*: NULL without the radiance net's parameters
         args = (q.meta.c_ref, P(q.grid16, "f16"), ctypes.byref(q.net), None, P(q.rays_o, "f32"), P(q.rays_d, "f32"), P(ctx.ridx, "i64"), P(ctx.t, "f32"),
-                L.c_i64(n), L.c_i32(q.ml), P(acts[0]), P(acts[1]), *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]), P(rgb, allow_none=True),
+                L.c_i64(n), L.c_level(q.ml), P(acts[0]), P(acts[1]), *([P(acts[2]), P(acts[3])] if ctx.rad else [None, None]), P(rgb, allow_none=True),
                 P(g_sdf, allow_none=True), P(g_nab, allow_none=True), P(g_rgb, allow_none=True), P(dh, allow_none=True), *ag)
         # the ray targets: the op's ray inputs (rows in ray order), or the step's buffers (ColorQuery.ray_grad, through its ray map)
         ro_t, rd_t, vd_t, ray_map = (d_ro, d_rd, d_vd, None) if q.ray_grad is None else q.ray_grad
@@ -167,13 +167,13 @@ class _FusedColor(autograd.Function):
                 L.call(L.lib().nsb_fused_color_bwd_grads, "fused_color_bwd_grads", *args, P(ctx.vd, "f32", allow_none=True),
                        P(ha_rows, allow_none=True), P(ray_map, "i64", allow_none=True), P(ha[0], "f32", allow_none=True), P(ray_rows),
                        P(ro_t, allow_none=True), P(rd_t, allow_none=True), P(vd_t if g_rgb is not None else None, allow_none=True), L.stream_ptr(),
-                       count=q.count)
+                       count=q.count, level=q.ml)
             elif appear is not None and g_rgb is not None:
                 ha_rows = torch.empty(n, 8, dtype=torch.float32, device=dev)        # per-sample code gradients, summed per ray in the call
                 L.call(L.lib().nsb_fused_color_bwd_appear, "fused_color_bwd_appear", *args, P(ha_rows), P(appear[1], "i64", allow_none=True),
-                       P(appear[0], "f32"), L.stream_ptr(), count=q.count)
+                       P(appear[0], "f32"), L.stream_ptr(), count=q.count, level=q.ml)
             else:
-                L.call(L.lib().nsb_fused_color_bwd, "fused_color_bwd", *args, L.stream_ptr(), count=q.count)
+                L.call(L.lib().nsb_fused_color_bwd, "fused_color_bwd", *args, L.stream_ptr(), count=q.count, level=q.ml)
         return ret
 
 

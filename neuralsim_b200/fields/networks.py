@@ -143,7 +143,8 @@ def sdf_decoder_c(t16, layers):
 
 def sdf_fwd(meta, grid16, dec, sdf, max_level, *, x=None, rays_o=None, rays_d=None, t=None, ridx=None, packs=None, collect=None, count=None):
     """one launch of the fused SDF query (nsb_fused_sdf_collect) into sdf: points x [n,3], or samples t [n] of rays ridx [n], or, with
-    packs = (pack_infos, pack ray | None[, block order | None]), the packs of t (ray-tiled; ridx unused)"""
+    packs = (pack_infos, pack ray | None[, block order | None]), the packs of t (ray-tiled; ridx unused).  max_level: a host int, or a device
+    int32 scalar the kernel reads (_lib.call)"""
     P = L.ptr
     if x is not None:
         pts = (P(x, "f32"), None, None, None, None, L.c_i64(x.shape[0]), None, None, None, L.c_i64(0), L.c_i32(0))
@@ -152,8 +153,8 @@ def sdf_fwd(meta, grid16, dec, sdf, max_level, *, x=None, rays_o=None, rays_d=No
     else:
         pts = (None, P(rays_o, "f32"), P(rays_d, "f32"), None, P(t, "f32"), L.c_i64(t.numel()), P(packs[0], "i64"), P(packs[1], "i64", allow_none=True),
                P(packs[2], "i64", allow_none=True) if len(packs) > 2 else None, L.c_i64(packs[0].shape[0]), L.c_i32(2))
-    L.call(L.lib().nsb_fused_sdf_collect, "fused_sdf", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), *pts, L.c_i32(max_level), P(sdf),
-           ctypes.byref(collect) if collect is not None else None, L.stream_ptr(), count=count)
+    L.call(L.lib().nsb_fused_sdf_collect, "fused_sdf", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), *pts, L.c_level(max_level), P(sdf),
+           ctypes.byref(collect) if collect is not None else None, L.stream_ptr(), count=count, level=max_level)
     return sdf
 
 
@@ -168,12 +169,13 @@ def sdf_bwd(meta, grid16, dec, d_sdf, n, max_level, grads, *, x=None, rays=None,
         ray_map = ray_grads[2] if len(ray_grads) > 2 else None
         L.call(L.lib().nsb_fused_sdf_bwd_rays, "fused_sdf_bwd_rays", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), P(rays[0], "f32"),
                P(rays[1], "f32"), P(rays[2], "i64"), P(rays[3], "f32"), P(d_sdf, "f32"), P(keep, "i64", allow_none=True), L.c_i64(n),
-               L.c_i32(max_level), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2), P(gx), P(ray_map, "i64", allow_none=True),
-               P(ray_grads[0], "f32", allow_none=True), P(ray_grads[1], "f32", allow_none=True), L.stream_ptr(), count=count)
+               L.c_level(max_level), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2), P(gx), P(ray_map, "i64", allow_none=True),
+               P(ray_grads[0], "f32", allow_none=True), P(ray_grads[1], "f32", allow_none=True), L.stream_ptr(), count=count, level=max_level)
         return
     pts = (P(x, "f32"), None, None, None, None) if x is not None else (None, P(rays[0], "f32"), P(rays[1], "f32"), P(rays[2], "i64"), P(rays[3], "f32"))
     L.call(L.lib().nsb_fused_sdf_bwd_indexed, "fused_sdf_bwd", meta.c_ref, P(grid16, "f16"), ctypes.byref(dec), *pts, P(d_sdf, "f32"),
-           P(keep, "i64", allow_none=True), L.c_i64(n), L.c_i32(max_level), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2), L.stream_ptr(), count=count)
+           P(keep, "i64", allow_none=True), L.c_i64(n), L.c_level(max_level), P(d_grid), P(d_W1), P(d_b1), P(d_W2), P(d_b2), L.stream_ptr(), count=count,
+           level=max_level)
 
 
 class _FusedSDF(autograd.Function):
@@ -261,6 +263,10 @@ class LoTDSDF(nn.Module):
         self._fused_cache = None
 
     # ---- reference API
+    def training_before_per_step(self, cur_it: int, logger=None):
+        """the encoding's level schedule (lotd_sdf.py:172-173)"""
+        self.encoding.set_anneal_iter(cur_it)
+
     def forward(self, x, *, return_h=False, max_level: int = None):
         h = self.encoding(x, max_level=max_level)
         sdf = self.decoder(h)[..., 0]

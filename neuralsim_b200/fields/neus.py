@@ -227,8 +227,10 @@ class LoTDNeuSModel(LoTDNeuS):
         return self.accel.init(self.query_sdf, logger=logger) if self.accel is not None else False
 
     def training_before_per_step(self, cur_it: int, logger=None):
+        # lotd_neus.py:116-121 then renderer_mixin.py:176-182: the level schedule is set before the accel queries the field
         self.it = cur_it
         self.ctrl_var.set_iter(cur_it)
+        self.implicit_surface.training_before_per_step(cur_it, logger=logger)
         if self.accel is not None:
             self.upsample_s_divisor = 2 ** self.accel.training_granularity
             if self.training:

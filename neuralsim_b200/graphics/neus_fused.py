@@ -444,9 +444,10 @@ def upsample_rays(meta, grid16, dec, ridx_hit, pack_infos, t_starts, rays_o, ray
     up = (ctypes.c_void_p * n_stage)(*[u.data_ptr() for u in us])
     with L.KERNEL_TIMER.time("ray_upsample", n_hit):
         L.call(lib.nsb_upsample_rays, "upsample_rays", meta.c_ref, L.ptr(grid16, "f16"), ctypes.byref(dec), L.ptr(rays_o, "f32"), L.ptr(rays_d, "f32"),
-               L.ptr(t_starts, "f32"), L.ptr(pack_infos, "i64"), L.ptr(ridx_hit, "i64"), L.c_i64(n_hit), L.c_i32(max_level), L.c_i32(n_stage), nf, invs, up,
+               L.ptr(t_starts, "f32"), L.ptr(pack_infos, "i64"), L.ptr(ridx_hit, "i64"), L.c_i64(n_hit), L.c_level(max_level), L.c_i32(n_stage), nf, invs, up,
                L.c_i32(1 if use_estimate_alpha else 0), L.c_f32(early_stop_eps), L.c_f32(alpha_thre), L.ptr(fine_all), L.ptr(overflow),
-               L.ptr(scratch, allow_none=True), L.c_i32(long_cap), ctypes.byref(collect) if collect is not None else None, L.stream_ptr(), count=count)
+               L.ptr(scratch, allow_none=True), L.c_i32(long_cap), ctypes.byref(collect) if collect is not None else None, L.stream_ptr(), count=count,
+               level=max_level)
     return fine_all, overflow
 
 

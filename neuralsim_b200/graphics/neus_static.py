@@ -179,14 +179,15 @@ def _fp16_images(model, radiance=True):
 
 
 def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=None, march_cap, kept_cap, coherent=False, with_rgb=True, with_normal=True,
-                  perturb=False, training=None, depth_use_normalized_vw=True, cnt=None, d_h_appear=None, d_rays=None):
+                  perturb=False, training=None, depth_use_normalized_vw=True, cnt=None, d_h_appear=None, d_rays=None, max_level_dev=None):
     """One chunk of rays, ray test -> query -> integration, without a host read.  -> (rendered dict of whole-chunk images, cnt int64[32]).
     `coherent`: image-ordered rays (the boundary / fine queries then walk the samples ray-tiled) -- a host decision here (the host-sized
     path measures it in the ray-test kernel).  `d_h_appear` [R, n_appear] (optional): zero-filled here, and the backward pass writes the
     gradient of the codes rays_h_appear into it, in the caller's ray order (the codes themselves are read detached).  `d_rays` =
     (d_rays_o, d_rays_d) [R, 3] (optional): the same for the rays -- zero-filled here, and the backward pass writes the gradient of the
     loss to rays_o and rays_d (the caller's frame and order; 0 for rays that miss the box or keep no sample), the depths held constant
-    as on the host-sized path."""
+    as on the host-sized path.  `max_level_dev` (optional): a device int32 scalar every LoTD kernel of the step reads its level bound from
+    (nsb_bind_device_max_level), so that a captured step follows a level schedule; None: the model's level at this call, fixed in a capture."""
     P, lib = L.ptr, L.lib()
     if with_rgb and getattr(model, "radiance_net", None) is None:
         raise RuntimeError("render_static(with_rgb=True): the model has no radiance net (radiance_cfg=False); render it with with_rgb=False")
@@ -213,7 +214,7 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         t16, st.dec, st.net, masters = _fp16_images(model, radiance=with_rgb)
         st.held, st.grid16 = t16, t16[0]
         st.meta = model.implicit_surface.encoding.meta
-        st.ml = model.implicit_surface._ml(model.max_level)
+        st.ml = max_level_dev if max_level_dev is not None else model.implicit_surface._ml(model.max_level)
         st.collect = model.accel.occ.collect_struct() if training else None
         # ---------------- ray test (fields/space.py:_ray_test_fused without the host read)
         c3, r3 = model.space._center_radius_c()
@@ -398,6 +399,11 @@ class StaticFrame:
     the per-sample buffers -- neuralsim_b200.loss.LidarLoss -- runs inside the captured step.  Per-step inputs of such a loss are static
     buffers the caller refreshes before `step()` (LidarLoss.set_step).
 
+    The LoTD level bound follows the model (`model.max_level`, else the encoding's annealed level) from replay to replay: `step()` refills a
+    device scalar the kernels read (`max_level_dev`), as it refills the variance schedule's weight, so one capture serves a whole level
+    schedule (LoTDEncoding's `anneal_cfg`; the trainer calls `model.training_before_per_step(it)` before `step()`).  A new level moves the
+    surface, so a step may need more samples than the arenas were sized for; `check()` then re-sizes them from the current level.
+
     The first call probes the sizes with the host-sized path (SingleVolumeRenderer.ray_query, no grad), sizes the arenas with `slack`,
     warms up and captures.  Gradients are accumulated into `p.grad` (kept in place; `zero_grads=True` or a `pre_hook` zeroes them inside the graph).
     Capture precondition (PyTorch): no autograd graph of an EARLIER backward on the default stream may still be referenced (a kept loss / rendered
@@ -425,6 +431,7 @@ class StaticFrame:
         if ray_grad:
             self.d_rays_o, self.d_rays_d = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)
         self.cnt = torch.zeros(32, dtype=torch.int64, device=dev)
+        self.max_level_dev = torch.zeros((), dtype=torch.int32, device=dev)
         self.graph, self.loss, self.rendered, self.buffers, self._occ_captured = None, None, None, None, None
         self.captures = 0
 
@@ -469,7 +476,8 @@ class StaticFrame:
         try:
             rendered, _, buffers = render_static(self.model, self.rays_o, self.rays_d, self.h_appear, near=self.near, far=self.far, march_cap=self.march_cap,
                                                  kept_cap=self.kept_cap, coherent=bool(self.coherent), with_rgb=self.with_rgb, with_normal=self.with_normal, cnt=self.cnt,
-                                                 d_h_appear=self.d_h_appear, d_rays=(self.d_rays_o, self.d_rays_d) if self.d_rays_o is not None else None)
+                                                 d_h_appear=self.d_h_appear, d_rays=(self.d_rays_o, self.d_rays_d) if self.d_rays_o is not None else None,
+                                                 max_level_dev=self.max_level_dev)
         finally:
             if cv is not None:
                 cv._use_w_dev = False
@@ -528,6 +536,7 @@ class StaticFrame:
             if getattr(cv, "_w_dev", None) is None:
                 cv._w_dev = torch.zeros((), device=self.device)
             cv._w_dev.fill_(cv.mix_weight())                  # the variance schedule's host-side weight of THIS iteration
+        self.max_level_dev.fill_(self.model.implicit_surface._ml(self.model.max_level))     # the LoTD level bound of THIS iteration
         if self.graph is None and (self.use_graph or self.march_cap is None):
             self.capture()
         if self.graph is not None:
