@@ -426,6 +426,27 @@ int nsb_gather_rays(const int64_t *idx, int64_t n, const float *o_n, const float
 int nsb_gather_rays_backward(const int64_t *idx, int64_t n, const float *radius3, const float *g_o, const float *g_d, const float *g_vd,
                              const float *vnorm, float *d_rays_o, float *d_rays_d, void *stream);
 
+/* ---------------------------------------------------------------- camera rays from refined poses (csrc/pose.cu)
+ * The StreetSurf camera pose refinement (app/models/scene/learnable_params.py:85-113; nr3d_lib/models/attributes/transform.py:107-130,
+ * attr.py:326-336): pose p is the quaternion q0[p] + dq[p] (real part first), normalised on every use, and the translation t0[p] + dt[p].
+ * Ray i of pose pidx[i] with camera-space direction dirs[i] is (app/resources/observers/cameras.py:299-310; nr3d_lib/maths/transforms.py:
+ * 41-72, 150-193):  rays_d = normalize(quat_apply(normalize_quat(q), dirs[i])),  rays_o = t  -- the direction normalised after the rotation,
+ * the origin the camera centre.  normalize(x) = x / max(|x|, 1e-12); normalize_quat also flips a quaternion whose real part is negative.
+ * The arithmetic is the reference's torch op sequence, each op rounded, so the rays are the reference's fp32 bits.
+ * nsb_pose_rays writes unit[n_poses, 4] (16-byte aligned; the normalised, standardised quaternion, once per pose) and nrm[n_poses] (|q|,
+ * negated where the quaternion was flipped; the backward's input), then rays_o, rays_d [n, 3] (count-aware: the rays below the count).
+ * pidx must lie in [0, n_poses): the caller checks it (the kernels do not).
+ * nsb_pose_rays_backward: from the cotangents d_rays_o, d_rays_d [n, 3] of the same rays (and the forward's unit, nrm), ADDS the gradient
+ * to dq into d_dq[n_poses, 4] and to dt into d_dt[n_poses, 3] (either may be NULL: not written).  Each pose's rays are summed in an order
+ * fixed by their positions (chunks of 4096 rays, lanes, a fixed butterfly, then the chunks in order): the same bits on every run, for rays
+ * in any pose order; a pose without rays gets 0.  Count-aware: rays past the count are not read.  scratch: 16-byte aligned,
+ * nsb_pose_grad_scratch_floats(n, n_poses) floats (n the capacity), no initialisation needed. */
+int64_t nsb_pose_grad_scratch_floats(int64_t n, int64_t n_poses);
+int nsb_pose_rays(const float *q0, const float *dq, const float *t0, const float *dt, int64_t n_poses, const int64_t *pidx, const float *dirs,
+                  int64_t n, float *unit, float *nrm, float *rays_o, float *rays_d, void *stream);
+int nsb_pose_rays_backward(const float *unit, const float *nrm, int64_t n_poses, const int64_t *pidx, const float *dirs, int64_t n,
+                           const float *d_rays_o, const float *d_rays_d, float *scratch, float *d_dq, float *d_dt, void *stream);
+
 /* ---------------------------------------------------------------- the StreetSurf LiDAR loss (csrc/lidar_loss.cu)
  * LidarLoss.forward with the depth term and the `neus_unisim` line-of-sight term (app/loss/lidar.py:174-210, 254-294) on the renderer's
  * own buffers, and its adjoint: the cotangents of the composite's depth_volume and vw (nsb_composite_backward's g_depth, g_vw).  R rays

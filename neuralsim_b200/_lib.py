@@ -63,6 +63,7 @@ def lib():
         _lib.nsb_color_tile_bytes.restype = ctypes.c_int64
         _lib.nsb_upsample_rays_scratch_floats.restype = ctypes.c_int64
         _lib.nsb_kth_smallest_scratch_bytes.restype = ctypes.c_int64
+        _lib.nsb_pose_grad_scratch_floats.restype = ctypes.c_int64
         # marching cubes (csrc/mesh.cu): `level` is a double, which an undeclared ctypes call would not pass
         vp, i32, i64, f64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_double
         _lib.nsb_mc_lattice_points.argtypes = [vp, vp, vp, i32, i32, i64, i64, vp, vp]

@@ -179,7 +179,8 @@ def _fp16_images(model, radiance=True):
 
 
 def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=None, march_cap, kept_cap, coherent=False, with_rgb=True, with_normal=True,
-                  perturb=False, training=None, depth_use_normalized_vw=True, cnt=None, d_h_appear=None, d_rays=None, max_level_dev=None):
+                  perturb=False, training=None, depth_use_normalized_vw=True, cnt=None, d_h_appear=None, d_rays=None, max_level_dev=None,
+                  ray_grad_hook=None):
     """One chunk of rays, ray test -> query -> integration, without a host read.  -> (rendered dict of whole-chunk images, cnt int64[32]).
     `coherent`: image-ordered rays (the boundary / fine queries then walk the samples ray-tiled) -- a host decision here (the host-sized
     path measures it in the ray-test kernel).  `d_h_appear` [R, n_appear] (optional): zero-filled here, and the backward pass writes the
@@ -187,7 +188,8 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     (d_rays_o, d_rays_d) [R, 3] (optional): the same for the rays -- zero-filled here, and the backward pass writes the gradient of the
     loss to rays_o and rays_d (the caller's frame and order; 0 for rays that miss the box or keep no sample), the depths held constant
     as on the host-sized path.  `max_level_dev` (optional): a device int32 scalar every LoTD kernel of the step reads its level bound from
-    (nsb_bind_device_max_level), so that a captured step follows a level schedule; None: the model's level at this call, fixed in a capture."""
+    (nsb_bind_device_max_level), so that a captured step follows a level schedule; None: the model's level at this call, fixed in a capture.
+    `ray_grad_hook` (optional, with d_rays): called in the backward pass right after d_rays is written (the pose adjoint of StaticFrame)."""
     P, lib = L.ptr, L.lib()
     if with_rgb and getattr(model, "radiance_net", None) is None:
         raise RuntimeError("render_static(with_rgb=True): the model has no radiance net (radiance_cfg=False); render it with with_rgb=False")
@@ -306,6 +308,8 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         # nodes run when no parameter requires grad: a pose refined against a fixed model)
         def ray_adjoint():
             NF.gather_rays_backward(rays_inds, R, r3, ray_g, vnorm, d_rays, count=(cnt, CNT_SLOTS["n_rays"]))
+            if ray_grad_hook is not None:
+                ray_grad_hook()
         anchor = _RayGradAdjoint.apply(ray_adjoint, torch.zeros((), device=dev, requires_grad=True))
     table = st.table_grad.route(s.encoding.flattened_params, anchor)    # the table as both backward nodes' input
     if not isinstance(inv_s, torch.Tensor):
@@ -394,6 +398,19 @@ class StaticFrame:
         loss = frame.step(o.detach(), d.detach(), codes)
         torch.autograd.backward([o, d], [frame.d_rays_o, frame.d_rays_d])      # -> pose.grad
 
+    `pose=CameraPoses(...)` (graphics/pose.py; off by default) moves that pose into the graph: the frame owns static buffers
+    `frame.dirs` [n_rays, 3] (camera-space directions) and `frame.pidx` [n_rays] (int64 pose indices), filled by `set_rays(dirs, pidx)` or
+    by `step(dirs=..., pidx=...)`; the graph first builds `frame.rays_o` / `frame.rays_d` from them (nsb_pose_rays) and, when dq or dt
+    requires grad, ends its backward with the pose adjoint (nsb_pose_rays_backward), which ADDS the gradient into `dq.grad` / `dt.grad`:
+
+        frame = StaticFrame(model, n_rays, loss_fn, near=0.01, pose=poses)
+        loss = frame.step(rays_h_appear=codes, dirs=dirs_cam, pidx=pidx)      # -> poses.dq.grad, poses.dt.grad; one graph launch
+
+    The gradient buffers stay the ones the graph writes: `step()` re-attaches them before each replay (a `.grad` set to None counts as
+    zeros, another tensor is copied in), and `zero_grads=True` zeroes them inside the graph with the model's.  `ray_grad=True` still fills
+    `d_rays_o` / `d_rays_d`.  Switching `requires_grad` of dq / dt (the reference's `enable_after`) re-captures once: the graph without
+    grad runs the forward kernel only.
+
     `loss_on_ret=True` (off by default: then `loss_fn(rendered)`): `loss_fn` receives the reference-shaped `ret = {"rendered": ...,
     "volume_buffer": vb}`, vb = static_volume_buffer(...) (the capacity-sized kept-sample buffers and their device counts), so a loss on
     the per-sample buffers -- neuralsim_b200.loss.LidarLoss -- runs inside the captured step.  Per-step inputs of such a loss are static
@@ -411,7 +428,7 @@ class StaticFrame:
 
     def __init__(self, model, n_rays, loss_fn=None, *, near=None, far=None, with_rgb=True, with_normal=True, slack=1.5, march_cap=None, kept_cap=None,
                  coherent=None, use_graph=True, zero_grads=False, h_appear_dim=None, pre_hook=None, h_appear_grad=False, ray_grad=False,
-                 loss_on_ret=False):
+                 loss_on_ret=False, pose=None):
         self.model, self.n_rays, self.loss_fn, self.loss_on_ret = model, int(n_rays), loss_fn, bool(loss_on_ret)
         self.near, self.far, self.with_rgb, self.with_normal, self.slack = near, far, with_rgb, with_normal, float(slack)
         self.march_cap, self.kept_cap, self.coherent = march_cap, kept_cap, coherent
@@ -432,6 +449,16 @@ class StaticFrame:
             self.d_rays_o, self.d_rays_d = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)
         self.cnt = torch.zeros(32, dtype=torch.int64, device=dev)
         self.max_level_dev = torch.zeros((), dtype=torch.int32, device=dev)
+        self.pose, self._pose_grad = pose, None
+        if pose is not None:
+            from .pose import scratch_floats
+            P = pose.n_poses
+            self.dirs = torch.zeros(self.n_rays, 3, device=dev)
+            self.pidx = torch.zeros(self.n_rays, dtype=torch.int64, device=dev)
+            self._pose_unit, self._pose_nrm = torch.zeros(P, 4, device=dev), torch.zeros(P, device=dev)
+            self._pose_scratch = torch.zeros(max(scratch_floats(self.n_rays, P), 4), device=dev)
+            self._pose_d_rays = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)       # the rays' gradient when ray_grad is off
+            self._pose_g = (torch.zeros(P, 4, device=dev), torch.zeros(P, 3, device=dev))   # what dq.grad / dt.grad are while the frame lives
         self.graph, self.loss, self.rendered, self.buffers, self._occ_captured = None, None, None, None, None
         self.captures = 0
 
@@ -460,6 +487,44 @@ class StaticFrame:
         self.march_cap = max(self.march_cap or 0, m)
         self.kept_cap = max(self.kept_cap or 0, k)
 
+    # -- the pose
+    def set_rays(self, dirs, pidx):
+        """copy camera-space directions [n_rays, 3] and pose indices [n_rays] (int64, each in [0, P): checked here, one host read) into the
+        frame's inputs"""
+        from .pose import check_pidx
+        if self.pose is None:
+            raise RuntimeError("StaticFrame.set_rays: the frame was built without pose=; pass rays_o / rays_d to step()")
+        if not isinstance(dirs, torch.Tensor) or tuple(dirs.shape) != (self.n_rays, 3) or not dirs.is_floating_point():
+            raise RuntimeError(f"StaticFrame.set_rays: dirs must be a float tensor [{self.n_rays}, 3], got {getattr(dirs, 'shape', type(dirs))}")
+        check_pidx(pidx.to(self.device) if isinstance(pidx, torch.Tensor) else pidx, self.n_rays, self.pose.n_poses)
+        self.dirs.copy_(dirs, non_blocking=True)
+        self.pidx.copy_(pidx, non_blocking=True)
+
+    def _pose_wants_grad(self):
+        return self.pose is not None and self.pose.requires_grad and torch.is_grad_enabled()
+
+    def _bind_pose_grads(self):
+        """dq.grad / dt.grad := the buffers the graph adds into (None counts as zeros; another tensor is copied in)"""
+        for p, buf in zip((self.pose.dq, self.pose.dt), self._pose_g):
+            if not p.requires_grad:
+                continue
+            if p.grad is None:
+                buf.zero_()
+            elif p.grad is not buf:
+                buf.copy_(p.grad)
+            p.grad = buf
+
+    def _pose_rays(self):
+        from .pose import pose_forward
+        with torch.no_grad():
+            pose_forward(self.pose, self.pidx, self.dirs, self._pose_unit, self._pose_nrm, self.rays_o, self.rays_d)
+
+    def _pose_adjoint(self, d_rays):
+        from .pose import pose_backward
+        pose = self.pose
+        pose_backward(self._pose_unit, self._pose_nrm, self.pidx, self.dirs, d_rays[0], d_rays[1], self._pose_scratch,
+                      self._pose_g[0] if pose.dq.requires_grad else None, self._pose_g[1] if pose.dt.requires_grad else None)
+
     # -- the step
     def _run(self):
         if self.pre_hook is not None:
@@ -468,6 +533,14 @@ class StaticFrame:
             for p in self.model.parameters():
                 if p.grad is not None:
                     p.grad.zero_()
+        pose_grad = self._pose_wants_grad()
+        if self.pose is not None:
+            if self.zero_grads and pose_grad:
+                for g in self._pose_g:
+                    g.zero_()
+            self._pose_rays()
+        d_rays = (self.d_rays_o, self.d_rays_d) if self.d_rays_o is not None else (self._pose_d_rays if pose_grad else None)
+        hook = (lambda: self._pose_adjoint(d_rays)) if pose_grad else None
         cv = getattr(self.model, "ctrl_var", None)
         if cv is not None and hasattr(cv, "mix_weight"):
             if getattr(cv, "_w_dev", None) is None:
@@ -476,8 +549,7 @@ class StaticFrame:
         try:
             rendered, _, buffers = render_static(self.model, self.rays_o, self.rays_d, self.h_appear, near=self.near, far=self.far, march_cap=self.march_cap,
                                                  kept_cap=self.kept_cap, coherent=bool(self.coherent), with_rgb=self.with_rgb, with_normal=self.with_normal, cnt=self.cnt,
-                                                 d_h_appear=self.d_h_appear, d_rays=(self.d_rays_o, self.d_rays_d) if self.d_rays_o is not None else None,
-                                                 max_level_dev=self.max_level_dev)
+                                                 d_h_appear=self.d_h_appear, d_rays=d_rays, max_level_dev=self.max_level_dev, ray_grad_hook=hook)
         finally:
             if cv is not None:
                 cv._use_w_dev = False
@@ -490,6 +562,10 @@ class StaticFrame:
         return rendered, buffers, loss
 
     def capture(self):
+        if self.pose is not None:
+            if not bool(self.dirs.any()):                   # (zero directions: see below)
+                raise RuntimeError("StaticFrame.capture: the pose inputs hold no rays yet; call set_rays(dirs, pidx) or step(dirs=..., pidx=...) first")
+            self._pose_rays()                               # the probe and the check below read the rays
         if self.march_cap is None or self.kept_cap is None or self.coherent is None:
             self._size()
         if not self.use_graph:
@@ -517,6 +593,7 @@ class StaticFrame:
             # stream BEFORE this and whose graph is still referenced -- a kept loss / rendered tensor -- pins those nodes to the default
             # stream and invalidates the capture: drop such references first.)
             self._occ_captured = self.model.accel.occ.occ_grid
+            self._pose_grad = self._pose_wants_grad()
             with torch.cuda.graph(g, stream=side):
                 self.rendered, self.buffers, self.loss = self._run()
             self.graph = g
@@ -525,10 +602,23 @@ class StaticFrame:
             L.KERNEL_TIMER.enabled = was
         return self
 
-    def step(self, rays_o, rays_d, rays_h_appear=None):
-        """copy the batch into the graph's inputs (H2D if the tensors are on the host) and launch.  -> loss (device scalar) or None"""
-        self.rays_o.copy_(rays_o, non_blocking=True)
-        self.rays_d.copy_(rays_d, non_blocking=True)
+    def step(self, rays_o=None, rays_d=None, rays_h_appear=None, *, dirs=None, pidx=None):
+        """copy the batch into the graph's inputs (H2D if the tensors are on the host) and launch.  -> loss (device scalar) or None.
+        With pose=: no rays_o / rays_d; dirs and pidx (set_rays), or neither to replay the rays set last."""
+        if self.pose is None:
+            if rays_o is None or rays_d is None or dirs is not None or pidx is not None:
+                raise RuntimeError("StaticFrame.step: a frame without pose= takes rays_o and rays_d (and no dirs / pidx)")
+            self.rays_o.copy_(rays_o, non_blocking=True)
+            self.rays_d.copy_(rays_d, non_blocking=True)
+        else:
+            if rays_o is not None or rays_d is not None or (dirs is None) != (pidx is None):
+                raise RuntimeError("StaticFrame.step: a frame with pose= takes dirs and pidx (or neither), not rays_o / rays_d")
+            if dirs is not None:
+                self.set_rays(dirs, pidx)
+            if self.pose.requires_grad:
+                self._bind_pose_grads()
+            if self.graph is not None and self._pose_grad != self._pose_wants_grad():
+                self.graph = None                           # requires_grad of the pose switched: re-capture (with / without the adjoint)
         if self.h_appear is not None and rays_h_appear is not None:
             self.h_appear.copy_(rays_h_appear, non_blocking=True)
         cv = getattr(self.model, "ctrl_var", None)
