@@ -447,6 +447,26 @@ int nsb_pose_rays(const float *q0, const float *dq, const float *t0, const float
 int nsb_pose_rays_backward(const float *unit, const float *nrm, int64_t n_poses, const int64_t *pidx, const float *dirs, int64_t n,
                            const float *d_rays_o, const float *d_rays_d, float *scratch, float *d_dq, float *d_dt, void *stream);
 
+/* ---------------------------------------------------------------- perturbed samples from torch's random stream (csrc/perturb.cu)
+ * With perturb=True a NeuS query draws from torch's CUDA generator, in order (nr3d_lib/graphics/neus/neus_ray_query.py:803, :821, :889):
+ * torch.rand([n_rays, nc1]) for the coarse depths (graphics/raysample.py:285-310), rand_like of the M marched samples' deltas
+ * (occgrid_raymarch.py:96-110) and torch.rand([n_hit, nf_i]) for up-sampling stage i (raysample.py:38-61).  Draw k starts at offset
+ * base + sum_{j<k} inc(N_j), inc(N) = ((N - 1) / (4 stride) + 1) * 4, stride = 256 min(ceil(N / 256), SMs (maxThreadsPerSM / 256))
+ * (torch's ATen/native/cuda/DistributionTemplates.h: calc_execution_policy, distribution_elementwise_grid_stride_kernel; element li is
+ * component (li / stride) % 4 of the (li / (4 stride))-th curand_uniform4 of Philox subsequence li % stride, 1 mapped to 0 by uniform_kernel).
+ * rng: device int64 {seed, base offset}.  draws_host: n_draws (<= 8) HOST int32 pairs (count slot, multiplier), N_j = counts[slot] * mult, in
+ * draw order; the last pair is the entry point's own draw: counts[slot] rows (clamped to the capacity n_rays / n_packs) of n_samples values.
+ * next_offset (may be NULL): the offset after the own draw, base + sum of every inc.  No host read: a CUDA graph can capture either call.
+ * nsb_coarse_depths_perturbed: t[r, j] = addcmul(near[r], j + u[r, j], (far[r] - near[r]) / n_samples) with torch's fp32 roundings
+ *   (the division a product with the fp32 reciprocal, the addcmul one FMA), r below the row count; other rows are not written.
+ * nsb_packed_invert_cdf_perturbed: samples[p, j] = nsb_packed_invert_cdf's sample at u = (j + u[p, j]) * (1 / n_samples) (the u of
+ *   packed_sample_cdf(perturb=True)), p below the row count; no u buffer. */
+int nsb_coarse_depths_perturbed(const float *near, const float *far, int64_t n_rays, int32_t n_samples, const int64_t *rng, const int64_t *counts,
+                                const int32_t *draws_host, int32_t n_draws, float *t, int64_t *next_offset, void *stream);
+int nsb_packed_invert_cdf_perturbed(const float *bins, const float *cdfs, const int64_t *pack_infos, int64_t n_packs, int32_t n_samples,
+                                    const int64_t *rng, const int64_t *counts, const int32_t *draws_host, int32_t n_draws, float *samples,
+                                    int64_t *next_offset, void *stream);
+
 /* ---------------------------------------------------------------- the StreetSurf LiDAR loss (csrc/lidar_loss.cu)
  * LidarLoss.forward with the depth term and the `neus_unisim` line-of-sight term (app/loss/lidar.py:174-210, 254-294) on the renderer's
  * own buffers, and its adjoint: the cotangents of the composite's depth_volume and vw (nsb_composite_backward's g_depth, g_vw).  R rays

@@ -75,13 +75,14 @@ def query_config(num_coarse=0, coarse_step_cfg=dict(step_mode="linear"), chunksi
 
 @torch.no_grad()
 def upsample_boundary(marched, rays_o, rays_d, coarse, cfg: QueryConfig, sdf_on_rays, block_order=None, *, table=None, perturb=False, counts=None,
-                      n_out=None, want_mid=True, want_ridx=True):
+                      n_out=None, want_mid=True, want_ridx=True, sampler=None):
     """sdf of the marched samples (ridx_hit, pack_infos, depth, ridx), the up-sampling stages (cdf -> inverse-cdf samples -> sdf -> merge)
     and the boundary samples of the coarse [R, num_coarse + 1] and fine depths -> neus_fused.assemble_boundary's (d1, mid, ridx_all, pack_infos).
     sdf_on_rays(ridx, t, packs, count) -> contiguous f32 sdf [t.numel()]: the caller's query (forward_sdf_on_rays' packs).  block_order(via):
     the pixel-block order of the packs on rays `via`; None: the rays are not image-ordered.  table = (meta, grid16, dec, max_level, collect)
     lets the persistent kernel run.  perturb: stratified samples (packed_sample_cdf).  counts = (cnt, CNT_SLOTS of graphics/neus_static.py):
-    sizes on the device, capacity-sized buffers (n_out merged samples); None: host sizes."""
+    sizes on the device, capacity-sized buffers (n_out merged samples); None: host sizes.  sampler(i, depth, cdf, pack_infos, nf) -> [n_packs,
+    nf]: the perturbed samples of stage i on the counted path (graphics/perturb.py: torch's draw, sized on the device)."""
     ridx_hit, pack_infos, depth, ridx = marched
     n_stage = len(cfg.factors)
 
@@ -89,6 +90,8 @@ def upsample_boundary(marched, rays_o, rays_d, coarse, cfg: QueryConfig, sdf_on_
         return None if counts is None else (counts[0], counts[1][name] + i)
 
     hit = count("hit")
+    if perturb and counts is not None and sampler is None:
+        raise RuntimeError("upsample_boundary(perturb=True, counts=...): the counted path draws through `sampler`")
     if use_persistent_upsample(rays_o.shape[0]) and not perturb and table is not None:
         # the whole no-grad half in ONE persistent per-ray kernel (csrc/ray_upsample.cu); same values as the stage kernels below
         meta, grid16, dec, max_level, collect = table
@@ -105,7 +108,7 @@ def upsample_boundary(marched, rays_o, rays_d, coarse, cfg: QueryConfig, sdf_on_
         for i, (factor, nf) in enumerate(zip(cfg.factors, cfg.num_fine)):
             cdf = neus_fused.upsample_cdf(sdf, depth, pack_infos, cfg.upsample_inv_s * factor, cfg.use_estimate_alpha, count=hit)
             if perturb:                  # one stratified u per pack and sample (raysample.py:38-61)
-                fine = packed_sample_cdf(depth, cdf, pack_infos, nf, perturb=True)[0]
+                fine = packed_sample_cdf(depth, cdf, pack_infos, nf, perturb=True)[0] if sampler is None else sampler(i, depth, cdf, pack_infos, nf)
             else:
                 fine = neus_fused.sample_cdf_uniform(depth, cdf, pack_infos, nf, count=hit)
             fine_stages.append(fine)

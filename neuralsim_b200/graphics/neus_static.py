@@ -26,6 +26,7 @@ from ..fields.networks import sdf_bwd, sdf_decoder_c, sdf_fwd
 from .neus import query_config, upsample_boundary
 from .raysample import batch_sample_step_linear
 from . import neus_fused as NF
+from . import perturb as PT
 
 __all__ = ["render_static", "StaticFrame", "CNT_SLOTS", "static_volume_buffer"]
 
@@ -180,7 +181,7 @@ def _fp16_images(model, radiance=True):
 
 def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=None, march_cap, kept_cap, coherent=False, with_rgb=True, with_normal=True,
                   perturb=False, training=None, depth_use_normalized_vw=True, cnt=None, d_h_appear=None, d_rays=None, max_level_dev=None,
-                  ray_grad_hook=None):
+                  ray_grad_hook=None, rng_dev=None):
     """One chunk of rays, ray test -> query -> integration, without a host read.  -> (rendered dict of whole-chunk images, cnt int64[32]).
     `coherent`: image-ordered rays (the boundary / fine queries then walk the samples ray-tiled) -- a host decision here (the host-sized
     path measures it in the ray-test kernel).  `d_h_appear` [R, n_appear] (optional): zero-filled here, and the backward pass writes the
@@ -189,13 +190,15 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     loss to rays_o and rays_d (the caller's frame and order; 0 for rays that miss the box or keep no sample), the depths held constant
     as on the host-sized path.  `max_level_dev` (optional): a device int32 scalar every LoTD kernel of the step reads its level bound from
     (nsb_bind_device_max_level), so that a captured step follows a level schedule; None: the model's level at this call, fixed in a capture.
-    `ray_grad_hook` (optional, with d_rays): called in the backward pass right after d_rays is written (the pose adjoint of StaticFrame)."""
+    `ray_grad_hook` (optional, with d_rays): called in the backward pass right after d_rays is written (the pose adjoint of StaticFrame).
+    `perturb`: stratified coarse depths and up-sampling quantiles, the values torch's CUDA generator gives the host-sized path
+    (graphics/neus.py:_query_fused) from the same state: the kernels of graphics/perturb.py draw them against the step's device counts.
+    `rng_dev` = int64 [2] (seed, offset) on the device, the state the step draws from (StaticFrame refills it before every replay); None:
+    the default CUDA generator's state at this call, which is then advanced by the step's reservation (perturb.reservation) -- eager calls
+    only, as a capture would fix the state."""
     P, lib = L.ptr, L.lib()
     if with_rgb and getattr(model, "radiance_net", None) is None:
         raise RuntimeError("render_static(with_rgb=True): the model has no radiance net (radiance_cfg=False); render it with with_rgb=False")
-    if perturb:
-        raise RuntimeError("render_static: perturb=True is not built (random streams of capacity-sized draws differ from the reference's); "
-                           "use the host-sized path (SingleVolumeRenderer.render)")
     training = model.training if training is None else training
     R, dev = rays_o.shape[0], rays_o.device
     cfg = query_config(**(model.ray_query_cfg.get("query_param", {}) or {}), upsample_s_divisor=model.upsample_s_divisor)
@@ -203,6 +206,13 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         raise RuntimeError("render_static: num_coarse=0 is not built (the boundary samples are the coarse and the fine ones)")
     nc1, max_steps = cfg.num_coarse + 1, cfg.max_steps
     march_cap, kept_cap = int(march_cap), int(kept_cap)
+    if perturb:
+        if ((model.ray_query_cfg.get("query_param", {}) or {}).get("march_cfg", {}) or {}).get("perturb_before_march", False):
+            raise RuntimeError("render_static(perturb=True): march_cfg.perturb_before_march=True is not built; use the host-sized path")
+        reserve = PT.reservation(R, cfg, PT.grid_cap(dev))
+        if rng_dev is None:
+            rng_dev = PT.take(PT.cuda_generator(None, dev), reserve)
+        draws_coarse, draws_stage = PT.step_draws(CNT_SLOTS, nc1, cfg.num_fine)
     if cnt is None:
         cnt = torch.zeros(32, dtype=torch.int64, device=dev)
     else:
@@ -252,7 +262,10 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
             ray_g = (ray_g[0], ray_g[1], ray_g[2] if with_rgb else None)           # g_o, g_d, g_vd (no view term without rgb)
             st.ray_grads = (ray_g[0], ray_g[1], rays_inds)
         # ---------------- coarse samples + march
-        coarse = batch_sample_step_linear(n_c, f_c, nc1, prefix_shape=[R], perturb=perturb).contiguous()
+        if perturb:           # rows past the ray count are not read (nsb_assemble_boundary)
+            coarse = PT.coarse_depths(n_c, f_c, nc1, rng_dev, cnt, draws_coarse, torch.empty(R, nc1, device=dev))
+        else:
+            coarse = batch_sample_step_linear(n_c, f_c, nc1, prefix_shape=[R]).contiguous()
         occ_grid = model.accel.occ.occ_grid
         res = occ_grid.shape[-3:]
         g8 = occ_grid.contiguous().view(torch.uint8)
@@ -297,7 +310,9 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
         d1, _mid, ridx_all, pinfo = upsample_boundary((ridx_hit, pack_infos, depth, ridx), o_c, d_c, coarse, cfg, sdf_on_rays,
                                                       (lambda via: _block_order(rays_inds, via, R, cnt, CNT_SLOTS["hit"])) if coherent else None,
                                                       table=(st.meta, st.grid16, st.dec, st.ml, st.collect), counts=(cnt, CNT_SLOTS), n_out=march_cap,
-                                                      want_mid=False, want_ridx=not coherent)
+                                                      want_mid=False, want_ridx=not coherent, perturb=perturb,
+                                                      sampler=(lambda i, dep, cdf, pi, nf: PT.invert_cdf(dep, cdf, pi, nf, rng_dev, cnt, draws_stage[i],
+                                                                                                         torch.empty(R, nf, device=dev))) if perturb else None)
     # ---------------- boundary SDF (grad) -> alpha -> compression
     s = model.implicit_surface
     dl = s.decoder.layers
@@ -421,6 +436,15 @@ class StaticFrame:
     schedule (LoTDEncoding's `anneal_cfg`; the trainer calls `model.training_before_per_step(it)` before `step()`).  A new level moves the
     surface, so a step may need more samples than the arenas were sized for; `check()` then re-sizes them from the current level.
 
+    `perturb=True` (off by default) trains with stratified samples, as the shipped StreetSurf configs do (`renderer.train.perturb`): the
+    graph draws the coarse depths and the up-sampling quantiles in its kernels from torch's CUDA generator (`generator`, else the default
+    one of the model's device; graphics/perturb.py).  `step()` writes the generator's (initial_seed(), get_offset()) into the device block
+    `frame.rng` and then advances the generator by `frame.rng_reservation` with set_offset -- host-side calls, no synchronisation.  From the
+    same generator state a replay draws exactly what the host-sized perturbed step draws, so its images, loss and gradients are that
+    step's.  The one difference: the host-sized step advances the generator by the sum of its draws (which depend on the batch), the graph
+    step by the fixed reservation that bounds them, so a run of graph steps and a run of host-sized steps drift apart after the first step.
+    `check()`'s retry replays the same draw.
+
     The first call probes the sizes with the host-sized path (SingleVolumeRenderer.ray_query, no grad), sizes the arenas with `slack`,
     warms up and captures.  Gradients are accumulated into `p.grad` (kept in place; `zero_grads=True` or a `pre_hook` zeroes them inside the graph).
     Capture precondition (PyTorch): no autograd graph of an EARLIER backward on the default stream may still be referenced (a kept loss / rendered
@@ -428,7 +452,7 @@ class StaticFrame:
 
     def __init__(self, model, n_rays, loss_fn=None, *, near=None, far=None, with_rgb=True, with_normal=True, slack=1.5, march_cap=None, kept_cap=None,
                  coherent=None, use_graph=True, zero_grads=False, h_appear_dim=None, pre_hook=None, h_appear_grad=False, ray_grad=False,
-                 loss_on_ret=False, pose=None):
+                 loss_on_ret=False, pose=None, perturb=False, generator=None):
         self.model, self.n_rays, self.loss_fn, self.loss_on_ret = model, int(n_rays), loss_fn, bool(loss_on_ret)
         self.near, self.far, self.with_rgb, self.with_normal, self.slack = near, far, with_rgb, with_normal, float(slack)
         self.march_cap, self.kept_cap, self.coherent = march_cap, kept_cap, coherent
@@ -448,6 +472,14 @@ class StaticFrame:
         if ray_grad:
             self.d_rays_o, self.d_rays_d = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)
         self.cnt = torch.zeros(32, dtype=torch.int64, device=dev)
+        self.perturb, self.rng, self.rng_reservation, self._gen = bool(perturb), None, 0, None
+        if generator is not None and not self.perturb:
+            raise RuntimeError("StaticFrame(generator=...): the generator is read only with perturb=True")
+        if self.perturb:
+            self._gen = PT.cuda_generator(generator, dev)
+            cfg = query_config(**(model.ray_query_cfg.get("query_param", {}) or {}), upsample_s_divisor=model.upsample_s_divisor)
+            self.rng_reservation = PT.reservation(self.n_rays, cfg, PT.grid_cap(dev))
+            self.rng = torch.zeros(2, dtype=torch.int64, device=dev)
         self.max_level_dev = torch.zeros((), dtype=torch.int32, device=dev)
         self.pose, self._pose_grad = pose, None
         if pose is not None:
@@ -549,7 +581,8 @@ class StaticFrame:
         try:
             rendered, _, buffers = render_static(self.model, self.rays_o, self.rays_d, self.h_appear, near=self.near, far=self.far, march_cap=self.march_cap,
                                                  kept_cap=self.kept_cap, coherent=bool(self.coherent), with_rgb=self.with_rgb, with_normal=self.with_normal, cnt=self.cnt,
-                                                 d_h_appear=self.d_h_appear, d_rays=d_rays, max_level_dev=self.max_level_dev, ray_grad_hook=hook)
+                                                 d_h_appear=self.d_h_appear, d_rays=d_rays, max_level_dev=self.max_level_dev, ray_grad_hook=hook,
+                                                 perturb=self.perturb, rng_dev=self.rng)
         finally:
             if cv is not None:
                 cv._use_w_dev = False
@@ -627,6 +660,8 @@ class StaticFrame:
                 cv._w_dev = torch.zeros((), device=self.device)
             cv._w_dev.fill_(cv.mix_weight())                  # the variance schedule's host-side weight of THIS iteration
         self.max_level_dev.fill_(self.model.implicit_surface._ml(self.model.max_level))     # the LoTD level bound of THIS iteration
+        if self.perturb:
+            PT.take(self._gen, self.rng_reservation, self.rng)                                 # the random state of THIS iteration
         if self.graph is None and (self.use_graph or self.march_cap is None):
             self.capture()
         if self.graph is not None:
