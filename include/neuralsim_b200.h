@@ -467,6 +467,32 @@ int nsb_packed_invert_cdf_perturbed(const float *bins, const float *cdfs, const 
                                     const int64_t *rng, const int64_t *counts, const int32_t *draws_host, int32_t n_draws, float *samples,
                                     int64_t *next_offset, void *stream);
 
+/* ---------------------------------------------------------------- error-map importance sampling (csrc/importance.cu)
+ * The training batch of one camera as ImpSampler.sample_img_pixel(n) draws it over one ErrorMap (nr3d_lib/models/importance.py:317-336):
+ * n_uniform rays from torch.randint(n_images, [n_uniform]) and torch.rand([n_uniform, 2]).clamp_(1e-6, 1 - 1e-6), the other n - n_uniform
+ * from torch.rand([n_e]) (the frame, searchsorted on cdf_img) and torch.rand([2, n_e]) (the 2-D inverse cdf), all clamped, drawn in that
+ * order from rng = device int64 {seed, offset} (torch_uniform.cuh).  rng_next (may be NULL) := {seed, offset after the four draws}.
+ * table: device int64 [n_cameras, NSB_IMP_TABLE_WIDTH], one row per camera: {cdf_img [F], cdf_y [F, res_y], cdf_x [F, res_y, res_x],
+ * intrinsics [F, 3, 3] (float32 device pointers), F, W, H, pose_base, appear_base, error_map, last (nsb_error_map_update's), gt_0 ..
+ * gt_4 (device pointers of [F, H, W] rows of gt_row_bytes[k] bytes)}; cam: device int64 scalar, the row.  dirs NULL: fidx and xy only (no
+ * camera: intrinsics, W, H, the bases and gt are not read).  Per ray r: fidx[r], xy[r] = (x, y) in (0, 1) (unsnapped), pidx[r] =
+ * pose_base + fidx, dirs[r] = pinhole_lift(w + 0.5, h + 0.5, 1) of the pixel (w, h) = (xy * WH).long().clamp_(0, WH - 1) (fp32, the
+ * reference's operation order, skew included), the n_gt ground-truth rows at (fidx, h, w) into gt_out[k] (HOST array of device
+ * pointers, rows of gt_row_bytes[k] (HOST) bytes, copied as stored), and with h_appear the code row appear_table[appear_base + fidx]
+ * ([*, n_appear] float32).  No host read.
+ * nsb_error_map_update: ErrorMap.update_error_map(fidx, xy, val) (importance.py:87-109) on error_map [n_images, res_y, res_x]: four corner
+ * statements in order, each `map[i, h, w] += v` with a cell hit by several rays receiving old + v of the last such ray in batch order.
+ * last: int32 [4, n_images, res_y, res_x] scratch, all -1 on entry and on return (the caller fills it once).  With table, error_map, last
+ * and the frame count come from row *cam (no host read), n_images then bounds every camera's.  flag |= 1 where a val < 0 (the update still
+ * runs).  skip (may be NULL): a device int64; when non-zero the map is left as it is (an overflowed step).  Two launches, deterministic. */
+#define NSB_IMP_TABLE_WIDTH 16
+#define NSB_IMP_MAX_GT 5
+int nsb_imp_sample(const int64_t *table, const int64_t *cam, const int64_t *rng, int64_t n, int64_t n_uniform, int32_t res_y, int32_t res_x,
+                   int32_t n_gt, const int64_t *gt_row_bytes, void *const *gt_out, const float *appear_table, int32_t n_appear, float *h_appear,
+                   int64_t *fidx, float *xy, int64_t *pidx, float *dirs, int64_t *rng_next, void *stream);
+int nsb_error_map_update(float *error_map, int32_t *last, int64_t n_images, const int64_t *table, const int64_t *cam, int32_t res_y, int32_t res_x,
+                         const int64_t *fidx, const float *xy, const float *val, int64_t n, int32_t *flag, const int64_t *skip, void *stream);
+
 /* ---------------------------------------------------------------- the StreetSurf LiDAR loss (csrc/lidar_loss.cu)
  * LidarLoss.forward with the depth term and the `neus_unisim` line-of-sight term (app/loss/lidar.py:174-210, 254-294) on the renderer's
  * own buffers, and its adjoint: the cotangents of the composite's depth_volume and vw (nsb_composite_backward's g_depth, g_vw).  R rays

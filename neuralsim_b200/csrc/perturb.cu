@@ -23,21 +23,6 @@ struct Draws {
     int32_t slot[kMaxDraws], mult[kMaxDraws];
 };
 
-// torch's cap on the grid of a draw (calc_execution_policy): SMs * (maxThreadsPerSM / 256) blocks, per device
-inline int64_t torch_rand_grid_cap() {
-    static std::atomic<int64_t> cache[64];
-    const int dev = current_device() & 63;
-    int64_t c = cache[dev].load(std::memory_order_relaxed);
-    if (c == 0) {
-        int threads = 0;
-        cudaDeviceGetAttribute(&threads, cudaDevAttrMaxThreadsPerMultiProcessor, current_device());
-        c = (int64_t)sm_count() * (threads / kTorchRandBlock);
-        if (c <= 0) c = 1;
-        cache[dev].store(c, std::memory_order_relaxed);
-    }
-    return c;
-}
-
 // this kernel's draw: Philox (seed, offset), its size n and its live rows (counts[slot] clamped to the capacity)
 struct Draw {
     uint64_t seed, offset;

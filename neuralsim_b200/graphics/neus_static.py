@@ -445,6 +445,17 @@ class StaticFrame:
     step by the fixed reservation that bounds them, so a run of graph steps and a run of host-sized steps drift apart after the first step.
     `check()`'s retry replays the same draw.
 
+    `sampler=CameraSampler(...)` (neuralsim_b200/importance.py; off by default; needs pose= and a loss_fn) draws every batch inside the
+    graph, as the shipped camera configs' ImpSampler.sample_img_pixel does over each camera's error map: `frame.step(cam=k)` fills a
+    device camera index and the generator block (the sampler's four draws come first, the perturbed ones after them), and the one replay
+    samples frames and pixels (nsb_imp_sample), gathers the ground truth into `frame.ground_truth` (a dict of [n_rays, ...] rows), writes
+    `frame.rays_fidx`, `frame.rays_pix`, the pose indices, the camera-space directions and the appearance codes, renders, calls
+    `loss, err = loss_fn(rendered_or_ret, frame.ground_truth)`, runs the backward and adds err [n_rays] (the per-ray rgb error the
+    reference feeds its error map) into camera k's error map (nsb_error_map_update).  After the replay, on the host, camera k's step
+    counter advances and its cdfs are rebuilt in place when the reference would (ErrorMap.count_step).  A negative error is recorded in a
+    device flag that `check()` raises on; a step that overflowed its arenas leaves the error map as it was.  `d_h_appear` keeps its
+    meaning: a trainer scatters it by `frame.rays_fidx`.
+
     The first call probes the sizes with the host-sized path (SingleVolumeRenderer.ray_query, no grad), sizes the arenas with `slack`,
     warms up and captures.  Gradients are accumulated into `p.grad` (kept in place; `zero_grads=True` or a `pre_hook` zeroes them inside the graph).
     Capture precondition (PyTorch): no autograd graph of an EARLIER backward on the default stream may still be referenced (a kept loss / rendered
@@ -452,7 +463,7 @@ class StaticFrame:
 
     def __init__(self, model, n_rays, loss_fn=None, *, near=None, far=None, with_rgb=True, with_normal=True, slack=1.5, march_cap=None, kept_cap=None,
                  coherent=None, use_graph=True, zero_grads=False, h_appear_dim=None, pre_hook=None, h_appear_grad=False, ray_grad=False,
-                 loss_on_ret=False, pose=None, perturb=False, generator=None):
+                 loss_on_ret=False, pose=None, perturb=False, generator=None, sampler=None):
         self.model, self.n_rays, self.loss_fn, self.loss_on_ret = model, int(n_rays), loss_fn, bool(loss_on_ret)
         self.near, self.far, self.with_rgb, self.with_normal, self.slack = near, far, with_rgb, with_normal, float(slack)
         self.march_cap, self.kept_cap, self.coherent = march_cap, kept_cap, coherent
@@ -473,10 +484,12 @@ class StaticFrame:
             self.d_rays_o, self.d_rays_d = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)
         self.cnt = torch.zeros(32, dtype=torch.int64, device=dev)
         self.perturb, self.rng, self.rng_reservation, self._gen = bool(perturb), None, 0, None
-        if generator is not None and not self.perturb:
-            raise RuntimeError("StaticFrame(generator=...): the generator is read only with perturb=True")
-        if self.perturb:
+        self.sampler = sampler
+        if generator is not None and not self.perturb and sampler is None:
+            raise RuntimeError("StaticFrame(generator=...): the generator is read only with perturb=True or a sampler")
+        if self.perturb or sampler is not None:
             self._gen = PT.cuda_generator(generator, dev)
+        if self.perturb:
             cfg = query_config(**(model.ray_query_cfg.get("query_param", {}) or {}), upsample_s_divisor=model.upsample_s_divisor)
             self.rng_reservation = PT.reservation(self.n_rays, cfg, PT.grid_cap(dev))
             self.rng = torch.zeros(2, dtype=torch.int64, device=dev)
@@ -491,6 +504,8 @@ class StaticFrame:
             self._pose_scratch = torch.zeros(max(scratch_floats(self.n_rays, P), 4), device=dev)
             self._pose_d_rays = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)       # the rays' gradient when ray_grad is off
             self._pose_g = (torch.zeros(P, 4, device=dev), torch.zeros(P, 3, device=dev))   # what dq.grad / dt.grad are while the frame lives
+        if sampler is not None:
+            self._init_sampler(sampler, pose, loss_fn)
         self.graph, self.loss, self.rendered, self.buffers, self._occ_captured = None, None, None, None, None
         self.captures = 0
 
@@ -518,6 +533,35 @@ class StaticFrame:
         k = int(max(need_k * self.slack, floor) * grow)
         self.march_cap = max(self.march_cap or 0, m)
         self.kept_cap = max(self.kept_cap or 0, k)
+
+    # -- the sampler
+    def _init_sampler(self, sampler, pose, loss_fn):
+        from ..importance import CameraSampler
+        if not isinstance(sampler, CameraSampler):
+            raise RuntimeError(f"StaticFrame(sampler=...): a neuralsim_b200.importance.CameraSampler, got {type(sampler)}")
+        if pose is None or loss_fn is None:
+            raise RuntimeError("StaticFrame(sampler=...): needs pose= (CameraPoses: the sampled rays are pose indices and camera-space directions) and a loss_fn")
+        if sampler.pose_end > pose.n_poses:
+            raise RuntimeError(f"StaticFrame(sampler=...): the cameras' frames reach pose {sampler.pose_end - 1}, the pose list holds {pose.n_poses}")
+        if sampler.device != self.device:
+            raise RuntimeError(f"StaticFrame(sampler=...): the sampler is on {sampler.device}, the model on {self.device}")
+        if sampler.appear_table is not None and (self.h_appear is None or sampler.appear_table.shape[1] != self.h_appear.shape[1]):
+            raise RuntimeError("StaticFrame(sampler=...): the sampler's appearance codes do not match the model's code width")
+        dev, n = self.device, self.n_rays
+        self.sampler_reservation = sampler.inc(n, PT.grid_cap(dev))
+        self.cam = torch.zeros((), dtype=torch.int64, device=dev)
+        self._rng_sampler = torch.zeros(2, dtype=torch.int64, device=dev)
+        self.rays_fidx = torch.zeros(n, dtype=torch.int64, device=dev)
+        self.rays_pix = torch.zeros(n, 2, device=dev)
+        self.ground_truth = {k: torch.zeros((n,) + tail, dtype=dt, device=dev) for k, (dt, tail) in sampler.gt_spec.items()}
+        self.err_flag = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._warming = False
+
+    def _sample(self):
+        """camera self.cam's batch into the frame's inputs (nsb_imp_sample)"""
+        s = self.sampler
+        s.sample(self.cam, self._rng_sampler, self.n_rays, self.rays_fidx, self.rays_pix, self.pidx, self.dirs, self.ground_truth,
+                 self.h_appear if s.appear_table is not None else None, self.rng if self.perturb else None)
 
     # -- the pose
     def set_rays(self, dirs, pidx):
@@ -566,6 +610,8 @@ class StaticFrame:
                 if p.grad is not None:
                     p.grad.zero_()
         pose_grad = self._pose_wants_grad()
+        if self.sampler is not None:
+            self._sample()
         if self.pose is not None:
             if self.zero_grads and pose_grad:
                 for g in self._pose_g:
@@ -588,13 +634,25 @@ class StaticFrame:
                 cv._use_w_dev = False
         loss = None
         if self.loss_fn is not None:
-            loss = self.loss_fn(dict(rendered=rendered, volume_buffer=static_volume_buffer(buffers, self.cnt)) if self.loss_on_ret else rendered)
+            arg = dict(rendered=rendered, volume_buffer=static_volume_buffer(buffers, self.cnt)) if self.loss_on_ret else rendered
+            if self.sampler is None:
+                loss = self.loss_fn(arg)
+            else:
+                loss, err = self.loss_fn(arg, self.ground_truth)
+                if not isinstance(err, torch.Tensor) or err.numel() != self.n_rays:
+                    raise RuntimeError(f"StaticFrame(sampler=...): loss_fn must return (loss, err), err holding {self.n_rays} per-ray errors")
+                err = err.detach().reshape(-1).float().contiguous()
             if loss.requires_grad:
                 loss.backward()
             loss = loss.detach()
+            if self.sampler is not None and not self._warming:       # the warm-up runs must not add into the error map
+                ov = CNT_SLOTS["overflow"]
+                self.sampler.update(self.cam, self.rays_fidx, self.rays_pix, err, self.err_flag, skip=self.cnt[ov:ov + 1])
         return rendered, buffers, loss
 
     def capture(self):
+        if self.sampler is not None:
+            self._sample()                                  # this step's batch: the probe and the check below read its rays
         if self.pose is not None:
             if not bool(self.dirs.any()):                   # (zero directions: see below)
                 raise RuntimeError("StaticFrame.capture: the pose inputs hold no rays yet; call set_rays(dirs, pidx) or step(dirs=..., pidx=...) first")
@@ -617,8 +675,12 @@ class StaticFrame:
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
-                for _ in range(2):                          # warm-up on a side stream (allocator, lazy module state)
-                    self._run()
+                self._warming = True
+                try:
+                    for _ in range(2):                      # warm-up on a side stream (allocator, lazy module state)
+                        self._run()
+                finally:
+                    self._warming = False
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
@@ -635,9 +697,18 @@ class StaticFrame:
             L.KERNEL_TIMER.enabled = was
         return self
 
-    def step(self, rays_o=None, rays_d=None, rays_h_appear=None, *, dirs=None, pidx=None):
+    def step(self, rays_o=None, rays_d=None, rays_h_appear=None, *, dirs=None, pidx=None, cam=None):
         """copy the batch into the graph's inputs (H2D if the tensors are on the host) and launch.  -> loss (device scalar) or None.
-        With pose=: no rays_o / rays_d; dirs and pidx (set_rays), or neither to replay the rays set last."""
+        With pose=: no rays_o / rays_d; dirs and pidx (set_rays), or neither to replay the rays set last.  With sampler=: cam alone, the
+        camera whose batch the graph draws."""
+        if self.sampler is not None:
+            if rays_o is not None or rays_d is not None or rays_h_appear is not None or dirs is not None or pidx is not None:
+                raise RuntimeError("StaticFrame.step: a frame with sampler= draws its own batch; pass cam= only")
+            if isinstance(cam, bool) or not isinstance(cam, int) or not 0 <= cam < self.sampler.n_cameras:
+                raise RuntimeError(f"StaticFrame.step: cam must be an int in [0, {self.sampler.n_cameras}), got {cam!r}")
+            self.cam.fill_(cam)
+        elif cam is not None:
+            raise RuntimeError("StaticFrame.step: cam= is read only with sampler=")
         if self.pose is None:
             if rays_o is None or rays_d is None or dirs is not None or pidx is not None:
                 raise RuntimeError("StaticFrame.step: a frame without pose= takes rays_o and rays_d (and no dirs / pidx)")
@@ -660,7 +731,9 @@ class StaticFrame:
                 cv._w_dev = torch.zeros((), device=self.device)
             cv._w_dev.fill_(cv.mix_weight())                  # the variance schedule's host-side weight of THIS iteration
         self.max_level_dev.fill_(self.model.implicit_surface._ml(self.model.max_level))     # the LoTD level bound of THIS iteration
-        if self.perturb:
+        if self.sampler is not None:        # the sampler's draws first; its kernel chains the offset after them into self.rng
+            PT.take(self._gen, self.sampler_reservation + self.rng_reservation, self._rng_sampler)
+        elif self.perturb:
             PT.take(self._gen, self.rng_reservation, self.rng)                                 # the random state of THIS iteration
         if self.graph is None and (self.use_graph or self.march_cap is None):
             self.capture()
@@ -672,6 +745,8 @@ class StaticFrame:
             self.graph.replay()
         else:
             self.rendered, self.buffers, self.loss = self._run()
+        if self.sampler is not None:
+            self.sampler.samplers[cam].error_map.count_step()     # the reference's per-camera schedule; rebuilds the cdfs in place
         return self.loss
 
     def counts(self):
@@ -681,7 +756,11 @@ class StaticFrame:
 
     def check(self, retry=True):
         """True if the last step fitted its arenas.  Otherwise the arenas are re-sized from this batch, the graph is re-captured and --
-        with `retry` -- the step is run again (gradients of the overflowed step were those of an empty render: nothing accumulated)."""
+        with `retry` -- the step is run again (gradients of the overflowed step were those of an empty render: nothing accumulated).
+        With sampler=: raises if loss_fn gave the error map a negative error since the last check."""
+        if self.sampler is not None and int(self.err_flag) != 0:
+            self.err_flag.zero_()
+            raise RuntimeError("StaticFrame.check: loss_fn returned a negative per-ray error; the error map accumulates non-negative errors only")
         if int(self.cnt[CNT_SLOTS["overflow"]]) == 0:
             return True
         self.march_cap = self.kept_cap = None
