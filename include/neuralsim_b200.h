@@ -226,9 +226,11 @@ typedef struct nsb_occ_collect {
     float inv_s;
 } nsb_occ_collect;
 
-/* The tensor-core SDF, colour and up-sampling entry points below take 3-D LoTD tables of L = 1..16 pseudo levels with
- * n_feat_per_pseudo_lvl == 2 and n_encoded_dims == 2L; the decoder's W1 is then [W x 2L].  Tables of more than 16 levels are refused
- * (the error names the limit) and run on the unfused LoTD entry points.  h_out of nsb_fused_sdf needs 16 levels. */
+/* The tensor-core SDF, colour and up-sampling entry points below take 3-D LoTD tables of L = 1..24 pseudo levels with
+ * n_feat_per_pseudo_lvl == 2 and n_encoded_dims == 2L; the decoder's W1 is then [W x 2L].  Tables of 1..16 levels run kernels with a
+ * 32-column feature tile, tables of 17..24 levels the same kernels with a 48-column one (chosen from L, not from max_level).  Tables of
+ * more than 24 levels are refused (the error names the limit) and run on the unfused LoTD entry points.  h_out of nsb_fused_sdf and its
+ * SIMT kernel need 16 levels. */
 /* forward_sdf on N points: x in network space [-1,1]^3 (not yet /2+0.5).  sdf fp32 (fp16-valued). */
 int nsb_fused_sdf(const nsb_lotd_meta *meta_host, const void *params_half, const nsb_sdf_decoder *dec_host,
                   const float *x, int64_t n, int32_t max_level, float *sdf, void *h_out_half, void *stream);
@@ -548,7 +550,7 @@ int nsb_occ_ema_update(const float *pts, const float *val, int64_t n, int32_t va
  * its backward including the second-order pass through nablas (LoTDFunctionBwdDydx.backward, lotd.py:193-268) as two.
  * All weight pointers are fp16 device images of the fp32 masters (what autocast feeds the GEMMs). */
 typedef struct nsb_color_net {
-    const void *W1, *b1, *W2, *b2;            /* sdf decoder: [width x 2L], [width], [1 x width], [1] (L levels, 1..16) */
+    const void *W1, *b1, *W2, *b2;            /* sdf decoder: [width x 2L], [width], [1 x width], [1] (L levels, 1..24) */
     const void *R1, *rb1, *R2, *rb2, *R3, *rb3; /* radiance net: [rw x rad_in], [rw], [rw x rw], [rw], [3 x rw], [3] */
     int32_t width, rad_width, rad_in, n_appear; /* rad_in = 3 + 16 + 3 + 2L + n_appear ([x, SH4(v), n, h, h_appear]) */
     float beta;                               /* Softplus beta of the decoder                                      */
@@ -557,9 +559,12 @@ typedef struct nsb_color_net {
 
 /* bytes of ONE saved activation buffer for n points (fp16 tiles of 128 points x 64 columns, core-matrix layout) */
 int64_t nsb_color_tile_bytes(int64_t n);
+/* bytes of ONE saved activation buffer for n points of an L-level table: nsb_color_tile_bytes(n) for L <= 16; for L = 17..24 the X tile
+ * is 80 columns wide (h takes 48), so every buffer is sized n_tiles x 20 KB */
+int64_t nsb_color_act_bytes(int64_t n, int32_t n_levels);
 /* Points are x[n,3] or rays_o/rays_d[R,3] + ridx[n] (NULL = identity) + t[n]; view_dirs[R,3] and h_appear[R,n_appear] are
  * indexed by ridx (by the point index when ridx is NULL).  Outputs fp32: sdf[n], nablas[n,3], rgb[n,3], x_out[n,3] (optional).
- * act_* : four buffers of nsb_color_tile_bytes(n) each kept for the backward, or all NULL for inference.
+ * act_* : four buffers of nsb_color_act_bytes(n, L) each kept for the backward, or all NULL for inference.
  * collect: NULL or the occupancy-evidence side effect of forward_sdf_nablas (see nsb_occ_collect).
  * rgb == NULL selects the geometry-only form (LoTDSDF.forward_sdf_nablas alone): sdf, nablas, x_out, act_z and the h half of act_x are
  * written exactly as with rgb, nothing of the radiance net is read, view_dirs, h_appear, act_y1 and act_y2 may be NULL (act_z and act_x
@@ -568,7 +573,7 @@ int nsb_fused_color_fwd(const nsb_lotd_meta *meta_host, const void *params_half,
                         const float *rays_o, const float *rays_d, const int64_t *ridx, const float *t, const float *view_dirs,
                         const float *h_appear, int64_t n, int32_t max_level, float *sdf, float *nablas, float *rgb, float *x_out,
                         void *act_z, void *act_x, void *act_y1, void *act_y2, const nsb_occ_collect *collect, void *stream);
-/* Cotangents g_sdf[n], g_nablas[n,3], g_rgb[n,3] (each may be NULL = zero); dh_scratch[n,32] fp32 workspace.
+/* Cotangents g_sdf[n], g_nablas[n,3], g_rgb[n,3] (each may be NULL = zero); dh_scratch[n,32] fp32 workspace ([n,48] for tables of 17..24 levels).
  * All gradient outputs are fp32 and ACCUMULATED into (caller zero-fills); d_R* use the reference's column order.
  * With g_rgb == NULL the radiance backward does not run: act_y1, act_y2, rgb, dh_scratch and d_R* / d_rb* may then be NULL, and net_host
  * may have rad_width == 0 with NULL radiance pointers (the activations of a geometry-only forward are enough). */

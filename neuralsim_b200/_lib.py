@@ -61,6 +61,8 @@ def lib():
         _lib.nsb_last_error.restype = ctypes.c_char_p
         _lib.nsb_launch_count.restype = ctypes.c_uint64
         _lib.nsb_color_tile_bytes.restype = ctypes.c_int64
+        _lib.nsb_color_act_bytes.restype = ctypes.c_int64
+        _lib.nsb_color_act_bytes.argtypes = [ctypes.c_int64, ctypes.c_int32]
         _lib.nsb_upsample_rays_scratch_floats.restype = ctypes.c_int64
         _lib.nsb_kth_smallest_scratch_bytes.restype = ctypes.c_int64
         _lib.nsb_pose_grad_scratch_floats.restype = ctypes.c_int64

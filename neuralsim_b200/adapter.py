@@ -88,9 +88,11 @@ def _share(dst: nn.Module, name: str, src):
         dst._buffers[name] = src
 
 
-def accelerate(ref_model, *, patch=True) -> LoTDNeuSModel:
-    """-> the LoTDNeuSModel that now backs `ref_model` (also stored as `ref_model._nsb`).  See the module docstring."""
+def accelerate(ref_model, *, patch=True, max_fused_levels: int = 16) -> LoTDNeuSModel:
+    """-> the LoTDNeuSModel that now backs `ref_model` (also stored as `ref_model._nsb`).  See the module docstring.
+    max_fused_levels = 24 runs tables of 17..24 levels (the shipped StreetSurf camera models) on the fused kernels too."""
     cfg = describe(ref_model)
+    cfg["surface_cfg"]["max_fused_levels"] = max_fused_levels
     dev = ref_model.implicit_surface.encoding.flattened_params.device
     ours = LoTDNeuSModel(device=dev, **cfg)
     rs, os_ = ref_model.implicit_surface, ours.implicit_surface

@@ -18,7 +18,9 @@
 // Numerics: the fp16 rounding points of the reference's autocast graph (oracle/nets.py); J and nablas use the exact
 // arithmetic of k_lotd_fwd<DYDX> / k_lotd_bwd_input, so nablas is bit-identical to the unfused kernels given the same g.
 // Radiance input columns are kept in the internal order [h | x | SH(v) | n | h_appear | 0] (h first, so the h tile IS the
-// first four chunks of X); weights are permuted when staged / flushed.
+// first NF / 8 chunks of X); weights are permuted when staged / flushed.
+// NF (a template parameter of every kernel here) is the width of the h tile: 32 for tables of 1..16 levels, 48 for 17..24
+// (feature_cols); the X tile is then NF + 32 columns wide: 64, or 80.
 #include "fused_tc_common.cuh"
 #include "sh_device.cuh"
 
@@ -31,14 +33,21 @@ struct ColorNetDev {
     float fac[3];                                       // sdf_scale / radius3d_original per axis
 };
 
-constexpr int XW = 64;                                  // padded radiance input width / hidden width
-constexpr int kTileBytes = kTile * XW * 2;              // one saved activation tile: 16 KB
+constexpr int XW = 64;                                  // padded hidden width of the radiance net
+constexpr int kTileBytes = kTile * XW * 2;              // one saved activation tile (Z, Y1, Y2; X at NF = 32): 16 KB
 constexpr int kChunk = kTile * 16;                      // bytes of one 8-column chunk of a 128-row tile
+template <int NF>
+constexpr int x_cols() { return NF + 32; }              // the radiance input tile [h(NF) | x sh n h_appear 0 (32)]
+template <int NF>
+constexpr int x_tile_bytes() { return kTile * x_cols<NF>() * 2; }   // one saved X tile: 16 KB, or 20 KB at NF = 48
+constexpr int kXVCols = 32;                             // the ray-gradient columns [x | SH | 0] of k_color_rad_bwd<., true>: 19 used
 
 // internal radiance-input column -> reference column (or -1 for padding); the reference input is [x(3), SH(16), n(3), h(nh), h_appear]
-// with nh = 2L h columns, so rad_in = 22 + nh + n_appear, and the internal h columns nh..31 are padding
-__host__ __device__ inline int ref_col(int k, int n_appear, int nh) {
-    if (k < 32) return k < nh ? 22 + k : -1;
+// with nh = 2L h columns, so rad_in = 22 + nh + n_appear, and the internal h columns nh..hc-1 are padding (hc = NF, the h tile's width;
+// the columns after it sit hc - 32 further right than in the 32-column layout)
+__host__ __device__ inline int ref_col(int k, int n_appear, int nh, int hc = 32) {
+    if (k < hc) return k < nh ? 22 + k : -1;
+    k -= hc - 32;
     if (k < 35) return k - 32;
     if (k < 51) return 3 + (k - 35);
     if (k < 54) return 19 + (k - 51);
@@ -118,9 +127,12 @@ constexpr int kColorGeoCtasPerSM = 2;
 
 // ===================================================================================================================== forward
 // kRad = false is the geometry-only form (models without a radiance net, and rays that render no rgb): it stops after nablas, writes the
-// Z tile and the h half of the X tile (at the X tile's 16 KB stride, so k_color_sdf_bwd reads them unchanged) and never reads the
+// Z tile and the h part of the X tile (at the X tile's stride, so k_color_sdf_bwd reads them unchanged) and never reads the
 // radiance weights, view_dirs, h_appear, rgb_out, Y1t or Y2t.
-template <bool kRad>
+// NF = 48: levels 0..15 are gathered with their Jacobian in registers (gather_row_and_jacobian), levels 16..La-1 by the plain gather;
+// once g is known, their Jacobian is formed from a second load of the same 8 corners (L1 / L2 hits) and added in level order, so
+// nablas keeps the arithmetic of k_lotd_bwd_input.
+template <bool kRad, int NF>
 __global__ void __launch_bounds__(kTile)
 k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev net, const PointSrc ps, const float *__restrict__ view_dirs,
             const float *__restrict__ h_appear, int64_t n, int max_level, float *__restrict__ sdf_out, float *__restrict__ nab_out,
@@ -131,28 +143,31 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
     const uint32_t La = active_levels(max_level, ml_dev, m.n_pseudo);
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
-    uint8_t *sX = tiles;                                       // 16 KB [h | x sh n ha 0] (geometry-only: 8 KB, the h half)
-    uint8_t *sU = sX + (kRad ? kTileBytes : 4 * kChunk);       // 16 KB u, later relu(y1)
-    uint8_t *sW1 = sU + kTileBytes;                            //  4 KB W1   [64 x 32]
-    uint8_t *sW1T = sW1 + HW * NF * 2;                         //  4 KB W1^T [32 x 64]
-    uint8_t *sR1 = sW1T + HW * NF * 2;                         //  8 KB R1 [64 x 64] (internal column order; radiance only)
-    uint8_t *sR2 = sR1 + XW * XW * 2;                          //  8 KB R2 [64 x 64] (radiance only)
+    constexpr int XC = x_cols<NF>();
+    uint8_t *sX = tiles;                                       // 16 KB (NF = 48: 20 KB) [h | x sh n ha 0] (geometry-only: the h part)
+    uint8_t *sU = sX + (kRad ? x_tile_bytes<NF>() : (NF / 8) * kChunk);   // 16 KB u, later relu(y1)
+    uint8_t *sW1 = sU + kTileBytes;                            //  4 KB (6 KB) W1   [64 x NF]
+    uint8_t *sW1T = sW1 + HW * NF * 2;                         //  4 KB (6 KB) W1^T [NF x 64]
+    uint8_t *sR1 = sW1T + HW * NF * 2;                         //  8 KB (10 KB) R1 [64 x XC] (internal column order; radiance only)
+    uint8_t *sR2 = sR1 + XW * XC * 2;                          //  8 KB R2 [64 x 64] (radiance only)
     constexpr int kS = tc::acc_stride(64);
     float *acc = reinterpret_cast<float *>(kRad ? sR2 + XW * XW * 2 : sR1);   // 34 KB staged accumulator rows (Z, g, Y1, Y2 in turn)
     __shared__ float sb1[HW], sW2[HW], srb1[XW], srb2[XW], sR3[3][XW];
     __shared__ float sb2, srb3[3];
 
     const int tid = threadIdx.x;
-    stage_W1(net.dec, sW1, tid);
-    stage_W1T(net.dec, sW1T, tid);
+    stage_W1<NF>(net.dec, sW1, tid);
+    stage_W1T<NF>(net.dec, sW1T, tid);
     if constexpr (kRad) {
-        for (int e = tid; e < XW * XW; e += kTile) {
+        for (int e = tid; e < XW * XC; e += kTile) {
             const int j = e % XW, k = e / XW;                  // (out j, in k)
-            const int rc = ref_col(k, net.n_appear, net.dec.nh);
+            const int rc = ref_col(k, net.n_appear, net.dec.nh, NF);
             const __half v1 = (j < net.rw && rc >= 0) ? net.R1[j * net.rin + rc] : __float2half_rn(0.f);
-            const __half v2 = (j < net.rw && k < net.rw) ? net.R2[j * net.rw + k] : __float2half_rn(0.f);
             *reinterpret_cast<__half *>(sR1 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v1;
-            *reinterpret_cast<__half *>(sR2 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v2;
+            if (k < XW) {
+                const __half v2 = (j < net.rw && k < net.rw) ? net.R2[j * net.rw + k] : __float2half_rn(0.f);
+                *reinterpret_cast<__half *>(sR2 + (k / 8) * (XW * 16) + j * 16 + (k % 8) * 2) = v2;
+            }
         }
     }
     stage_decoder_vectors(net.dec, sb1, sW2, &sb2, tid);
@@ -182,6 +197,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         load_point(ps, ps.x == nullptr, i, valid, xn, xs, ray);
         float J0[16][3], J1[16][3];
         gather_row_and_jacobian(m, grid, xs, La, sX, tid, J0, J1);                  // h -> chunks 0..3 of X, J -> registers
+        if constexpr (NF > 32) gather_row_to_tile<kTile, NF, kColorGatherU>(m, grid, xs, La, sX, tid, 16);   // levels 16.. -> chunks 4..5
         tc::fence_async_smem();
         __syncthreads();
         tc::mma_to_rows<64, 0, 0, NF / 16>(acc, kS, 0, tc::kmajor(x_addr, kTile), tc::kmajor(w1_addr, HW), false);   // Z = H . W1^T
@@ -209,12 +225,12 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         const float sdf = r16(out + sb2);
         tc::fence_async_smem();
         __syncthreads();
-        tc::mma_to_rows<32, 0, 0, HW / 16>(acc, kS, 0, tc::kmajor(u_addr, kTile), tc::kmajor(w1t_addr, NF), false);   // g = U . W1
+        tc::mma_to_rows<NF, 0, 0, HW / 16>(acc, kS, 0, tc::kmajor(u_addr, kTile), tc::kmajor(w1t_addr, NF), false);   // g = U . W1
         __syncthreads();
-        // ---- nablas01 = J^T g, f ascending (k_lotd_bwd_input order), J from the gather
+        // ---- nablas01 = J^T g, f ascending (k_lotd_bwd_input order), J from the gather (levels >= 16: from a second corner load)
         float nacc[3] = {0.f, 0.f, 0.f};
 #pragma unroll
-        for (uint32_t g4 = 0; g4 < 4; ++g4) {
+        for (uint32_t g4 = 0; g4 < NF / 8; ++g4) {
             float gg[8];
             tc::acc_ld8(acc, kS, tid, g4 * 8, gg);
 #pragma unroll
@@ -222,10 +238,13 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
                 const uint32_t p = g4 * 4 + q;
                 if (p < La) {
                     const float g0 = r16(gg[2 * q]), g1 = r16(gg[2 * q + 1]);
+                    float Jr0[3], Jr1[3];
+                    if (p >= 16) level_jacobian(m, p, xs, grid, Jr0, Jr1);
+                    const uint32_t pj = p < 16 ? p : 15;       // p is a constant after unrolling: J stays statically indexed
 #pragma unroll
-                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g0, J0[p][d], nacc[d]);
+                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g0, p < 16 ? J0[pj][d] : Jr0[d], nacc[d]);
 #pragma unroll
-                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g1, J1[p][d], nacc[d]);
+                    for (int d = 0; d < 3; ++d) nacc[d] = __fmaf_rn(g1, p < 16 ? J1[pj][d] : Jr1[d], nacc[d]);
                 }
             }
         }
@@ -234,7 +253,7 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
         for (int d = 0; d < 3; ++d) nab[d] = __fmul_rn(__fmul_rn(nacc[d], 0.5f), net.fac[d]);
         float o3[3] = {0.f, 0.f, 0.f};
         if constexpr (kRad) {
-            // ---- radiance input, columns 32..63: [x | SH(v) | clamp(n) | h_appear | 0]
+            // ---- radiance input, columns NF..NF+31: [x | SH(v) | clamp(n) | h_appear | 0]
             {
                 float xr[32];
 #pragma unroll
@@ -250,23 +269,28 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
                 }
 #pragma unroll
                 for (int d = 0; d < 3; ++d) xr[19 + d] = fminf(fmaxf(nab[d], -1.f), 1.f);
-                uint8_t *xt = Xt ? Xt + tile * kTileBytes : nullptr;
+                uint8_t *xt = Xt ? Xt + tile * x_tile_bytes<NF>() : nullptr;
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {
                     float v8[8];
 #pragma unroll
                     for (int k = 0; k < 8; ++k) v8[k] = xr[c * 8 + k];
                     const uint4 q = tc::pack8_f16(v8);
-                    *reinterpret_cast<uint4 *>(sX + (4 + c) * kChunk + tid * 16) = q;
+                    *reinterpret_cast<uint4 *>(sX + (NF / 8 + c) * kChunk + tid * 16) = q;
                     if (xt) {
-                        __stcs(reinterpret_cast<uint4 *>(xt + (4 + c) * kChunk + tid * 16), q);
+                        __stcs(reinterpret_cast<uint4 *>(xt + (NF / 8 + c) * kChunk + tid * 16), q);
                         __stcs(reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16), *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16));
                     }
+                }
+                if (xt) {
+#pragma unroll
+                    for (int c = 4; c < NF / 8; ++c)
+                        __stcs(reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16), *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16));
                 }
             }
             tc::fence_async_smem();
             __syncthreads();
-            tc::mma_to_rows<64, 0, 0, XW / 16>(acc, kS, 0, tc::kmajor(x_addr, kTile), tc::kmajor(r1_addr, XW), false);   // Y1 = X . R1^T
+            tc::mma_to_rows<64, 0, 0, XC / 16>(acc, kS, 0, tc::kmajor(x_addr, kTile), tc::kmajor(r1_addr, XW), false);   // Y1 = X . R1^T
             __syncthreads();
             uint8_t *y1t = Y1t ? Y1t + tile * kTileBytes : nullptr;
 #pragma unroll 1
@@ -296,10 +320,10 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
                 }
                 if (y2t) __stcs(reinterpret_cast<uint4 *>(y2t + c * kChunk + tid * 16), tc::pack8_f16(y));
             }
-        } else if (Xt) {                                       // the h half of the saved X tile (what k_color_sdf_bwd fetches)
-            uint8_t *xt = Xt + tile * kTileBytes;
+        } else if (Xt) {                                       // the h part of the saved X tile (what k_color_sdf_bwd fetches)
+            uint8_t *xt = Xt + tile * x_tile_bytes<NF>();
 #pragma unroll
-            for (int c = 0; c < 4; ++c)
+            for (int c = 0; c < NF / 8; ++c)
                 __stcs(reinterpret_cast<uint4 *>(xt + c * kChunk + tid * 16), *reinterpret_cast<const uint4 *>(sX + c * kChunk + tid * 16));
         }
         if (valid) {
@@ -320,25 +344,26 @@ k_color_fwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev n
 }
 
 // ===================================================================================================================== radiance backward
-// T = [dZ2 | dZ1 | y2] (128 points x 192, three 16 KB blocks).  MMAs per tile:
+// T = [dZ2 | dZ1 | y2] (128 points x 192, three 16 KB blocks).  MMAs per tile (NF = 32; at NF = 48 dh is N48 and XB N96):
 //   dY1 = dZ2 . R2                 (M128 N64 K64)    A = T block 0 (K-major),           B = R2^T tile
-//   dh  = dZ1 . R1[:, h columns]   (M128 N32 K64)    A = T block 1,                     B = R1h^T tile
+//   dh  = dZ1 . R1[:, h columns]   (M128 NF  K64)    A = T block 1,                     B = R1h^T tile
 //   XA += dZ2^T . [Y1 | 1 | 0]               (M64 N80 K128, MN-major) = [dR2 | drb2]
-//   XB += dZ1^T . [X | 1 gy3 | 0]            (M64 N80 K128, MN-major) = [dR1 | drb1]
+//   XB += dZ1^T . [X | 1 gy3 | 0]            (M64 N(NF+48) K128, MN-major) = [dR1 | drb1]
 //   X3 += y2^T  . [1 gy3 0..]                (M64 N8  K128, MN-major): cols 1..3 = dR3^T
 // XA, XB and X3 are register fragments carried over all tiles of the persistent CTA; the dY1 ReLU mask runs on the dY1 fragments, and
-// dh goes from its fragments straight to global memory, so the kernel stages no fp32 rows (~104 KB of shared memory: 2 CTAs / SM).
-// kAppear adds the appearance-code gradient of every point (the codes are the radiance input's columns 54..54 + n_appear):
+// dh goes from its fragments straight to global memory, so the kernel stages no fp32 rows (~104 KB of shared memory, 112 KB at NF = 48:
+// 2 CTAs / SM).
+// kAppear adds the appearance-code gradient of every point (the codes are the internal radiance input's columns NF+22..NF+22+n_appear):
 //   da  = dZ1 . R1[:, h_appear]    (M128 N8 K64)     A = T block 1,                     B = R1a^T tile (1 KB more shared memory)
 // written from its fragments like dh, as rows of 8 floats (zero beyond n_appear); k_ray_row_sum adds them up per ray.
 // kRays adds the gradient of every point's position and SH view embedding (the reference's radiance input columns 0..18):
 //   dxv = dZ1 . R1[:, 0:19]       (M128 N32 K64)     A = T block 1,                     B = R1x^T tile (4 KB more shared memory)
 // written as rows of 24 floats [dL/dx (3) | dL/dSH (16) | 0]; k_color_sdf_bwd<true> adds dL/dx to the table's input gradient and maps
 // dL/dSH to the view direction.
-// The three saved activation tiles of a point tile (X, Y1, Y2: 3 x 16 KB, each contiguous in global memory and in shared memory) are
+// The three saved activation tiles of a point tile (X, Y1, Y2: 3 x 16 KB (X: 20 KB at NF = 48), each contiguous in global memory and in shared memory) are
 // fetched by the bulk async copy engine (cp.async.bulk -> mbarrier), issued by one thread; the fetch of the NEXT tile starts as soon
 // as the last MMA that reads the current tiles has completed, so it overlaps the dh store and the next prologue.
-template <bool kAppear, bool kRays>
+template <bool kAppear, bool kRays, int NF>
 __global__ void __launch_bounds__(kTile, kColorBwdCtasPerSM)
 k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uint8_t *__restrict__ Y1t, const uint8_t *__restrict__ Y2t,
                 const float *__restrict__ rgb, const float *__restrict__ g_rgb, int64_t n, float *__restrict__ dh_out,
@@ -347,13 +372,14 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
                 float *__restrict__ xv_out) {
     n = eff_n(n, n_dev);
     constexpr int NE = 80;                                     // 64 columns + the [1, gy3, 0..] chunk + a zero chunk (N % 16 == 0)
+    constexpr int XC = x_cols<NF>(), NEX = XC + 16;            // the X tile, and the same with its two extra chunks (80, or 96)
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
     uint8_t *sT = tiles;                                       // 48 KB
     uint8_t *sY1 = sT + 3 * kTileBytes;                        // 20 KB [Y1 | 1 | 0]
-    uint8_t *sXe = sY1 + kTile * NE * 2;                       // 20 KB [X | 1 gy3 | 0]
-    uint8_t *sR2T = sXe + kTile * NE * 2;                      //  8 KB (N = in i, K = out j) = R2[j][i]
-    uint8_t *sR1h = sR2T + XW * XW * 2;                        //  4 KB (N = h column k, K = out j) = R1[j][22 + k], zero for k >= 2L
+    uint8_t *sXe = sY1 + kTile * NE * 2;                       // 20 KB (NF = 48: 24 KB) [X | 1 gy3 | 0]
+    uint8_t *sR2T = sXe + kTile * NEX * 2;                     //  8 KB (N = in i, K = out j) = R2[j][i]
+    uint8_t *sR1h = sR2T + XW * XW * 2;                        //  4 KB (6 KB) (N = h column k, K = out j) = R1[j][22 + k], zero for k >= 2L
     uint8_t *sR1a = sR1h + NF * XW * 2;                        //  1 KB (kAppear; N = code column k, K = out j) = R1[j][22 + 2L + k], zero for k >= n_appear
     uint8_t *sR1x = sR1a + 8 * XW * 2;                         //  4 KB (kRays; N = input column k, K = out j) = R1[j][k], zero for k >= 19
     __shared__ float sR3[3][XW];
@@ -379,10 +405,10 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         }
     }
     if constexpr (kRays) {
-        for (int e = tid; e < NF * XW; e += kTile) {
-            const int k = e % NF, j = e / NF;
+        for (int e = tid; e < kXVCols * XW; e += kTile) {
+            const int k = e % kXVCols, j = e / kXVCols;
             const __half v = (j < net.rw && k < 19) ? net.R1[j * net.rin + k] : __float2half_rn(0.f);
-            *reinterpret_cast<__half *>(sR1x + (j / 8) * (NF * 16) + k * 16 + (j % 8) * 2) = v;
+            *reinterpret_cast<__half *>(sR1x + (j / 8) * (kXVCols * 16) + k * 16 + (j % 8) * 2) = v;
         }
     }
     if (tid < XW) {
@@ -391,10 +417,12 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     }
     *reinterpret_cast<uint4 *>(sY1 + 8 * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);       // [1, 0, ...]
     *reinterpret_cast<uint4 *>(sY1 + 9 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
-    *reinterpret_cast<uint4 *>(sXe + 9 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
-    float xa[NE / 2], xb[NE / 2], x3[4];
+    *reinterpret_cast<uint4 *>(sXe + (XC / 8 + 1) * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
+    float xa[NE / 2], xb[NEX / 2], x3[4];
 #pragma unroll
-    for (int k = 0; k < NE / 2; ++k) xa[k] = xb[k] = 0.f;
+    for (int k = 0; k < NE / 2; ++k) xa[k] = 0.f;
+#pragma unroll
+    for (int k = 0; k < NEX / 2; ++k) xb[k] = 0.f;
 #pragma unroll
     for (int k = 0; k < 4; ++k) x3[k] = 0.f;
     if (tid == 0) {
@@ -410,11 +438,11 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
     bool first_tile = true;
 
     const int64_t n_tiles = (n + kTile - 1) / kTile;
-    auto fetch = [&](int64_t tile) {                          // one thread: 48 KB of saved activations -> the three shared-memory tiles
-        tc::mbar_arrive_expect_tx(&mbar_ld, 3 * kTileBytes);
+    auto fetch = [&](int64_t tile) {                          // one thread: 48 KB (52 KB) of saved activations -> the three shared-memory tiles
+        tc::mbar_arrive_expect_tx(&mbar_ld, 2 * kTileBytes + x_tile_bytes<NF>());
         tc::tma_load_bulk(sT + 2 * kTileBytes, Y2t + tile * kTileBytes, kTileBytes, &mbar_ld);
         tc::tma_load_bulk(sY1, Y1t + tile * kTileBytes, kTileBytes, &mbar_ld);
-        tc::tma_load_bulk(sXe, Xt + tile * kTileBytes, kTileBytes, &mbar_ld);
+        tc::tma_load_bulk(sXe, Xt + tile * x_tile_bytes<NF>(), x_tile_bytes<NF>(), &mbar_ld);
     };
     if (tid == 0 && (int64_t)blockIdx.x < n_tiles) fetch(blockIdx.x);
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -432,7 +460,7 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         }
         {
             float e8[8] = {1.f, gy[0], gy[1], gy[2], 0.f, 0.f, 0.f, 0.f};
-            *reinterpret_cast<uint4 *>(sXe + 8 * kChunk + tid * 16) = tc::pack8_f16(e8);
+            *reinterpret_cast<uint4 *>(sXe + (XC / 8) * kChunk + tid * 16) = tc::pack8_f16(e8);
         }
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
@@ -470,17 +498,17 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
         tc::fence_async_smem();
         __syncthreads();
         float dh[2][NF / 2];
-        tc::mma_m128<32, 0, 0, XW / 16>(dh, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(r1h_addr, NF), false);   // dh = dZ1 . R1[:, h]
+        tc::mma_m128<NF, 0, 0, XW / 16>(dh, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(r1h_addr, NF), false);   // dh = dZ1 . R1[:, h]
         float da[2][4];
         if constexpr (kAppear)
             tc::mma_m128<8, 0, 0, XW / 16>(da, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(tc::smem_u32(sR1a), 8), false);   // da = dZ1 . R1[:, h_appear]
-        float dxv[2][NF / 2];
+        float dxv[2][kXVCols / 2];
         if constexpr (kRays)
-            tc::mma_m128<32, 0, 0, XW / 16>(dxv, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(tc::smem_u32(sR1x), NF), false);   // dxv = dZ1 . R1[:, 0:19]
+            tc::mma_m128<kXVCols, 0, 0, XW / 16>(dxv, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(tc::smem_u32(sR1x), kXVCols), false);   // dxv = dZ1 . R1[:, 0:19]
         // weight gradients: contract over the 128 points
         tc::mma_m64<NE, 1, 1, kTile / 16>(xa, tc::mnmajor(t_addr, kTile), tc::mnmajor(y1_addr, kTile), true);
-        tc::mma_m64<NE, 1, 1, kTile / 16>(xb, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(xe_addr, kTile), true);
-        tc::mma_m64<8, 1, 1, kTile / 16>(x3, tc::mnmajor(t_addr + 2 * kTileBytes, kTile), tc::mnmajor(xe_addr + 8 * kChunk, kTile), true);
+        tc::mma_m64<NEX, 1, 1, kTile / 16>(xb, tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(xe_addr, kTile), true);
+        tc::mma_m64<8, 1, 1, kTile / 16>(x3, tc::mnmajor(t_addr + 2 * kTileBytes, kTile), tc::mnmajor(xe_addr + (XC / 8) * kChunk, kTile), true);
         first_tile = false;
         __syncthreads();
         if (tid == 0 && tile + gridDim.x < n_tiles) {
@@ -515,19 +543,23 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
             const int row = tc::frag_row(r);
             if (row >= net.rw) continue;
 #pragma unroll
-            for (int c = 0; c < NE / 8; ++c)
+            for (int c = 0; c < NEX / 8; ++c)
 #pragma unroll
                 for (int j = 0; j < 2; ++j) {
                     const int col = tc::frag_col(c) + j;
-                    const float a = xa[4 * c + 2 * r + j], b = xb[4 * c + 2 * r + j];
-                    if (col < XW) {
-                        if (col < net.rw) atomicAdd(dR2 + row * net.rw + col, a);
-                        const int rc = ref_col(col, net.n_appear, net.dec.nh);
-                        if (rc >= 0) atomicAdd(dR1 + row * net.rin + rc, b);
-                    } else if (col == XW) {
-                        atomicAdd(drb2 + row, a);
-                        atomicAdd(drb1 + row, b);
+                    const float b = xb[4 * c + 2 * r + j];
+                    if (c < NE / 8) {
+                        const float a = xa[(4 * c + 2 * r + j) % (NE / 2)];   // (the modulo only keeps the index in range for c >= NE / 8)
+                        if (col < XW) {
+                            if (col < net.rw) atomicAdd(dR2 + row * net.rw + col, a);
+                        } else if (col == XW)
+                            atomicAdd(drb2 + row, a);
                     }
+                    if (col < XC) {
+                        const int rc = ref_col(col, net.n_appear, net.dec.nh, NF);
+                        if (rc >= 0) atomicAdd(dR1 + row * net.rin + rc, b);
+                    } else if (col == XC)
+                        atomicAdd(drb1 + row, b);
                 }
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
@@ -542,17 +574,17 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
 // ===================================================================================================================== sdf / nablas backward
 // T = [dz | u | v] (128 x 192).  gin = dL/dnablas * fac * 0.5 (cotangent of nablas01), dsdf optional, dh_r = dL/dh from the radiance net.
 //   dg_f = sum_d gin_d J[f][d]  (k_lotd_ddLdy)                                   -> fp16 tile Ge = [dG | 1 0..]
-//   du = dG . W1^T (M128 N64 K32);  g = U . W1 (M128 N32 K64)
+//   du = dG . W1^T (M128 N64 K=NF);  g = U . W1 (M128 N=NF K64)
 //   dz_j = fp16(du_j) w2_j beta s_j (1 - s_j) + dsdf w2_j s_j ;  v_j = fp16(du_j) s_j + dsdf a16_j
-//   dhz = dZ . W1 (M128 N32 K64)
-//   W  += dz^T . [H | 1 | 0]     (M64 N48 K128, MN-major) = [dW1 (z part) | db1]
-//   W[:, 0..31] += u^T . dG      (M64 N32 K128, MN-major): dW1 (second-order part); N = 32 keeps sum(u) out of db1
+//   dhz = dZ . W1 (M128 N=NF K64)
+//   W  += dz^T . [H | 1 | 0]     (M64 N=NF+16 K128, MN-major) = [dW1 (z part) | db1]
+//   W[:, 0..NF-1] += u^T . dG    (M64 N=NF K128, MN-major): dW1 (second-order part); N = NF keeps sum(u) out of db1
 //   V  += v^T . [1 0..]          (M64 N8  K128, MN-major): col 0 = dW2
 //   scatter per level / corner:  g_f * wsum_c(gin) + (dhz_f + dh_r_f) * w_c
 // W and V are register fragments carried over all tiles of the persistent CTA, dz and v are computed on the du fragments, and only g and
 // dhz -- the scatter needs a point's whole row of them -- are staged as fp32 rows, in T once its last MMA has completed (~97 KB of
-// shared memory: 2 CTAs / SM).
-// The saved Z tile (16 KB) and the H half of the saved X tile (8 KB) are fetched by the bulk async copy engine into shared memory, and
+// shared memory, 109 KB at NF = 48: 2 CTAs / SM; at NF = 48 the rows also take the head of Ge, which follows T and is free then).
+// The saved Z tile (16 KB) and the H part of the saved X tile (8 KB, 12 KB at NF = 48) are fetched by the bulk async copy engine into shared memory, and
 // the NEXT tile's fetch is issued right after the last MMA of the current tile -- it runs behind the whole scatter phase.  (Reading Z
 // straight from global memory in the two epilogue loops costs 16 dependent round trips per tile at 8 warps per SM.)
 // kXGrad adds the gradient of every point's ray (the depths t are constants): the scatter loop loads the corners of each level it scatters
@@ -560,7 +592,7 @@ k_color_rad_bwd(const ColorNetDev net, const uint8_t *__restrict__ Xt, const uin
 // not reach x), which is mapped to network space and added to dL/dx of the radiance input (xv rows of k_color_rad_bwd<., true>, NULL
 // without rgb); dL/dSH of those rows is mapped to the view direction through the SH Jacobian.  Each point writes a row of 12 floats
 // [g_x | t g_x | g_v | 0 0 0], which k_ray_row_sum adds up per ray.
-template <bool kXGrad>
+template <bool kXGrad, int NF>
 __global__ void __launch_bounds__(kTile, kColorBwdCtasPerSM)
 k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetDev net, const PointSrc ps, const uint8_t *__restrict__ Zt,
                 const uint8_t *__restrict__ Xt, const float *__restrict__ g_nab, const float *__restrict__ g_sdf, const float *__restrict__ dh_r,
@@ -569,30 +601,32 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
                 const float *__restrict__ view_dirs, float *__restrict__ gx_out, const int32_t *__restrict__ ml_dev) {
     n = eff_n(n, n_dev);
     const uint32_t La = active_levels(max_level, ml_dev, m.n_pseudo);
-    constexpr int NX = 48;                                     // 32 + the [1 0..] chunk + a zero chunk (N % 16 == 0)
+    constexpr int NX = NF + 16;                                // NF + the [1 0..] chunk + a zero chunk (N % 16 == 0)
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
     uint8_t *sT = tiles;                                       // 48 KB [dz | u | v]
-    uint8_t *sHe = sT + 3 * kTileBytes;                        // 12 KB [H | 1 | 0]
-    uint8_t *sGe = sHe + kTile * NX * 2;                       // 12 KB [dG | 1 | 0]
-    uint8_t *sW1 = sGe + kTile * NX * 2;                       //  4 KB
-    uint8_t *sW1T = sW1 + HW * NF * 2;                         //  4 KB
+    uint8_t *sGe = sT + 3 * kTileBytes;                        // 12 KB (NF = 48: 16 KB) [dG | 1 | 0]
+    uint8_t *sHe = sGe + kTile * NX * 2;                       // 12 KB (16 KB) [H | 1 | 0]
+    uint8_t *sW1 = sHe + kTile * NX * 2;                       //  4 KB (6 KB)
+    uint8_t *sW1T = sW1 + HW * NF * 2;                         //  4 KB (6 KB)
     uint8_t *sZ = sW1T + NF * HW * 2;                          // 16 KB saved pre-activations
-    constexpr int kS = tc::acc_stride(2 * NF);                 // staged rows [g | dhz] for the scatter: 34 KB, aliasing T
+    constexpr int kS = tc::acc_stride(2 * NF);                 // staged rows [g | dhz] for the scatter: 34 KB (50 KB), aliasing T (and Ge)
     float *stage = reinterpret_cast<float *>(sT);
-    static_assert(kTile * kS * 4 <= 3 * kTileBytes, "the staged rows must fit in T");
+    // the rows may run into Ge's feature chunks (free after the MMAs), never into its constant [1 0..] and zero chunks at NF / 8 and
+    // NF / 8 + 1, which are written once before the tile loop
+    static_assert(kTile * kS * 4 <= 3 * kTileBytes + (NF / 8) * kChunk, "the staged rows must end before Ge's constant chunks");
     __shared__ float sW2[HW], sdsdf[kTile];
     __shared__ float sdb2;
     __shared__ __align__(8) uint64_t mbar_ld;
 
     const int tid = threadIdx.x, lane = tid & 31;
-    stage_W1(net.dec, sW1, tid);
-    stage_W1T(net.dec, sW1T, tid);
+    stage_W1<NF>(net.dec, sW1, tid);
+    stage_W1T<NF>(net.dec, sW1T, tid);
     stage_decoder_vectors(net.dec, nullptr, sW2, nullptr, tid);
-    *reinterpret_cast<uint4 *>(sHe + 4 * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);
-    *reinterpret_cast<uint4 *>(sGe + 4 * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);
-    *reinterpret_cast<uint4 *>(sHe + 5 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
-    *reinterpret_cast<uint4 *>(sGe + 5 * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(sHe + (NF / 8) * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(sGe + (NF / 8) * kChunk + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(sHe + (NF / 8 + 1) * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(sGe + (NF / 8 + 1) * kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
     float wacc[NX / 2], vacc[4];
 #pragma unroll
     for (int k = 0; k < NX / 2; ++k) wacc[k] = 0.f;
@@ -613,9 +647,9 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
 
     const int64_t n_tiles = (n + kTile - 1) / kTile;
     auto fetch = [&](int64_t tile) {                          // one thread: Z tile + the H chunks of the X tile -> shared memory
-        tc::mbar_arrive_expect_tx(&mbar_ld, kTileBytes + 4 * kChunk);
+        tc::mbar_arrive_expect_tx(&mbar_ld, kTileBytes + (NF / 8) * kChunk);
         tc::tma_load_bulk(sZ, Zt + tile * kTileBytes, kTileBytes, &mbar_ld);
-        tc::tma_load_bulk(sHe, Xt + tile * kTileBytes, 4 * kChunk, &mbar_ld);
+        tc::tma_load_bulk(sHe, Xt + tile * x_tile_bytes<NF>(), (NF / 8) * kChunk, &mbar_ld);
     };
     if (tid == 0 && (int64_t)blockIdx.x < n_tiles) fetch(blockIdx.x);
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -646,9 +680,9 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
             }
             *reinterpret_cast<uint4 *>(sT + kTileBytes + c * kChunk + tid * 16) = tc::pack8_f16(uu);
         }
-        // dg = J gin (fp16), level by level, into my row of Ge; zero for the levels >= La (columns 2La..31)
+        // dg = J gin (fp16), level by level, into my row of Ge; zero for the levels >= La (columns 2La..NF-1)
 #pragma unroll 4
-        for (uint32_t p = 0; p < 16; ++p) {               // four levels per trip: 32 independent corner loads in flight (2 CTAs / SM: registers are free)
+        for (uint32_t p = 0; p < NF / 2; ++p) {               // four levels per trip: 32 independent corner loads in flight (2 CTAs / SM: registers are free)
             uint32_t packed = 0;
             if (p < La) {
                 float J0[3], J1[3];
@@ -667,7 +701,7 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         {
             float du[2][HW / 2];
             tc::mma_m128<64, 0, 0, NF / 16>(du, tc::kmajor(ge_addr, kTile), tc::kmajor(w1_addr, HW), false);                  // du = dG . W1^T
-            tc::mma_m128<32, 0, 0, HW / 16>(gfr, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(w1t_addr, NF), false);   // g = U . W1
+            tc::mma_m128<NF, 0, 0, HW / 16>(gfr, tc::kmajor(t_addr + kTileBytes, kTile), tc::kmajor(w1t_addr, NF), false);   // g = U . W1
             // dz -> T block 0, v -> T block 2, on the du fragments (no MMA in flight reads those blocks)
 #pragma unroll
             for (int h = 0; h < 2; ++h)
@@ -699,16 +733,17 @@ k_color_sdf_bwd(const PLMeta m, const __half *__restrict__ grid, const ColorNetD
         tc::fence_async_smem();
         __syncthreads();
         float dhz[2][NF / 2];
-        tc::mma_m128<32, 0, 0, HW / 16>(dhz, tc::kmajor(t_addr, kTile), tc::kmajor(w1t_addr, NF), false);                        // dhz = dZ . W1
+        tc::mma_m128<NF, 0, 0, HW / 16>(dhz, tc::kmajor(t_addr, kTile), tc::kmajor(w1t_addr, NF), false);                        // dhz = dZ . W1
         tc::mma_m64<NX, 1, 1, kTile / 16>(wacc, tc::mnmajor(t_addr, kTile), tc::mnmajor(he_addr, kTile), true);
         tc::mma_m64<NF, 1, 1, kTile / 16>(*reinterpret_cast<float(*)[NF / 2]>(wacc), tc::mnmajor(t_addr + kTileBytes, kTile), tc::mnmajor(ge_addr, kTile), true);
-        tc::mma_m64<8, 1, 1, kTile / 16>(vacc, tc::mnmajor(t_addr + 2 * kTileBytes, kTile), tc::mnmajor(ge_addr + 4 * kChunk, kTile), true);
+        tc::mma_m64<8, 1, 1, kTile / 16>(vacc, tc::mnmajor(t_addr + 2 * kTileBytes, kTile), tc::mnmajor(ge_addr + (NF / 8) * kChunk, kTile), true);
         first_tile = false;
         const float dsum = warp_sum(dsdf);
         if (lane == 0 && dsum != 0.f) atomicAdd(&sdb2, dsum);
         __syncthreads();
         if (tid == 0 && tile + gridDim.x < n_tiles) {
             // sZ was last read by the threads before the __syncthreads that precedes the MMAs above, sHe by those MMAs, which have completed
+            // (the staged rows below overlap Ge, never He)
             tc::fence_async_smem();
             fetch(tile + gridDim.x);
         }
@@ -834,6 +869,36 @@ static int64_t n_tiles(int64_t n) { return (n + kTile - 1) / kTile; }
 
 extern "C" int64_t nsb_color_tile_bytes(int64_t n) { return n_tiles(n) * (int64_t)kTileBytes; }
 
+extern "C" int64_t nsb_color_act_bytes(int64_t n, int32_t n_levels) {
+    return n_tiles(n) * (int64_t)(n_levels <= kMaxNarrowLevels ? x_tile_bytes<32>() : x_tile_bytes<48>());
+}
+
+// dynamic shared memory of the colour kernels at tile width NF (the 1 KB is the alignment slack of the tiles)
+template <int NF>       // k_color_fwd<false>: the h part of X, U, W1, W1^T, the staged rows (67 KB; 75 KB at NF = 48)
+constexpr int color_geo_smem() { return (NF / 8) * kChunk + kTileBytes + 2 * HW * NF * 2 + kTile * tc::acc_stride(64) * 4 + 1024; }
+template <int NF>       // k_color_fwd<true>: X, U, W1, W1^T, R1, R2, the staged rows (91 KB; 101 KB at NF = 48)
+constexpr int color_fwd_smem() {
+    return x_tile_bytes<NF>() + kTileBytes + 2 * HW * NF * 2 + XW * x_cols<NF>() * 2 + XW * XW * 2 + kTile * tc::acc_stride(64) * 4 + 1024;
+}
+template <int NF, bool kAppear, bool kRays>   // k_color_rad_bwd: T, [Y1 | 1 | 0], [X | 1 gy3 | 0], R2^T, R1h, R1a, R1x (101-106 KB; 107-112 KB)
+constexpr int color_rad_bwd_smem() {
+    return 3 * kTileBytes + kTile * 80 * 2 + kTile * (x_cols<NF>() + 16) * 2 + XW * XW * 2 + NF * XW * 2 + (kAppear || kRays ? 8 * XW * 2 : 0) +
+           (kRays ? kXVCols * XW * 2 : 0) + 1024;
+}
+template <int NF>       // k_color_sdf_bwd: T, Ge, He, W1, W1^T, Z (97 KB; 109 KB at NF = 48)
+constexpr int color_sdf_bwd_smem() { return 3 * kTileBytes + 2 * kTile * (NF + 16) * 2 + 2 * HW * NF * 2 + kTileBytes + 1024; }
+static_assert(color_geo_smem<32>() == 4 * kChunk + kTileBytes + 2 * HW * 32 * 2 + kTile * tc::acc_stride(64) * 4 + 1024, "32-column budget");
+static_assert(color_fwd_smem<32>() == 2 * kTileBytes + 2 * HW * 32 * 2 + 2 * XW * XW * 2 + kTile * tc::acc_stride(64) * 4 + 1024, "32-column budget");
+static_assert(color_rad_bwd_smem<32, true, true>() == 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + 32 * XW * 2 + 8 * XW * 2 + 32 * XW * 2 + 1024,
+              "32-column budget");
+static_assert(color_sdf_bwd_smem<32>() == 3 * kTileBytes + 2 * kTile * 48 * 2 + 2 * HW * 32 * 2 + kTileBytes + 1024, "32-column budget");
+
+// calls f(std::integral_constant<int, NF>{}) with the tile width of an L-level table
+template <typename F>
+static int with_feature_cols(uint32_t L, F &&f) {
+    return feature_cols(L) == 32 ? f(std::integral_constant<int, 32>{}) : f(std::integral_constant<int, 48>{});
+}
+
 extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params_half, const nsb_color_net *net, const float *x, const float *rays_o,
                                    const float *rays_d, const int64_t *ridx, const float *t, const float *view_dirs, const float *h_appear,
                                    int64_t n, int32_t max_level, float *sdf, float *nablas, float *rgb, float *x_out, void *act_z, void *act_x,
@@ -853,29 +918,32 @@ extern "C" int nsb_fused_color_fwd(const nsb_lotd_meta *meta, const void *params
     if (int rc = make_net(net, meta, &m, &d, "nsb_fused_color_fwd", rad)) return rc;
     const PointSrc ps{x, rays_o, rays_d, t, ridx};
     const int ml = max_level < 0 ? -1 : max_level;
-    if (!rad) {                                                // geometry only: sdf, nablas, x, Z and the h half of X
-        constexpr int kSmemG = 4 * kChunk + kTileBytes + 2 * HW * NF * 2 + kTile * tc::acc_stride(64) * 4 + 1024;   // 67 KB
-        // carve-out for kColorGeoCtasPerSM CTAs (dynamic + static shared memory + the 1 KB the hardware reserves per CTA), in % of 228 KB;
-        // the driver rounds it up to the next configuration it supports
-        constexpr int kCarveout = (100 * kColorGeoCtasPerSM * (kSmemG + 2 * 1024) + 228 * 1024 - 1) / (228 * 1024);
-        if (smem_opt_in_needed(reinterpret_cast<const void *>(k_color_fwd<false>), current_device(), kSmemG)) {
-            cudaFuncSetAttribute(k_color_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemG);
-            cudaFuncSetAttribute(k_color_fwd<false>, cudaFuncAttributePreferredSharedMemoryCarveout, kCarveout);
-        }
-        if (int rc = require_ctas_per_sm(k_color_fwd<false>, kTile, kSmemG, kColorGeoCtasPerSM, "nsb_fused_color_fwd(geometry)")) return rc;
-        k_color_fwd<false><<<persistent_grid(n_tiles(n), kColorGeoCtasPerSM), kTile, kSmemG, (cudaStream_t)stream>>>(
-            m, (const __half *)params_half, d, ps, nullptr, nullptr, n, ml, sdf, nablas, nullptr, x_out, (uint8_t *)act_z, (uint8_t *)act_x,
-            nullptr, nullptr, occ_collect_of(collect), dn.a, ml_dev);
-        return check_launch("nsb_fused_color_fwd");
+    if (!rad) {                                                // geometry only: sdf, nablas, x, Z and the h part of X
+        return with_feature_cols(m.n_pseudo, [&](auto nf) -> int {
+            constexpr int NF = decltype(nf)::value, kSmemG = color_geo_smem<NF>();
+            // carve-out for kColorGeoCtasPerSM CTAs (dynamic + static shared memory + the 1 KB the hardware reserves per CTA), in % of 228 KB;
+            // the driver rounds it up to the next configuration it supports
+            constexpr int kCarveout = (100 * kColorGeoCtasPerSM * (kSmemG + 2 * 1024) + 228 * 1024 - 1) / (228 * 1024);
+            if (smem_opt_in_needed(reinterpret_cast<const void *>(k_color_fwd<false, NF>), current_device(), kSmemG)) {
+                cudaFuncSetAttribute(k_color_fwd<false, NF>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemG);
+                cudaFuncSetAttribute(k_color_fwd<false, NF>, cudaFuncAttributePreferredSharedMemoryCarveout, kCarveout);
+            }
+            if (int rc = require_ctas_per_sm(k_color_fwd<false, NF>, kTile, kSmemG, kColorGeoCtasPerSM, "nsb_fused_color_fwd(geometry)")) return rc;
+            k_color_fwd<false, NF><<<persistent_grid(n_tiles(n), kColorGeoCtasPerSM), kTile, kSmemG, (cudaStream_t)stream>>>(
+                m, (const __half *)params_half, d, ps, nullptr, nullptr, n, ml, sdf, nablas, nullptr, x_out, (uint8_t *)act_z, (uint8_t *)act_x,
+                nullptr, nullptr, occ_collect_of(collect), dn.a, ml_dev);
+            return check_launch("nsb_fused_color_fwd");
+        });
     }
     NSB_REQUIRE(d.n_appear == 0 || h_appear, "nsb_fused_color_fwd: h_appear is NULL but the net has %d appearance channels", d.n_appear);
-    constexpr int kSmem = 2 * kTileBytes + 2 * HW * NF * 2 + 2 * XW * XW * 2 + kTile * tc::acc_stride(64) * 4 + 1024;   // 91 KB: 2 CTAs / SM
-    opt_in_smem(k_color_fwd<true>, kSmem);
-    k_color_fwd<true><<<persistent_grid(n_tiles(n), 2), kTile, kSmem, (cudaStream_t)stream>>>(m, (const __half *)params_half, d, ps, view_dirs, h_appear, n,
-                                                                                             ml, sdf, nablas, rgb, x_out, (uint8_t *)act_z,
-                                                                                             (uint8_t *)act_x, (uint8_t *)act_y1, (uint8_t *)act_y2,
-                                                                                             occ_collect_of(collect), dn.a, ml_dev);
-    return check_launch("nsb_fused_color_fwd");
+    return with_feature_cols(m.n_pseudo, [&](auto nf) -> int {
+        constexpr int NF = decltype(nf)::value, kSmem = color_fwd_smem<NF>();   // 91 KB (101 KB): 2 CTAs / SM
+        opt_in_smem(k_color_fwd<true, NF>, kSmem);
+        k_color_fwd<true, NF><<<persistent_grid(n_tiles(n), 2), kTile, kSmem, (cudaStream_t)stream>>>(
+            m, (const __half *)params_half, d, ps, view_dirs, h_appear, n, ml, sdf, nablas, rgb, x_out, (uint8_t *)act_z, (uint8_t *)act_x,
+            (uint8_t *)act_y1, (uint8_t *)act_y2, occ_collect_of(collect), dn.a, ml_dev);
+        return check_launch("nsb_fused_color_fwd");
+    });
 }
 
 // the two backward kernels (k_color_rad_bwd only with g_rgb), then with kAppear the per-ray sum of the code gradients and with kRays the
@@ -910,14 +978,16 @@ static int color_bwd(const char *who, const nsb_lotd_meta *meta, const void *par
     const float *dh = nullptr;
     float *xv_rows = (kRays && g_rgb) ? ray_scratch + n * 12 : nullptr;   // [n, 24] after the [n, 12] ray rows
     if (g_rgb) {
-        constexpr int kSmemR = 3 * kTileBytes + 2 * kTile * 80 * 2 + XW * XW * 2 + NF * XW * 2 + (kAppear || kRays ? 8 * XW * 2 : 0) +
-                               (kRays ? NF * XW * 2 : 0) + 1024;   // 101 (102 with codes, 106 with rays) KB
-        opt_in_smem(k_color_rad_bwd<kAppear, kRays>, kSmemR);
-        if (int rc = require_ctas_per_sm(k_color_rad_bwd<kAppear, kRays>, kTile, kSmemR, kColorBwdCtasPerSM, "nsb_fused_color_bwd(radiance)")) return rc;
-        k_color_rad_bwd<kAppear, kRays><<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemR, s>>>(
-            d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n, dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3, d_rb3,
-            dn.a, ha_scratch, xv_rows);
-        if (int rc = check_launch("nsb_fused_color_bwd(radiance)")) return rc;
+        const int rc = with_feature_cols(m.n_pseudo, [&](auto nf) -> int {
+            constexpr int NF = decltype(nf)::value, kSmemR = color_rad_bwd_smem<NF, kAppear, kRays>();
+            opt_in_smem(k_color_rad_bwd<kAppear, kRays, NF>, kSmemR);
+            if (int rc = require_ctas_per_sm(k_color_rad_bwd<kAppear, kRays, NF>, kTile, kSmemR, kColorBwdCtasPerSM, "nsb_fused_color_bwd(radiance)")) return rc;
+            k_color_rad_bwd<kAppear, kRays, NF><<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemR, s>>>(
+                d, (const uint8_t *)act_x, (const uint8_t *)act_y1, (const uint8_t *)act_y2, rgb, g_rgb, n, dh_scratch, d_R1, d_rb1, d_R2, d_rb2, d_R3,
+                d_rb3, dn.a, ha_scratch, xv_rows);
+            return check_launch("nsb_fused_color_bwd(radiance)");
+        });
+        if (rc) return rc;
         dh = dh_scratch;
         if (kAppear) {
             k_ray_row_sum<8><<<row_sum_blocks(n), 256, 0, s>>>(ha_scratch, ridx, nullptr, n, d.n_appear, ray_map,
@@ -925,14 +995,17 @@ static int color_bwd(const char *who, const nsb_lotd_meta *meta, const void *par
             if (int rc = check_launch("nsb_fused_color_bwd(code sum)")) return rc;
         }
     }
-    constexpr int kSmemS = 3 * kTileBytes + 2 * kTile * 48 * 2 + 2 * HW * NF * 2 + kTileBytes + 1024;   // 97 KB
-    opt_in_smem(k_color_sdf_bwd<kRays>, kSmemS);
-    if (int rc = require_ctas_per_sm(k_color_sdf_bwd<kRays>, kTile, kSmemS, kColorBwdCtasPerSM, "nsb_fused_color_bwd(sdf)")) return rc;
     const PointSrc ps{x, rays_o, rays_d, t, ridx};
-    k_color_sdf_bwd<kRays><<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemS, s>>>(
-        m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x, g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level,
-        d_grid, d_W1, d_b1, d_W2, d_b2, dn.a, xv_rows, view_dirs, ray_scratch, ml_dev);
-    if (int rc = check_launch("nsb_fused_color_bwd(sdf)")) return rc;
+    const int rc = with_feature_cols(m.n_pseudo, [&](auto nf) -> int {
+        constexpr int NF = decltype(nf)::value, kSmemS = color_sdf_bwd_smem<NF>();
+        opt_in_smem(k_color_sdf_bwd<kRays, NF>, kSmemS);
+        if (int rc = require_ctas_per_sm(k_color_sdf_bwd<kRays, NF>, kTile, kSmemS, kColorBwdCtasPerSM, "nsb_fused_color_bwd(sdf)")) return rc;
+        k_color_sdf_bwd<kRays, NF><<<persistent_grid(n_tiles(n), kColorBwdCtasPerSM), kTile, kSmemS, s>>>(
+            m, (const __half *)params_half, d, ps, (const uint8_t *)act_z, (const uint8_t *)act_x, g_nablas, g_sdf, dh, n, max_level < 0 ? -1 : max_level,
+            d_grid, d_W1, d_b1, d_W2, d_b2, dn.a, xv_rows, view_dirs, ray_scratch, ml_dev);
+        return check_launch("nsb_fused_color_bwd(sdf)");
+    });
+    if (rc) return rc;
     if (kRays) {
         k_ray_row_sum<12><<<row_sum_blocks(n), 256, 0, s>>>(ray_scratch, ridx, nullptr, n, 9, ray_map, RowSumOut{{d_rays_o, d_rays_d, d_view_dirs}, 3},
                                                              dn.a);

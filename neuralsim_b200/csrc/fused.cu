@@ -135,9 +135,9 @@ static int launch_fused_sdf(const nsb_lotd_meta *meta, const void *params_half, 
     NSB_REQUIRE(meta && dec && sdf, "nsb_fused_sdf: NULL argument");
     if (n == 0) return 0;
     NSB_REQUIRE(params_half && dec->W1 && dec->b1 && dec->W2 && dec->b2, "nsb_fused_sdf: NULL weights");
-    NSB_REQUIRE(meta->n_dims_to_encode == 3 && meta->n_feat_per_pseudo_lvl == 2 && meta->n_pseudo_levels >= 1 && meta->n_pseudo_levels <= 16 &&
+    NSB_REQUIRE(meta->n_dims_to_encode == 3 && meta->n_feat_per_pseudo_lvl == 2 && meta->n_pseudo_levels >= 1 && meta->n_pseudo_levels <= 24 &&
                 meta->n_encoded_dims == 2 * meta->n_pseudo_levels,
-                "nsb_fused_sdf: built for 3-D LoTD with 1 to 16 levels of 2 features (got D=%u F=%u levels=%u NF=%u)", meta->n_dims_to_encode,
+                "nsb_fused_sdf: built for 3-D LoTD with 1 to 24 levels of 2 features (got D=%u F=%u levels=%u NF=%u)", meta->n_dims_to_encode,
                 meta->n_feat_per_pseudo_lvl, meta->n_pseudo_levels, meta->n_encoded_dims);
     NSB_REQUIRE(dec->width >= 1 && dec->width <= kMaxW, "nsb_fused_sdf: decoder width %d out of range (<= %d)", dec->width, kMaxW);
     if (!g_opt_sdf_simt.load() && h_out == nullptr)   // tensor-core kernel (csrc/fused_tc.cu)
@@ -179,8 +179,8 @@ extern "C" int nsb_fused_sdf_packs(const nsb_lotd_meta *meta, const void *params
     NSB_REQUIRE(meta && dec && (sdf || n_packs == 0), "nsb_fused_sdf_packs: NULL argument");
     if (n_packs == 0) return 0;
     NSB_REQUIRE(rays_o && rays_d && pack_infos && t && params_half && dec->W1 && dec->b1 && dec->W2 && dec->b2, "nsb_fused_sdf_packs: NULL argument");
-    NSB_REQUIRE(meta->n_dims_to_encode == 3 && meta->n_feat_per_pseudo_lvl == 2 && meta->n_pseudo_levels >= 1 && meta->n_pseudo_levels <= 16 &&
-                meta->n_encoded_dims == 2 * meta->n_pseudo_levels, "nsb_fused_sdf_packs: built for 3-D LoTD with 1 to 16 levels of 2 features (got %u levels)",
+    NSB_REQUIRE(meta->n_dims_to_encode == 3 && meta->n_feat_per_pseudo_lvl == 2 && meta->n_pseudo_levels >= 1 && meta->n_pseudo_levels <= 24 &&
+                meta->n_encoded_dims == 2 * meta->n_pseudo_levels, "nsb_fused_sdf_packs: built for 3-D LoTD with 1 to 24 levels of 2 features (got %u levels)",
                 meta->n_pseudo_levels);
     NSB_REQUIRE(dec->width >= 1 && dec->width <= kMaxW, "nsb_fused_sdf_packs: decoder width %d out of range (<= %d)", dec->width, kMaxW);
     return nsb_fused_sdf_tc_launch(meta, params_half, dec, nullptr, rays_o, rays_d, nullptr, t, 0, max_level, sdf, stream, 2, pack_infos, pack_ray, nullptr, n_packs, nullptr);
@@ -194,8 +194,8 @@ extern "C" int nsb_fused_sdf_collect(const nsb_lotd_meta *meta, const void *para
     NSB_REQUIRE(mode >= 0 && mode <= 2, "nsb_fused_sdf_collect: mode must be 0 (points), 1 (rays) or 2 (packs)");
     if ((mode == 2 && n_packs == 0) || (mode != 2 && n == 0)) return 0;
     NSB_REQUIRE(sdf && (mode == 0 ? x != nullptr : (rays_o && rays_d && t)) && (mode != 2 || pack_infos), "nsb_fused_sdf_collect: NULL argument");
-    NSB_REQUIRE(meta->n_dims_to_encode == 3 && meta->n_feat_per_pseudo_lvl == 2 && meta->n_pseudo_levels >= 1 && meta->n_pseudo_levels <= 16 &&
-                meta->n_encoded_dims == 2 * meta->n_pseudo_levels, "nsb_fused_sdf_collect: built for 3-D LoTD with 1 to 16 levels of 2 features (got %u levels)",
+    NSB_REQUIRE(meta->n_dims_to_encode == 3 && meta->n_feat_per_pseudo_lvl == 2 && meta->n_pseudo_levels >= 1 && meta->n_pseudo_levels <= 24 &&
+                meta->n_encoded_dims == 2 * meta->n_pseudo_levels, "nsb_fused_sdf_collect: built for 3-D LoTD with 1 to 24 levels of 2 features (got %u levels)",
                 meta->n_pseudo_levels);
     NSB_REQUIRE(dec->width >= 1 && dec->width <= kMaxW, "nsb_fused_sdf_collect: decoder width %d out of range (<= %d)", dec->width, kMaxW);
     NSB_REQUIRE(!collect || !collect->grid_pcl || (collect->res[0] > 0 && collect->res[1] > 0 && collect->res[2] > 0), "nsb_fused_sdf_collect: bad grid resolution");

@@ -2,9 +2,10 @@
 //
 // One CTA = 128 threads = one warpgroup = one tile of 128 points; thread r owns point r for the gather and the scatter (the ray-tiled
 // query, MODE 2 below, gives the gather and the MMA + epilogue to different warps of a larger CTA, with the same per-row arithmetic):
-//   gather   thread r walks the L (1..16) LoTD levels of its point (8 corner loads each); every level's two fp16 features go
-//            straight into its row of the A tile in shared memory (core-matrix layout of tc_util.cuh), columns 2L..31 are zero
-//   MMA      the warpgroup issues wgmma (M=64, N=64, K=16) x2 per 64-row half: Z[128 x 64] (fp32, registers) = H[128 x 32] . W1^T
+//   gather   thread r walks the L (1..24) LoTD levels of its point (8 corner loads each); every level's two fp16 features go
+//            straight into its row of the A tile in shared memory (core-matrix layout of tc_util.cuh), columns 2L..NF-1 are zero
+//   MMA      the warpgroup issues wgmma (M=64, N=64, K=16) x NF/16 per 64-row half: Z[128 x 64] (fp32, registers) = H[128 x NF] . W1^T
+//            (NF = 32 feature columns for tables of 1..16 levels, 48 for 17..24: feature_cols, fused_tc_common.cuh)
 //   epilogue bias + Softplus(beta) with the autocast rounding points on the accumulator fragments, the 64 -> 1 layer as a
 //            dot product per row (16 hidden units per lane, summed over the lane quad) -> sdf[r]
 // The loop over levels is rolled on purpose (instruction cache: a fully unrolled gather is several thousand instructions).
@@ -40,11 +41,13 @@ constexpr int kPackSets = 5, kPackSlots = 7, kPackCtasPerSM = 1;
 constexpr int kPackProducerRegs = 72, kPackConsumerRegs = 120;
 static_assert(kPackSets * kTile * kPackProducerRegs + kTile * kPackConsumerRegs <= kTile * (1 + kPackSets) * 80, "register split");
 constexpr int kPackThreads = kTile * (1 + kPackSets);
-constexpr int kPackSmem = kPackSlots * (kTile * NF * 2 + kTile * 12) + HW * NF * 2 + 2 * HW * 4 + kPackSlots * 20 + 16 + 128;
+// ~71 KB at NF = 32, ~98 KB at NF = 48: one CTA per SM either way
+template <int NF>
+constexpr int pack_smem() { return kPackSlots * (kTile * NF * 2 + kTile * 12) + HW * NF * 2 + 2 * HW * 4 + kPackSlots * 20 + 16 + 128; }
 
-// one slot of the ring: the A tile (8 KB) and, per row, the output index (-1: no sample) and the occupancy voxel of the sample
+// one slot of the ring: the A tile (8 KB, 12 KB at NF = 48) and, per row, the output index (-1: no sample) and the occupancy voxel of the sample
 struct PackSlots {
-    uint8_t *a;                            // [kPackSlots][kTile * NF * 2]
+    uint8_t *a;                            // [kPackSlots][kTile * NF * 2 bytes]
     int64_t *out;                          // [kPackSlots][kTile]
     int *voxel;                            // [kPackSlots][kTile]
     uint64_t *full, *empty;                // [kPackSlots]: 128 producer arrivals / 128 consumer arrivals per phase
@@ -53,6 +56,7 @@ struct PackSlots {
 
 // the producer side of MODE 2: set `set` walks every group of this CTA, gathers its tiles j (j % kPackSets == set) into the ring and,
 // when it owns the index past the last tile, posts the end marker there.  Lane = pack (ray), warp w of the set = sample ordinal k0 + w.
+template <int NF>
 __device__ __forceinline__ void sdf_packs_produce(const PLMeta &m, const __half *__restrict__ grid, uint32_t La, const float *__restrict__ rays_o,
                                                   const float *__restrict__ rays_d, const float *__restrict__ t, const int64_t *__restrict__ pack_infos,
                                                   const int64_t *__restrict__ pack_ray, const int64_t *__restrict__ order, int64_t n_packs,
@@ -91,7 +95,7 @@ __device__ __forceinline__ void sdf_packs_produce(const PLMeta &m, const __half 
                 for (int q = 0; q < 3; ++q) xs[q] = to_table_space(xs[q]);
                 const uint32_t s = mine % kPackSlots;
                 tc::mbar_wait(&ring.empty[s], ((mine / kPackSlots) & 1u) ^ 1u);
-                gather_row_to_tile<kTile>(m, grid, xs, La, ring.a + s * (kTile * NF * 2), row);
+                gather_row_to_tile<kTile, NF>(m, grid, xs, La, ring.a + s * (kTile * NF * 2), row);
                 ring.out[s * kTile + row] = valid ? first + k : -1;
                 ring.voxel[s * kTile + row] = (valid && oc.pcl) ? occ_voxel(oc, xs) : 0;
                 tc::fence_async_smem();                        // the tile's generic-proxy writes -> visible to the wgmma (async proxy)
@@ -108,7 +112,7 @@ __device__ __forceinline__ void sdf_packs_produce(const PLMeta &m, const __half 
     }
 }
 
-template <int MODE>
+template <int MODE, int NF>
 __global__ void __launch_bounds__(MODE == 2 ? kPackThreads : kTile, MODE == 2 ? kPackCtasPerSM : 0)
 k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ x,
                const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
@@ -124,7 +128,7 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
         uint8_t *base = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 127) & ~uintptr_t(127));
         PackSlots ring;
         ring.a = base;                                                            // kPackSlots x 8 KB : the A tiles
-        uint8_t *sB = ring.a + kPackSlots * (kTile * NF * 2);                     //  4 KB : W1 [64 x 32]
+        uint8_t *sB = ring.a + kPackSlots * (kTile * NF * 2);                     //  4 KB : W1 [64 x NF]
         ring.out = reinterpret_cast<int64_t *>(sB + HW * NF * 2);
         ring.voxel = reinterpret_cast<int *>(ring.out + kPackSlots * kTile);
         float *sb1 = reinterpret_cast<float *>(ring.voxel + kPackSlots * kTile), *sW2 = sb1 + HW;
@@ -133,7 +137,7 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
         ring.end = reinterpret_cast<int *>(ring.empty + kPackSlots);
         float *sb2 = reinterpret_cast<float *>(ring.end + kPackSlots);
         if (tid < kTile) {
-            stage_W1(dec, sB, tid);
+            stage_W1<NF>(dec, sB, tid);
             stage_decoder_vectors(dec, sb1, sW2, sb2, tid);
         }
         if (tid < kPackSlots) {
@@ -146,7 +150,7 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
         __syncthreads();
         if (warp >= 4) {                                       // producers
             tc::setmaxnreg_dec<kPackProducerRegs>();
-            sdf_packs_produce(m, grid, La, rays_o, rays_d, t, pack_infos, pack_ray, order, n_packs, oc, ring, (warp - 4) >> 2, warp & 3, lane);
+            sdf_packs_produce<NF>(m, grid, La, rays_o, rays_d, t, pack_infos, pack_ray, order, n_packs, oc, ring, (warp - 4) >> 2, warp & 3, lane);
             return;
         }
         tc::setmaxnreg_inc<kPackConsumerRegs>();
@@ -187,11 +191,11 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
         }
     } else {
         n = eff_n(n, n_dev);                                   // device-resident count (nsb_bind_device_counts)
-        __shared__ __align__(128) uint8_t sA[kTile * NF * 2];    // 8 KB : features, chunk-major core-matrix layout
-        __shared__ __align__(128) uint8_t sB[HW * NF * 2];       // 4 KB : W1 [64 x 32], same layout
+        __shared__ __align__(128) uint8_t sA[kTile * NF * 2];    // 8 KB (NF = 48: 12 KB) : features, chunk-major core-matrix layout
+        __shared__ __align__(128) uint8_t sB[HW * NF * 2];       // 4 KB (6 KB) : W1 [64 x NF], same layout
         __shared__ float sb1[HW], sW2[HW], srow[kTile];
         __shared__ float sb2;
-        stage_W1(dec, sB, tid);
+        stage_W1<NF>(dec, sB, tid);
         stage_decoder_vectors(dec, sb1, sW2, &sb2, tid);
         tc::fence_async_smem();
         __syncthreads();
@@ -202,7 +206,7 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
             const bool valid = i < n;
             float xs[3];
             load_point(PointSrc{x, rays_o, rays_d, t, ridx}, MODE == 1, i, valid, xs);
-            const float v = sdf_of_tile(ctx, xs, tid);
+            const float v = sdf_of_tile<NF>(ctx, xs, tid);
             if (valid) {
                 sdf[i] = v;
                 if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -217,23 +221,31 @@ k_fused_sdf_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDev
 //   recompute  gather -> A tile [H | 1 | 0..];  MMA1: Z = H.W1^T (registers);  z = fp16(Z + b1); s = sigmoid(beta z), a = fp16(softplus)
 //   G tile [128 x 128] fp16 :=  [ dz_0..dz_63 | d*a_0..d*a_63 ],  dz_j = d * w2_j * s_j, written from the Z fragments
 //              (the reference rounds grad_z to fp16 at the same place, layers.py autocast backward)
-//   MMA2: dH[128 x 32]  = dZ . W1                 A = G cols 0..63 (K-major), B = W1^T tile          -> registers
-//   MMA3: X[64 x 40]   += dZ^T . [H | 1 | 0..]    both operands are the tiles above read MN-major, K = the 128 points: [ dW1 | db1 ]
+//   MMA2: dH[128 x NF]  = dZ . W1                 A = G cols 0..63 (K-major), B = W1^T tile          -> registers
+//   MMA3: X[64 x NF+8] += dZ^T . [H | 1 | 0..]    both operands are the tiles above read MN-major, K = the 128 points: [ dW1 | db1 ]
 //   MMA4: V[64 x 8]    += (d*a)^T . [1 0..]       column 0 = dW2
 //              X and V are register fragments carried over all tiles of the persistent CTA
 //   dH staged as fp32 rows in G (free once the MMAs have completed) -> scatter into the fp32 table gradient (8 corners x L levels,
-//   red.global.add.v2.f32);  db2 via a warp sum.  Columns 2L..31 of H and dH are zero and neither scattered nor flushed.
+//   red.global.add.v2.f32);  db2 via a warp sum.  Columns 2L..NF-1 of H and dH are zero and neither scattered nor flushed.
 // =====================================================================================================================
 // Resident CTAs per SM of the persistent grid of k_sdf_bwd_tc: 51 KB of shared memory and 120 registers fit four.  On an H100
 // (NVIDIA H100 80GB HBM3, 400 W power limit) the kernel took 2.43 / 2.43 ms per bench step at 2 CTAs / SM, 2.24 / 2.19 ms at 3 and
 // 2.16 / 2.13 ms at 4 (profiles/bwd_kernels.py, the three builds alternated in one run; 2.48 ms before its sums moved to registers).
 constexpr int kSdfBwdCtasPerSM = 4;
+// The 48-column form (tables of 17..24 levels) needs 58 KB of shared memory per CTA (wider H tile, W1 and W1^T): three fit an SM.
+constexpr int kSdfBwdWideCtasPerSM = 3;
+template <int NF>
+constexpr int sdf_bwd_ctas() { return NF == 32 ? kSdfBwdCtasPerSM : kSdfBwdWideCtasPerSM; }
+// dynamic shared memory of k_sdf_bwd_tc: [H | 1 | 0..], G, W1, W1^T and the 128 B alignment slack (50 KB at NF = 32, 58 KB at 48)
+template <int NF>
+constexpr int sdf_bwd_smem() { return (kTile * (NF + 8) + kTile * 128 + HW * NF + NF * HW) * 2 + 128; }
+static_assert(sdf_bwd_smem<32>() == (128 * 40 + 128 * 128 + 64 * 32 + 32 * 64) * 2 + 128, "the 32-column budget is unchanged");
 
 // kXGrad (points from rays only) adds the gradient of every point's ray, the depths t being constants: the scatter loads the corners of
 // each level it scatters to once more and adds J^T dH to the point's table-space input gradient g, which is mapped to network space and
 // written as row i_ (the kernel's row, not keep[i_]) of gx_out [n, 8] = [g | t g | 0 0]; k_ray_row_sum adds the rows up per ray.
-template <bool FROM_RAYS, bool kXGrad>
-__global__ void __launch_bounds__(kTile, kSdfBwdCtasPerSM)
+template <bool FROM_RAYS, bool kXGrad, int NF>
+__global__ void __launch_bounds__(kTile, sdf_bwd_ctas<NF>())
 k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ x,
              const float *__restrict__ rays_o, const float *__restrict__ rays_d, const int64_t *__restrict__ ridx,
              const float *__restrict__ t, const float *__restrict__ d_sdf, int64_t n, int max_level, float *__restrict__ d_grid,
@@ -241,24 +253,24 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
              const int64_t *__restrict__ keep, const int64_t *__restrict__ n_dev, float *__restrict__ gx_out, const int32_t *__restrict__ ml_dev) {
     n = eff_n(n, n_dev);
     const uint32_t La = active_levels(max_level, ml_dev, m.n_pseudo);
-    constexpr int NX = 40, GW = 128;                          // NX: features + [1,0,..] chunk; GW: dz | d*a
-    constexpr int kS = tc::acc_stride(NF);                    // staged dH rows for the scatter: 18 KB, aliasing G
-    extern __shared__ uint8_t dyn_smem[];                     // 50 KB of tiles (> the 48 KB static limit)
+    constexpr int NX = NF + 8, GW = 128;                      // NX: features + [1,0,..] chunk; GW: dz | d*a
+    constexpr int kS = tc::acc_stride(NF);                    // staged dH rows for the scatter: 18 KB (26 KB), aliasing G
+    extern __shared__ uint8_t dyn_smem[];                     // 50 KB (NF = 48: 58 KB) of tiles (> the 48 KB static limit)
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(dyn_smem) + 127) & ~uintptr_t(127));
-    uint8_t *sA = tiles;                                      // 10 KB : [H | 1 | 0..]
+    uint8_t *sA = tiles;                                      // 10 KB (14 KB) : [H | 1 | 0..]
     uint8_t *sG = sA + kTile * NX * 2;                        // 32 KB : [dz | d*a]
-    uint8_t *sB = sG + kTile * GW * 2;                        //  4 KB : W1   [64 x 32]  (B of MMA1)
-    uint8_t *sBT = sB + HW * NF * 2;                          //  4 KB : W1^T [32 x 64]  (B of MMA2)
+    uint8_t *sB = sG + kTile * GW * 2;                        //  4 KB (6 KB) : W1   [64 x NF]  (B of MMA1)
+    uint8_t *sBT = sB + HW * NF * 2;                          //  4 KB (6 KB) : W1^T [NF x 64]  (B of MMA2)
     float *stage = reinterpret_cast<float *>(sG);
     static_assert(kTile * kS * 4 <= kTile * GW * 2, "the staged dH rows must fit in G");
     __shared__ float sb1[HW], sW2[HW], sdd[kTile];
     __shared__ float sdb2;
 
     const int tid = threadIdx.x, lane = tid & 31;
-    stage_W1(dec, sB, tid);
-    stage_W1T(dec, sBT, tid);
+    stage_W1<NF>(dec, sB, tid);
+    stage_W1T<NF>(dec, sBT, tid);
     stage_decoder_vectors(dec, sb1, sW2, nullptr, tid);
-    *reinterpret_cast<uint4 *>(sA + 4 * (kTile * 16) + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);   // constant chunk: [1,0,..]
+    *reinterpret_cast<uint4 *>(sA + (NF / 8) * (kTile * 16) + tid * 16) = make_uint4(0x00003C00u, 0, 0, 0);   // constant chunk: [1,0,..]
     float xacc[NX / 2], vacc[4];
 #pragma unroll
     for (int k = 0; k < NX / 2; ++k) xacc[k] = 0.f;
@@ -280,7 +292,7 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         load_point(PointSrc{x, rays_o, rays_d, t, ridx}, FROM_RAYS, i, valid, xs);
         const float dd = valid ? d_sdf[i] : 0.f;
         sdd[tid] = dd;                                           // read by the fragment owners of my row
-        gather_row_to_tile<kTile>(m, grid, xs, La, sA, tid);
+        gather_row_to_tile<kTile, NF>(m, grid, xs, La, sA, tid);
         tc::fence_async_smem();
         __syncthreads();
         {
@@ -315,7 +327,7 @@ k_sdf_bwd_tc(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC
         float dh_fr[2][NF / 2];
         tc::mma_m128<NF, 0, 0, HW / 16>(dh_fr, tc::kmajor(g_addr, kTile), tc::kmajor(bt_addr, NF), false);                          // dH = dZ . W1 : K = 64 hidden
         tc::mma_m64<NX, 1, 1, kTile / 16>(xacc, tc::mnmajor(g_addr, kTile), tc::mnmajor(a_addr, kTile), true);                      // X += dZ^T . [H|1] : K = 128 points
-        tc::mma_m64<8, 1, 1, kTile / 16>(vacc, tc::mnmajor(g_addr + 8 * (kTile * 16), kTile), tc::mnmajor(a_addr + 4 * (kTile * 16), kTile), true);   // V += (d*a)^T . 1
+        tc::mma_m64<8, 1, 1, kTile / 16>(vacc, tc::mnmajor(g_addr + 8 * (kTile * 16), kTile), tc::mnmajor(a_addr + (NF / 8) * (kTile * 16), kTile), true);   // V += (d*a)^T . 1
         first_tile = false;
         const float dsum = warp_sum(dd);
         if (lane == 0 && dsum != 0.f) atomicAdd(&sdb2, dsum);
@@ -403,16 +415,21 @@ extern "C" int nsb_fused_sdf_tc_launch(const nsb_lotd_meta *meta, const void *pa
     const __half *g = (const __half *)params_half;
     const OccCollect oc = occ_collect_of(collect);
     const unsigned tiles = persistent_grid((n + kTile - 1) / kTile, kSdfCtasPerSM);
-    if (mode == 2) {          // a work unit of mode 2 is a group of 32 packs
-        opt_in_smem(k_fused_sdf_tc<2>, kPackSmem);
-        if (int rc = require_ctas_per_sm(k_fused_sdf_tc<2>, kPackThreads, kPackSmem, kPackCtasPerSM, "nsb_fused_sdf (packs)")) return rc;
-        k_fused_sdf_tc<2><<<persistent_grid((n_packs + 31) / 32, kPackCtasPerSM), kPackThreads, kPackSmem, s>>>(
-            m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf, pack_infos, pack_ray, pack_order, n_packs, oc, dn.a, ml_dev);
-    } else if (mode == 1)
-        k_fused_sdf_tc<1><<<tiles, kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, ridx, t, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a, ml_dev);
-    else
-        k_fused_sdf_tc<0><<<tiles, kTile, 0, s>>>(m, g, d, x, nullptr, nullptr, nullptr, nullptr, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a, ml_dev);
-    return check_launch("nsb_fused_sdf(tc)");
+    auto launch = [&](auto nf) -> int {
+        constexpr int NF = decltype(nf)::value;
+        if (mode == 2) {      // a work unit of mode 2 is a group of 32 packs
+            constexpr int kPackSmem = pack_smem<NF>();
+            opt_in_smem(k_fused_sdf_tc<2, NF>, kPackSmem);
+            if (int rc = require_ctas_per_sm(k_fused_sdf_tc<2, NF>, kPackThreads, kPackSmem, kPackCtasPerSM, "nsb_fused_sdf (packs)")) return rc;
+            k_fused_sdf_tc<2, NF><<<persistent_grid((n_packs + 31) / 32, kPackCtasPerSM), kPackThreads, kPackSmem, s>>>(
+                m, g, d, nullptr, rays_o, rays_d, nullptr, t, n, ml, sdf, pack_infos, pack_ray, pack_order, n_packs, oc, dn.a, ml_dev);
+        } else if (mode == 1)
+            k_fused_sdf_tc<1, NF><<<tiles, kTile, 0, s>>>(m, g, d, nullptr, rays_o, rays_d, ridx, t, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a, ml_dev);
+        else
+            k_fused_sdf_tc<0, NF><<<tiles, kTile, 0, s>>>(m, g, d, x, nullptr, nullptr, nullptr, nullptr, n, ml, sdf, nullptr, nullptr, nullptr, 0, oc, dn.a, ml_dev);
+        return check_launch("nsb_fused_sdf(tc)");
+    };
+    return feature_cols(m.n_pseudo) == 32 ? launch(std::integral_constant<int, 32>{}) : launch(std::integral_constant<int, 48>{});
 }
 
 extern "C" int nsb_fused_sdf_bwd(const nsb_lotd_meta *meta, const void *params_half, const nsb_sdf_decoder *dec, const float *x,
@@ -438,16 +455,19 @@ static int sdf_bwd(const char *who, const nsb_lotd_meta *meta, const void *param
     PLMeta m;
     DecoderDevTC d;
     if (int rc = make_decoder(meta, dec, &m, &d, who)) return rc;
-    constexpr int kBwdSmem = (128 * 40 + 128 * 128 + 64 * 32 + 32 * 64) * 2 + 128;       // 50 KB
-    auto kern = x == nullptr ? k_sdf_bwd_tc<true, kXGrad> : k_sdf_bwd_tc<false, false>;
-    opt_in_smem(kern, kBwdSmem);
-    if (int rc = require_ctas_per_sm(kern, kTile, kBwdSmem, kSdfBwdCtasPerSM, who)) return rc;
-    const unsigned grid = persistent_grid((n + kTile - 1) / kTile, kSdfBwdCtasPerSM);
     cudaStream_t s = (cudaStream_t)stream;
     const int ml = max_level < 0 ? -1 : max_level;
-    kern<<<grid, kTile, kBwdSmem, s>>>(m, (const __half *)params_half, d, x, x ? nullptr : rays_o, x ? nullptr : rays_d, x ? nullptr : ridx,
-                                       x ? nullptr : t, d_sdf, n, ml, d_grid, d_W1, d_b1, d_W2, d_b2, keep, dn.a, gx_scratch, ml_dev);
-    if (int rc = check_launch(who)) return rc;
+    auto launch = [&](auto nf) -> int {
+        constexpr int NF = decltype(nf)::value, kBwdSmem = sdf_bwd_smem<NF>(), kCtas = sdf_bwd_ctas<NF>();
+        auto kern = x == nullptr ? k_sdf_bwd_tc<true, kXGrad, NF> : k_sdf_bwd_tc<false, false, NF>;
+        opt_in_smem(kern, kBwdSmem);
+        if (int rc = require_ctas_per_sm(kern, kTile, kBwdSmem, kCtas, who)) return rc;
+        const unsigned grid = persistent_grid((n + kTile - 1) / kTile, kCtas);
+        kern<<<grid, kTile, kBwdSmem, s>>>(m, (const __half *)params_half, d, x, x ? nullptr : rays_o, x ? nullptr : rays_d, x ? nullptr : ridx,
+                                           x ? nullptr : t, d_sdf, n, ml, d_grid, d_W1, d_b1, d_W2, d_b2, keep, dn.a, gx_scratch, ml_dev);
+        return check_launch(who);
+    };
+    if (int rc = feature_cols(m.n_pseudo) == 32 ? launch(std::integral_constant<int, 32>{}) : launch(std::integral_constant<int, 48>{})) return rc;
     if (kXGrad) {
         if (!d_rays_o && !d_rays_d) return 0;
         k_ray_row_sum<8><<<row_sum_blocks(n), 256, 0, s>>>(gx_scratch, ridx, keep, n, 6, ray_map, RowSumOut{{d_rays_o, d_rays_d, nullptr}, 3}, dn.a);

@@ -9,7 +9,7 @@ namespace nsb {
 struct DecoderDevTC {
     const __half *W1, *b1, *W2, *b2;
     int width;
-    int nh;                                // 2L: the decoder's input width = the row stride of W1 (L = PLMeta::n_pseudo, 1..16)
+    int nh;                                // 2L: the decoder's input width = the row stride of W1 (L = PLMeta::n_pseudo, 1..24)
     float beta;
 };
 
@@ -43,7 +43,11 @@ __device__ __forceinline__ void occ_collect_point(const OccCollect &oc, const fl
 }
 
 constexpr int kTile = 128;
-constexpr int NF = 32, HW = 64;           // features, hidden width (zero padded to 64)
+constexpr int HW = 64;                    // hidden width (zero padded to 64)
+// Feature columns of the A tile (the template parameter NF of every wgmma kernel): 32 for tables of 1..16 two-feature levels, 48 for
+// 17..24.  The width follows the table's L, not the active level count, so one instantiation serves every level bound of a schedule.
+constexpr int kMaxNarrowLevels = 16, kMaxWideLevels = 24;
+inline int feature_cols(uint32_t L) { return L <= (uint32_t)kMaxNarrowLevels ? 32 : 48; }
 
 // The levels a launch uses: 0..max_level of the L = m.n_pseudo levels (make_decoder: pseudo level p is level p), i.e. the prefix of
 // clamp(max_level + 1, 0, L) levels.  max_level is the host argument, or -- with a device level bound to the launch (ml_dev,
@@ -54,20 +58,21 @@ __device__ __forceinline__ uint32_t active_levels(int max_level, const int32_t *
     return ml < 0 ? 0u : (ml >= (int)L - 1 ? L : (uint32_t)ml + 1u);
 }
 
-// the La active levels of one point -> row `r` of a chunk-major [R x >=32] fp16 tile (4 bytes per level); the feature columns 2La..31
+// the La active levels of one point -> row `r` of a chunk-major [R x >=NF] fp16 tile (4 bytes per level); the feature columns 2La..NF-1
 // are written as zeros, so that nothing a previous tile left in shared memory reaches a wgmma (a stale fp16 Inf times a zero weight is
 // NaN), and levels >= La are not read: a masked level costs its zero columns, not its 8 corner loads.
 // U levels per loop trip: the 8 U corner loads of a trip are independent, so U = 2 doubles the loads in flight per thread (the
 // latency-bound backward kernels run at 8-16 warps / SM; one level per trip thrashes L1 in the ray-major order of k_fused_sdf_tc);
-// full unrolling is avoided on purpose (instruction cache, see fused_tc.cu).  An odd La ends with one level alone.
+// full unrolling is avoided on purpose (instruction cache, see fused_tc.cu).  An odd La ends with one level alone.  p_begin > 0 skips the
+// first levels (written by the caller).
 template <int R>
 __device__ __forceinline__ void put_level_to_tile(uint8_t *tile, int r, uint32_t p, uint32_t v) {
     *reinterpret_cast<uint32_t *>(tile + (p >> 2) * (R * 16) + r * 16 + (p & 3) * 4) = v;
 }
-template <int R, int U = 2>
+template <int R, int NF, int U = 2>
 __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half *__restrict__ grid, const float (&xs)[3],
-                                                   uint32_t La, uint8_t *tile, int r) {
-    uint32_t p0 = 0;
+                                                   uint32_t La, uint8_t *tile, int r, uint32_t p_begin = 0) {
+    uint32_t p0 = p_begin;
 #pragma unroll 1
     for (; p0 + U <= La; p0 += U) {
         uint32_t cell[U][8];
@@ -88,7 +93,7 @@ __device__ __forceinline__ void gather_row_to_tile(const PLMeta &m, const __half
         put_level_to_tile<R>(tile, r, p0, level_feat2_cells(level_cells_ptr(m, p0, grid), cell, w));
     }
 #pragma unroll 1
-    for (; p0 < 16; ++p0) put_level_to_tile<R>(tile, r, p0, 0u);
+    for (; p0 < NF / 2; ++p0) put_level_to_tile<R>(tile, r, p0, 0u);
 }
 
 // d(y_f)/d(x_d) of one level (both features) from its 8 corner cells as loaded, exactly as k_lotd_fwd<3,2,true,true> computes dy_dx
@@ -198,7 +203,8 @@ __device__ __forceinline__ void softplus_as(float zz, const SoftplusK &K, float 
     s = lin ? 1.f : e * rcp_approx(d);
 }
 
-// W1 [width x 2L] (fp16, row-major) -> chunk-major [64 x 32] B tile, rows >= width and columns >= 2L zero
+// W1 [width x 2L] (fp16, row-major) -> chunk-major [64 x NF] B tile, rows >= width and columns >= 2L zero
+template <int NF>
 __device__ __forceinline__ void stage_W1(const DecoderDevTC &dec, uint8_t *sB, int tid) {
     for (int e = tid; e < HW * (NF / 8); e += kTile) {
         const int j = e % HW, c = e / HW;
@@ -209,7 +215,8 @@ __device__ __forceinline__ void stage_W1(const DecoderDevTC &dec, uint8_t *sB, i
     }
 }
 
-// W1^T [32 x 64] -> chunk-major B tile (row = feature k, column = hidden j), columns >= width and rows >= 2L zero
+// W1^T [NF x 64] -> chunk-major B tile (row = feature k, column = hidden j), columns >= width and rows >= 2L zero
+template <int NF>
 __device__ __forceinline__ void stage_W1T(const DecoderDevTC &dec, uint8_t *sBT, int tid) {
     for (int e = tid; e < NF * HW; e += kTile) {
         const int k = e % NF, j = e / NF;
@@ -300,10 +307,11 @@ inline unsigned row_sum_blocks(int64_t n) {
 }
 
 // Host: the LoTD layout and decoder the wgmma kernels are built for -> their kernel arguments (0, or 2 with the error set).
-// L = 1..16 levels of 2 features each in 3-D; the decoder's W1 is [width x 2L].
+// L = 1..24 levels of 2 features each in 3-D (feature_cols(L) picks the kernels' tile width); the decoder's W1 is [width x 2L].
 inline int make_decoder(const nsb_lotd_meta *meta, const nsb_sdf_decoder *dec, PLMeta *m, DecoderDevTC *d, const char *who) {
     if (make_plmeta(meta, m)) return 2;
-    NSB_REQUIRE(m->n_pseudo >= 1 && m->n_pseudo <= 16, "%s: built for 1 to 16 LoTD levels (got %u)", who, m->n_pseudo);
+    NSB_REQUIRE(m->n_pseudo >= 1 && m->n_pseudo <= (uint32_t)kMaxWideLevels, "%s: built for 1 to %d LoTD levels (got %u)", who, kMaxWideLevels,
+                m->n_pseudo);
     NSB_REQUIRE(m->F == 2 && m->D == 3 && m->n_out == 2 * m->n_pseudo && plmeta_two_feature_cells(*m), "%s: built for L x 2 LoTD features in 3-D", who);
     NSB_REQUIRE(plmeta_cell_key_fits(*m), "%s: a level resolution exceeds %u cells per axis (the backward's merge key)", who, 1u << kCellKeyBits);
     for (uint32_t p = 0; p < m->n_pseudo; ++p)        // 2-feature levels: the active levels are a prefix (active_levels)
@@ -353,8 +361,9 @@ __device__ __forceinline__ void sdf_rows_of_frags(const float (&z)[2][HW / 2], c
 }
 
 // all 128 threads: my point's table coordinates -> my sdf (fp16-rounded, as fp32).  Ends with the CTA barrier that frees the tile.
+template <int NF>
 __device__ __forceinline__ float sdf_of_tile(const SdfTile &c, const float (&xs)[3], int tid) {
-    gather_row_to_tile<kTile>(c.m, c.grid, xs, c.La, c.sA, tid);
+    gather_row_to_tile<kTile, NF>(c.m, c.grid, xs, c.La, c.sA, tid);
     tc::fence_async_smem();                // generic-proxy smem writes -> visible to the tensor core (async proxy)
     __syncthreads();
     float z[2][HW / 2];

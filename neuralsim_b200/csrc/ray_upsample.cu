@@ -35,6 +35,9 @@ struct UpsampleArgs {
     float eps, thre;
 };
 
+// NF: the feature columns of the A tile (feature_cols: 32 for tables of 1..16 levels, 48 for 17..24; 37 KB of static shared memory
+// instead of 31 KB, still five CTAs per SM)
+template <int NF>
 __global__ void __launch_bounds__(kTile)
 k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const DecoderDevTC dec, const float *__restrict__ rays_o,
                       const float *__restrict__ rays_d, const float *__restrict__ t_starts, const int64_t *__restrict__ pack_infos,
@@ -53,7 +56,7 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
     __shared__ float *p_t[2][kG], *p_sdf[2][kG], *p_cdf[kG];          // where ray q's samples live: shared memory, or its slice of `scratch`
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    stage_W1(dec, sB, tid);
+    stage_W1<NF>(dec, sB, tid);
     stage_decoder_vectors(dec, sb1, sW2, &sb2, tid);
     tc::fence_async_smem();
     __syncthreads();
@@ -110,7 +113,7 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
                 }
 #pragma unroll
                 for (int c = 0; c < 3; ++c) xs[c] = to_table_space(xs[c]);
-                const float v = sdf_of_tile(ctx, xs, tid);
+                const float v = sdf_of_tile<NF>(ctx, xs, tid);
                 if (valid) {
                     p_sdf[0][q][r] = v;
                     if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -145,7 +148,7 @@ k_upsample_persistent(const PLMeta m, const __half *__restrict__ grid, const Dec
                 }
 #pragma unroll
                 for (int c = 0; c < 3; ++c) xs[c] = to_table_space(xs[c]);
-                const float v = sdf_of_tile(ctx, xs, tid);
+                const float v = sdf_of_tile<NF>(ctx, xs, tid);
                 if (valid) {
                     s_fsdf[q][k] = v;
                     if (oc.pcl) occ_collect_point(oc, xs, v);
@@ -214,7 +217,8 @@ extern "C" int nsb_upsample_rays(const nsb_lotd_meta *meta, const void *params_h
     }
     NSB_REQUIRE(merged < kCap, "nsb_upsample_persistent: the merged stages alone exceed the per-ray capacity");
     NSB_REQUIRE(scratch == nullptr || long_cap > kCap, "nsb_upsample_rays: long_cap must exceed the shared-memory capacity (%d)", kCap);
-    k_upsample_persistent<<<upsample_grid(n_hit), kTile, 0, (cudaStream_t)stream>>>(
+    auto kern = feature_cols(m.n_pseudo) == 32 ? k_upsample_persistent<32> : k_upsample_persistent<48>;
+    kern<<<upsample_grid(n_hit), kTile, 0, (cudaStream_t)stream>>>(
         m, (const __half *)params_half, d, rays_o, rays_d, t_starts, pack_infos, ridx_hit, n_hit, max_level < 0 ? -1 : max_level, ua, fine_all, nf_total,
         overflow, scratch, long_cap, occ_collect_of(collect), dn.a, ml_dev);
     return check_launch("nsb_upsample_rays");

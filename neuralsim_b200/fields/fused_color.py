@@ -17,6 +17,11 @@ from torch import autograd
 from .. import _lib as L
 
 
+def h_tile_cols(n_levels):
+    """the width of the kernels' feature tile for an n_levels-level table (csrc/fused_tc_common.cuh feature_cols): the columns of dh_scratch"""
+    return 32 if n_levels <= 16 else 48
+
+
 def color_net_c(t16, dec, rad, fac):
     """nsb_color_net over the fp16 images t16 = (W1, b1, W2, b2[, R1, rb1, R2, rb2, R3, rb3]) of the decoder layers `dec` and the radiance
     layers `rad` (None: the geometry-only net, rad_width = 0); fac: sdf_scale / radius3d_original per axis"""
@@ -101,7 +106,7 @@ class _FusedColor(autograd.Function):
         n_act = 4 if rad else 2                                  # Z, X (+ Y1, Y2)
         acts = None
         if keep:
-            acts = torch.empty(n_act, int(L.lib().nsb_color_tile_bytes(L.c_i64(n))), dtype=torch.uint8, device=dev)
+            acts = torch.empty(n_act, int(L.lib().nsb_color_act_bytes(n, q.meta.n_pseudo_levels)), dtype=torch.uint8, device=dev)
         ap = [L.ptr(acts[k]) if keep and k < n_act else None for k in range(4)]
         P = L.ptr
         with L.KERNEL_TIMER.time("fused_color_fwd", n):
@@ -149,7 +154,7 @@ class _FusedColor(autograd.Function):
             return ret
         c = lambda g: None if g is None else g.contiguous().float()
         g_sdf, g_nab, g_rgb = c(g_sdf), c(g_nab), c(g_rgb)
-        dh = torch.empty(n, 32, dtype=torch.float32, device=dev) if g_rgb is not None else None
+        dh = torch.empty(n, h_tile_cols(q.meta.n_pseudo_levels), dtype=torch.float32, device=dev) if g_rgb is not None else None
         P = L.ptr
         ag = [P(g) for g in grads] + [None] * (11 - len(grads))          # d_R* / d_rb*: NULL without the radiance net's parameters
         args = (q.meta.c_ref, P(q.grid16, "f16"), ctypes.byref(q.net), None, P(q.rays_o, "f32"), P(q.rays_d, "f32"), P(ctx.ridx, "i64"), P(ctx.t, "f32"),

@@ -244,12 +244,21 @@ class _FusedSDF(autograd.Function):
         return None, None, None, None, d_grid, d_W1, d_b1, d_W2, d_b2, d_ro, d_rd
 
 
+# the largest LoTD tables the fused kernels may take, per model: 16 (the default) or 24.  Tables of 17..24 levels run the kernels'
+# 48-column feature tile (csrc/fused_tc_common.cuh feature_cols); with the default they keep the module path.
+FUSED_LEVEL_BOUNDS = (16, 24)
+
+
 class LoTDSDF(nn.Module):
-    """LoTD encoding + MLP decoder -> sdf (and nablas by analytic back-propagation through decoder and table)."""
+    """LoTD encoding + MLP decoder -> sdf (and nablas by analytic back-propagation through decoder and table).
+    max_fused_levels: 16 or 24, the most LoTD levels a table may have to run on the fused kernels (see _fusable)."""
 
     def __init__(self, encoding_cfg: dict = None, decoder_cfg: dict = None, dtype=torch.half, device=None, generator=None,
-                 sdf_scale=1.0, radius3d_original=1.0, aabb=None):
+                 sdf_scale=1.0, radius3d_original=1.0, aabb=None, max_fused_levels: int = 16):
         super().__init__()
+        if isinstance(max_fused_levels, bool) or max_fused_levels not in FUSED_LEVEL_BOUNDS:
+            raise ValueError(f"LoTDSDF: max_fused_levels must be one of {FUSED_LEVEL_BOUNDS} (got {max_fused_levels!r})")
+        self.max_fused_levels = int(max_fused_levels)
         self.dtype = dtype
         self.encoding = LoTDEncoding(3, **(encoding_cfg or {}), dtype=dtype, device=device, generator=generator, aabb=aabb)
         dc = dict(D=1, W=64, activation=dict(type="softplus", beta=100.0))
@@ -324,13 +333,13 @@ class LoTDSDF(nn.Module):
 
     # ---- fused no-grad query (csrc/fused.cu)
     def _fusable(self):
-        """the preconditions of the fused kernels (csrc/fused_tc_common.cuh make_decoder: 1 to 16 levels of 2 features, `plmeta_two_feature_cells`),
-        width <= 64, both biases, CUDA parameters); any other valid LoTD / decoder configuration, such as a table of 17 or more levels, takes
-        the generic encoding -> decoder path of forward()"""
+        """the preconditions of the fused kernels (csrc/fused_tc_common.cuh make_decoder: 1 to max_fused_levels (16, or 24) levels of 2
+        features, `plmeta_two_feature_cells`), width <= 64, both biases, CUDA parameters); any other valid LoTD / decoder configuration, such
+        as a table of more than max_fused_levels levels, takes the generic encoding -> decoder path of forward()"""
         e, d = self.encoding, self.decoder
         m = e.meta
         return (self.dtype == torch.half and e.window is None and d.D == 1 and e.in_features == 3
-                and 1 <= m.n_pseudo_levels <= 16 and e.out_features == 2 * m.n_pseudo_levels
+                and 1 <= m.n_pseudo_levels <= self.max_fused_levels and e.out_features == 2 * m.n_pseudo_levels
                 and m.n_feat_per_pseudo_lvl == 2 and all(f == 2 for f in m.level_n_feats)
                 and d.layers[0].out_features <= 64 and isinstance(d.layers[0].activation, nn.Softplus)
                 and d.layers[0].bias is not None and d.layers[1].bias is not None and e.flattened_params.is_cuda)

@@ -42,7 +42,8 @@ class LoTDNeuS(nn.Module):
         self.space = AABBSpace(bounding_size, aabb=aabb, device=device)
         self.implicit_surface = LoTDSDF(encoding_cfg=sc.get("encoding_cfg"), decoder_cfg=sc.get("decoder_cfg"), dtype=dtype, device=device,
                                         generator=generator, sdf_scale=sc.get("sdf_scale", 1.0), aabb=self.space.aabb.cpu(),
-                                        radius3d_original=(self.space.radius3d_original.cpu() if aabb is not None else bounding_size / 2.))
+                                        radius3d_original=(self.space.radius3d_original.cpu() if aabb is not None else bounding_size / 2.),
+                                        max_fused_levels=sc.get("max_fused_levels", 16))
         if radiance_cfg is False:
             self.radiance_net = None
         else:
