@@ -495,6 +495,31 @@ int nsb_imp_sample(const int64_t *table, const int64_t *cam, const int64_t *rng,
 int nsb_error_map_update(float *error_map, int32_t *last, int64_t n_images, const int64_t *table, const int64_t *cam, int32_t res_y, int32_t res_x,
                          const int64_t *fidx, const float *xy, const float *val, int64_t n, int32_t *flag, const int64_t *skip, void *stream);
 
+/* ---------------------------------------------------------------- the LiDAR batch of a frame (csrc/lidar_sample.cu)
+ * LidarDataset.sample_merged(frame, n) in the merged_weighted / merged_equal modes (dataio/data_loader/lidar_loader.py:119-204) and the
+ * beams' world transform (MultiRaysLidarBundle.get_selected_rays, app/resources/observers/lidars.py:65-78).  table: device int64
+ * [n_frames, NSB_LIDAR_TABLE_WIDTH], one row per frame, written by the host once: the frame's first beam in the concatenated arrays
+ * (DATA_OFF), its first row of l2w (POSE_BASE: lidar li's transform is row POSE_BASE + li), the generator offsets its draws advance
+ * (INC = sum_li inc(num_li)), the lidar count L <= NSB_LIDAR_MAX, the ray segments RAY_START[0 .. L] (lidar li draws the rays
+ * [RAY_START[li], RAY_START[li + 1]), RAY_START[L] = n), the cumulative beam counts CUMU[0 .. L] (lidar li's beams are
+ * CUMU[li] .. CUMU[li + 1] - 1 of the frame, fewer than 2^32) and each lidar's draw offset DRAW_OFF[li] = sum_{k < li} inc(num_k).
+ * frame: device int64 scalar, the row.  rng: device int64 {seed, offset}; lidar li's torch.randint(CUMU[li], CUMU[li + 1], [num_li])
+ * starts at offset + DRAW_OFF[li] (torch_uniform.cuh).  Per ray r: the beam b = DATA_OFF + the draw, out_rays_o[r] = R rays_o[b] + t and
+ * out_rays_d[r] = R rays_d[b] with (R | t) = l2w[POSE_BASE + li] ([*, 3, 4] float32; a fixed fma order, csrc/lidar_sample.cu),
+ * out_ranges[r] = ranges[b], li[r] = li, rays_fidx[r] = *frame.  rng_next (may be NULL) := {seed, offset + INC}.  No host read. */
+#define NSB_LIDAR_MAX 8
+#define NSB_LIDAR_TABLE_WIDTH 32
+#define NSB_LIDAR_ROW_DATA_OFF 0
+#define NSB_LIDAR_ROW_POSE_BASE 1
+#define NSB_LIDAR_ROW_INC 2
+#define NSB_LIDAR_ROW_N_LIDARS 3
+#define NSB_LIDAR_ROW_RAY_START 4
+#define NSB_LIDAR_ROW_CUMU (NSB_LIDAR_ROW_RAY_START + NSB_LIDAR_MAX + 1)
+#define NSB_LIDAR_ROW_DRAW_OFF (NSB_LIDAR_ROW_CUMU + NSB_LIDAR_MAX + 1)
+int nsb_lidar_sample(const int64_t *table, const int64_t *frame, const int64_t *rng, int64_t n, const float *rays_o, const float *rays_d,
+                     const float *ranges, const float *l2w, float *out_rays_o, float *out_rays_d, float *out_ranges, int64_t *li,
+                     int64_t *rays_fidx, int64_t *rng_next, void *stream);
+
 /* ---------------------------------------------------------------- the StreetSurf LiDAR loss (csrc/lidar_loss.cu)
  * LidarLoss.forward with the depth term and the `neus_unisim` line-of-sight term (app/loss/lidar.py:174-210, 254-294) on the renderer's
  * own buffers, and its adjoint: the cotangents of the composite's depth_volume and vw (nsb_composite_backward's g_depth, g_vw).  R rays

@@ -456,6 +456,15 @@ class StaticFrame:
     device flag that `check()` raises on; a step that overflowed its arenas leaves the error map as it was.  `d_h_appear` keeps its
     meaning: a trainer scatters it by `frame.rays_fidx`.
 
+    `sampler=LidarSampler(...)` (neuralsim_b200/lidar_sampler.py; needs a loss_fn and with_rgb=False, takes no pose=) draws every LiDAR
+    batch inside the graph, as the shipped LiDAR configs' LidarDataset.sample_merged does, and moves the beams to world with each (lidar,
+    frame)'s transform: `frame.step(frame_ind=f)` fills a device frame index and the generator block (the sampler's per-lidar draws first,
+    the perturbed ones after them), and the one replay writes `frame.rays_o` / `frame.rays_d` (world), `frame.rays_li` (the reference's
+    `rays_sel`), `frame.rays_fidx` and `frame.ground_truth = {"ranges": [n_rays]}` (nsb_lidar_sample), renders, calls `loss =
+    loss_fn(rendered_or_ret, frame.ground_truth)` and runs the backward.  With LidarLoss the ranges reach the loss inside the replay:
+    `loss_fn = lambda ret, gt: sum(lidar_loss(None, ret, ground_truth=gt).values())`, the iteration's weights set on the host by
+    `lidar_loss.set_step(None, it)` before `step()`.
+
     The first call probes the sizes with the host-sized path (SingleVolumeRenderer.ray_query, no grad), sizes the arenas with `slack`,
     warms up and captures.  Gradients are accumulated into `p.grad` (kept in place; `zero_grads=True` or a `pre_hook` zeroes them inside the graph).
     Capture precondition (PyTorch): no autograd graph of an EARLIER backward on the default stream may still be referenced (a kept loss / rendered
@@ -484,7 +493,7 @@ class StaticFrame:
             self.d_rays_o, self.d_rays_d = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)
         self.cnt = torch.zeros(32, dtype=torch.int64, device=dev)
         self.perturb, self.rng, self.rng_reservation, self._gen = bool(perturb), None, 0, None
-        self.sampler = sampler
+        self.sampler, self._lidar = sampler, False
         if generator is not None and not self.perturb and sampler is None:
             raise RuntimeError("StaticFrame(generator=...): the generator is read only with perturb=True or a sampler")
         if self.perturb or sampler is not None:
@@ -505,7 +514,7 @@ class StaticFrame:
             self._pose_d_rays = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)       # the rays' gradient when ray_grad is off
             self._pose_g = (torch.zeros(P, 4, device=dev), torch.zeros(P, 3, device=dev))   # what dq.grad / dt.grad are while the frame lives
         if sampler is not None:
-            self._init_sampler(sampler, pose, loss_fn)
+            self._init_sampler(sampler, pose, loss_fn, with_rgb)
         self.graph, self.loss, self.rendered, self.buffers, self._occ_captured = None, None, None, None, None
         self.captures = 0
 
@@ -535,10 +544,16 @@ class StaticFrame:
         self.kept_cap = max(self.kept_cap or 0, k)
 
     # -- the sampler
-    def _init_sampler(self, sampler, pose, loss_fn):
+    def _init_sampler(self, sampler, pose, loss_fn, with_rgb):
         from ..importance import CameraSampler
+        from ..lidar_sampler import LidarSampler
+        self._lidar = isinstance(sampler, LidarSampler)
+        if self._lidar:
+            self._init_lidar_sampler(sampler, pose, loss_fn, with_rgb)
+            return
         if not isinstance(sampler, CameraSampler):
-            raise RuntimeError(f"StaticFrame(sampler=...): a neuralsim_b200.importance.CameraSampler, got {type(sampler)}")
+            raise RuntimeError(f"StaticFrame(sampler=...): a neuralsim_b200.importance.CameraSampler or neuralsim_b200.lidar_sampler.LidarSampler, "
+                               f"got {type(sampler)}")
         if pose is None or loss_fn is None:
             raise RuntimeError("StaticFrame(sampler=...): needs pose= (CameraPoses: the sampled rays are pose indices and camera-space directions) and a loss_fn")
         if sampler.pose_end > pose.n_poses:
@@ -557,9 +572,27 @@ class StaticFrame:
         self.err_flag = torch.zeros(1, dtype=torch.int32, device=dev)
         self._warming = False
 
+    def _init_lidar_sampler(self, sampler, pose, loss_fn, with_rgb):
+        if pose is not None or loss_fn is None or with_rgb:
+            raise RuntimeError("StaticFrame(sampler=LidarSampler): needs a loss_fn and with_rgb=False, and takes no pose= (the sampler writes the "
+                               "world rays)")
+        if sampler.device != self.device:
+            raise RuntimeError(f"StaticFrame(sampler=...): the sampler is on {sampler.device}, the model on {self.device}")
+        dev, n = self.device, self.n_rays
+        self.sampler_reservation = sampler.inc(n, PT.grid_cap(dev))
+        self.frame_ind = torch.zeros((), dtype=torch.int64, device=dev)
+        self._rng_sampler = torch.zeros(2, dtype=torch.int64, device=dev)
+        self.rays_li = torch.zeros(n, dtype=torch.int64, device=dev)
+        self.rays_fidx = torch.zeros(n, dtype=torch.int64, device=dev)
+        self.ground_truth = dict(ranges=torch.zeros(n, device=dev))
+
     def _sample(self):
-        """camera self.cam's batch into the frame's inputs (nsb_imp_sample)"""
+        """camera self.cam's (or LiDAR frame self.frame_ind's) batch into the frame's inputs (nsb_imp_sample, nsb_lidar_sample)"""
         s = self.sampler
+        if self._lidar:
+            s.launch(self.frame_ind, self._rng_sampler, self.rays_o, self.rays_d, self.ground_truth["ranges"], self.rays_li, self.rays_fidx,
+                     self.rng if self.perturb else None)
+            return
         s.sample(self.cam, self._rng_sampler, self.n_rays, self.rays_fidx, self.rays_pix, self.pidx, self.dirs, self.ground_truth,
                  self.h_appear if s.appear_table is not None else None, self.rng if self.perturb else None)
 
@@ -637,6 +670,8 @@ class StaticFrame:
             arg = dict(rendered=rendered, volume_buffer=static_volume_buffer(buffers, self.cnt)) if self.loss_on_ret else rendered
             if self.sampler is None:
                 loss = self.loss_fn(arg)
+            elif self._lidar:
+                loss = self.loss_fn(arg, self.ground_truth)
             else:
                 loss, err = self.loss_fn(arg, self.ground_truth)
                 if not isinstance(err, torch.Tensor) or err.numel() != self.n_rays:
@@ -645,7 +680,7 @@ class StaticFrame:
             if loss.requires_grad:
                 loss.backward()
             loss = loss.detach()
-            if self.sampler is not None and not self._warming:       # the warm-up runs must not add into the error map
+            if self.sampler is not None and not self._lidar and not self._warming:       # the warm-up runs must not add into the error map
                 ov = CNT_SLOTS["overflow"]
                 self.sampler.update(self.cam, self.rays_fidx, self.rays_pix, err, self.err_flag, skip=self.cnt[ov:ov + 1])
         return rendered, buffers, loss
@@ -697,11 +732,17 @@ class StaticFrame:
             L.KERNEL_TIMER.enabled = was
         return self
 
-    def step(self, rays_o=None, rays_d=None, rays_h_appear=None, *, dirs=None, pidx=None, cam=None):
+    def step(self, rays_o=None, rays_d=None, rays_h_appear=None, *, dirs=None, pidx=None, cam=None, frame_ind=None):
         """copy the batch into the graph's inputs (H2D if the tensors are on the host) and launch.  -> loss (device scalar) or None.
-        With pose=: no rays_o / rays_d; dirs and pidx (set_rays), or neither to replay the rays set last.  With sampler=: cam alone, the
-        camera whose batch the graph draws."""
-        if self.sampler is not None:
+        With pose=: no rays_o / rays_d; dirs and pidx (set_rays), or neither to replay the rays set last.  With sampler=CameraSampler: cam
+        alone, the camera whose batch the graph draws; with sampler=LidarSampler: frame_ind alone, the frame whose beams it draws."""
+        if self._lidar:
+            if rays_o is not None or rays_d is not None or rays_h_appear is not None or dirs is not None or pidx is not None or cam is not None:
+                raise RuntimeError("StaticFrame.step: a frame with sampler=LidarSampler draws its own batch; pass frame_ind= only")
+            self.frame_ind.fill_(self.sampler.check_frame(frame_ind))
+        elif frame_ind is not None:
+            raise RuntimeError("StaticFrame.step: frame_ind= is read only with sampler=LidarSampler")
+        elif self.sampler is not None:
             if rays_o is not None or rays_d is not None or rays_h_appear is not None or dirs is not None or pidx is not None:
                 raise RuntimeError("StaticFrame.step: a frame with sampler= draws its own batch; pass cam= only")
             if isinstance(cam, bool) or not isinstance(cam, int) or not 0 <= cam < self.sampler.n_cameras:
@@ -709,7 +750,9 @@ class StaticFrame:
             self.cam.fill_(cam)
         elif cam is not None:
             raise RuntimeError("StaticFrame.step: cam= is read only with sampler=")
-        if self.pose is None:
+        if self._lidar:
+            pass                                            # the graph writes the world rays
+        elif self.pose is None:
             if rays_o is None or rays_d is None or dirs is not None or pidx is not None:
                 raise RuntimeError("StaticFrame.step: a frame without pose= takes rays_o and rays_d (and no dirs / pidx)")
             self.rays_o.copy_(rays_o, non_blocking=True)
@@ -745,7 +788,7 @@ class StaticFrame:
             self.graph.replay()
         else:
             self.rendered, self.buffers, self.loss = self._run()
-        if self.sampler is not None:
+        if self.sampler is not None and not self._lidar:
             self.sampler.samplers[cam].error_map.count_step()     # the reference's per-camera schedule; rebuilds the cdfs in place
         return self.loss
 
@@ -758,7 +801,7 @@ class StaticFrame:
         """True if the last step fitted its arenas.  Otherwise the arenas are re-sized from this batch, the graph is re-captured and --
         with `retry` -- the step is run again (gradients of the overflowed step were those of an empty render: nothing accumulated).
         With sampler=: raises if loss_fn gave the error map a negative error since the last check."""
-        if self.sampler is not None and int(self.err_flag) != 0:
+        if self.sampler is not None and not self._lidar and int(self.err_flag) != 0:
             self.err_flag.zero_()
             raise RuntimeError("StaticFrame.check: loss_fn returned a negative per-ray error; the error map accumulates non-negative errors only")
         if int(self.cnt[CNT_SLOTS["overflow"]]) == 0:

@@ -9,6 +9,11 @@ fused, count-aware CUDA kernels (csrc/lidar_loss.cu) that read the renderer's bu
     frame = StaticFrame(model, n, loss_fn=lambda ret: sum(lidar_loss(None, ret).values()), loss_on_ret=True, with_rgb=False)
     lidar_loss.set_step(ranges, it)
     frame.step(rays_o, rays_d)
+    # the graph step that draws its own batch: the ranges come with the step's ground truth, the iteration's weights from set_step
+    frame = StaticFrame(model, n, loss_fn=lambda ret, gt: sum(lidar_loss(None, ret, ground_truth=gt).values()), loss_on_ret=True,
+                        with_rgb=False, sampler=LidarSampler(...))
+    lidar_loss.set_step(None, it)
+    frame.step(frame_ind=f)
 
 `ret["volume_buffer"]` is either the reference's exact-size `"packed"` dict or the capacity-sized `"packed_static"` dict of
 `StaticFrame(loss_on_ret=True)` (its sizes in the step's device count block).  The per-step values -- the ranges and the annealed weights
@@ -161,28 +166,43 @@ class LidarLoss(nn.Module):
         self.mask = None                   # [n_rays] the last step's validity mask (after the outlier discard)
 
     @torch.no_grad()
-    def set_step(self, ranges, it):
+    def set_step(self, ranges, it, device=None):
         """the step's ranges [n_rays] and iteration -> the static buffers the loss reads (device copies and fills: no host read).  Call it
-        before StaticFrame.step; the buffers keep their addresses, so a captured step follows them on replay."""
-        r = ranges.reshape(-1)
-        if self.ranges is None or self.ranges.shape != r.shape or self.ranges.device != r.device:
-            self.ranges = torch.empty(r.shape, dtype=torch.float32, device=r.device)
-            self._blk = torch.zeros(3, dtype=torch.float32, device=r.device)
-        self.ranges.copy_(r, non_blocking=True)
+        before StaticFrame.step; the buffers keep their addresses, so a captured step follows them on replay.  ranges None: the weights
+        of iteration `it` only (a step whose ranges come with its ground truth, StaticFrame(sampler=LidarSampler(...)); the weights are
+        made on `device`, default the current CUDA device, when no step set them before)."""
+        if ranges is not None:
+            r = ranges.reshape(-1)
+            if self.ranges is None or self.ranges.shape != r.shape or self.ranges.device != r.device:
+                self.ranges = torch.empty(r.shape, dtype=torch.float32, device=r.device)
+            if self._blk is None or self._blk.device != r.device:
+                self._blk = torch.zeros(3, dtype=torch.float32, device=r.device)
+            self.ranges.copy_(r, non_blocking=True)
+        elif self._blk is None:
+            self._blk = torch.zeros(3, dtype=torch.float32, device=device if device is not None else torch.device("cuda", torch.cuda.current_device()))
         d, s = self.depth_loss, self.line_of_sight_loss
         self._blk[0].fill_(d.weight(it) if d is not None else 0.0)
         self._blk[1].fill_(s.weight(it) if s is not None else 0.0)
         self._blk[2].fill_(s.epsilon(it) if s is not None else 0.0)
 
     def forward(self, scene, ret: dict, sample: dict = None, ground_truth: dict = None, *, it: int = None, far: float = None, logger=None):
-        """the reference's call; with ground_truth None the ranges and iteration of the last set_step are used (the graph step)"""
-        if ground_truth is not None:
+        """the reference's call; with ground_truth None the ranges and iteration of the last set_step are used (the graph step).  With
+        ground_truth and it None, once a set_step has run: ground_truth["ranges"] is read in place (a float32 device buffer the step
+        fills, StaticFrame(sampler=LidarSampler(...)).ground_truth) with the weights of the last set_step(None, it)."""
+        if ground_truth is not None and it is None and self._blk is not None:
+            ranges = ground_truth["ranges"].reshape(-1)
+            if ranges.dtype != torch.float32 or ranges.device != self._blk.device or not ranges.is_contiguous():
+                raise RuntimeError(f"LidarLoss: ground_truth['ranges'] read in place must be a contiguous float32 tensor on {self._blk.device}")
+        elif ground_truth is not None:
             self.set_step(ground_truth["ranges"], it)
+            ranges = self.ranges
         elif self.ranges is None:
             raise RuntimeError("LidarLoss: no ranges: pass ground_truth={'ranges': ...} or call set_step(ranges, it) before the step")
+        else:
+            ranges = self.ranges
         depth_pred, mask_pred = ret["rendered"]["depth_volume"], ret["rendered"]["mask_volume"]
-        if depth_pred.numel() != self.ranges.numel():
-            raise RuntimeError(f"LidarLoss: {depth_pred.numel()} rendered rays, {self.ranges.numel()} ranges")
+        if depth_pred.numel() != ranges.numel():
+            raise RuntimeError(f"LidarLoss: {depth_pred.numel()} rendered rays, {ranges.numel()} ranges")
         vw = t = pinfo = rih = count = None
         if self.line_of_sight_loss is not None:
             vb = ret["volume_buffer"]
@@ -198,7 +218,7 @@ class LidarLoss(nn.Module):
         cfg = (FN_TYPES[self.depth_loss.fn_type] if self.depth_loss is not None else None, float(self.mask_pred_thresh),
                float(self.discard_toofar) if self.discard_toofar is not None and self.discard_toofar > 0 else None,
                float(self.discard_outliers_median))
-        out, self.mask = _LidarLossFn.apply(cfg, depth_pred, vw, mask_pred, t, pinfo, rih, self.ranges, self._blk, count)
+        out, self.mask = _LidarLossFn.apply(cfg, depth_pred, vw, mask_pred, t, pinfo, rih, ranges, self._blk, count)
         losses = {}
         if self.depth_loss is not None:
             losses["lidar_loss.depth"] = out[0]
