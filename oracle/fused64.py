@@ -44,7 +44,8 @@ class Fused64:
     table: fp32 master or fp16 image of the LoTD parameters [P];  lotd_cfg: the LoTD configuration (dict of LoDMeta);
     W1 [width, 32], b1 [width], W2 [1, width], b2 [1];  R1 [rw, 54 + n_appear], rb1, R2 [rw, rw], rb2, R3 [3, rw], rb3 (optional);
     beta: softplus beta of the decoder;  fac [3]: sdf_scale / radius3d_original (the nablas scale, fp32 in the kernels);
-    max_level: highest LoTD level that contributes (None: all)."""
+    max_level: highest LoTD level that contributes (None: all).  h_cols: the columns of h in R1's input; the codes follow them."""
+    h_cols = H_COLS
 
     def __init__(self, table, lotd_cfg, W1, b1, W2, b2, R1=None, rb1=None, R2=None, rb2=None, R3=None, rb3=None, *, beta=100.0,
                  fac=(1.0, 1.0, 1.0), max_level=None, rounding=True):
@@ -208,7 +209,7 @@ class Fused64:
         gy = self.r16(self.r16(g_rgb) * ((1.0 - rgb) * rgb))
         dZ2 = self.r16((Y2 > 0) * (gy @ self.R3))
         dZ1 = self.r16((Y1 > 0) * (dZ2 @ self.R2))
-        dh_r = dZ1 @ self.R1[:, H_COLS]
+        dh_r = dZ1 @ self.R1[:, self.h_cols]
         out.update(R3=gy.T @ Y2, rb3=gy.sum(0), R2=dZ2.T @ Y1, rb2=dZ2.sum(0), R1=dZ1.T @ X, rb1=dZ1.sum(0))
         # decoder, first and second order
         h, J, lin, s, a16, u, g16 = fwd["h"], fwd["J"], fwd["lin"], fwd["s"], fwd["a16"], fwd["u"], fwd["g16"]

@@ -2,7 +2,8 @@
 
 The codes are the last n_appear columns of the radiance input X = [x | SH4(v) | n | h | h_appear], so with the radiance backward's
 rounding points of Fused64 (gy = r16(r16(g_rgb) (1-rgb) rgb);  dZ2 = r16([Y2>0] gy R3);  dZ1 = r16([Y1>0] dZ2 R2)) the gradient of a
-point's code is  dZ1 . R1[:, 54:]  (what k_color_rad_bwd<true> computes), and a ray's is the sum over its points (k_appear_ray_sum).
+point's code is  dZ1 . R1[:, h_cols.stop:]  (what k_color_rad_bwd<true> computes: R1[:, 54:] in the 16-level layout of Fused64, R1[:, 70:]
+in the 48-column layout of tests/fused64_wide.py), and a ray's is the sum over its points (k_appear_ray_sum).
 """
 import numpy as np
 
@@ -10,14 +11,15 @@ from oracle import neus64, step64
 
 
 def code_grad(ref, fwd, g_rgb):
-    """ref: oracle.fused64.Fused64 with n_appear >= 1; fwd: its color_forward; g_rgb [N, 3] -> d loss / d h_appear [N, n_appear]"""
+    """ref: oracle.fused64.Fused64 (or a subclass with its own h_cols) with n_appear >= 1; fwd: its color_forward; g_rgb [N, 3]
+    -> d loss / d h_appear [N, n_appear]"""
     assert ref.n_appear >= 1
     g = np.asarray(g_rgb, dtype=ref.f32).astype(np.float64)
     rgb, Y1, Y2 = fwd["rgb"], fwd["Y1"], fwd["Y2"]
     gy = ref.r16(ref.r16(g) * ((1.0 - rgb) * rgb))
     dZ2 = ref.r16((Y2 > 0) * (gy @ ref.R3))
     dZ1 = ref.r16((Y1 > 0) * (dZ2 @ ref.R2))
-    return dZ1 @ ref.R1[:, 54:]
+    return dZ1 @ ref.R1[:, ref.h_cols.stop:]
 
 
 def ray_sum(rows, ray, n_rays):

@@ -32,6 +32,8 @@ def ref_col_wide(k, n_appear, nh, hc=H_WIDE):
 
 
 class Fused64Wide(fused64.Fused64):
+    h_cols = H_COLS_WIDE
+
     def __init__(self, table, lotd_cfg, W1, b1, W2, b2, R1=None, rb1=None, R2=None, rb2=None, R3=None, rb3=None, **kw):
         nh = int(olotd.LoDMeta(3, **lotd_cfg).n_encoded_dims)
         assert 2 <= nh <= H_WIDE and nh % 2 == 0, nh
@@ -77,29 +79,4 @@ class Fused64Wide(fused64.Fused64):
         return self._unpad(super().sdf_backward(x, d_sdf))
 
     def color_backward(self, fwd, g_sdf=None, g_nablas=None, g_rgb=None):
-        """Fused64.color_backward in the 48-column layout.  The base class reads the h columns of R1 through its 32-column module constant,
-        so the method is restated here term for term with the 48 h columns (H_COLS_WIDE), the only difference."""
-        N = fwd["sdf"].shape[0]
-        f32 = lambda v, shape: np.zeros(shape) if v is None else np.asarray(v, dtype=self.f32).astype(np.float64)
-        g_sdf, g_nab, g_rgb = f32(g_sdf, (N,)), f32(g_nablas, (N, 3)), f32(g_rgb, (N, 3))
-        rgb, X, Y1, Y2 = fwd["rgb"], fwd["X"], fwd["Y1"], fwd["Y2"]
-        out = {}
-        # radiance net
-        gy = self.r16(self.r16(g_rgb) * ((1.0 - rgb) * rgb))
-        dZ2 = self.r16((Y2 > 0) * (gy @ self.R3))
-        dZ1 = self.r16((Y1 > 0) * (dZ2 @ self.R2))
-        dh_r = dZ1 @ self.R1[:, H_COLS_WIDE]
-        out.update(R3=gy.T @ Y2, rb3=gy.sum(0), R2=dZ2.T @ Y1, rb2=dZ2.sum(0), R1=dZ1.T @ X, rb1=dZ1.sum(0))
-        # decoder, first and second order
-        h, J, lin, s, a16, u, g16 = fwd["h"], fwd["J"], fwd["lin"], fwd["s"], fwd["a16"], fwd["u"], fwd["g16"]
-        w2, dsdf = self.W2[0], g_sdf[:, None]
-        gin = g_nab * self.fac * 0.5
-        dG = self.r16(np.einsum("nd,nfd->nf", gin, J))
-        dd = self.r16(dG @ self.W1.T)
-        curv = np.where(lin, 0.0, self.beta * s * (1.0 - s))
-        dz = self.r16(dd * w2 * curv + dsdf * w2 * s)
-        v = self.r16(dd * s + dsdf * a16)
-        dhz = dz @ self.W1
-        out.update(W1=dz.T @ h + u.T @ dG, b1=dz.sum(0), W2=v.sum(0)[None], b2=g_sdf.sum(0, keepdims=True))
-        out["grid"] = self._scatter(fwd["xs"], row_w=dhz + dh_r, row_dw=g16, gin=gin)
-        return self._unpad(out)
+        return self._unpad(super().color_backward(fwd, g_sdf, g_nablas, g_rgb))

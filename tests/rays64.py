@@ -4,13 +4,13 @@ The reference differentiates a sample x = o + d t of ray r with t a constant, vi
 input gradient first order (dy_dx is not differentiated).  With Fused64's rounding points that gives, per sample,
     g_x = 0.5 J^T h_hat + dZ1 . R1[:, 0:3]          g_v = (dSH4/dv)^T (dZ1 . R1[:, 3:19])
 with h_hat = dH = r16(d w2 s) . W1 for the SDF query (k_sdf_bwd_tc) and h_hat = dz . W1 + dZ1 . R1[:, h] for the colour query
-(k_color_sdf_bwd: its dz has the softplus'' term of the nablas cotangent), and per ray  dL/do = sum g_x, dL/dd = sum t g_x, dL/dv = sum g_v.
+(k_color_sdf_bwd: its dz has the softplus'' term of the nablas cotangent; h = ref.h_cols, 32 or 48 columns), and per ray  dL/do = sum g_x, dL/dd = sum t g_x, dL/dv = sum g_v.
 """
 import numpy as np
 import torch
 
 from appear64 import ray_sum
-from oracle import fused64, nets as onets
+from oracle import nets as onets
 
 
 def sh_vjp(v, dsh):
@@ -45,7 +45,7 @@ def color_rows(ref, fwd, view_dirs, g_sdf=None, g_nablas=None, g_rgb=None):
     g_x, g_v = np.zeros((N, 3)), np.zeros((N, 3))
     if g_rgb is not None:
         dZ1 = _radiance_dZ1(ref, fwd, g_rgb)
-        h_hat = h_hat + dZ1 @ ref.R1[:, fused64.H_COLS]
+        h_hat = h_hat + dZ1 @ ref.R1[:, ref.h_cols]
         g_x = dZ1 @ ref.R1[:, 0:3]
         g_v = sh_vjp(view_dirs, dZ1 @ ref.R1[:, 3:19])
     return g_x + 0.5 * np.einsum("nf,nfd->nd", h_hat, J), g_v

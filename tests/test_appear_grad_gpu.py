@@ -68,6 +68,7 @@ def _direct(model, inp, *, appear=True, cap_extra=0, ray_map=None):
     """nsb_fused_color_fwd + nsb_fused_color_bwd(_appear) on inp's samples.  cap_extra > 0: the capacity is that many samples larger
     than the device-resident count; the extra samples name ray R (a ray no counted sample names) and carry NaN cotangents"""
     from neuralsim_b200 import _lib as L
+    from neuralsim_b200.fields.fused_color import h_tile_cols
     from neuralsim_b200.graphics.neus_static import CNT_SLOTS, _call
     P = L.ptr
     n, R = inp["t"].shape[0], inp["R"]
@@ -80,10 +81,10 @@ def _direct(model, inp, *, appear=True, cap_extra=0, ray_map=None):
     t = cu(torch.cat([inp["t"], inp["t"][:cap_extra]]))
     cot = [cu(torch.cat([c, torch.full((cap_extra, *c.shape[1:]), float("nan"))])) for c in inp["cot"]]
     out = {k: torch.empty(m, *s, device="cuda") for k, s in (("sdf", ()), ("nab", (3,)), ("rgb", (3,)), ("x", (3,)))}
-    acts = torch.empty(4, int(L.lib().nsb_color_tile_bytes(L.c_i64(m))), dtype=torch.uint8, device="cuda")
+    acts = torch.empty(4, int(L.lib().nsb_color_act_bytes(L.c_i64(m), meta.n_pseudo_levels)), dtype=torch.uint8, device="cuda")
     ps = tk._params(model)
     grads = {k: torch.zeros(p.shape, dtype=torch.float32, device="cuda") for k, p in ps.items()}
-    dh = torch.full((m, 32), SENT, device="cuda")
+    dh = torch.full((m, h_tile_cols(meta.n_pseudo_levels)), SENT, device="cuda")
     rows = torch.full((m, 8), SENT, device="cuda")
     d_ha = torch.zeros(R + 1, ha.shape[1], device="cuda")
     d_ha[R] = SENT
@@ -116,11 +117,13 @@ def _model(n_appear):
     return _MODELS[n_appear]
 
 
-def _check_against_f64(model, inp, got, what):
+def _check_against_f64(model, inp, got, what, ref=None, fwd=None):
+    """ref: the float64 reference (default: Fused64 of the model), fwd: its colour forward on inp (computed when None)"""
     n, R, na = inp["t"].shape[0], inp["R"], inp["ha"].shape[1]
-    ref = fused64.Fused64.from_model(model)
+    ref = fused64.Fused64.from_model(model) if ref is None else ref
     ridx = inp["ridx"].numpy()
-    fwd = ref.color_forward(inp["x"].numpy(), inp["v"].numpy()[ridx], inp["ha"].numpy()[ridx])
+    if fwd is None:
+        fwd = ref.color_forward(inp["x"].numpy(), inp["v"].numpy()[ridx], inp["ha"].numpy()[ridx])
     want = code_grad(ref, fwd, inp["cot"][2].numpy())
     want_ray = ray_sum(want, ridx, R)
     rows = got["rows"].cpu().numpy()

@@ -58,7 +58,8 @@ def _launch(model, inp, rad, *, max_level=None, count=None, collect_res=(16, 16,
     out = dict(sdf=torch.full((n,), nan, device="cuda"), nablas=torch.full((n, 3), nan, device="cuda"), x=torch.full((n, 3), nan, device="cuda"))
     rgb = torch.full((n, 3), nan, device="cuda") if rad else None
     tb = int(lib.nsb_color_tile_bytes(L.c_i64(n)))
-    acts = torch.zeros(4 if rad else 2, max(tb, 1), dtype=torch.uint8, device="cuda")
+    acts = torch.zeros(4 if rad else 2, max(int(lib.nsb_color_act_bytes(L.c_i64(n), s.encoding.meta.n_pseudo_levels)), 1), dtype=torch.uint8,
+                       device="cuda")        # a saved X tile is 20 KB at more than 16 levels
     pcl = torch.zeros(int(np.prod(collect_res)), device="cuda")
     oc = L.OccCollectC(pcl.data_ptr(), (ctypes.c_int32 * 3)(*collect_res), 256.0)
     ap = [L.ptr(acts[k]) if k < acts.shape[0] else None for k in range(4)]
@@ -76,7 +77,7 @@ def _launch(model, inp, rad, *, max_level=None, count=None, collect_res=(16, 16,
     L.check(rc, "fused_color_fwd")
     torch.cuda.synchronize()
     out["Z"] = acts[0]
-    out["Xh"] = acts[1].view(-1, 16384)[:, :8192] if tb else acts[1][:0]       # per 16 KB tile: the four h chunks
+    out["Xh"] = acts[1][:tb].view(-1, 16384)[:, :8192] if tb else acts[1][:0]  # per 16 KB tile (up to 16 levels): the four h chunks
     out["collect"] = pcl
     return out
 

@@ -50,6 +50,7 @@ def _entry(model, inp, ml, *, cap_extra=0, rgb=True, sdf=False):
     """nsb_fused_color_fwd + nsb_fused_color_bwd_grads (sdf=False) or nsb_fused_sdf_bwd_rays (sdf=True) on inp's samples, with the
     device-resident count n and a capacity cap_extra larger (the extra samples name ray R and carry NaN cotangents)"""
     from neuralsim_b200 import _lib as L
+    from neuralsim_b200.fields.fused_color import h_tile_cols
     from neuralsim_b200.graphics.neus_static import CNT_SLOTS, _call
     P = L.ptr
     n, R = inp["t"].shape[0], inp["R"]
@@ -78,10 +79,10 @@ def _entry(model, inp, ml, *, cap_extra=0, rgb=True, sdf=False):
     else:
         grid16, net, _alive = model._fused_color_state() if rgb else model._fused_geometry_state()
         out = {k: torch.empty(m, *sh, device="cuda") for k, sh in (("sdf", ()), ("nab", (3,)), ("rgb", (3,)), ("x", (3,)))}
-        acts = torch.empty(4, int(L.lib().nsb_color_tile_bytes(L.c_i64(m))), dtype=torch.uint8, device="cuda")
+        acts = torch.empty(4, int(L.lib().nsb_color_act_bytes(L.c_i64(m), meta.n_pseudo_levels)), dtype=torch.uint8, device="cuda")
         ps = tk._params(model)
         grads = {k: torch.zeros(p.shape, dtype=torch.float32, device="cuda") for k, p in ps.items()}
-        dh = torch.empty(m, 32, device="cuda")
+        dh = torch.empty(m, h_tile_cols(meta.n_pseudo_levels), device="cuda")
         rows = torch.full((m, 36), SENT, device="cuda")
         fwd = (meta.c_ref, P(grid16, "f16"), ctypes.byref(net), None, P(o), P(d), P(ridx), P(t), P(v) if rgb else None, P(ha) if rgb else None,
                L.c_i64(m), L.c_i32(ml), P(out["sdf"]), P(out["nab"]), P(out["rgb"]) if rgb else None, P(out["x"]), P(acts[0]), P(acts[1]),

@@ -39,10 +39,10 @@ def _cfg(hashmap_size=None):
     return cfg
 
 
-def _model(cfg, seed):
+def _model(cfg, seed, **surface):
     from neuralsim_b200.fields.neus import LoTDNeuS
     gen = torch.Generator("cuda").manual_seed(seed)
-    model = LoTDNeuS(surface_cfg=dict(aabb=AABB, sdf_scale=SDF_SCALE, encoding_cfg=dict(lotd_cfg=cfg)),
+    model = LoTDNeuS(surface_cfg=dict(aabb=AABB, sdf_scale=SDF_SCALE, encoding_cfg=dict(lotd_cfg=cfg), **surface),
                      radiance_cfg=dict(n_appear_embedding=4), device="cuda", generator=gen)
     with torch.no_grad():
         model.implicit_surface.encoding.flattened_params.uniform_(-0.5, 0.5, generator=gen)
@@ -50,20 +50,26 @@ def _model(cfg, seed):
     return model
 
 
+def _lidar_beam(rng):
+    """a LiDAR beam (one of 64 elevations -17.6 .. 2.4 deg, random azimuth) from a sensor 2.2 m above z = -5.5 along the street
+    -> (o, d) in network space (world / radius, so t is in metres), the unit world direction, and the t where the beam leaves the box"""
+    elev = np.radians(rng.choice(np.linspace(-17.6, 2.4, 64)))
+    az = rng.uniform(0, 2 * np.pi)
+    dw = np.array([np.cos(elev) * np.sin(az), np.cos(elev) * np.cos(az), np.sin(elev)])
+    ow = np.array([rng.uniform(-3, 3), rng.uniform(-60, 60), -3.3])
+    o, d = ow / RADIUS, dw / RADIUS
+    with np.errstate(divide="ignore"):
+        a, b = (-0.995 - o) / d, (0.995 - o) / d
+    return o, d, dw, float(np.maximum(a, b).min())
+
+
 def _lidar_samples(n, seed):
-    """n samples of LiDAR beams (64 elevations -17.6 .. 2.4 deg, random azimuth) from sensors 2.2 m above z = -5.5 along the street, in
-    ray order with t ascending, 0.2 m apart, until the beam leaves the box.  Network space: x = o / radius + (d / radius) t, t in metres."""
+    """n samples of LiDAR beams (_lidar_beam) in ray order with t ascending, 0.2 m apart from 1 m on, until the beam leaves the box.
+    Network space: x = o / radius + (d / radius) t, t in metres."""
     rng = np.random.default_rng(seed)
     os_, ds, ts, total = [], [], [], 0
     while True:
-        elev = np.radians(rng.choice(np.linspace(-17.6, 2.4, 64)))
-        az = rng.uniform(0, 2 * np.pi)
-        dw = np.array([np.cos(elev) * np.sin(az), np.cos(elev) * np.cos(az), np.sin(elev)])
-        ow = np.array([rng.uniform(-3, 3), rng.uniform(-60, 60), -3.3])
-        o, d = ow / RADIUS, dw / RADIUS
-        with np.errstate(divide="ignore"):
-            a, b = (-0.995 - o) / d, (0.995 - o) / d
-        t1 = float(np.maximum(a, b).min())
+        o, d, _, t1 = _lidar_beam(rng)
         t = 1.0 + rng.uniform(0, 0.2) + 0.2 * np.arange(int((t1 - 1.0) / 0.2))
         if total + len(t) >= n:
             t = t[:n - total]

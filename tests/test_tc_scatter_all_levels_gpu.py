@@ -57,26 +57,32 @@ def census(x, cfg, order=None, active=None):
 
 
 # ===================================================================================================================== inputs
-def _cluster_rays(n, n_appear, seed):
-    """n samples of rays through the box in ray order, t ascending: 8..14 coarse samples over the ray's interval and, around a surface
-    point inside it, 33 samples within +-0.003 (the last up-sampling stage at inv_s 1024 places them so), then 0..3 more coarse samples.
-    No ray length is a multiple of 32; ~30 % of the sdf cotangents are zero (runs and isolated)."""
+def _box_beam(rng):
+    """a ray through the box from outside it -> (o, d, view direction, entry t, exit t)"""
+    d = rng.normal(size=3)
+    d /= np.linalg.norm(d)
+    o = rng.uniform(-0.6, 0.6, 3) - 2.5 * d
+    return (o, d, d, *ts._slab(o, d, 0.99))
+
+
+def _cluster_rays(n, n_appear, seed, beam=_box_beam, half=0.003):
+    """n samples of rays (beam(rng) -> o, d, view direction, entry and exit t) in ray order, t ascending: 8..14 coarse samples over the
+    ray's interval and, around a surface point inside it, 33 samples within +-half (the last up-sampling stage at inv_s 1024 places them
+    within +-0.003 in the unit box), then 0..3 more coarse samples.  No ray length is a multiple of 32; ~30 % of the sdf cotangents are
+    zero (runs and isolated)."""
     rng = np.random.default_rng(seed)
-    os_, ds, ts_, total = [], [], [], 0
+    os_, ds, vs, ts_, total = [], [], [], [], 0
     while total < n:
-        d = rng.normal(size=3)
-        d /= np.linalg.norm(d)
-        o = rng.uniform(-0.6, 0.6, 3) - 2.5 * d
-        t0, t1 = ts._slab(o, d, 0.99)
+        o, d, v, t0, t1 = beam(rng)
         s = rng.uniform(t0 + 0.2 * (t1 - t0), t1 - 0.3 * (t1 - t0))
-        near = np.sort(s + rng.uniform(-0.003, 0.003, 33))
+        near = np.sort(s + rng.uniform(-half, half, 33))
         a = np.linspace(t0, s - 0.01, rng.integers(8, 15))
         b = np.linspace(s + 0.01, t1, 4)[:rng.integers(0, 4)]
         t = np.concatenate([a, near, b])
         if len(t) % 32 == 0:
             t = t[1:]
         t = t[:n - total]
-        os_.append(o), ds.append(d), ts_.append(t)
+        os_.append(o), ds.append(d), vs.append(v), ts_.append(t)
         total += len(t)
     lens = np.array([len(t) for t in ts_])
     o = torch.tensor(np.stack(os_), dtype=torch.float32)
@@ -91,7 +97,8 @@ def _cluster_rays(n, n_appear, seed):
     zero = torch.rand(n, generator=g) < 0.1
     for s in np.flatnonzero(rng.random(n) < 0.025):
         zero[s:s + rng.integers(2, 17)] = True
-    return dict(x=x, o=o, d=d, t=t, ridx=ridx, v=d.clone(), ha=ha, cot=cot, zero=zero, perm=torch.from_numpy(rng.permutation(n)))
+    return dict(x=x, o=o, d=d, t=t, ridx=ridx, v=torch.tensor(np.stack(vs), dtype=torch.float32), ha=ha, cot=cot, zero=zero,
+                perm=torch.from_numpy(rng.permutation(n)))
 
 
 def _assert_merges_on(x, cfg, levels, what, zero=None):
@@ -203,21 +210,23 @@ def test_color_backward_clusters_order_invariant():
 
 
 # ===================================================================================================================== hand-built warps
-def _hand_layouts_level15():
-    """ts._hand_layouts with the run structures set on level 15 (2049 cells per axis).  Label j of structure k sits in level-15 cell
-    (200 + 1024 (1 - j % 2) + 3 (j // 2), 600 + j % 2, 700 + 3 k): labels 2 m and 2 m + 1 are cells (x + 1024, y) and (x, y + 1) with y
-    even, whose keys coincide when packed with 10 bits per axis, so a narrower key would merge lanes that must stay apart.  Lanes are
-    jittered by 1e-6 per lane (a level-15 cell is ~4.9e-4 wide in table space), so lanes share a level-15 cell exactly when they share a
-    label.  The nomerge layout interleaves filler lanes in cells far away on every level."""
+def _hand_layouts(cfg, level):
+    """ts._hand_layouts with the run structures set on `level` of the table `cfg` (level 15 of the bench table: 2049 cells per axis).
+    Label j of structure k sits in cell (200 + 1024 (1 - j % 2) + 3 (j // 2), 600 + j % 2, 700 + 3 k) of the level: labels 2 m and 2 m + 1
+    are cells (x + 1024, y) and (x, y + 1) with y even, whose keys coincide when packed with 10 bits per axis, so a narrower key would
+    merge lanes that must stay apart.  Lanes are jittered by 1e-6 per lane in table space (a level-15 cell is ~4.9e-4 wide), or by an
+    eighth of the smallest cell / 32 on a finer level, so lanes share a cell of the level exactly when they share a label.  The nomerge
+    layout interleaves filler lanes in cells far away on every level."""
     structs = ts._hand_structures()
     names = list(structs)
-    sc = np.float64(olotd.LoDMeta(3, **CFG).level_res_multidim[15][0] - 2)
+    sc = np.array(olotd.LoDMeta(3, **cfg).level_res_multidim[level], dtype=np.float64) - 2
+    jitter = min(1e-6, 0.125 / sc.max() / 32)
     pts, zero = [], []
     for k, name in enumerate(names):
         labels, zl = structs[name][:2]
         for lane, lab in enumerate(labels):
             cell = np.array([200 + 1024 * (1 - lab % 2) + 3 * (lab // 2), 600 + lab % 2, 700 + 3 * k])
-            xs = cell / sc + 1e-6 * lane
+            xs = cell / sc + jitter * lane
             pts.append(2 * xs - 1)
             zero.append(lane in zl)
     nh = len(pts)
@@ -235,24 +244,22 @@ def _hand_layouts_level15():
     return names, np.stack(pts).astype(np.float32), dict(merged=merged.ravel(), nomerge=nomerge.ravel()), np.array(zero)
 
 
-@pytest.mark.parametrize("kernel", ["sdf", "color"])
-def test_hand_built_warps_level15(kernel):
-    """one hand-built warp's cotangent at a time: the table gradient is that warp's sum, against float64 (per level) and against the
-    same 32 points in a layout where nothing merges"""
-    c = _case("cubic")
-    model, ref = c["model"], c["ref"]
-    names, x, orders, zero = _hand_layouts_level15()
+def hand_built_warps(model, ref, cfg, level, kernel, what):
+    """one hand-built warp's cotangent at a time (_hand_layouts(cfg, level)): the table gradient is that warp's sum, against float64 (per
+    level) and against the same 32 points in a layout where nothing merges"""
+    meta = olotd.LoDMeta(3, **cfg)
+    names, x, orders, zero = _hand_layouts(cfg, level)
     structs = ts._hand_structures()
     for k, name in enumerate(names):
         lanes = orders["merged"][k * 128:(k + 1) * 128]
-        heads = census(x, CFG, order=lanes, active=~zero[lanes] if kernel == "sdf" else None)["heads"][0]
+        heads = census(x, cfg, order=lanes, active=~zero[lanes] if kernel == "sdf" else None)["heads"][0]
         want = structs[name][2] if kernel == "sdf" else structs[name][3]
-        assert heads[15] == want, (name, heads[15], want)
-    nm = census(x, CFG, order=orders["nomerge"])["heads"].reshape(len(names), 4, -1)[:, :2]
+        assert heads[level] == want, (name, heads[level], want)
+    nm = census(x, cfg, order=orders["nomerge"])["heads"].reshape(len(names), 4, -1)[:, :2]
     assert (nm > MERGE_MAX_HEADS).all(), int(nm.min())
-    # the 32-heads warp: lanes 2 m and 2 m + 1 are different level-15 cells whose 10-bit-per-axis keys are equal
+    # the 32-heads warp: lanes 2 m and 2 m + 1 are different cells of the level whose 10-bit-per-axis keys are equal
     k32 = names.index("32_heads")
-    cell = merge_census(x, CFG, order=orders["merged"][k32 * 128:k32 * 128 + 32])["cells"][15].astype(np.int64)
+    cell = merge_census(x, cfg, order=orders["merged"][k32 * 128:k32 * 128 + 32])["cells"][level].astype(np.int64)
     packed10 = cell[:, 0] | (cell[:, 1] << 10) | (cell[:, 2] << 20)
     assert (cell[0::2] != cell[1::2]).any(1).all() and (packed10[0::2] == packed10[1::2]).all() and (cell[0::2, 0] >= 1024).all()
     g = torch.Generator().manual_seed(89)
@@ -287,10 +294,17 @@ def test_hand_built_warps_level15(kernel):
         else:
             want = ref.color_backward(ref.color_forward(x[rows], v_all.numpy()[rows], ha_all.numpy()[rows]), *(v.numpy()[rows] for v in cot))
             keys = tuple(tk.BWD_REL)
-        ts._compare(got["merged"], want, f"hand L15 {kernel} {name} vs f64", HAND_REL, {k_: tk.TILE_REL[k_] for k_ in keys}, fails=fails)
-        ts._compare(got["merged"], got["nomerge"], f"hand L15 {kernel} {name} vs nomerge", HAND_ORDER_LEVEL_REL, {k_: ORDER_REL for k_ in keys},
-                    fails=fails)
+        ts._compare(got["merged"], want, f"{what} {kernel} {name} vs f64", HAND_REL, {k_: tk.TILE_REL[k_] for k_ in keys}, fails=fails,
+                    meta=meta)
+        ts._compare(got["merged"], got["nomerge"], f"{what} {kernel} {name} vs nomerge", HAND_ORDER_LEVEL_REL, {k_: ORDER_REL for k_ in keys},
+                    fails=fails, meta=meta)
     assert not fails, fails
+
+
+@pytest.mark.parametrize("kernel", ["sdf", "color"])
+def test_hand_built_warps_level15(kernel):
+    c = _case("cubic")
+    hand_built_warps(c["model"], c["ref"], CFG, 15, kernel, "hand L15")
 
 
 # ===================================================================================================================== host rejection

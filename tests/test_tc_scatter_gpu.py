@@ -9,7 +9,8 @@ and tile boundaries), the same points shuffled (the no-merge reference), and han
 the merge (one run, 32 heads, 24 and 25 heads, a run that starts at lane 31, A A B A A keys, zero cotangents on a head and inside a
 run).  Every test asserts with tests/util.py:merge_census that its inputs do (or do not) exercise the merge, so an edit to the inputs
 cannot silently stop covering it.  The graph step's calls are covered too: nsb_fused_sdf_bwd_indexed over a device-built keep list,
-and the backward and colour kernels under a device-resident count smaller than their capacity.
+and the backward and colour kernels under a device-resident count smaller than their capacity (tests/test_wide_scatter_gpu.py runs the
+same bodies on the 17-level street table, the 48-column kernels).
 
 The table gradient is compared per level (a whole-table rel-L2 lets the dominant levels hide one level).  Bounds are about 3x the
 errors measured on an H100 80GB HBM3 (132 SMs, 700 W power limit); DESIGN.md §4 lists them."""
@@ -193,23 +194,23 @@ def _color_fwd(model, inp, perm=None):
 
 
 # ===================================================================================================================== comparisons
-def _level_slices(max_level=None):
-    top = META.n_levels - 1 if max_level is None else max_level
-    return [(l, slice(META.level_offsets[l], META.level_offsets[l + 1]), l <= top) for l in range(META.n_levels)]
+def _level_slices(max_level=None, meta=META):
+    top = meta.n_levels - 1 if max_level is None else max_level
+    return [(l, slice(meta.level_offsets[l], meta.level_offsets[l + 1]), l <= top) for l in range(meta.n_levels)]
 
 
 def _np(v):
     return v.detach().double().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v, dtype=np.float64)
 
 
-def _compare(got, want, what, level_bound, weight_bounds, max_level=None, fails=None):
-    """per-level rel-L2 of the table gradient (levels above max_level must be exactly zero in `got`) and rel-L2 of every other gradient.
-    Prints one METRIC line; appends failures to `fails` (asserts right away when it is None)."""
+def _compare(got, want, what, level_bound, weight_bounds, max_level=None, fails=None, meta=META):
+    """per-level rel-L2 of the table gradient of the table `meta` (levels above max_level must be exactly zero in `got`) and rel-L2 of
+    every other gradient.  Prints one METRIC line; appends failures to `fails` (asserts right away when it is None)."""
     own = fails is None
     fails = [] if own else fails
     g, w = _np(got["grid"]), _np(want["grid"])
     lv = {}
-    for l, sl, on in _level_slices(max_level):
+    for l, sl, on in _level_slices(max_level, meta):
         if on:
             if not np.abs(w[sl]).max() > 0:
                 fails.append((what, "level has no reference gradient", l))
@@ -467,14 +468,27 @@ def _count_block(slot, value):
     return cnt
 
 
+def _bench_graph_case():
+    """the graph-step calls' case on the bench table: the production model on its ray-ordered samples.  tests/test_wide_scatter_gpu.py
+    builds the same dict for the 17-level street table (the 48-column kernels)."""
+    c = _case(tk.PRODUCTION)
+    return dict(name="bench16", model=c["model"], inp=c["inp"], ref=c["ref"], cfg=CFG, meta=META, bwd_rel=tk.BWD_REL,
+                merge_levels=list(range(5)))
+
+
 def test_indexed_sdf_backward_keep_list_and_device_count():
     """nsb_fused_sdf_bwd_indexed as _StaticSDF.backward (graphics/neus_static.py) calls it: the samples with a non-zero cotangent
     compacted by nsb_flag_nonzero + a scan into a keep list; once with the count on the host, once with the count device-resident
     and the capacity larger.  Slots past the counts hold in-range indices of samples whose cotangent is NaN."""
+    indexed_sdf_backward_keep_list_and_device_count(_bench_graph_case())
+
+
+def indexed_sdf_backward_keep_list_and_device_count(c):
+    """the body of the test above for a case dict(name, model, inp, ref, cfg, meta, bwd_rel, merge_levels): merge_levels are the levels
+    on which the census of the kept samples must show the merge on most warps"""
     from neuralsim_b200 import _lib as L
     from neuralsim_b200.graphics.neus_static import CNT_SLOTS, _call, _scan
-    c = _case(tk.PRODUCTION)
-    model, inp, ref = c["model"], c["inp"], c["ref"]
+    name, model, inp, ref, meta = c["name"], c["model"], c["inp"], c["ref"], c["meta"]
     n, extra = inp["x"].shape[0], 1000
     cap = n + extra
     cot = _masked(inp["cot"], inp["zero"])[0]
@@ -491,24 +505,30 @@ def test_indexed_sdf_backward_keep_list_and_device_count():
     K = int(cnt[CNT_SLOTS["nonzero"]])
     kept = torch.nonzero(cot).flatten()
     assert K == kept.shape[0] and torch.equal(keep[:K].cpu(), kept)
-    c_k = merge_census(inp["x"].numpy(), CFG, order=kept.numpy())
-    assert (c_k["heads"][:, :5] <= MERGE_MAX_HEADS).mean() >= 0.5
+    c_k = merge_census(inp["x"].numpy(), c["cfg"], order=kept.numpy())
+    frac = (c_k["heads"] <= MERGE_MAX_HEADS).mean(0)
+    assert (frac[c["merge_levels"]] >= 0.5).all(), frac
     rays = (o, d, ridx_c, t_c)
     a = _sdf_bwd(model, None, d_c, rays=rays, keep=keep[:K].clone(), n=K)
-    _compare(a, ref.sdf_backward(inp["x"].numpy()[kept], cot.numpy()[kept]), "f64 sdf_bwd indexed", LEVEL_REL, tk.BWD_REL)
+    _compare(a, ref.sdf_backward(inp["x"].numpy()[kept], cot.numpy()[kept]), f"f64 sdf_bwd indexed {name}", LEVEL_REL, c["bwd_rel"], meta=meta)
     keep[K:] = n + torch.arange(cap - K, device="cuda") % extra          # in range; the samples they name carry NaN cotangents
     b = _sdf_bwd(model, None, d_c, rays=rays, keep=keep, n=cap, count=(cnt, CNT_SLOTS["nonzero"]))
     assert _all_finite(b)
-    _compare(b, a, "sdf_bwd indexed count-bound vs count-sized", ORDER_LEVEL_REL, {k: ORDER_REL for k in SDF_KEYS})
+    _compare(b, a, f"sdf_bwd indexed count-bound vs count-sized {name}", ORDER_LEVEL_REL, {k: ORDER_REL for k in SDF_KEYS}, meta=meta)
 
 
 def test_color_device_count():
     """nsb_fused_color_fwd / nsb_fused_color_bwd as _StaticColor calls them: capacity larger than the device-resident count; slots past
     the count hold in-range ray indices and NaN cotangents, and the outputs there must stay untouched"""
+    color_device_count(_bench_graph_case())
+
+
+def color_device_count(c):
+    """the body of the test above for a case dict as indexed_sdf_backward_keep_list_and_device_count takes it"""
     from neuralsim_b200 import _lib as L
+    from neuralsim_b200.fields.fused_color import h_tile_cols
     from neuralsim_b200.graphics.neus_static import CNT_SLOTS, _call
-    c = _case(tk.PRODUCTION)
-    model, inp = c["model"], c["inp"]
+    name, model, inp = c["name"], c["model"], c["inp"]
     n, extra = inp["x"].shape[0], 1000
     cap = n + extra
     P = L.ptr
@@ -528,12 +548,12 @@ def test_color_device_count():
     def run(m, count):
         out = dict(sdf=torch.full((m,), SENT, device="cuda"), nab=torch.full((m, 3), SENT, device="cuda"),
                    rgb=torch.full((m, 3), SENT, device="cuda"), x=torch.full((m, 3), SENT, device="cuda"))
-        acts = torch.empty(4, int(L.lib().nsb_color_tile_bytes(L.c_i64(m))), dtype=torch.uint8, device="cuda")
+        acts = torch.empty(4, int(L.lib().nsb_color_act_bytes(L.c_i64(m), meta.n_pseudo_levels)), dtype=torch.uint8, device="cuda")
         fwd = (meta.c_ref, P(grid16, "f16"), ctypes.byref(net), None, P(o, "f32"), P(d, "f32"), P(ridx_c, "i64"), P(t_c, "f32"), P(v, "f32"),
                P(ha, "f32"), L.c_i64(m), L.c_i32(model.implicit_surface._ml(None)), P(out["sdf"]), P(out["nab"]), P(out["rgb"]), P(out["x"]),
                *[P(acts[k]) for k in range(4)], None, L.stream_ptr())
         grads = {k: torch.zeros(p.shape, dtype=torch.float32, device="cuda") for k, p in ps.items()}
-        dh = torch.empty(m, 32, dtype=torch.float32, device="cuda")
+        dh = torch.empty(m, h_tile_cols(meta.n_pseudo_levels), dtype=torch.float32, device="cuda")
         cm = [x[:m].contiguous() for x in cot]
         bwd = (meta.c_ref, P(grid16, "f16"), ctypes.byref(net), None, P(o, "f32"), P(d, "f32"), P(ridx_c, "i64"), P(t_c, "f32"), L.c_i64(m),
                L.c_i32(model.implicit_surface._ml(None)), *[P(acts[k]) for k in range(4)], P(out["rgb"]), P(cm[0]), P(cm[1]), P(cm[2]), P(dh),
@@ -552,4 +572,4 @@ def test_color_device_count():
         assert bool((b_out[k][n:] == SENT).all()), k
     assert torch.equal(a_out["x"].cpu(), inp["x"])
     assert _all_finite(b)
-    _compare(b, a, "color_bwd count-bound vs count-sized", ORDER_LEVEL_REL, {k: ORDER_REL for k in tk.BWD_REL})
+    _compare(b, a, f"color_bwd count-bound vs count-sized {name}", ORDER_LEVEL_REL, {k: ORDER_REL for k in tk.BWD_REL}, meta=c["meta"])
