@@ -65,10 +65,11 @@ class Fused64:
     def from_model(cls, model, max_level=None, rounding=True):
         """From a product LoTDNeuS (fields/neus.py): the parameters as the fused kernels see them."""
         s = model.implicit_surface
-        d, r = s.decoder.layers, model.radiance_net.blocks.layers
+        d = s.decoder.layers
+        # a geometry-only model (radiance_cfg=False) has no radiance net: sdf and nablas only
+        r = [None] * 6 if model.radiance_net is None else [p for l in model.radiance_net.blocks.layers for p in (l.weight, l.bias)]
         fac = (s.sdf_scale / s.radius3d_original.detach().float().cpu()).tolist()
-        return cls(s.encoding.flattened_params, s.encoding.lotd_cfg, d[0].weight, d[0].bias, d[1].weight, d[1].bias,
-                   r[0].weight, r[0].bias, r[1].weight, r[1].bias, r[2].weight, r[2].bias,
+        return cls(s.encoding.flattened_params, s.encoding.lotd_cfg, d[0].weight, d[0].bias, d[1].weight, d[1].bias, *r,
                    beta=float(d[0].activation.beta), fac=fac, max_level=max_level, rounding=rounding)
 
     @property
@@ -161,10 +162,11 @@ class Fused64:
         z, lin, s, a16, sdf = self._decoder(h)
         return (sdf, self.sdf_scale(a16)) if with_scale else sdf
 
-    def color_forward(self, x, view_dirs, h_appear=None):
+    def color_forward(self, x, view_dirs, h_appear=None, with_rgb=True):
         """k_color_fwd at the points x [N, 3] with per-point view directions [N, 3] and appearance codes [N, n_appear].
         -> dict(sdf, nablas, rgb; sdf_scale (see sdf_scale); nablas_scale = 0.5 fac sum |r16(g) J| per point and axis, the
-        scale of the nablas rounding error; and the intermediates the backward passes use)."""
+        scale of the nablas rounding error; and the intermediates the backward passes use).  with_rgb=False (or no radiance net):
+        the geometry-only query k_color_fwd<false>, sdf and nablas; rgb is None and no radiance input is formed."""
         x = np.asarray(x, dtype=np.float32)
         xs = self.xs_of(x)
         h, J = self.features(xs)
@@ -173,6 +175,10 @@ class Fused64:
         g16 = self.r16(u @ self.W1)
         nab = np.einsum("nf,nfd->nd", g16, J) * 0.5 * self.fac
         nab_scale = np.einsum("nf,nfd->nd", np.abs(g16), np.abs(J)) * 0.5 * self.fac
+        out = dict(sdf=sdf, nablas=nab, rgb=None, sdf_scale=self.sdf_scale(a16), nablas_scale=nab_scale, xs=xs, h=h, J=J, z=z, lin=lin,
+                   s=s, a16=a16, u=u, g16=g16)
+        if not with_rgb or self.R1 is None:
+            return out
         v = torch.as_tensor(np.asarray(view_dirs), dtype=torch.float32 if self.rounding else torch.float64)
         sh = onets.sh_encode(v, 4).double().numpy()
         parts = [x.astype(np.float64), sh, np.clip(nab, -1.0, 1.0), h]
@@ -182,8 +188,8 @@ class Fused64:
         Y1 = np.maximum(self.r16(X @ self.R1.T + self.rb1), 0.0)
         Y2 = np.maximum(self.r16(Y1 @ self.R2.T + self.rb2), 0.0)
         rgb = self.r16(_sigmoid(self.r16(Y2 @ self.R3.T + self.rb3)))
-        return dict(sdf=sdf, nablas=nab, rgb=rgb, sdf_scale=self.sdf_scale(a16), nablas_scale=nab_scale, xs=xs, h=h, J=J, z=z, lin=lin,
-                    s=s, a16=a16, u=u, g16=g16, X=X, Y1=Y1, Y2=Y2)
+        out.update(rgb=rgb, X=X, Y1=Y1, Y2=Y2)
+        return out
 
     # ------------------------------------------------------------------ backward passes
     def sdf_backward(self, x, d_sdf):
@@ -199,18 +205,26 @@ class Fused64:
 
     def color_backward(self, fwd, g_sdf=None, g_nablas=None, g_rgb=None):
         """k_color_rad_bwd + k_color_sdf_bwd: gradients of sum(g_sdf sdf + g_nablas nablas + g_rgb rgb) through the forward
-        `fwd` (color_forward) -> dict(grid [P], W1, b1, W2, b2, R1, rb1, R2, rb2, R3, rb3), float64"""
+        `fwd` (color_forward) -> dict(grid [P], W1, b1, W2, b2, R1, rb1, R2, rb2, R3, rb3), float64.  A geometry-only forward
+        (rgb None) takes no g_rgb: the radiance net's gradients are exact zeros (absent without a radiance net)."""
         N = fwd["sdf"].shape[0]
         f32 = lambda v, shape: np.zeros(shape) if v is None else np.asarray(v, dtype=self.f32).astype(np.float64)
-        g_sdf, g_nab, g_rgb = f32(g_sdf, (N,)), f32(g_nablas, (N, 3)), f32(g_rgb, (N, 3))
-        rgb, X, Y1, Y2 = fwd["rgb"], fwd["X"], fwd["Y1"], fwd["Y2"]
+        g_sdf, g_nab = f32(g_sdf, (N,)), f32(g_nablas, (N, 3))
         out = {}
-        # radiance net
-        gy = self.r16(self.r16(g_rgb) * ((1.0 - rgb) * rgb))
-        dZ2 = self.r16((Y2 > 0) * (gy @ self.R3))
-        dZ1 = self.r16((Y1 > 0) * (dZ2 @ self.R2))
-        dh_r = dZ1 @ self.R1[:, self.h_cols]
-        out.update(R3=gy.T @ Y2, rb3=gy.sum(0), R2=dZ2.T @ Y1, rb2=dZ2.sum(0), R1=dZ1.T @ X, rb1=dZ1.sum(0))
+        if fwd["rgb"] is None:
+            assert g_rgb is None, "a geometry-only forward has no rgb"
+            dh_r = 0.0
+            if self.R1 is not None:
+                out.update({k: np.zeros(getattr(self, k).shape) for k in ("R1", "rb1", "R2", "rb2", "R3", "rb3")})
+        else:
+            g_rgb = f32(g_rgb, (N, 3))
+            rgb, X, Y1, Y2 = fwd["rgb"], fwd["X"], fwd["Y1"], fwd["Y2"]
+            # radiance net
+            gy = self.r16(self.r16(g_rgb) * ((1.0 - rgb) * rgb))
+            dZ2 = self.r16((Y2 > 0) * (gy @ self.R3))
+            dZ1 = self.r16((Y1 > 0) * (dZ2 @ self.R2))
+            dh_r = dZ1 @ self.R1[:, self.h_cols]
+            out.update(R3=gy.T @ Y2, rb3=gy.sum(0), R2=dZ2.T @ Y1, rb2=dZ2.sum(0), R1=dZ1.T @ X, rb1=dZ1.sum(0))
         # decoder, first and second order
         h, J, lin, s, a16, u, g16 = fwd["h"], fwd["J"], fwd["lin"], fwd["s"], fwd["a16"], fwd["u"], fwd["g16"]
         w2, dsdf = self.W2[0], g_sdf[:, None]
