@@ -568,6 +568,30 @@ int nsb_lidar_los_backward(const float *t, const float *vw, const int64_t *pack_
 int nsb_occ_ema_update(const float *pts, const float *val, int64_t n, int32_t val_is_sdf, float inv_s, int32_t rx, int32_t ry, int32_t rz,
                        float *pcl_or_null, float *occ_val_grid, uint8_t *occ_grid, uint32_t *occ_bits_or_null, float ema_decay, float occ_thre,
                        float *scratch_cells, void *stream);
+/* nsb_occ_ema_update over the first *n_dev of n_capacity points (a device-resident count); with skip_or_null pointing at a non-zero
+ * int64 the update changes nothing (neither grid nor pcl). */
+int nsb_occ_ema_update_count(const float *pts, const float *val, const int64_t *n_dev, int64_t n_capacity, int32_t val_is_sdf, float inv_s,
+                             int32_t rx, int32_t ry, int32_t rz, float *pcl_or_null, float *occ_val_grid, uint8_t *occ_grid,
+                             uint32_t *occ_bits_or_null, float ema_decay, float occ_thre, float *scratch_cells, const int64_t *skip_or_null,
+                             void *stream);
+
+/* ---------------------------------------------------------------- the grid's update from the network (csrc/occ_update.cu)
+ * OccGridEma._step (ema_single.py:133-175) and sample_pts_in_voxels (occgrid/utils.py:17-41) without a host read.
+ * nsb_occ_voxel_lists: the occupied and the empty cells of occ_grid[cells] (bool bytes) as flat indices (row-major, last axis fastest:
+ *   nonzero()'s order) in occupied[cells] / empty[cells]; counts[0] = occupied cells, counts[1] = empty cells (device).  flags, first:
+ *   int32 [cells] scratch; workspace: nsb_scan_workspace_bytes() of device memory (zeroed here).  One scan (nsb_scan_counts).
+ * nsb_occ_draw_pts: the points of one update's num_steps iterations, in the reference's order, drawn from torch's CUDA generator at
+ *   (rng[0] seed, rng[1] offset): per iteration, with *warmup != 0, num_pts points in all cells; else num_pts / 2 in all cells,
+ *   num_pts / 4 in the empty cells (none if there are none) and num_pts / 4 in the occupied cells (the voxel lists above).  Each part is
+ *   sample_pts_in_voxels's torch.randint + torch.rand (n < 2 nv) or torch.rand of nv (n / nv + 1) points, each draw at the offset the
+ *   previous one's left, the values and fp32 roundings torch gives.  pts[capacity, 3]; out[0] = the points drawn, out[1] = 1 when the
+ *   steady phase found no occupied cell (then nothing is drawn: the reference asserts), else 0.  capacity >= num_steps times the
+ *   larger phase's sum over its parts of n + min(cells, n / 2) (a part of n points draws at most that many). */
+int nsb_occ_voxel_lists(const uint8_t *occ_grid, int64_t cells, int32_t *flags, int32_t *first, int64_t *occupied, int64_t *empty,
+                        int64_t *counts, void *workspace, void *stream);
+int nsb_occ_draw_pts(const int64_t *rng, const int32_t *warmup, const int64_t *counts, const int64_t *occupied, const int64_t *empty,
+                     int32_t rx, int32_t ry, int32_t rz, int32_t num_steps, int64_t num_pts, int64_t capacity, float *pts, int64_t *out,
+                     void *stream);
 
 /* ---------------------------------------------------------------- fused colour / normal query (csrc/color_tc.cu)
  * The whole LoTDNeuS.forward of the reference for packed samples (nr3d_lib/models/fields/neus/lotd_neus.py:141-167 =

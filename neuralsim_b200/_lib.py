@@ -79,6 +79,11 @@ def lib():
         _lib.nsb_fused_sdf_bwd_rays.argtypes = [vp] * 9 + [i64, i32] + [vp] * 9 + [vp]
         # the adjoint of the ray test's normalisation and gather (count-aware): idx, n, radius3 (host float[3]), 6 pointers, stream
         _lib.nsb_gather_rays_backward.argtypes = [vp, i64] + [vp] * 7 + [vp]
+        # the occupancy grid's update from the network (csrc/occ_update.cu, csrc/occ_ema.cu)
+        f32 = ctypes.c_float
+        _lib.nsb_occ_voxel_lists.argtypes = [vp, i64] + [vp] * 7
+        _lib.nsb_occ_draw_pts.argtypes = [vp] * 5 + [i32] * 4 + [i64, i64, vp, vp, vp]
+        _lib.nsb_occ_ema_update_count.argtypes = [vp, vp, vp, i64, i32, f32, i32, i32, i32, vp, vp, vp, vp, f32, f32, vp, vp, vp]
     return _lib
 
 

@@ -17,7 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "_build")
 LIB = os.path.join(HERE, "libneuralsim_b200.so")
-SOURCES = ["common.cu", "lotd.cu", "march.cu", "pack_ops.cu", "sh.cu", "fused.cu", "fused_tc.cu", "neus_fused.cu", "neus_glue.cu", "color_tc.cu", "ray_upsample.cu", "occ_ema.cu", "mesh.cu", "lidar_loss.cu", "pose.cu", "perturb.cu", "importance.cu", "lidar_sample.cu"]
+SOURCES = ["common.cu", "lotd.cu", "march.cu", "pack_ops.cu", "sh.cu", "fused.cu", "fused_tc.cu", "neus_fused.cu", "neus_glue.cu", "color_tc.cu", "ray_upsample.cu", "occ_ema.cu", "mesh.cu", "lidar_loss.cu", "pose.cu", "perturb.cu", "importance.cu", "lidar_sample.cu", "occ_update.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = [*ARCH, "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",

@@ -31,7 +31,8 @@ __global__ void __launch_bounds__(256) k_occ_fill(float *__restrict__ ev, int64_
 // pts [n,3] in [-1,1]^3 (network space), val [n]: sdf (is_sdf) or ready-made evidence >= 0
 __global__ void __launch_bounds__(256)
 k_occ_scatter(const float *__restrict__ pts, const float *__restrict__ val, int64_t n, int rx, int ry, int rz, float inv_s, int is_sdf,
-              float *__restrict__ ev) {
+              float *__restrict__ ev, const int64_t *__restrict__ n_dev) {
+    n = eff_n(n, n_dev);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const float ux = __fadd_rn(__fmul_rn(pts[i * 3], 0.5f), 0.5f), uy = __fadd_rn(__fmul_rn(pts[i * 3 + 1], 0.5f), 0.5f),
                     uz = __fadd_rn(__fmul_rn(pts[i * 3 + 2], 0.5f), 0.5f);
@@ -46,7 +47,8 @@ k_occ_scatter(const float *__restrict__ pts, const float *__restrict__ val, int6
 
 __global__ void __launch_bounds__(256)
 k_occ_finalize(float *__restrict__ ev, float *__restrict__ pcl, float *__restrict__ grid, uint8_t *__restrict__ occ, uint32_t *__restrict__ bits,
-               int64_t cells, float decay, float thre) {
+               int64_t cells, float decay, float thre, const int64_t *__restrict__ skip) {
+    if (skip && *skip) return;                                 // an update that drew nothing changes nothing, the collected evidence included
     for (int64_t c0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) & ~31ll; c0 < cells; c0 += (int64_t)gridDim.x * blockDim.x) {
         const int64_t c = c0 + (threadIdx.x & 31);
         bool o = false;
@@ -81,9 +83,30 @@ extern "C" int nsb_occ_ema_update(const float *pts, const float *val, int64_t n,
     k_occ_fill<<<wave_grid(cells, 256, 8), 256, 0, s>>>(scratch_cells, cells);
     if (int rc = check_launch("nsb_occ_ema_update(fill)")) return rc;
     if (n > 0) {
-        k_occ_scatter<<<wave_grid(n, 256, 8), 256, 0, s>>>(pts, val, n, rx, ry, rz, inv_s, val_is_sdf, scratch_cells);
+        k_occ_scatter<<<wave_grid(n, 256, 8), 256, 0, s>>>(pts, val, n, rx, ry, rz, inv_s, val_is_sdf, scratch_cells, nullptr);
         if (int rc = check_launch("nsb_occ_ema_update(scatter)")) return rc;
     }
-    k_occ_finalize<<<wave_grid(cells, 256, 8), 256, 0, s>>>(scratch_cells, pcl_or_null, occ_val_grid, occ_grid, occ_bits_or_null, cells, ema_decay, occ_thre);
+    k_occ_finalize<<<wave_grid(cells, 256, 8), 256, 0, s>>>(scratch_cells, pcl_or_null, occ_val_grid, occ_grid, occ_bits_or_null, cells, ema_decay, occ_thre,
+                                                            nullptr);
     return check_launch("nsb_occ_ema_update(finalize)");
+}
+
+extern "C" int nsb_occ_ema_update_count(const float *pts, const float *val, const int64_t *n_dev, int64_t n_capacity, int32_t val_is_sdf, float inv_s,
+                                        int32_t rx, int32_t ry, int32_t rz, float *pcl_or_null, float *occ_val_grid, uint8_t *occ_grid,
+                                        uint32_t *occ_bits_or_null, float ema_decay, float occ_thre, float *scratch_cells, const int64_t *skip_or_null,
+                                        void *stream) {
+    NSB_REQUIRE(occ_val_grid && occ_grid && scratch_cells && n_dev, "nsb_occ_ema_update_count: NULL grid or count");
+    NSB_REQUIRE(rx > 0 && ry > 0 && rz > 0, "nsb_occ_ema_update_count: bad resolution");
+    NSB_REQUIRE(n_capacity == 0 || (pts && val), "nsb_occ_ema_update_count: NULL points");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int64_t cells = (int64_t)rx * ry * rz;
+    k_occ_fill<<<wave_grid(cells, 256, 8), 256, 0, s>>>(scratch_cells, cells);
+    if (int rc = check_launch("nsb_occ_ema_update_count(fill)")) return rc;
+    if (n_capacity > 0) {
+        k_occ_scatter<<<wave_grid(n_capacity, 256, 8), 256, 0, s>>>(pts, val, n_capacity, rx, ry, rz, inv_s, val_is_sdf, scratch_cells, n_dev);
+        if (int rc = check_launch("nsb_occ_ema_update_count(scatter)")) return rc;
+    }
+    k_occ_finalize<<<wave_grid(cells, 256, 8), 256, 0, s>>>(scratch_cells, pcl_or_null, occ_val_grid, occ_grid, occ_bits_or_null, cells, ema_decay, occ_thre,
+                                                            skip_or_null);
+    return check_launch("nsb_occ_ema_update_count(finalize)");
 }

@@ -4,3 +4,4 @@ from .networks import MLP, DenseLayer, LoTDSDF, RadianceNet, SHEncoder, VarSingl
 from .accel import OccGridAccel, OccGridEma  # noqa: F401
 from .space import AABBSpace  # noqa: F401
 from .neus import LoTDNeuS, LoTDNeuSModel  # noqa: F401
+from .occ_update import OccGridUpdate  # noqa: F401

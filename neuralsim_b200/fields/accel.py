@@ -56,6 +56,7 @@ class OccGridEma(nn.Module):
         self.n_steps_between_update, self.n_steps_warmup = n_steps_between_update, n_steps_warmup
         if self.should_collect_samples:
             self.register_buffer("_occ_val_grid_pcl", torch.zeros(res.tolist(), dtype=dtype, device=device), persistent=False)
+        self.net_update = None          # an attached fields/occ_update.py:OccGridUpdate runs step()'s update as one graph replay
 
     def occ_val_fn(self, sdf):
         # the model's sdf is fp16-valued (autocast decoder): evaluate like the reference does on its half tensor, then widen
@@ -143,6 +144,10 @@ class OccGridEma(nn.Module):
 
     @torch.no_grad()
     def step(self, cur_it, val_query_fn, logger=None, generator=None):
+        if self.net_update is not None:
+            if generator is not None:
+                raise RuntimeError("OccGridEma.step: the attached OccGridUpdate draws from its own generator; pass it to OccGridUpdate(generator=...)")
+            return self.net_update.step(cur_it, val_query_fn)
         assert bool(self.is_initialized), "init() first"
         if cur_it <= 0 or cur_it % self.n_steps_between_update != 0:
             return False
