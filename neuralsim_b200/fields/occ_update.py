@@ -4,14 +4,13 @@ The host-sized step (fields/accel.py:OccGridEma.step, the reference's ema_single
 back with nonzero() -- a synchronisation that drains every graph step queued before it -- and sizes its draws and queries from them.  Here
 one replay builds both lists on the device, draws the num_steps iterations' points from torch's CUDA generator (the values
 sample_pts_in_voxels draws from the same state), queries the SDF with the fused kernel at the model's device level bound and runs the EMA
-over the device count of points.  The generator contract is the perturbed step's (graphics/perturb.py): before each replay, `take` writes
-(seed, offset) into a device block and advances the generator by `reservation(...)`, a bound on what an update can draw."""
+over the device count of points, with torch_rng.py's generator contract: `reservation(...)` bounds what an update can draw."""
 from __future__ import annotations
 
 import torch
 
 from .. import _lib as L
-from ..graphics import perturb as PT
+from .. import torch_rng as TR
 from .accel import OccGridEma, OccGridEmaBatched
 from .networks import sdf_fwd
 
@@ -41,8 +40,8 @@ def reservation(cells: int, num_steps: int, num_pts: int, cap: int) -> int:
     part_points(n, cells); inc() is monotone in N, so the larger of the two branches' bounds bounds the part whatever nv is.  Refuses a draw
     of 2^31 or more values."""
     def part(n):
-        return max(PT.uniform_inc(n, cap) + PT.uniform_inc(3 * n, cap), PT.uniform_inc(3 * part_points(n, cells), cap))
-    PT._check_draw(3 * part_points(int(num_pts), cells), "occupancy update")
+        return max(TR.uniform_inc(n, cap) + TR.uniform_inc(3 * n, cap), TR.uniform_inc(3 * part_points(n, cells), cap))
+    TR.check_draw(3 * part_points(int(num_pts), cells), "the occupancy update")
     return int(num_steps) * max(sum(part(n) for n in ph) for ph in _phases(int(num_pts)))
 
 
@@ -76,10 +75,8 @@ class OccGridUpdate:
     Both phases (warm-up: it < n_steps_warmup; steady) come from the one capture: a device scalar holds the phase.  `occ_grid` and
     `occ_val_grid` are updated in place, so a captured StaticFrame step sees the new grid.
 
-    Random state: before each replay the generator's (initial_seed(), get_offset()) goes to a device block and the generator advances by
-    `self.reservation` (graphics/perturb.py:take).  From the same generator state the replay draws exactly the host-sized update's points,
-    so it leaves the same grids; the host-sized update advances the generator by what it drew, this one by the reservation, so the two
-    drift apart after the first update (StaticFrame(perturb=True)'s contract).
+    Random state: torch_rng.take before each replay, with `self.reservation`; from the same generator state the replay draws exactly the
+    host-sized update's points, so it leaves the same grids (runs of the two drift apart: torch_rng.py).
 
     If the steady phase finds no occupied voxel the update changes nothing and records it; `check()` (one device-to-host read) then raises the
     reference's error.  The update's size (`update_from_net_cfg`, the grid's resolution) is read when the object is made.  Memory: an arena
@@ -100,12 +97,12 @@ class OccGridUpdate:
             raise RuntimeError("OccGridUpdate: the grid must be a contiguous 3-D CUDA grid with a float32 occ_val_grid")
         self.model, self.occ = model, occ
         dev = g.device
-        self.gen = PT.cuda_generator(generator, dev)
+        self.gen = TR.cuda_generator(generator, dev)
         cfg = occ.update_from_net_cfg
         self.num_steps, self.num_pts = int(cfg.get("num_steps", 4)), int(cfg.get("num_pts", 2 ** 18))       # OccGridEma.step's defaults
         self.res = [int(r) for r in g.shape]
         cells = g.numel()
-        self.reservation = reservation(cells, self.num_steps, self.num_pts, PT.grid_cap(dev))
+        self.reservation = reservation(cells, self.num_steps, self.num_pts, TR.grid_cap(dev))
         self.capacity = capacity(cells, self.num_steps, self.num_pts)
         i64 = dict(dtype=torch.int64, device=dev)
         self.rng = torch.zeros(2, **i64)
@@ -148,7 +145,7 @@ class OccGridUpdate:
             raise RuntimeError("OccGridUpdate: init() the occupancy grid first")
         self.model._nablas_fac()             # _fp16_images reads it; its first call reads the device, which a capture must not do
         saved = [t.clone() if t is not None else None for t in self._targets()]
-        PT.take(self.gen, 0, self.rng)
+        TR.take(self.gen, 0, self.rng)
         self._run()
         for t, s in zip(self._targets(), saved):
             if t is not None:
@@ -176,7 +173,7 @@ class OccGridUpdate:
             self.graph = None                                        # a grid buffer was re-assigned (set_occ_grid): capture again
         if self.graph is None:
             self.capture()
-        PT.take(self.gen, self.reservation, self.rng)
+        TR.take(self.gen, self.reservation, self.rng)
         self.graph.replay()
         return True
 

@@ -27,6 +27,8 @@ from .neus import query_config, upsample_boundary
 from .raysample import batch_sample_step_linear
 from . import neus_fused as NF
 from . import perturb as PT
+from .pose import FramePose
+from .. import torch_rng as TR
 
 __all__ = ["render_static", "StaticFrame", "CNT_SLOTS", "static_volume_buffer"]
 
@@ -209,9 +211,9 @@ def render_static(model, rays_o, rays_d, rays_h_appear=None, *, near=None, far=N
     if perturb:
         if ((model.ray_query_cfg.get("query_param", {}) or {}).get("march_cfg", {}) or {}).get("perturb_before_march", False):
             raise RuntimeError("render_static(perturb=True): march_cfg.perturb_before_march=True is not built; use the host-sized path")
-        reserve = PT.reservation(R, cfg, PT.grid_cap(dev))
+        reserve = PT.reservation(R, cfg, TR.grid_cap(dev))
         if rng_dev is None:
-            rng_dev = PT.take(PT.cuda_generator(None, dev), reserve)
+            rng_dev = TR.take(TR.cuda_generator(None, dev), reserve)
         draws_coarse, draws_stage = PT.step_draws(CNT_SLOTS, nc1, cfg.num_fine)
     if cnt is None:
         cnt = torch.zeros(32, dtype=torch.int64, device=dev)
@@ -438,32 +440,16 @@ class StaticFrame:
 
     `perturb=True` (off by default) trains with stratified samples, as the shipped StreetSurf configs do (`renderer.train.perturb`): the
     graph draws the coarse depths and the up-sampling quantiles in its kernels from torch's CUDA generator (`generator`, else the default
-    one of the model's device; graphics/perturb.py).  `step()` writes the generator's (initial_seed(), get_offset()) into the device block
-    `frame.rng` and then advances the generator by `frame.rng_reservation` with set_offset -- host-side calls, no synchronisation.  From the
-    same generator state a replay draws exactly what the host-sized perturbed step draws, so its images, loss and gradients are that
-    step's.  The one difference: the host-sized step advances the generator by the sum of its draws (which depend on the batch), the graph
-    step by the fixed reservation that bounds them, so a run of graph steps and a run of host-sized steps drift apart after the first step.
-    `check()`'s retry replays the same draw.
+    one of the model's device; graphics/perturb.py).  `step()` writes the generator's state into the device block `frame.rng` and advances
+    it by `frame.rng_reservation` (torch_rng.take: no synchronisation), so a replay draws exactly what the host-sized perturbed step draws
+    from the same state, and its images, loss and gradients are that step's; runs of the two drift apart (torch_rng.py).  `check()`'s
+    retry replays the same draw.
 
-    `sampler=CameraSampler(...)` (neuralsim_b200/importance.py; off by default; needs pose= and a loss_fn) draws every batch inside the
-    graph, as the shipped camera configs' ImpSampler.sample_img_pixel does over each camera's error map: `frame.step(cam=k)` fills a
-    device camera index and the generator block (the sampler's four draws come first, the perturbed ones after them), and the one replay
-    samples frames and pixels (nsb_imp_sample), gathers the ground truth into `frame.ground_truth` (a dict of [n_rays, ...] rows), writes
-    `frame.rays_fidx`, `frame.rays_pix`, the pose indices, the camera-space directions and the appearance codes, renders, calls
-    `loss, err = loss_fn(rendered_or_ret, frame.ground_truth)`, runs the backward and adds err [n_rays] (the per-ray rgb error the
-    reference feeds its error map) into camera k's error map (nsb_error_map_update).  After the replay, on the host, camera k's step
-    counter advances and its cdfs are rebuilt in place when the reference would (ErrorMap.count_step).  A negative error is recorded in a
-    device flag that `check()` raises on; a step that overflowed its arenas leaves the error map as it was.  `d_h_appear` keeps its
-    meaning: a trainer scatters it by `frame.rays_fidx`.
-
-    `sampler=LidarSampler(...)` (neuralsim_b200/lidar_sampler.py; needs a loss_fn and with_rgb=False, takes no pose=) draws every LiDAR
-    batch inside the graph, as the shipped LiDAR configs' LidarDataset.sample_merged does, and moves the beams to world with each (lidar,
-    frame)'s transform: `frame.step(frame_ind=f)` fills a device frame index and the generator block (the sampler's per-lidar draws first,
-    the perturbed ones after them), and the one replay writes `frame.rays_o` / `frame.rays_d` (world), `frame.rays_li` (the reference's
-    `rays_sel`), `frame.rays_fidx` and `frame.ground_truth = {"ranges": [n_rays]}` (nsb_lidar_sample), renders, calls `loss =
-    loss_fn(rendered_or_ret, frame.ground_truth)` and runs the backward.  With LidarLoss the ranges reach the loss inside the replay:
-    `loss_fn = lambda ret, gt: sum(lidar_loss(None, ret, ground_truth=gt).values())`, the iteration's weights set on the host by
-    `lidar_loss.set_step(None, it)` before `step()`.
+    `sampler=` (off by default; needs a loss_fn) draws every batch inside the graph: a CameraSampler (neuralsim_b200/importance.py;
+    `step(cam=k)`) or a LidarSampler (neuralsim_b200/lidar_sampler.py; `step(frame_ind=f)`).  `step()` fills the sampler's index and
+    generator block (its draws first, the perturbed ones after them); the replay draws the batch into the frame's inputs and
+    `frame.ground_truth`, renders, calls `loss_fn(rendered_or_ret, frame.ground_truth)` and runs the backward (the samplers' `attach`,
+    `select`, `draw`, `loss` and `check` say what else each one needs, writes and updates).
 
     The first call probes the sizes with the host-sized path (SingleVolumeRenderer.ray_query, no grad), sizes the arenas with `slack`,
     warms up and captures.  Gradients are accumulated into `p.grad` (kept in place; `zero_grads=True` or a `pre_hook` zeroes them inside the graph).
@@ -493,30 +479,26 @@ class StaticFrame:
             self.d_rays_o, self.d_rays_d = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)
         self.cnt = torch.zeros(32, dtype=torch.int64, device=dev)
         self.perturb, self.rng, self.rng_reservation, self._gen = bool(perturb), None, 0, None
-        self.sampler, self._lidar = sampler, False
         if generator is not None and not self.perturb and sampler is None:
             raise RuntimeError("StaticFrame(generator=...): the generator is read only with perturb=True or a sampler")
         if self.perturb or sampler is not None:
-            self._gen = PT.cuda_generator(generator, dev)
+            self._gen = TR.cuda_generator(generator, dev)
         if self.perturb:
             cfg = query_config(**(model.ray_query_cfg.get("query_param", {}) or {}), upsample_s_divisor=model.upsample_s_divisor)
-            self.rng_reservation = PT.reservation(self.n_rays, cfg, PT.grid_cap(dev))
+            self.rng_reservation = PT.reservation(self.n_rays, cfg, TR.grid_cap(dev))
             self.rng = torch.zeros(2, dtype=torch.int64, device=dev)
         self.max_level_dev = torch.zeros((), dtype=torch.int32, device=dev)
-        self.pose, self._pose_grad = pose, None
+        self.pose, self._pose = pose, (FramePose(pose, self.n_rays, dev) if pose is not None else None)
         if pose is not None:
-            from .pose import scratch_floats
-            P = pose.n_poses
-            self.dirs = torch.zeros(self.n_rays, 3, device=dev)
-            self.pidx = torch.zeros(self.n_rays, dtype=torch.int64, device=dev)
-            self._pose_unit, self._pose_nrm = torch.zeros(P, 4, device=dev), torch.zeros(P, device=dev)
-            self._pose_scratch = torch.zeros(max(scratch_floats(self.n_rays, P), 4), device=dev)
-            self._pose_d_rays = torch.zeros(2, self.n_rays, 3, device=dev).unbind(0)       # the rays' gradient when ray_grad is off
-            self._pose_g = (torch.zeros(P, 4, device=dev), torch.zeros(P, 3, device=dev))   # what dq.grad / dt.grad are while the frame lives
+            self.dirs, self.pidx = self._pose.dirs, self._pose.pidx
+        self.sampler = sampler
         if sampler is not None:
-            self._init_sampler(sampler, pose, loss_fn, with_rgb)
-        self.graph, self.loss, self.rendered, self.buffers, self._occ_captured = None, None, None, None, None
-        self.captures = 0
+            if loss_fn is None or sampler.device != dev:
+                raise RuntimeError(f"StaticFrame(sampler=...): needs a loss_fn, and the sampler on the model's device {dev} (it is on {sampler.device})")
+            self._rng_sampler = torch.zeros(2, dtype=torch.int64, device=dev)      # the sampler's (seed, offset); it chains its end into self.rng
+            self.sampler_reservation = sampler.attach(self)
+        self.graph, self.loss, self.rendered, self.buffers, self._occ_captured, self._grad_captured = None, None, None, None, None, None
+        self.captures, self._warming = 0, False
 
     # -- sizes
     @torch.no_grad()
@@ -543,96 +525,18 @@ class StaticFrame:
         self.march_cap = max(self.march_cap or 0, m)
         self.kept_cap = max(self.kept_cap or 0, k)
 
-    # -- the sampler
-    def _init_sampler(self, sampler, pose, loss_fn, with_rgb):
-        from ..importance import CameraSampler
-        from ..lidar_sampler import LidarSampler
-        self._lidar = isinstance(sampler, LidarSampler)
-        if self._lidar:
-            self._init_lidar_sampler(sampler, pose, loss_fn, with_rgb)
-            return
-        if not isinstance(sampler, CameraSampler):
-            raise RuntimeError(f"StaticFrame(sampler=...): a neuralsim_b200.importance.CameraSampler or neuralsim_b200.lidar_sampler.LidarSampler, "
-                               f"got {type(sampler)}")
-        if pose is None or loss_fn is None:
-            raise RuntimeError("StaticFrame(sampler=...): needs pose= (CameraPoses: the sampled rays are pose indices and camera-space directions) and a loss_fn")
-        if sampler.pose_end > pose.n_poses:
-            raise RuntimeError(f"StaticFrame(sampler=...): the cameras' frames reach pose {sampler.pose_end - 1}, the pose list holds {pose.n_poses}")
-        if sampler.device != self.device:
-            raise RuntimeError(f"StaticFrame(sampler=...): the sampler is on {sampler.device}, the model on {self.device}")
-        if sampler.appear_table is not None and (self.h_appear is None or sampler.appear_table.shape[1] != self.h_appear.shape[1]):
-            raise RuntimeError("StaticFrame(sampler=...): the sampler's appearance codes do not match the model's code width")
-        dev, n = self.device, self.n_rays
-        self.sampler_reservation = sampler.inc(n, PT.grid_cap(dev))
-        self.cam = torch.zeros((), dtype=torch.int64, device=dev)
-        self._rng_sampler = torch.zeros(2, dtype=torch.int64, device=dev)
-        self.rays_fidx = torch.zeros(n, dtype=torch.int64, device=dev)
-        self.rays_pix = torch.zeros(n, 2, device=dev)
-        self.ground_truth = {k: torch.zeros((n,) + tail, dtype=dt, device=dev) for k, (dt, tail) in sampler.gt_spec.items()}
-        self.err_flag = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._warming = False
-
-    def _init_lidar_sampler(self, sampler, pose, loss_fn, with_rgb):
-        if pose is not None or loss_fn is None or with_rgb:
-            raise RuntimeError("StaticFrame(sampler=LidarSampler): needs a loss_fn and with_rgb=False, and takes no pose= (the sampler writes the "
-                               "world rays)")
-        if sampler.device != self.device:
-            raise RuntimeError(f"StaticFrame(sampler=...): the sampler is on {sampler.device}, the model on {self.device}")
-        dev, n = self.device, self.n_rays
-        self.sampler_reservation = sampler.inc(n, PT.grid_cap(dev))
-        self.frame_ind = torch.zeros((), dtype=torch.int64, device=dev)
-        self._rng_sampler = torch.zeros(2, dtype=torch.int64, device=dev)
-        self.rays_li = torch.zeros(n, dtype=torch.int64, device=dev)
-        self.rays_fidx = torch.zeros(n, dtype=torch.int64, device=dev)
-        self.ground_truth = dict(ranges=torch.zeros(n, device=dev))
-
-    def _sample(self):
-        """camera self.cam's (or LiDAR frame self.frame_ind's) batch into the frame's inputs (nsb_imp_sample, nsb_lidar_sample)"""
-        s = self.sampler
-        if self._lidar:
-            s.launch(self.frame_ind, self._rng_sampler, self.rays_o, self.rays_d, self.ground_truth["ranges"], self.rays_li, self.rays_fidx,
-                     self.rng if self.perturb else None)
-            return
-        s.sample(self.cam, self._rng_sampler, self.n_rays, self.rays_fidx, self.rays_pix, self.pidx, self.dirs, self.ground_truth,
-                 self.h_appear if s.appear_table is not None else None, self.rng if self.perturb else None)
-
-    # -- the pose
     def set_rays(self, dirs, pidx):
-        """copy camera-space directions [n_rays, 3] and pose indices [n_rays] (int64, each in [0, P): checked here, one host read) into the
-        frame's inputs"""
-        from .pose import check_pidx
-        if self.pose is None:
+        """copy camera-space directions [n_rays, 3] and pose indices [n_rays] (int64 in [0, P), checked: one host read) into `dirs`, `pidx`"""
+        if self._pose is None:
             raise RuntimeError("StaticFrame.set_rays: the frame was built without pose=; pass rays_o / rays_d to step()")
-        if not isinstance(dirs, torch.Tensor) or tuple(dirs.shape) != (self.n_rays, 3) or not dirs.is_floating_point():
-            raise RuntimeError(f"StaticFrame.set_rays: dirs must be a float tensor [{self.n_rays}, 3], got {getattr(dirs, 'shape', type(dirs))}")
-        check_pidx(pidx.to(self.device) if isinstance(pidx, torch.Tensor) else pidx, self.n_rays, self.pose.n_poses)
-        self.dirs.copy_(dirs, non_blocking=True)
-        self.pidx.copy_(pidx, non_blocking=True)
+        self._pose.set_rays(dirs, pidx)
 
-    def _pose_wants_grad(self):
-        return self.pose is not None and self.pose.requires_grad and torch.is_grad_enabled()
-
-    def _bind_pose_grads(self):
-        """dq.grad / dt.grad := the buffers the graph adds into (None counts as zeros; another tensor is copied in)"""
-        for p, buf in zip((self.pose.dq, self.pose.dt), self._pose_g):
-            if not p.requires_grad:
-                continue
-            if p.grad is None:
-                buf.zero_()
-            elif p.grad is not buf:
-                buf.copy_(p.grad)
-            p.grad = buf
-
-    def _pose_rays(self):
-        from .pose import pose_forward
-        with torch.no_grad():
-            pose_forward(self.pose, self.pidx, self.dirs, self._pose_unit, self._pose_nrm, self.rays_o, self.rays_d)
-
-    def _pose_adjoint(self, d_rays):
-        from .pose import pose_backward
-        pose = self.pose
-        pose_backward(self._pose_unit, self._pose_nrm, self.pidx, self.dirs, d_rays[0], d_rays[1], self._pose_scratch,
-                      self._pose_g[0] if pose.dq.requires_grad else None, self._pose_g[1] if pose.dt.requires_grad else None)
+    def _variance_control(self):
+        """the model's variance schedule (ctrl_var with a host-side mix_weight), its device weight `_w_dev` made on first use; or None"""
+        cv = getattr(self.model, "ctrl_var", None)
+        if hasattr(cv, "mix_weight") and getattr(cv, "_w_dev", None) is None:
+            cv._w_dev = torch.zeros((), device=self.device)
+        return cv if hasattr(cv, "mix_weight") else None
 
     # -- the step
     def _run(self):
@@ -642,20 +546,13 @@ class StaticFrame:
             for p in self.model.parameters():
                 if p.grad is not None:
                     p.grad.zero_()
-        pose_grad = self._pose_wants_grad()
         if self.sampler is not None:
-            self._sample()
-        if self.pose is not None:
-            if self.zero_grads and pose_grad:
-                for g in self._pose_g:
-                    g.zero_()
-            self._pose_rays()
-        d_rays = (self.d_rays_o, self.d_rays_d) if self.d_rays_o is not None else (self._pose_d_rays if pose_grad else None)
-        hook = (lambda: self._pose_adjoint(d_rays)) if pose_grad else None
-        cv = getattr(self.model, "ctrl_var", None)
-        if cv is not None and hasattr(cv, "mix_weight"):
-            if getattr(cv, "_w_dev", None) is None:
-                cv._w_dev = torch.zeros((), device=self.device)
+            self.sampler.draw(self, self._rng_sampler)
+        d_rays, hook = ((self.d_rays_o, self.d_rays_d) if self.d_rays_o is not None else None), None
+        if self._pose is not None:
+            d_rays, hook = self._pose.run(self.rays_o, self.rays_d, d_rays, self.zero_grads)
+        cv = self._variance_control()
+        if cv is not None:
             cv._use_w_dev = True                             # inv_s annealing weight from a device scalar (refreshed in step())
         try:
             rendered, _, buffers = render_static(self.model, self.rays_o, self.rays_d, self.h_appear, near=self.near, far=self.far, march_cap=self.march_cap,
@@ -668,30 +565,22 @@ class StaticFrame:
         loss = None
         if self.loss_fn is not None:
             arg = dict(rendered=rendered, volume_buffer=static_volume_buffer(buffers, self.cnt)) if self.loss_on_ret else rendered
-            if self.sampler is None:
-                loss = self.loss_fn(arg)
-            elif self._lidar:
-                loss = self.loss_fn(arg, self.ground_truth)
-            else:
-                loss, err = self.loss_fn(arg, self.ground_truth)
-                if not isinstance(err, torch.Tensor) or err.numel() != self.n_rays:
-                    raise RuntimeError(f"StaticFrame(sampler=...): loss_fn must return (loss, err), err holding {self.n_rays} per-ray errors")
-                err = err.detach().reshape(-1).float().contiguous()
+            loss, after_backward = self.sampler.loss(self, arg) if self.sampler is not None else (self.loss_fn(arg), None)
             if loss.requires_grad:
                 loss.backward()
             loss = loss.detach()
-            if self.sampler is not None and not self._lidar and not self._warming:       # the warm-up runs must not add into the error map
+            if after_backward is not None and not self._warming:         # the warm-up runs leave the sampler's state alone
                 ov = CNT_SLOTS["overflow"]
-                self.sampler.update(self.cam, self.rays_fidx, self.rays_pix, err, self.err_flag, skip=self.cnt[ov:ov + 1])
+                after_backward(self.cnt[ov:ov + 1])                       # (an overflowed step rendered nothing: skipped on the device)
         return rendered, buffers, loss
 
     def capture(self):
         if self.sampler is not None:
-            self._sample()                                  # this step's batch: the probe and the check below read its rays
-        if self.pose is not None:
+            self.sampler.draw(self, self._rng_sampler)      # this step's batch: the probe and the check below read its rays
+        if self._pose is not None:
             if not bool(self.dirs.any()):                   # (zero directions: see below)
                 raise RuntimeError("StaticFrame.capture: the pose inputs hold no rays yet; call set_rays(dirs, pidx) or step(dirs=..., pidx=...) first")
-            self._pose_rays()                               # the probe and the check below read the rays
+            self._pose.run(self.rays_o, self.rays_d)        # the probe and the check below read the rays
         if self.march_cap is None or self.kept_cap is None or self.coherent is None:
             self._size()
         if not self.use_graph:
@@ -723,7 +612,7 @@ class StaticFrame:
             # stream BEFORE this and whose graph is still referenced -- a kept loss / rendered tensor -- pins those nodes to the default
             # stream and invalidates the capture: drop such references first.)
             self._occ_captured = self.model.accel.occ.occ_grid
-            self._pose_grad = self._pose_wants_grad()
+            self._grad_captured = self._pose is not None and self._pose.wants_grad()
             with torch.cuda.graph(g, stream=side):
                 self.rendered, self.buffers, self.loss = self._run()
             self.graph = g
@@ -734,50 +623,36 @@ class StaticFrame:
 
     def step(self, rays_o=None, rays_d=None, rays_h_appear=None, *, dirs=None, pidx=None, cam=None, frame_ind=None):
         """copy the batch into the graph's inputs (H2D if the tensors are on the host) and launch.  -> loss (device scalar) or None.
-        With pose=: no rays_o / rays_d; dirs and pidx (set_rays), or neither to replay the rays set last.  With sampler=CameraSampler: cam
-        alone, the camera whose batch the graph draws; with sampler=LidarSampler: frame_ind alone, the frame whose beams it draws."""
-        if self._lidar:
-            if rays_o is not None or rays_d is not None or rays_h_appear is not None or dirs is not None or pidx is not None or cam is not None:
-                raise RuntimeError("StaticFrame.step: a frame with sampler=LidarSampler draws its own batch; pass frame_ind= only")
-            self.frame_ind.fill_(self.sampler.check_frame(frame_ind))
-        elif frame_ind is not None:
-            raise RuntimeError("StaticFrame.step: frame_ind= is read only with sampler=LidarSampler")
-        elif self.sampler is not None:
-            if rays_o is not None or rays_d is not None or rays_h_appear is not None or dirs is not None or pidx is not None:
-                raise RuntimeError("StaticFrame.step: a frame with sampler= draws its own batch; pass cam= only")
-            if isinstance(cam, bool) or not isinstance(cam, int) or not 0 <= cam < self.sampler.n_cameras:
-                raise RuntimeError(f"StaticFrame.step: cam must be an int in [0, {self.sampler.n_cameras}), got {cam!r}")
-            self.cam.fill_(cam)
-        elif cam is not None:
-            raise RuntimeError("StaticFrame.step: cam= is read only with sampler=")
-        if self._lidar:
-            pass                                            # the graph writes the world rays
-        elif self.pose is None:
+        With pose=: no rays_o / rays_d; dirs and pidx (set_rays), or neither to replay the rays set last.  With sampler=: the camera cam
+        (CameraSampler) or the LiDAR frame frame_ind (LidarSampler) whose batch the graph draws, alone."""
+        after_step = None
+        if self.sampler is not None:
+            after_step = self.sampler.select(self, cam=cam, frame_ind=frame_ind, rays=(rays_o, rays_d, rays_h_appear, dirs, pidx))
+        elif cam is not None or frame_ind is not None:
+            raise RuntimeError("StaticFrame.step: cam= and frame_ind= are read only with sampler=")
+        elif self._pose is None:
             if rays_o is None or rays_d is None or dirs is not None or pidx is not None:
                 raise RuntimeError("StaticFrame.step: a frame without pose= takes rays_o and rays_d (and no dirs / pidx)")
             self.rays_o.copy_(rays_o, non_blocking=True)
             self.rays_d.copy_(rays_d, non_blocking=True)
-        else:
-            if rays_o is not None or rays_d is not None or (dirs is None) != (pidx is None):
-                raise RuntimeError("StaticFrame.step: a frame with pose= takes dirs and pidx (or neither), not rays_o / rays_d")
-            if dirs is not None:
-                self.set_rays(dirs, pidx)
-            if self.pose.requires_grad:
-                self._bind_pose_grads()
-            if self.graph is not None and self._pose_grad != self._pose_wants_grad():
+        elif rays_o is not None or rays_d is not None or (dirs is None) != (pidx is None):
+            raise RuntimeError("StaticFrame.step: a frame with pose= takes dirs and pidx (or neither), not rays_o / rays_d")
+        elif dirs is not None:
+            self.set_rays(dirs, pidx)
+        if self._pose is not None:
+            self._pose.bind_grads()
+            if self.graph is not None and self._grad_captured != self._pose.wants_grad():
                 self.graph = None                           # requires_grad of the pose switched: re-capture (with / without the adjoint)
         if self.h_appear is not None and rays_h_appear is not None:
             self.h_appear.copy_(rays_h_appear, non_blocking=True)
-        cv = getattr(self.model, "ctrl_var", None)
-        if cv is not None and hasattr(cv, "mix_weight"):
-            if getattr(cv, "_w_dev", None) is None:
-                cv._w_dev = torch.zeros((), device=self.device)
+        cv = self._variance_control()
+        if cv is not None:
             cv._w_dev.fill_(cv.mix_weight())                  # the variance schedule's host-side weight of THIS iteration
         self.max_level_dev.fill_(self.model.implicit_surface._ml(self.model.max_level))     # the LoTD level bound of THIS iteration
         if self.sampler is not None:        # the sampler's draws first; its kernel chains the offset after them into self.rng
-            PT.take(self._gen, self.sampler_reservation + self.rng_reservation, self._rng_sampler)
+            TR.take(self._gen, self.sampler_reservation + self.rng_reservation, self._rng_sampler)
         elif self.perturb:
-            PT.take(self._gen, self.rng_reservation, self.rng)                                 # the random state of THIS iteration
+            TR.take(self._gen, self.rng_reservation, self.rng)                                 # the random state of THIS iteration
         if self.graph is None and (self.use_graph or self.march_cap is None):
             self.capture()
         if self.graph is not None:
@@ -788,8 +663,8 @@ class StaticFrame:
             self.graph.replay()
         else:
             self.rendered, self.buffers, self.loss = self._run()
-        if self.sampler is not None and not self._lidar:
-            self.sampler.samplers[cam].error_map.count_step()     # the reference's per-camera schedule; rebuilds the cdfs in place
+        if after_step is not None:
+            after_step()
         return self.loss
 
     def counts(self):
@@ -801,9 +676,8 @@ class StaticFrame:
         """True if the last step fitted its arenas.  Otherwise the arenas are re-sized from this batch, the graph is re-captured and --
         with `retry` -- the step is run again (gradients of the overflowed step were those of an empty render: nothing accumulated).
         With sampler=: raises if loss_fn gave the error map a negative error since the last check."""
-        if self.sampler is not None and not self._lidar and int(self.err_flag) != 0:
-            self.err_flag.zero_()
-            raise RuntimeError("StaticFrame.check: loss_fn returned a negative per-ray error; the error map accumulates non-negative errors only")
+        if self.sampler is not None:
+            self.sampler.check(self)
         if int(self.cnt[CNT_SLOTS["overflow"]]) == 0:
             return True
         self.march_cap = self.kept_cap = None

@@ -1,42 +1,21 @@
 """Perturbed samples of the one-launch step from torch's own CUDA random stream (csrc/perturb.cu, csrc/torch_uniform.cuh).
 
 A perturbed NeuS query draws, in order, torch.rand([n_rays, nc1]) (coarse depths), rand_like of the M marched samples (the marcher's
-jitter, discarded) and torch.rand([n_hit, nf_i]) per up-sampling stage (graphics/neus.py:_query_fused).  torch advances its generator's
-offset by `uniform_inc(N)` per draw, so draw k starts at base + sum_{j<k} uniform_inc(N_j); every N_j is a count of the step's device
-block (graphics/neus_static.py CNT_SLOTS), so the kernels find their offsets on the device.  A step takes its (seed, base offset) from a
-device block `rng` = int64 [2] and reserves `reservation(...)` offsets of the generator: a bound on every draw the step can make."""
+jitter, discarded) and torch.rand([n_hit, nf_i]) per up-sampling stage (graphics/neus.py:_query_fused).  Draw k starts at base +
+sum_{j<k} uniform_inc(N_j) (torch_rng.py); every N_j is a count of the step's device block (graphics/neus_static.py CNT_SLOTS), so the
+kernels find their offsets on the device.  A step takes its (seed, base offset) from a device block `rng` = int64 [2] and reserves
+`reservation(...)` offsets of the generator: a bound on every draw the step can make."""
 from __future__ import annotations
 
 import ctypes
 
-import torch
-
 from .. import _lib as L
+from .. import torch_rng as TR
+from ..torch_rng import cuda_generator, grid_cap, seed_i64, take, uniform_inc  # noqa: F401 -- public here before torch_rng.py held them
 
 __all__ = ["grid_cap", "uniform_inc", "reservation", "cuda_generator", "take", "step_draws", "coarse_depths", "invert_cdf"]
 
-MAX_DRAW = 2 ** 31          # torch splits a draw of 2^31 or more values into 32-bit sub-iterators, each with its own offset
 MAX_DRAWS = 8               # entries of a draw list (csrc/perturb.cu kMaxDraws)
-
-
-def grid_cap(device) -> int:
-    """torch's cap on the grid of a draw on `device` (calc_execution_policy): SMs * (maxThreadsPerSM / 256) blocks"""
-    p = torch.cuda.get_device_properties(device)
-    return int(p.multi_processor_count) * (int(p.max_threads_per_multi_processor) // 256)
-
-
-def uniform_inc(n: int, cap: int) -> int:
-    """the generator offset a draw of n float32 values advances by (0 for an empty draw)"""
-    n = int(n)
-    if n <= 0:
-        return 0
-    stride = 256 * min((n + 255) // 256, int(cap))
-    return ((n - 1) // (4 * stride) + 1) * 4
-
-
-def _check_draw(n, what):
-    if n >= MAX_DRAW:
-        raise RuntimeError(f"perturb=True: the {what} draw may hold {n} >= 2^31 values, which torch splits into 32-bit sub-draws; use fewer rays per step")
 
 
 def reservation(n_rays: int, cfg, cap: int) -> int:
@@ -45,41 +24,10 @@ def reservation(n_rays: int, cfg, cap: int) -> int:
     nc1 = cfg.num_coarse + 1
     sizes = [(n_rays * nc1, "coarse"), (n_rays * cfg.max_steps, "marcher")] + [(n_rays * nf, f"stage {i}") for i, nf in enumerate(cfg.num_fine)]
     for n, what in sizes:
-        _check_draw(n, what)
+        TR.check_draw(n, f"perturb=True: the {what}")
     if 2 + len(cfg.num_fine) > MAX_DRAWS:
         raise RuntimeError(f"perturb=True: at most {MAX_DRAWS - 2} up-sampling stages, got {len(cfg.num_fine)}")
-    return sum(uniform_inc(n, cap) for n, _ in sizes)
-
-
-def cuda_generator(generator, device):
-    """the CUDA generator a perturbed step draws from: `generator`, or torch's default one of `device`"""
-    if generator is not None and (not isinstance(generator, torch.Generator) or generator.device.type != "cuda"):
-        raise RuntimeError(f"perturb=True: the generator must be a CUDA torch.Generator, got {getattr(generator, 'device', type(generator))}")
-    device = torch.device(device)
-    idx = device.index if device.index is not None else torch.cuda.current_device()
-    if generator is None:
-        return torch.cuda.default_generators[idx]
-    if (generator.device.index if generator.device.index is not None else torch.cuda.current_device()) != idx:
-        raise RuntimeError(f"perturb=True: the generator is on {generator.device}, the step on cuda:{idx}")
-    return generator
-
-
-def seed_i64(seed: int) -> int:
-    """a uint64 Philox seed as the int64 of the same bits"""
-    seed = int(seed)
-    return seed - 2 ** 64 if seed >= 2 ** 63 else seed
-
-
-def take(gen, reserve: int, out=None):
-    """(seed, offset) of `gen` into the device block `out` (int64 [2]; made when None) by two fills -- no host read, no synchronisation --
-    then the generator advanced by `reserve`.  -> out"""
-    seed, off = seed_i64(gen.initial_seed()), int(gen.get_offset())
-    if out is None:
-        out = torch.empty(2, dtype=torch.int64, device=gen.device)
-    out[0].fill_(seed)
-    out[1].fill_(off)
-    gen.set_offset(off + int(reserve))
-    return out
+    return sum(TR.uniform_inc(n, cap) for n, _ in sizes)
 
 
 def step_draws(slots, nc1, num_fine):

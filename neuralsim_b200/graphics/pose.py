@@ -9,7 +9,7 @@ frame): q0, dq [P, 4] (real part first), t0, dt [P, 3].  A ray is the pose index
     rays_o = t0 + dt,    rays_d = normalize(quat_apply(normalize_quat(q0 + dq), dirs))
 
 in the reference's fp32 operation order (app/resources/observers/cameras.py:299-310).  `pose_rays` is the differentiable op; the
-one-launch step (`StaticFrame(..., pose=...)`) runs the same two kernels inside its graph, so both give the same bits.
+one-launch step (`StaticFrame(..., pose=...)`) runs the same two kernels inside its graph through a `FramePose`, so both give the same bits.
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ import torch
 
 from .. import _lib as L
 
-__all__ = ["CameraPoses", "PoseRays", "pose_rays", "check_pose_cfg", "check_pidx", "pose_forward", "pose_backward"]
+__all__ = ["CameraPoses", "PoseRays", "pose_rays", "FramePose", "check_pose_cfg", "check_pidx", "pose_forward", "pose_backward"]
 
 _UNSUPPORTED_ROT = ("RotationAxisAngle", "Rotation6D", "RotationMat3x3")
 
@@ -143,3 +143,56 @@ def pose_rays(poses, pidx, dirs):
         _check_f32(t, (poses.n_poses, w), name)
     check_pidx(pidx, n, poses.n_poses)
     return PoseRays.apply(poses, pidx, dirs, poses.dq, poses.dt)
+
+
+class FramePose:
+    """The pose's part of a one-launch step (StaticFrame(pose=poses)): the inputs `dirs` [n_rays, 3] (camera-space directions) and `pidx`
+    [n_rays] (int64 pose indices), the rays built from them and the pose adjoint, which ADDS into `grads` (bound as dq.grad / dt.grad)."""
+
+    def __init__(self, poses, n_rays, device):
+        P, n = poses.n_poses, int(n_rays)
+        self.poses, self.n_rays = poses, n
+        self.dirs = torch.zeros(n, 3, device=device)
+        self.pidx = torch.zeros(n, dtype=torch.int64, device=device)
+        self.unit, self.nrm = torch.zeros(P, 4, device=device), torch.zeros(P, device=device)
+        self.scratch = torch.zeros(max(scratch_floats(n, P), 4), device=device)
+        self.d_rays = torch.zeros(2, n, 3, device=device).unbind(0)           # the rays' gradient when the step keeps none of its own
+        self.grads = (torch.zeros(P, 4, device=device), torch.zeros(P, 3, device=device))
+
+    def set_rays(self, dirs, pidx):
+        """StaticFrame.set_rays: dirs [n_rays, 3] and pidx [n_rays] (int64 in [0, P), checked: one host read) into the inputs"""
+        if not isinstance(dirs, torch.Tensor) or tuple(dirs.shape) != (self.n_rays, 3) or not dirs.is_floating_point():
+            raise RuntimeError(f"StaticFrame.set_rays: dirs must be a float tensor [{self.n_rays}, 3], got {getattr(dirs, 'shape', type(dirs))}")
+        check_pidx(pidx.to(self.pidx.device) if isinstance(pidx, torch.Tensor) else pidx, self.n_rays, self.poses.n_poses)
+        self.dirs.copy_(dirs, non_blocking=True)
+        self.pidx.copy_(pidx, non_blocking=True)
+
+    def wants_grad(self):
+        return self.poses.requires_grad and torch.is_grad_enabled()
+
+    def bind_grads(self):
+        """dq.grad / dt.grad := `grads`, for the deltas that require grad (a None .grad counts as zeros, another tensor is copied in)"""
+        for p, buf in zip((self.poses.dq, self.poses.dt), self.grads):
+            if not p.requires_grad:
+                continue
+            if p.grad is None:
+                buf.zero_()
+            elif p.grad is not buf:
+                buf.copy_(p.grad)
+            p.grad = buf
+
+    def run(self, rays_o, rays_d, d_rays=None, zero_grads=False):
+        """the world rays into rays_o, rays_d [n_rays, 3].  -> (d_rays, None) without grad; with grad (`grads` zeroed first if zero_grads)
+        the buffers the rays' gradient goes to (d_rays, else the pose's own) and the hook that adds their pose adjoint into `grads`"""
+        grad = self.wants_grad()
+        if grad and zero_grads:
+            for g in self.grads:
+                g.zero_()
+        with torch.no_grad():
+            pose_forward(self.poses, self.pidx, self.dirs, self.unit, self.nrm, rays_o, rays_d)
+        if not grad:
+            return d_rays, None
+        d = d_rays if d_rays is not None else self.d_rays
+        q = self.poses
+        return d, lambda: pose_backward(self.unit, self.nrm, self.pidx, self.dirs, d[0], d[1], self.scratch,
+                                        self.grads[0] if q.dq.requires_grad else None, self.grads[1] if q.dt.requires_grad else None)

@@ -22,6 +22,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib as L
+from . import torch_rng as TR
 
 __all__ = ["ErrorMap", "ImpSampler", "CameraSampler", "check_error_map_cfg", "split", "sampler_inc", "recipe_update_error_map",
            "recipe_sample_img_pixel", "recipe_pixels", "TABLE_WIDTH", "MAX_GT"]
@@ -53,15 +54,10 @@ def split(n, frac_uniform):
     return n_u, n - n_u
 
 
-def _inc(n, cap):
-    from .graphics.perturb import uniform_inc
-    return uniform_inc(n, cap)
-
-
 def sampler_inc(n, frac_uniform, cap):
     """the generator offsets one draw of n rays advances: randint and rand of the uniform rays, rand of the frames and rand of the pixels"""
     n_u, n_e = split(n, frac_uniform)
-    return _inc(n_u, cap) + _inc(2 * n_u, cap) + _inc(n_e, cap) + _inc(2 * n_e, cap)
+    return TR.uniform_inc(n_u, cap) + TR.uniform_inc(2 * n_u, cap) + TR.uniform_inc(n_e, cap) + TR.uniform_inc(2 * n_e, cap)
 
 
 # ---------------------------------------------------------------------------------------------------------------- the reference's torch ops
@@ -182,13 +178,6 @@ def error_map_update(fidx, xy, val, flag, *, error_map=None, last=None, table=No
                                          P(table, "i64", "table", allow_none=True), P(cam, "i64", "cam", allow_none=True), L.c_i32(res_yx[0]),
                                          L.c_i32(res_yx[1]), P(fidx, "i64", "fidx"), P(xy, "f32", "xy"), P(val, "f32", "val"), L.c_i64(fidx.shape[0]),
                                          P(flag, "i32", "flag"), P(skip, "i64", "skip", allow_none=True), L.stream_ptr()), "error_map_update")
-
-
-def _take(n, frac_uniform, generator, device):
-    """(seed, offset) of the generator into a device block, then the generator advanced past the draw (graphics/perturb.py:take)"""
-    from .graphics import perturb as PT
-    gen = PT.cuda_generator(generator, device)
-    return PT.take(gen, sampler_inc(n, frac_uniform, PT.grid_cap(device)))
 
 
 # ---------------------------------------------------------------------------------------------------------------- modules
@@ -325,7 +314,7 @@ class ErrorMap(nn.Module):
         dev = self.device
         if self._table is None:
             self._table = (torch.tensor([self.table_row()], dtype=torch.int64).to(dev), torch.zeros((), dtype=torch.int64, device=dev))
-        rng = _take(n, frac_uniform, generator, dev)
+        rng = TR.take(TR.cuda_generator(generator, dev), sampler_inc(n, frac_uniform, TR.grid_cap(dev)))
         fidx = torch.empty(n, dtype=torch.int64, device=dev)
         xy = torch.empty(n, 2, dtype=torch.float32, device=dev)
         imp_sample(self._table[0], self._table[1], rng, n, split(n, frac_uniform)[0], (self.res_y, self.res_x), fidx, xy)
@@ -415,7 +404,8 @@ class CameraSampler:
     """The batch source of StaticFrame(sampler=...): per camera k an ImpSampler, the ground-truth image stacks gts[k] = {key: [F_k, H_k,
     W_k, ...] device tensor} (float32 `image_rgb`, bool / uint8 masks; the same keys, dtypes and trailing shapes for every camera), the
     intrinsics intrs[k] [F_k, 3, 3] (float32), and the bases of its frames in the pose list (CameraPoses) and in the appearance-code table.
-    `frame.step(cam=k)` draws camera k's batch inside the graph and updates its error map; one capture serves every camera."""
+    `frame.step(cam=k)` draws camera k's batch inside the graph, as ImpSampler.sample_img_pixel does over its error map, and updates that
+    map; one capture serves every camera.  `frame.d_h_appear` keeps its meaning: a trainer scatters it by `frame.rays_fidx`."""
 
     def __init__(self, samplers, gts, intrs, wh, pose_bases, appear_bases=None, appear_table=None):
         k = len(samplers)
@@ -482,3 +472,49 @@ class CameraSampler:
     def update(self, cam, fidx, xy, err, flag, skip=None):
         """camera *cam's error map += the batch's errors (nsb_error_map_update from the table)"""
         error_map_update(fidx, xy, err, flag, table=self.table, cam=cam, n_images=self.max_images, res_yx=self.res_yx, skip=skip)
+
+    # -- the batch source of a StaticFrame: every per-frame buffer lives on the frame, so one sampler serves several frames
+    def attach(self, frame):
+        """check the frame, give it `cam` (a device index), `rays_fidx`, `rays_pix`, `ground_truth`, `err_flag`.  -> the draw's reservation"""
+        if frame.pose is None:
+            raise RuntimeError("StaticFrame(sampler=...): needs pose= (CameraPoses: the sampled rays are pose indices and camera-space directions)")
+        if self.pose_end > frame.pose.n_poses:
+            raise RuntimeError(f"StaticFrame(sampler=...): the cameras' frames reach pose {self.pose_end - 1}, the pose list holds {frame.pose.n_poses}")
+        if self.appear_table is not None and (frame.h_appear is None or self.appear_table.shape[1] != frame.h_appear.shape[1]):
+            raise RuntimeError("StaticFrame(sampler=...): the sampler's appearance codes do not match the model's code width")
+        dev, n = frame.device, frame.n_rays
+        frame.cam = torch.zeros((), dtype=torch.int64, device=dev)
+        frame.rays_fidx = torch.zeros(n, dtype=torch.int64, device=dev)
+        frame.rays_pix = torch.zeros(n, 2, device=dev)
+        frame.ground_truth = {k: torch.zeros((n,) + tail, dtype=dt, device=dev) for k, (dt, tail) in self.gt_spec.items()}
+        frame.err_flag = torch.zeros(1, dtype=torch.int32, device=dev)
+        return self.inc(n, TR.grid_cap(dev))
+
+    def select(self, frame, cam, frame_ind, rays):
+        """frame.step(cam=k), which takes no frame_ind or rays: k into frame.cam.  -> camera k's ErrorMap.count_step, run after the step"""
+        if frame_ind is not None or any(v is not None for v in rays):
+            raise RuntimeError("StaticFrame.step: a frame with sampler= draws its own batch; pass cam= only")
+        if isinstance(cam, bool) or not isinstance(cam, int) or not 0 <= cam < self.n_cameras:
+            raise RuntimeError(f"StaticFrame.step: cam must be an int in [0, {self.n_cameras}), got {cam!r}")
+        frame.cam.fill_(cam)
+        return self.samplers[cam].error_map.count_step
+
+    def draw(self, frame, rng):
+        """camera frame.cam's batch, drawn at the device block rng: `rays_fidx`, `rays_pix`, `ground_truth`, `pidx`, `dirs`, codes"""
+        self.sample(frame.cam, rng, frame.n_rays, frame.rays_fidx, frame.rays_pix, frame.pidx, frame.dirs, frame.ground_truth,
+                    frame.h_appear if self.appear_table is not None else None, frame.rng)
+
+    def loss(self, frame, arg):
+        """loss, err = frame.loss_fn(arg, frame.ground_truth), err [n_rays] the per-ray rgb error the reference feeds its error map.
+        -> (loss, what runs after the backward: camera frame.cam's error map += err, unless the device flag `skip` is set)"""
+        loss, err = frame.loss_fn(arg, frame.ground_truth)
+        if not isinstance(err, torch.Tensor) or err.numel() != frame.n_rays:
+            raise RuntimeError(f"StaticFrame(sampler=...): loss_fn must return (loss, err), err holding {frame.n_rays} per-ray errors")
+        err = err.detach().reshape(-1).float().contiguous()
+        return loss, lambda skip: self.update(frame.cam, frame.rays_fidx, frame.rays_pix, err, frame.err_flag, skip=skip)
+
+    def check(self, frame):
+        """raises if loss_fn gave the error map a negative error since the last check (one device-to-host read)"""
+        if int(frame.err_flag) != 0:
+            frame.err_flag.zero_()
+            raise RuntimeError("StaticFrame.check: loss_fn returned a negative per-ray error; the error map accumulates non-negative errors only")

@@ -21,6 +21,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from . import torch_rng as TR
 
 __all__ = ["LidarSampler", "lidar_split", "recipe_sample_merged", "LIDAR_MAX", "TABLE_WIDTH"]
 
@@ -76,11 +77,6 @@ def recipe_sample_merged(rays_o, rays_d, ranges, li, n_lidars, num_rays, weight,
     return dict(split=num_rays_each_lidar, inds=inds, li=li[inds], rays_o=rays_o[inds], rays_d=rays_d[inds], ranges=ranges[inds])
 
 
-def _inc(n, cap):
-    from .graphics.perturb import uniform_inc
-    return uniform_inc(n, cap)
-
-
 class LidarSampler:
     """The batch source of StaticFrame(sampler=LidarSampler(...)).
 
@@ -93,7 +89,9 @@ class LidarSampler:
         multi_lidar_weight, lidar_sample_mode, equal_mode: the `lidar_dataset` settings
 
     The split of every frame is computed here, once (`split[f]`).  `sample(frame_ind, generator)` draws one batch on the kernel outside
-    a graph; `frame.step(frame_ind=f)` draws frame f's batch inside the graph."""
+    a graph; `frame.step(frame_ind=f)` draws frame f's batch inside the graph.  With LidarLoss the ranges reach the loss inside the
+    replay: `loss_fn = lambda ret, gt: sum(lidar_loss(None, ret, ground_truth=gt).values())`, its weights set by
+    `lidar_loss.set_step(None, it)` before `step()`."""
 
     def __init__(self, rays_o, rays_d, ranges, counts, l2w, num_rays, multi_lidar_weight=None, *, lidar_sample_mode="merged_weighted",
                  equal_mode="ray_batch"):
@@ -152,7 +150,7 @@ class LidarSampler:
             o = 0
             for li, num in enumerate(split):
                 row[_DRAW_OFF + li] = o
-                o += _inc(num, cap)
+                o += TR.uniform_inc(num, cap)
             row[_INC] = o
         return [list(r) for r in self._rows]
 
@@ -164,7 +162,7 @@ class LidarSampler:
 
     def frame_inc(self, f, cap):
         """the generator offsets frame f's draws advance: sum over its lidars of inc(num_li)"""
-        return sum(_inc(num, cap) for num in self.split[f])
+        return sum(TR.uniform_inc(num, cap) for num in self.split[f])
 
     def inc(self, n, cap):
         """the reservation of one draw of n (= num_rays) rays: the largest frame_inc over the frames (bounds every frame's draws)"""
@@ -179,9 +177,8 @@ class LidarSampler:
 
     def launch(self, frame, rng, rays_o, rays_d, ranges, li, rays_fidx, rng_next=None):
         """nsb_lidar_sample: frame *frame's batch (frame: device int64 scalar) from rng = device int64 {seed, offset} into the buffers"""
-        from .graphics import perturb as PT
         P = L.ptr
-        table = self._table(PT.grid_cap(self.device))
+        table = self._table(TR.grid_cap(self.device))
         L.check(L.lib().nsb_lidar_sample(P(table, "i64", "table"), P(frame, "i64", "frame"), P(rng, "i64", "rng"), L.c_i64(self.num_rays),
                                          P(self.rays_o, "f32", "rays_o"), P(self.rays_d, "f32", "rays_d"), P(self.ranges, "f32", "ranges"),
                                          P(self.l2w, "f32", "l2w"), P(rays_o, "f32", "out rays_o"), P(rays_d, "f32", "out rays_d"),
@@ -192,11 +189,10 @@ class LidarSampler:
     def sample(self, frame_ind, generator=None):
         """frame frame_ind's batch on the kernel from torch's CUDA generator (`generator`, else the default one), which then moves past
         the draws as the reference's randints move it.  -> dict(rays_o, rays_d (world), ranges, li, rays_fidx)"""
-        from .graphics import perturb as PT
         f = self.check_frame(frame_ind)
         n, dev = self.num_rays, self.device
         self.frame.fill_(f)
-        rng = PT.take(PT.cuda_generator(generator, dev), self.frame_inc(f, PT.grid_cap(dev)))
+        rng = TR.take(TR.cuda_generator(generator, dev), self.frame_inc(f, TR.grid_cap(dev)))
         out = dict(rays_o=torch.empty(n, 3, device=dev), rays_d=torch.empty(n, 3, device=dev), ranges=torch.empty(n, device=dev),
                    li=torch.empty(n, dtype=torch.int64, device=dev), rays_fidx=torch.empty(n, dtype=torch.int64, device=dev))
         self.launch(self.frame, rng, out["rays_o"], out["rays_d"], out["ranges"], out["li"], out["rays_fidx"])
@@ -214,3 +210,32 @@ class LidarSampler:
         """recipe_sample_merged on frame frame_ind's data"""
         o, d, r, li = self.frame_data(frame_ind)
         return recipe_sample_merged(o, d, r, li, self.n_lidars, self.num_rays, self.weight, generator)
+
+    # -- the batch source of a StaticFrame: every per-frame buffer lives on the frame, so one sampler serves several frames
+    def attach(self, frame):
+        """check the frame, give it `frame_ind` (a device index), `rays_li`, `rays_fidx`, `ground_truth` = {"ranges"}.  -> the draw's reservation"""
+        if frame.pose is not None or frame.with_rgb:
+            raise RuntimeError("StaticFrame(sampler=LidarSampler): needs with_rgb=False, and takes no pose= (the sampler writes the world rays)")
+        dev, n = frame.device, frame.n_rays
+        frame.frame_ind = torch.zeros((), dtype=torch.int64, device=dev)
+        frame.rays_li = torch.zeros(n, dtype=torch.int64, device=dev)
+        frame.rays_fidx = torch.zeros(n, dtype=torch.int64, device=dev)
+        frame.ground_truth = dict(ranges=torch.zeros(n, device=dev))
+        return self.inc(n, TR.grid_cap(dev))
+
+    def select(self, frame, cam, frame_ind, rays):
+        """frame.step(frame_ind=f), which takes no cam or rays: f into frame.frame_ind.  -> None: nothing runs on the host after the step"""
+        if cam is not None or any(v is not None for v in rays):
+            raise RuntimeError("StaticFrame.step: a frame with sampler=LidarSampler draws its own batch; pass frame_ind= only")
+        frame.frame_ind.fill_(self.check_frame(frame_ind))
+
+    def draw(self, frame, rng):
+        """frame frame.frame_ind's batch, drawn at the device block rng: world rays, `rays_li` (the reference's rays_sel), `rays_fidx`, ranges"""
+        self.launch(frame.frame_ind, rng, frame.rays_o, frame.rays_d, frame.ground_truth["ranges"], frame.rays_li, frame.rays_fidx, frame.rng)
+
+    def loss(self, frame, arg):
+        """-> (frame.loss_fn(arg, frame.ground_truth), None: nothing runs after the backward)"""
+        return frame.loss_fn(arg, frame.ground_truth), None
+
+    def check(self, frame):
+        """nothing to check: a LiDAR draw records no error"""

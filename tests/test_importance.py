@@ -167,8 +167,8 @@ def test_refusals():
 
 
 def test_offsets_of_a_draw():
-    """the generator offsets a batch advances: the four draws' increments, torch's policy (graphics/perturb.py:uniform_inc)"""
-    from neuralsim_b200.graphics.perturb import uniform_inc
+    """the generator offsets a batch advances: the four draws' increments, torch's policy (torch_rng.py:uniform_inc)"""
+    from neuralsim_b200.torch_rng import uniform_inc
     cap = 132 * 8
     for n, f in ((8192, 0.5), (4097, 0.5), (7, 0.0), (7, 1.0), (1, 0.5)):
         n_u, n_e = I.split(n, f)

@@ -30,8 +30,8 @@ def _I():
 
 
 def _cap():
-    from neuralsim_b200.graphics import perturb as PT
-    return PT.grid_cap(torch.device("cuda"))
+    from neuralsim_b200 import torch_rng as TR
+    return TR.grid_cap(torch.device("cuda"))
 
 
 def _same(a, b, what):

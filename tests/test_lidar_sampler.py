@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from neuralsim_b200 import lidar_sampler as LS
-from neuralsim_b200.graphics.perturb import uniform_inc
+from neuralsim_b200.torch_rng import uniform_inc
 
 GOLD = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_lidar_sampler.npz"))
 CASES = [k for k in range(3)]

@@ -118,8 +118,8 @@ def test_kernel_equals_recipe(n, mode):
 
 
 def _cap():
-    from neuralsim_b200.graphics import perturb as PT
-    return PT.grid_cap(torch.device("cuda"))
+    from neuralsim_b200 import torch_rng as TR
+    return TR.grid_cap(torch.device("cuda"))
 
 
 # ===================================================================================================================== 2. world rays

@@ -14,7 +14,7 @@ import bench_cfg3 as C
 from neuralsim_b200.fields import OccGridUpdate
 from neuralsim_b200.fields import occ_update as U
 from neuralsim_b200.fields.accel import OccGridEma, sample_pts_in_voxels
-from neuralsim_b200.graphics import perturb as PT
+from neuralsim_b200 import torch_rng as TR
 from util import rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -85,7 +85,7 @@ def _draw(occ, warmup, num_steps, num_pts, seed):
     cells = occ.occ_grid.numel()
     gen = torch.Generator(dev).manual_seed(seed)
     gen.set_offset(4 * seed)
-    rng = PT.take(gen, 0)
+    rng = TR.take(gen, 0)
     occupied, empty, counts = _lists(occ.occ_grid)
     cap = U.capacity(cells, num_steps, num_pts)
     pts = torch.full((cap, 3), float("nan"), device=dev)
@@ -94,7 +94,7 @@ def _draw(occ, warmup, num_steps, num_pts, seed):
     off0 = gen.get_offset()
     host = _host_pts(occ, warmup, num_steps, num_pts, gen)
     assert int(out[1]) == 0 and int(out[0]) == host.shape[0] <= cap
-    return pts[:host.shape[0]], host, gen.get_offset() - off0, U.reservation(cells, num_steps, num_pts, PT.grid_cap(dev))
+    return pts[:host.shape[0]], host, gen.get_offset() - off0, U.reservation(cells, num_steps, num_pts, TR.grid_cap(dev))
 
 
 def _occ_with(res, occupied_cells):
@@ -134,7 +134,7 @@ def test_draws_without_empty_voxels_and_without_occupied_ones(cuda):
     occupied, empty, counts = _lists(none.occ_grid)
     out = torch.full((2,), -5, dtype=torch.int64, device=cuda)
     pts = torch.zeros(U.capacity(512, 2, 64), 3, device=cuda)
-    U.draw_pts(PT.take(torch.Generator(cuda).manual_seed(1), 0), torch.tensor(0, dtype=torch.int32, device=cuda), counts, occupied, empty, (8, 8, 8),
+    U.draw_pts(TR.take(torch.Generator(cuda).manual_seed(1), 0), torch.tensor(0, dtype=torch.int32, device=cuda), counts, occupied, empty, (8, 8, 8),
                2, 64, pts, out)
     assert out.tolist() == [0, 1]
 

@@ -1,5 +1,5 @@
 """The perturbed one-launch step's bookkeeping of torch's random stream, on the host: the offset increment of a draw against a restatement
-of torch's launch policy, the element -> Philox call mapping, the step's reservation, and the refusals (graphics/perturb.py)."""
+of torch's launch policy, the element -> Philox call mapping, the step's reservation, and the refusals (torch_rng.py, graphics/perturb.py)."""
 import random
 import types
 
@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import torch_uniform as TU
+from neuralsim_b200 import torch_rng as TR
 from neuralsim_b200.graphics import perturb as PT
 from neuralsim_b200.graphics.neus import query_config
 
@@ -20,8 +21,8 @@ def test_inc_matches_torchs_policy(sms, threads):
     edges = [256 * cap, 4 * 256 * cap, 8 * 256 * cap]
     ns = list(range(1, 3000)) + [e + d for e in edges for d in (-257, -256, -255, -1, 0, 1, 255, 256, 257)] + [12 * 256 * cap + 3]
     for n in ns:
-        assert PT.uniform_inc(n, cap) == TU.calc_execution_policy(n, sms, threads)[0], n
-    assert PT.uniform_inc(0, cap) == 0                          # an empty draw is not launched and does not advance the offset
+        assert TR.uniform_inc(n, cap) == TU.calc_execution_policy(n, sms, threads)[0], n
+    assert TR.uniform_inc(0, cap) == 0                          # an empty draw is not launched and does not advance the offset
 
 
 @pytest.mark.parametrize("sms,threads", [(1, 1024), (2, 512)])
@@ -30,7 +31,7 @@ def test_element_mapping_matches_the_grid_stride_loop(sms, threads):
     for n in [1, 5, 255, 256, 257, 256 * cap - 1, 256 * cap, 256 * cap + 1, 4 * 256 * cap, 4 * 256 * cap + 1, 9 * 256 * cap + 77]:
         calls = TU.element_calls(n, sms, threads)
         assert sorted(calls) == list(range(n))
-        inc = PT.uniform_inc(n, cap)
+        inc = TR.uniform_inc(n, cap)
         for li, (idx, k, c) in calls.items():
             assert TU.element_call(li, n, cap) == (idx, k, c)
             assert 4 * k < inc                                  # every call lies inside the offsets the draw reserves
@@ -40,7 +41,7 @@ def test_inc_is_monotone():
     for cap in (4, 912, 1056):
         prev = 0
         for n in sorted(set(range(0, 20000, 7)) | set(range(256 * cap - 600, 256 * cap * 9, 911))):
-            v = PT.uniform_inc(n, cap)
+            v = TR.uniform_inc(n, cap)
             assert v >= prev, (cap, n)
             prev = v
 
@@ -55,9 +56,9 @@ def test_reservation_bounds_every_step():
                 n = rng.randint(0, n_rays)
                 m = rng.randint(0, n * cfg.max_steps)
                 hit = rng.randint(0, n)
-                used = PT.uniform_inc(n * 129, cap) + PT.uniform_inc(m, cap) + sum(PT.uniform_inc(hit * nf, cap) for nf in cfg.num_fine)
+                used = TR.uniform_inc(n * 129, cap) + TR.uniform_inc(m, cap) + sum(TR.uniform_inc(hit * nf, cap) for nf in cfg.num_fine)
                 assert used <= res
-            full = PT.uniform_inc(n_rays * 129, cap) + PT.uniform_inc(n_rays * cfg.max_steps, cap) + sum(PT.uniform_inc(n_rays * nf, cap) for nf in cfg.num_fine)
+            full = TR.uniform_inc(n_rays * 129, cap) + TR.uniform_inc(n_rays * cfg.max_steps, cap) + sum(TR.uniform_inc(n_rays * nf, cap) for nf in cfg.num_fine)
             assert res == full and res % 4 == 0
 
 
@@ -76,10 +77,10 @@ def test_refusals():
         PT.reservation(2 ** 31 // 129 + 1, query_config(num_coarse=128, march_cfg=dict(max_steps=1)), 1056)
     PT.reservation(2 ** 31 // 512 - 1, cfg, 1056)
     with pytest.raises(RuntimeError, match="CUDA torch.Generator"):
-        PT.cuda_generator(torch.Generator(), "cuda:0")
+        TR.cuda_generator(torch.Generator(), "cuda:0")
     with pytest.raises(RuntimeError, match="CUDA torch.Generator"):
-        PT.cuda_generator(object(), "cuda:0")
-    assert PT.seed_i64(2 ** 64 - 1) == -1 and PT.seed_i64(5) == 5
+        TR.cuda_generator(object(), "cuda:0")
+    assert TR.seed_i64(2 ** 64 - 1) == -1 and TR.seed_i64(5) == 5
 
 
 def test_static_frame_argument_checks():

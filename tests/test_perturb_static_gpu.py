@@ -28,8 +28,8 @@ ORDER_REL = ll.ORDER_REL
 
 
 def _cap():
-    from neuralsim_b200.graphics import perturb as PT
-    return PT.grid_cap(torch.device("cuda"))
+    from neuralsim_b200 import torch_rng as TR
+    return TR.grid_cap(torch.device("cuda"))
 
 
 def _gen(seed=1234, offset=40):
@@ -59,6 +59,7 @@ def _coarse_sizes():
 
 @pytest.mark.parametrize("k", range(15))
 def test_coarse_draw_equals_torch(k):
+    from neuralsim_b200 import torch_rng as TR
     from neuralsim_b200.graphics import perturb as PT
     from neuralsim_b200.graphics.raysample import batch_sample_step_linear
     n, nc1 = _coarse_sizes()[k]
@@ -79,7 +80,7 @@ def test_coarse_draw_equals_torch(k):
         ref = batch_sample_step_linear(near, far, nc1, prefix_shape=[n], perturb=True, generator=g)
         _same(t[:n], ref, f"n={n} nc1={nc1}")
         assert bool(t[n:].isnan().all())
-        assert int(nxt) == g.get_offset() and g.get_offset() - 8 * k == PT.uniform_inc(n * nc1, _cap())
+        assert int(nxt) == g.get_offset() and g.get_offset() - 8 * k == TR.uniform_inc(n * nc1, _cap())
 
 
 def _packs(P, seed):

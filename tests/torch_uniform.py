@@ -1,6 +1,6 @@
 """torch.rand on a CUDA generator restated in Python (torch's ATen/native/cuda/DistributionTemplates.h): the launch policy of a draw of
 N float32 values, the offset it advances the generator by, and which Philox call produces each element.  The perturbed one-launch step
-(neuralsim_b200/graphics/perturb.py, csrc/torch_uniform.cuh) computes the same things on the device."""
+(neuralsim_b200/torch_rng.py, csrc/torch_uniform.cuh) computes the same things on the device."""
 BLOCK = 256
 CURAND_OFFSETS = 4        # max_generator_offsets_per_curand_call
 UNROLL = 4                # float4 / float: one curand_uniform4 per loop iteration
